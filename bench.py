@@ -8,7 +8,7 @@ gradient all-reduce + Adam) on synthetic N=2048, d=256, 9-layer pairs (BASELINE.
         --master-port 29511 bench.py --gpus 8 --steps 10 --warmup 3
     python bench.py --impl reference ...      # the reference algorithm on the host CPU cores (oracle port)
 
-Prints ONE JSON line on rank 0 (contract: see the task statement / DESIGN.md section "Measurement").
+Prints ONE JSON line on rank 0 (fields: see main() and kernel_roofline()).
 """
 import argparse
 import json
@@ -23,7 +23,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-METRIC = "image-pairs/sec training SuperPoint+LightGlue N=2048 at 1/2/4/8 B200"
+METRIC = "image-pairs/sec training SuperPoint+LightGlue N=2048 at 1/2/4/8 H100"
 UNIT = "image-pairs/s"
 N_KPTS, D_DESC, N_LAYERS, N_HEADS = 2048, 256, 9, 4
 # algorithmic attention FLOPs per pair, forward + backward, no recompute counted (SURVEY.md 8d):
@@ -38,7 +38,8 @@ def measured_peaks():
             p = json.load(f)
         return {"hbm_gbs": p["hbm_gbs"], "tflops_burst": p["bf16_tflops"], "tflops_sustained": p["bf16_tflops_sustained"],
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "tflops_burst": 1590.0, "tflops_sustained": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth and dense BF16 tensor rate, not measured here
+    return {"hbm_gbs": 3350.0, "tflops_burst": 989.0, "tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
@@ -126,7 +127,7 @@ def nbytes(data):
 # ------------------------------------------------------------------------------------------------
 class CpuArm:
     """The reference's own implementation of the path on the host CPU cores (BASELINE.md section 4): the UNMODIFIED
-    reference matcher driven through its real TwoViewPipeline (oracle/reference_runner.py; installed under baseline/_ref
+    reference matcher driven through its real TwoViewPipeline (oracle/reference_runner.py; installed under oracle/_ref
     by the build, `kind: "reference"`), or, when that copy did not travel, the oracle port (`kind: "port"`).
     One step = zero_grad + forward + loss + backward + Adam on `B` pairs of the N=2048 / 9-layer workload, fp32."""
 
@@ -243,13 +244,13 @@ def cpu_baseline_sample(seconds=25.0):
 
 def gpu_eager_baseline(dev, B=4, steps=5, warmup=3):
     """The same-box GPU competitor (BASELINE.md section 4, SURVEY section 0 fact 1): the reference ships no GPU kernels,
-    so its PyTorch modules on this B200 (`.cuda()`; fp32 and `--mp bfloat16` autocast) are what the plugin replaces.
+    so its PyTorch modules on this GPU (`.cuda()`; fp32 and `--mp bfloat16` autocast) are what the plugin replaces.
     Bounded: B pairs per step (the reference YAML's per-GPU batch), a few steps, rank 0 at N=1 only."""
     from gluefactory_b200 import synthetic
     from oracle import reference_runner as R
 
     if not R.available():
-        return {"unavailable": "baseline/_ref did not travel (reference not installed)"}
+        return {"unavailable": "oracle/_ref is missing (reference not installed)"}
     conf = dict(synthetic.DEFAULT_CONF)
     w = synthetic.make_weights(conf, seed=0)
     batch = synthetic.to_device(R.pipeline_batch(synthetic.make_pairs(B, N_KPTS, seed=1234)), dev)
@@ -287,11 +288,13 @@ def main():
     ap.add_argument("--batch", type=int, default=int(os.environ.get("LGB200_BENCH_BATCH", "32")), help="pairs per GPU per step")
     ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
     ap.add_argument("--kpts", type=int, default=2048, help="keypoints per image: 2048 = BASELINE configs[2] (the headline), "
-                    "1024 = configs[1] (recorded under profiles/, not the driver's line)")
+                    "1024 = configs[1]")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-kernel-timing", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel from the host instead of replaying "
                     "one CUDA graph of the whole training step")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last timed step computed "
+                    "(losses, and a fixed sample of the updated parameters and their gradients) as DIR/<name>.npy")
     args = ap.parse_args()
 
     global N_KPTS, ATTN_FLOPS_PER_PAIR
@@ -357,11 +360,13 @@ def main():
     if use_graph:
         trainer.capture(pool_dev[0], dev, warmup=2)
 
+    last = {}
+
     def step_resident(i):
         if use_graph:
-            trainer.step_graphed(pool_dev[i % len(pool_dev)])  # device-to-device copy into the static inputs + replay
+            last["out"] = trainer.step_graphed(pool_dev[i % len(pool_dev)])  # D2D copy into the static inputs + replay
         else:
-            trainer.step(pool_dev[i % len(pool_dev)])
+            last["out"] = trainer.step(pool_dev[i % len(pool_dev)])
 
     host_loss = []
 
@@ -380,6 +385,8 @@ def main():
         ms = timed(step_resident, args.steps)
         launches = launches_per_step * args.steps
     clocks = clk.summary()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, trainer, *last["out"])
     # dominant kernel, timed live with CUDA events on the launching stream (second pass, so the
     # event records do not perturb the headline number)
     roof = None
@@ -400,7 +407,7 @@ def main():
                                "all-reduce+Adam",
                    "pairs_per_gpu_per_step": B, "global_batch": B * world, "parallelism": f"dp{world}",
                    "launch": "cuda-graph replay of the whole step" if use_graph else "eager (host launches)",
-                   "l2": "per-step working set (activations + N x N similarities, >1 GB) exceeds the 126 MB L2; inputs rotate",
+                   "l2": "per-step working set (activations + N x N similarities, >1 GB) exceeds the 50 MB L2; inputs rotate",
                    "attention_roofline_frac": value / world * ATTN_FLOPS_PER_PAIR / (measured_peaks()["tflops_sustained"] * 1e12)},
         "clocks": clocks,
         "e2e": {"value": pairs / (ms_e2e / 1e3), "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4,
@@ -424,6 +431,26 @@ def main():
         dist.barrier()
         sys.stdout.flush()
         os._exit(0)
+
+
+def dump_outputs(out_dir, trainer, loss, losses, sample=1 << 20):
+    """The last timed step's results as .npy files: the loss (float64), every per-pair loss term, and the updated flat
+    parameters and their gradients at a fixed, seeded sample of `sample` positions (the full vectors exceed 64 MB)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": loss.detach().double().reshape(-1)}
+    for k, v in losses.items():
+        if torch.is_tensor(v):
+            arrays[f"losses_{k}"] = v.detach().float().reshape(-1)
+    flat, grad = trainer.fp.flat, trainer.fp.grad
+    n = flat.numel()
+    idx = torch.randperm(n, generator=torch.Generator().manual_seed(0))[:min(sample, n)].sort().values.to(flat.device)
+    arrays["sample_index"] = idx.double()
+    arrays["params_sample"] = flat[idx].float()
+    arrays["grads_sample"] = grad.reshape(-1)[idx].float()
+    for k, v in arrays.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), v.cpu().numpy())
 
 
 def kernel_roofline(trainer, pool_dev, B, dev):
@@ -455,14 +482,6 @@ def kernel_roofline(trainer, pool_dev, B, dev):
     C = 2 * N_KPTS * N_KPTS * D_DESC * B  # one all-heads contraction for every pair of the batch
     alg = {("lgb200_attn_fwd", "self"): 4 * C, ("lgb200_attn_fwd", "cross"): 3 * C,
            ("lgb200_attn_bwd", "self"): 8 * C, ("lgb200_attn_bwd", "cross"): 6 * C}
-    traffic = {}
-    tpath = os.path.join(ROOT, "profiles", "r02_roofline_traffic.json")
-    if os.path.exists(tpath):
-        with open(tpath) as f:
-            tj = json.load(f)
-        # only quote a capture taken at this run's batch size and keypoint count
-        if tj.get("sequences_per_launch") == 2 * B and tj.get("keypoints", 2048) == N_KPTS:
-            traffic = tj.get("dram_bytes_per_launch", {})
     kernels = {}
     for (name, kind), ts in sorted(groups.items()):
         avg_ms = sum(ts) / len(ts)
@@ -474,10 +493,9 @@ def kernel_roofline(trainer, pool_dev, B, dev):
     secs = sum(v["avg_launch_ms"] * v["launches_timed"] for _, v in bw) * 1e-3
     n = sum(v["launches_timed"] for _, v in bw)
     achieved = flops / secs / 1e12
-    return {"kernel": "lgb200_attn_bwd (attn_bwd_prep_fused + attn_bwd_fused + dq_convert; self 8C and cross 6C launches)",
+    return {"kernel": "lgb200_attn_bwd (attn_bwd_prep_fused + attn_bwd_dq + attn_bwd_dkv; self 8C and cross 6C launches)",
             "bound": "tensor", "achieved": achieved, "peak": peaks["tflops_sustained"], "unit": "TFLOP/s",
-            "frac": achieved / peaks["tflops_sustained"], "traffic": traffic.get("lgb200_attn_bwd"),
-            "traffic_source": "profiles/r02_roofline_traffic.json (ncu --set full of this command at this batch size)" if traffic else None,
+            "frac": achieved / peaks["tflops_sustained"],
             "avg_launch_ms": secs / n * 1e3, "launches_timed": n, "kernels": kernels,
             "peak_source": peaks["source"] + ", sustained (kernel timed inside a long step)"}
 

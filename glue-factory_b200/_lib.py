@@ -2,7 +2,7 @@
 
 The shared library is built in-tree by `__graft_entry__.build()` at
 glue-factory_b200/csrc/liblgb200.so.  There is no fallback: if the library is
-missing, or the device is not a B200, every entry point raises.
+missing, or the device is not an H100 (sm_90), every entry point raises.
 """
 import ctypes
 import os
@@ -97,7 +97,7 @@ def load(check_device=True):
         import torch
 
         if not torch.cuda.is_available():
-            raise Lgb200Error("no CUDA device: the lgb200 matcher runs on B200 (sm_100a) only, there is no CPU fallback")
+            raise Lgb200Error("no CUDA device: the lgb200 matcher runs on H100 (sm_90a) only, there is no CPU fallback")
         rc = _lib.lgb200_check_device()
         if rc != 0:
             raise Lgb200Error(_lib.lgb200_last_error().decode())

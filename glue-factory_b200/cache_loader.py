@@ -9,7 +9,7 @@ box -- `random_c` --, descriptors with uniform noise between their min and max -
 depths with zeros; models/utils/misc.py:18-55).  Padding keypoints are real inputs of the matcher (they are NOT
 masked, SURVEY Appendix C.9), so only the distributions matter, not the random stream.
 
-What is different on a B200 feeding thousands of pairs per second:
+What is different on an H100 feeding thousands of pairs per second:
   * storage back end `FeaturePack`: one flat little-endian file per export + a JSON index, memory-mapped; a record is the
     fp16 arrays of one image laid out back to back, so assembling a batch is B memcpys into a PINNED staging buffer
     (no per-key Python objects, no HDF5 chunk decoding).  `FeaturePack.write` builds it from any mapping

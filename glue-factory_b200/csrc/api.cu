@@ -119,7 +119,7 @@ int device_sm_count() {
   if (dev >= 0 && dev < 16 && counts[dev]) return counts[dev];
   int n = 0;
   cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  if (n <= 0) n = 148;
+  if (n <= 0) n = 132;  // H100 SXM
   if (dev >= 0 && dev < 16) counts[dev] = n;
   return n;
 }
@@ -145,8 +145,8 @@ int lgb200_check_device(void) {
   int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-  LGB_REQUIRE(major == 10, kErrUnsupported, "device %d is sm_%d%d; this library is built for sm_100a only", dev, major,
-              minor);
+  LGB_REQUIRE(major == 9 && minor == 0, kErrUnsupported, "device %d is sm_%d%d; this library is built for sm_90a only", dev,
+              major, minor);
   return 0;
 }
 

@@ -1,24 +1,23 @@
 // Assignment head fused with its similarity GEMM (SURVEY K8+K9; lightglue.py:256-290, losses.py:6-25):
-// sim = mdesc0 . mdesc1^T is produced tile by tile in tensor memory and consumed there -- it is never written to HBM
-// (round 1 wrote 16.8 MB fp32 per pair per supervised layer, re-read it three times and kept it for backward).
+// sim = mdesc0 . mdesc1^T is produced tile by tile in registers and consumed there -- it is never written to HBM.
 //
 // Three passes over the same skeleton (persistent CTAs, one per SM):
 //   work item = (direction, pair b, 128-row panel).  direction 0: panel rows = keypoints of image 0, columns = all
-//   keypoints of image 1 (thread == row i == TMEM lane: everything per ROW of sim); direction 1: the transposed
-//   problem (thread == column j of sim: everything per COLUMN).  Running both directions doubles the (cheap, tensor-
-//   core) contraction but makes every reduction a per-thread running value: no column partials, no merge kernels,
-//   no atomics, deterministic.
-//   The panel (A, 128 x D bf16) stays resident in shared memory for the item; 128-column tiles of the other image
-//   (B, 128 x D) stream through a 2-stage TMA ring; S = A B^T (M128 N128, D/16 MMAs) lands in one of two TMEM buffers
-//   so the MMA warp runs a tile ahead of the 16 epilogue warps (four per TMEM lane quarter, 32 columns each).
+//   keypoints of image 1 (everything per ROW of sim); direction 1: the transposed problem (everything per COLUMN).
+//   Running both directions doubles the (cheap, tensor-core) contraction but makes every reduction a per-row running
+//   value: no column partials, no merge kernels, no atomics, deterministic.
+//   The panel (A, 128 x D bf16) stays resident in shared memory for the item; 64-column tiles of the other image
+//   (B, 64 x D) stream through a 3-stage TMA ring.  Two consumer warpgroups own 64 panel rows each and form
+//   S = A B^T (64 x 64 per warpgroup, D/16 wgmma m64n64k16) in registers; a row is shared by the four lanes of a
+//   quad (16 of the tile's columns each), whose running values are merged at the end of the item.
 //
-//   LSE  : running (max, sum exp2) per thread -> lse_row [B,M] (dir 0), lse_col [B,N] (dir 1).
+//   LSE  : running (max, sum exp2) per row -> lse_row [B,M] (dir 0), lse_col [B,N] (dir 1).
 //   STATS: scores in the reference's association order ((s - lse_r) + (s - lse_c)) + (lsig0 + lsig1); running
-//          max / first argmax per thread -> rowmax/rowarg (dir 0), colmax/colarg (dir 1); dir 0 also gathers
+//          max / first argmax per row -> rowmax/rowarg (dir 0), colmax/colarg (dir 1); dir 0 also gathers
 //          sum_j gt_ij (2 s_ij - lse_r_i - lse_c_j) from the boolean assignment.  No MUFU work at all.
 //   BWD  : dsim = gc (2 gt - softmax_row rowcnt - softmax_col colcnt) recomputed from S and the two LSE vectors,
-//          rounded to bf16 and written IN PLACE over the S columns it came from (tcgen05.st), then
-//          d(mdesc) panel (128 x D fp32, TMEM) += dsim (TMEM A operand) . B tile (the same smem bytes, MN-major):
+//          rounded to bf16 into register A fragments, then
+//          d(mdesc) panel (64 x D fp32 per warpgroup, registers) += dsim . B tile (the same smem bytes, MN-major):
 //          dir 0 yields d(mdesc0) = dsim mdesc1, dir 1 yields d(mdesc1) = dsim^T mdesc0.  dsim never exists in HBM.
 // All three are exact restatements of assign_lse / assign_scores / assign_bwd (assign.cu) on the fp32 accumulator.
 #include "common.cuh"
@@ -28,16 +27,16 @@
 namespace lgb {
 
 constexpr int AT_R = 128;                  // panel rows
-constexpr int AT_C = 128;                  // columns per tile
+constexpr int AT_C = 64;                   // columns per tile
 constexpr int AT_KBLK = 64;                // K elements per smem block (one 128-byte swizzle row)
-constexpr int AT_BLK = AT_R * AT_KBLK * 2; // 16 KiB
+constexpr int AT_ABLK = AT_R * AT_KBLK * 2; // 16 KiB
+constexpr int AT_BBLK = AT_C * AT_KBLK * 2; // 8 KiB
 constexpr int AT_MAXKB = 4;                // D <= 256
-constexpr int AT_STAGES = 2;
-constexpr int AT_EWARPS = 16;
-constexpr int AT_THREADS = (AT_EWARPS + 2) * 32;
-constexpr int AT_SCR = AT_EWARPS * 2 * 32 * 4 + 3 * 384 * 4;  // per-warp column vectors + quarter-merge scratch
-constexpr int AT_SMEM = (1 + AT_STAGES) * AT_MAXKB * AT_BLK + AT_SCR + 256;
-constexpr int AT_ACC_COL = 256;            // TMEM: S0 [0,128) S1 [128,256) | d(mdesc) accumulator [256, 256 + D)
+constexpr int AT_STAGES = 3;
+constexpr int AT_THREADS = 2 * 128 + 32;   // two consumer warpgroups + the producer warp
+constexpr int AT_PRODUCER = 8;
+constexpr float kLog2e_at = 1.4426950408889634f;
+constexpr int AT_SMEM = AT_MAXKB * AT_ABLK + AT_STAGES * AT_MAXKB * AT_BBLK + 256;
 
 enum { AT_LSE = 0, AT_STATS = 1, AT_BWD = 2 };
 
@@ -54,26 +53,17 @@ struct AssignTcArgs {
   __nv_bfloat16* dmd0; __nv_bfloat16* dmd1;  // BWD out: [B*M, D], [B*N, D]
 };
 
-__device__ __forceinline__ void bar_epi() { asm volatile("bar.sync 1, %0;" ::"n"(AT_EWARPS * 32) : "memory"); }
-
 template <int MODE>
 __global__ void __launch_bounds__(AT_THREADS, 1)
     assign_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1, AssignTcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sA = smem;
-  uint8_t* sB = smem + AT_MAXKB * AT_BLK;
-  float* sVec = reinterpret_cast<float*>(smem + (1 + AT_STAGES) * AT_MAXKB * AT_BLK);  // [16 warps][2][32]
-  float* sMerge = sVec + AT_EWARPS * 2 * 32;                                              // [3][3][128]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (1 + AT_STAGES) * AT_MAXKB * AT_BLK + AT_SCR);
-  uint64_t* a_full = bars;          // 1
-  uint64_t* a_empty = bars + 1;     // 1
-  uint64_t* b_full = bars + 2;      // [2]
-  uint64_t* b_empty = bars + 4;     // [2]
-  uint64_t* s_full = bars + 6;      // [2]
-  uint64_t* s_done = bars + 8;      // [2]  epilogue finished with S buffer (LSE/STATS: free; BWD: dsim written)
-  uint64_t* acc_full = bars + 10;   // BWD
-  uint64_t* acc_empty = bars + 11;  // BWD
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 12);
+  uint8_t* sB = smem + AT_MAXKB * AT_ABLK;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + AT_STAGES * AT_MAXKB * AT_BBLK);
+  uint64_t* a_full = bars;                   // 1
+  uint64_t* a_empty = bars + 1;              // 1
+  uint64_t* b_full = bars + 2;               // [AT_STAGES]
+  uint64_t* b_empty = b_full + AT_STAGES;    // [AT_STAGES]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int B = a.B, M = a.M, N = a.N, D = a.D;
@@ -84,26 +74,18 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
   if (threadIdx.x == 0) {
     if (smem_u32(smem) & 1023u) __trap();
     mbar_init(a_full, 1);
-    mbar_init(a_empty, 1);
-    for (int s = 0; s < 2; ++s) {
+    mbar_init(a_empty, 2);
+    for (int s = 0; s < AT_STAGES; ++s) {
       mbar_init(&b_full[s], 1);
-      mbar_init(&b_empty[s], 1);
-      mbar_init(&s_full[s], 1);
-      mbar_init(&s_done[s], AT_EWARPS);
+      mbar_init(&b_empty[s], 2);
     }
-    mbar_init(acc_full, 1);
-    mbar_init(acc_empty, AT_EWARPS);
     mbar_fence_init();
   }
-  if (warp == AT_EWARPS && lane == 0) {
+  if (warp == AT_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tm0);
     tma_prefetch_desc(&tm1);
   }
-  if (warp == AT_EWARPS + 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // item -> (dir, b, panel); items of one pair are consecutive so its tiles are shared through L2
   auto decode = [&](int item, int& dir, int& b, int& p) {
@@ -113,7 +95,7 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
     p = dir ? r - PM : r;
   };
 
-  if (warp == AT_EWARPS) {
+  if (warp == AT_PRODUCER) {
     // ------------------------------------------------------------------ TMA producer
     if (lane == 0) {
       int it = 0, g = 0;
@@ -125,312 +107,221 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
         const int ncols = dir ? M : N;
         const int ntiles = (ncols + AT_C - 1) / AT_C;
         mbar_wait(a_empty, (it & 1) ^ 1);
-        mbar_expect_tx(a_full, KB * AT_BLK);
-        for (int kb = 0; kb < KB; ++kb) tma_load_3d(sA + kb * AT_BLK, tA, a_full, kb * AT_KBLK, p * AT_R, b);
+        mbar_expect_tx(a_full, KB * AT_ABLK);
+        for (int kb = 0; kb < KB; ++kb)
+          for (int hf = 0; hf < 2; ++hf)  // two 64-row boxes per block: the same bytes as one 128-row box
+            tma_load_3d(sA + kb * AT_ABLK + hf * AT_BBLK, tA, a_full, kb * AT_KBLK, p * AT_R + hf * AT_C, b);
         for (int t = 0; t < ntiles; ++t, ++g) {
-          const int s = g & 1;
-          mbar_wait(&b_empty[s], ((g >> 1) & 1) ^ 1);
-          mbar_expect_tx(&b_full[s], KB * AT_BLK);
+          const int s = g % AT_STAGES;
+          mbar_wait(&b_empty[s], ((g / AT_STAGES) & 1) ^ 1);
+          mbar_expect_tx(&b_full[s], KB * AT_BBLK);
           for (int kb = 0; kb < KB; ++kb)
-            tma_load_3d(sB + (s * AT_MAXKB + kb) * AT_BLK, tB, &b_full[s], kb * AT_KBLK, t * AT_C, b);
+            tma_load_3d(sB + (s * AT_MAXKB + kb) * AT_BBLK, tB, &b_full[s], kb * AT_KBLK, t * AT_C, b);
         }
       }
     }
-  } else if (warp == AT_EWARPS + 1) {
-    // ------------------------------------------------------------------ MMA issuer (warp-convergent, elected lane)
-    constexpr uint32_t idesc_s = make_idesc_bf16(AT_R, AT_C, 0, 0);
-    const uint32_t idesc_acc = make_idesc_bf16(AT_R, D, 0, 1);  // dsim (TMEM) x B tile MN-major, N = D
-    const uint64_t dA = make_smem_desc(smem_u32(sA), 16, 1024);
-    const uint64_t dBk = make_smem_desc(smem_u32(sB), 16, 1024);
-    const uint64_t dBm = make_smem_desc(smem_u32(sB), AT_BLK, 1024);  // 64-wide channel chunks AT_BLK apart
-    const bool leader = elect_one();
-    int it = 0, g = 0;
-    for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++it) {
-      int dir, b, p;
-      decode(item, dir, b, p);
-      const int ncols = dir ? M : N;
-      const int ntiles = (ncols + AT_C - 1) / AT_C;
-      mbar_wait(a_full, it & 1);
-      tc_fence_after();
-      auto issue_acc = [&](int gg, bool first) {  // d(mdesc) += dsim(gg) . B(gg)
-        const int s = gg & 1;
-        mbar_wait(&s_done[s], (gg >> 1) & 1);
-        tc_fence_after();
-        if (first) {
-          mbar_wait(acc_empty, (it & 1) ^ 1);
-          tc_fence_after();
-        }
-        if (leader) {
-          const uint64_t so = (uint64_t)((s * AT_MAXKB * AT_BLK) >> 4);
-          const uint32_t abase = tmem_base + s * AT_C;
+    return;
+  }
+  // ------------------------------------------------------------------ consumer warpgroups
+  const int wg = threadIdx.x >> 7, t4 = lane & 3;
+  const bool signal = (threadIdx.x & 127) == 0;
+  const uint64_t dA = make_smem_desc(smem_u32(sA) + wg * 8192, 8192, 1024);
+  const uint64_t dB = make_smem_desc(smem_u32(sB), 8192, 1024);
+  const float c2 = a.alpha * kLog2e_at;
+  int it = 0, g = 0;
+  for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++it) {
+    int dir, b, p;
+    decode(item, dir, b, p);
+    const int nrows = dir ? N : M, ncols = dir ? M : N;
+    const int ntiles = (ncols + AT_C - 1) / AT_C;
+    // per-row constants of this thread's two rows
+    bool rok[2];
+    int64_t ro[2];
+    float lse_mine[2] = {0.f, 0.f}, ls_mine[2] = {0.f, 0.f}, coef_mine[2] = {0.f, 0.f};
+    const uint8_t* grow[2] = {nullptr, nullptr};  // the rows of the boolean assignment (or of its transpose)
+    const float gc = MODE == AT_BWD ? a.gcoef[b] : 0.f;
 #pragma unroll
-          for (int kk = 0; kk < AT_C / 16; ++kk)  // quarter cq of the tile wrote its packed dsim at column cq*32
-            umma_bf16_ts(tmem_base + AT_ACC_COL, abase + (kk >> 1) * 32 + (kk & 1) * 8, dBm + so + (uint64_t)(kk * 128),
-                         idesc_acc, (first && kk == 0) ? 0u : 1u);
-          umma_commit(&b_empty[s]);
-        }
-        __syncwarp();
-      };
-      for (int t = 0; t < ntiles; ++t, ++g) {
-        const int s = g & 1;
-        mbar_wait(&b_full[s], (g >> 1) & 1);
-        if (MODE != AT_BWD) mbar_wait(&s_done[s], ((g >> 1) & 1) ^ 1);  // epilogue drained this S buffer (2 tiles ago)
-        tc_fence_after();
-        if (leader) {
-          const uint64_t so = (uint64_t)((s * AT_MAXKB * AT_BLK) >> 4);
-          for (int kb = 0; kb < KB; ++kb) {
-#pragma unroll
-            for (int kk = 0; kk < AT_KBLK / 16; ++kk)
-              umma_bf16(tmem_base + s * AT_C, dA + (uint64_t)((kb * AT_BLK) >> 4) + (uint64_t)(kk * 2),
-                        dBk + so + (uint64_t)((kb * AT_BLK) >> 4) + (uint64_t)(kk * 2), idesc_s, (kb | kk) != 0 ? 1u : 0u);
-          }
-          umma_commit(&s_full[s]);
-          if (MODE != AT_BWD) umma_commit(&b_empty[s]);
-          if (t == ntiles - 1) umma_commit(a_empty);
-        }
-        __syncwarp();
-        if (MODE == AT_BWD && t >= 1) issue_acc(g - 1, t == 1);
-      }
+    for (int i = 0; i < 2; ++i) {
+      const int row = p * AT_R + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+      rok[i] = row < nrows;
+      ro[i] = (int64_t)b * nrows + (rok[i] ? row : 0);
+      if (MODE != AT_LSE) lse_mine[i] = (dir ? a.lse_col : a.lse_row)[ro[i]];
+      if (MODE == AT_STATS) ls_mine[i] = (dir ? a.ls1 : a.ls0)[ro[i]];
       if (MODE == AT_BWD) {
-        issue_acc(g - 1, ntiles == 1);
-        if (leader) umma_commit(acc_full);
-        __syncwarp();
+        coef_mine[i] = rok[i] ? gc * (dir ? a.colcnt : a.rowcnt)[ro[i]] : 0.f;
+        lse_mine[i] *= kLog2e_at;
+        grow[i] = (dir ? a.gt_t : a.gt) + ro[i] * ncols;
       }
+      if (MODE == AT_STATS && !dir && a.gt) grow[i] = a.gt + ro[i] * ncols;
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue warps
-    // 16 warps = 4 per scheduler: TMEM lane quarter q (rows), column quarter cq (32 of the tile's 128 columns)
-    const int q = warp & 3, cq = warp >> 2;
-    const int r = q * 32 + lane;                   // row within the panel == TMEM lane
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    float* myvec = sVec + warp * 64;               // [2][32]: this warp's slice of the two per-column vectors
-    constexpr float kLog2e = 1.4426950408889634f;
-    const float c2 = a.alpha * kLog2e;
-    int it = 0, g = 0;
-    for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++it) {
-      int dir, b, p;
-      decode(item, dir, b, p);
-      const int nrows = dir ? N : M, ncols = dir ? M : N;
-      const int ntiles = (ncols + AT_C - 1) / AT_C;
-      const int row = p * AT_R + r;
-      const bool rok = row < nrows;
-      const int64_t ro = (int64_t)b * nrows + (rok ? row : 0);
-      // per-row constants
-      float lse_mine = 0.f, ls_mine = 0.f, coef_mine = 0.f, gc = 0.f;
-      if (MODE != AT_LSE) lse_mine = (dir ? a.lse_col : a.lse_row)[ro];
-      if (MODE == AT_STATS) ls_mine = (dir ? a.ls1 : a.ls0)[ro];
-      if (MODE == AT_BWD) {
-        gc = a.gcoef[b];
-        coef_mine = rok ? gc * (dir ? a.colcnt : a.rowcnt)[ro] : 0.f;
-        lse_mine *= kLog2e;
+    const float* cvec_lse = (dir ? a.lse_row : a.lse_col) + (int64_t)b * ncols;  // per-column vectors of the tile
+    const float* cvec_b = MODE == AT_STATS ? (dir ? a.ls0 : a.ls1) + (int64_t)b * ncols
+                          : MODE == AT_BWD ? (dir ? a.rowcnt : a.colcnt) + (int64_t)b * ncols : nullptr;
+    // running values (this lane's 16 columns of every tile)
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // LSE (log2 domain)
+    float best[2] = {-INFINITY, -INFINITY}, psum[2] = {0.f, 0.f};    // STATS
+    int besti[2] = {0x7fffffff, 0x7fffffff};
+    float acc[AT_MAXKB][32];                                         // BWD: d(mdesc) rows, 64 channels per block
+    if (MODE == AT_BWD) {
+#pragma unroll
+      for (int c = 0; c < AT_MAXKB; ++c)
+#pragma unroll
+        for (int e = 0; e < 32; ++e) acc[c][e] = 0.f;
+    }
+    mbar_wait(a_full, it & 1);
+    for (int t = 0; t < ntiles; ++t, ++g) {
+      const int s = g % AT_STAGES;
+      const uint64_t sb = dB + (uint64_t)((s * AT_MAXKB * AT_BBLK) >> 4);
+      mbar_wait(&b_full[s], (g / AT_STAGES) & 1);
+      float sv[32];
+      wgmma_fence();
+      for (int kb = 0; kb < KB; ++kb) {
+#pragma unroll
+        for (int kk = 0; kk < AT_KBLK / 16; ++kk)
+          wgmma_m64n64_ss<0, 0>(sv, dA + (uint64_t)((kb * AT_ABLK) >> 4) + kk * 2,
+                                sb + (uint64_t)((kb * AT_BBLK) >> 4) + kk * 2, (kb | kk) != 0);
       }
-      const float* cvec_lse = (dir ? a.lse_row : a.lse_col) + (int64_t)b * ncols;  // per-column vectors of the tile
-      const float* cvec_b = MODE == AT_STATS ? (dir ? a.ls0 : a.ls1) + (int64_t)b * ncols
-                            : MODE == AT_BWD ? (dir ? a.rowcnt : a.colcnt) + (int64_t)b * ncols : nullptr;
-      const uint8_t* grow = nullptr;  // this thread's row of the boolean assignment (or of its transpose)
-      if (MODE == AT_BWD) grow = (dir ? a.gt_t : a.gt) + ro * ncols;
-      if (MODE == AT_STATS && !dir && a.gt) grow = a.gt + ro * ncols;
-      const bool gvec = (ncols & 15) == 0;
-      // running values
-      float m_run = -INFINITY, l_run = 0.f;     // LSE (log2 domain)
-      float best = -INFINITY, psum = 0.f;       // STATS
-      int besti = 0x7fffffff;
-
-      for (int t = 0; t < ntiles; ++t, ++g) {
-        const int s = g & 1;
-        const int j0 = t * AT_C + cq * 32;      // first column of this warp's quarter
-        const bool tail = j0 + 32 > ncols;
-        if (MODE != AT_LSE) {                   // stage this warp's 32 per-column values, coalesced
-          __syncwarp();
-          const int j = j0 + lane;
-          float v0 = 0.f, v1 = 0.f;
-          if (j < ncols) {
-            v0 = cvec_lse[j];
-            v1 = cvec_b[j];
-          }
-          if (MODE == AT_BWD) {
-            v0 = j < ncols ? v0 * kLog2e : INFINITY;  // exp2(x - inf) = 0 for columns past the end
-            v1 *= gc;
-          } else {
-            v0 = j < ncols ? v1 - v0 : -INFINITY;     // STATS: other side's (log sigmoid - lse); -inf masks the tail
-          }
-          myvec[lane] = v0;
-          myvec[32 + lane] = v1;
-          __syncwarp();
-        }
-        uint32_t gw[8];  // 32 mask bytes of this thread's row (registers: constant indices only)
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_hold(sv);
+      if (MODE != AT_BWD && signal) mbar_arrive(&b_empty[s]);  // S is in registers: the tile's stage is free
+      const int j0 = t * AT_C + 2 * t4;  // column of sv[0]; sv[4jj + 2i + e] is column j0 + 8jj + e of row i
+      if (MODE == AT_LSE) {
 #pragma unroll
-        for (int e = 0; e < 8; ++e) gw[e] = 0u;
-        if (grow && !tail && gvec) {
+        for (int i = 0; i < 2; ++i) {
+          float mx = -INFINITY;
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const uint4 u = *reinterpret_cast<const uint4*>(grow + j0 + 16 * e);
-            gw[4 * e] = u.x; gw[4 * e + 1] = u.y; gw[4 * e + 2] = u.z; gw[4 * e + 3] = u.w;
-          }
-        } else if (grow) {
+          for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
-          for (int e = 0; e < 8; ++e) {
-#pragma unroll
-            for (int u = 0; u < 4; ++u)
-              if (j0 + 4 * e + u < ncols) gw[e] |= (uint32_t)grow[j0 + 4 * e + u] << (8 * u);
-          }
-        }
-        mbar_wait(&s_full[s], (g >> 1) & 1);
-        tc_fence_after();
-        float sv[32];
-        tmem_ld32(t_lane + s * AT_C + cq * 32, sv);
-        tmem_ld_wait();
-        if (MODE == AT_LSE) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&s_done[s]);  // S is in registers: the MMA warp may overwrite the buffer
-          if (tail) {
-#pragma unroll
-            for (int e = 0; e < 32; ++e)
-              if (j0 + e >= ncols) sv[e] = -INFINITY;
-          }
-          float mx = sv[0];
-#pragma unroll
-          for (int e = 1; e < 32; ++e) mx = fmaxf(mx, sv[e]);
-          // alpha > 0: max commutes with the scale.  All-masked quarter (j0 >= ncols): mx = -inf, contributes nothing.
-          const float m_new = fmaxf(m_run, mx * c2);
+            for (int e = 0; e < 2; ++e) {
+              float& x = sv[4 * jj + 2 * i + e];
+              if (j0 + 8 * jj + e >= ncols) x = -INFINITY;
+              mx = fmaxf(mx, x);
+            }
+          // alpha > 0: max commutes with the scale.  All-masked columns: mx = -inf, contributes nothing.
+          const float m_new = fmaxf(m_run[i], mx * c2);
           if (m_new > -INFINITY) {
             float sum = 0.f;
 #pragma unroll
-            for (int e = 0; e < 32; ++e) sum += fast_exp2(fmaf(sv[e], c2, -m_new));
-            l_run = l_run * fast_exp2(m_run - m_new) + sum;
-            m_run = m_new;
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) sum += fast_exp2(fmaf(sv[4 * jj + 2 * i + e], c2, -m_new));
+            l_run[i] = l_run[i] * fast_exp2(m_run[i] - m_new) + sum;
+            m_run[i] = m_new;
           }
-        } else if (MODE == AT_STATS) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&s_done[s]);
-          // score_ij = (2 alpha S_ij + [lsig - lse]_other(j)) + [lsig - lse]_mine: the second bracket is constant along
-          // this thread's sweep, so the running max / first argmax is taken over the first term only (an FMA and an
-          // FMNMX per element) and the constant is added when the result is written.  (assign_scores in assign.cu keeps
-          // the reference's association order for the fp32 parity path; the two agree to fp32 rounding.)
-          const float a2 = 2.f * a.alpha;
-          float cmax = -INFINITY;
-#pragma unroll
-          for (int e4 = 0; e4 < 8; ++e4) {
-            const float4 cv = *reinterpret_cast<const float4*>(myvec + e4 * 4);
-            sv[e4 * 4] = fmaf(sv[e4 * 4], a2, cv.x); sv[e4 * 4 + 1] = fmaf(sv[e4 * 4 + 1], a2, cv.y);
-            sv[e4 * 4 + 2] = fmaf(sv[e4 * 4 + 2], a2, cv.z); sv[e4 * 4 + 3] = fmaf(sv[e4 * 4 + 3], a2, cv.w);
-            cmax = fmaxf(fmaxf(cmax, fmaxf(sv[e4 * 4], sv[e4 * 4 + 1])), fmaxf(sv[e4 * 4 + 2], sv[e4 * 4 + 3]));
-            if (gw[e4] != 0u) {  // a ground-truth positive in these four columns (rare): sum_j gt (2 s - lse_r - lse_c)
-#pragma unroll
-              for (int u = 0; u < 4; ++u)
-                if ((gw[e4] >> (8 * u)) & 0xffu) {
-                  const int e = e4 * 4 + u;
-                  // 2 alpha S = sv[e] - cv; the other side's lse comes from memory, mine from the register
-                  const float two_x = sv[e] - myvec[e];
-                  psum += two_x - lse_mine - cvec_lse[j0 + e];
-                }
-            }
-          }
-          if (cmax > best) {  // a new running maximum is rare (~ln(columns) times per row): find its first position
-            best = cmax;
-#pragma unroll
-            for (int e = 31; e >= 0; --e)
-              if (sv[e] == cmax) besti = j0 + e;
-          }
-        } else {  // AT_BWD
-          const float two_gc = 2.f * gc;
-          uint32_t pw[16];
-#pragma unroll
-          for (int e4 = 0; e4 < 8; ++e4) {
-            const float4 lc = *reinterpret_cast<const float4*>(myvec + e4 * 4);
-            const float4 cc = *reinterpret_cast<const float4*>(myvec + 32 + e4 * 4);
-            const float lcv[4] = {lc.x, lc.y, lc.z, lc.w}, ccv[4] = {cc.x, cc.y, cc.z, cc.w};
-            float d[4];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              const int e = e4 * 4 + u;
-              float v = ((gw[e4] >> (8 * u)) & 0xffu) ? two_gc : 0.f;
-              v = fmaf(-fast_exp2(fmaf(sv[e], c2, -lse_mine)), coef_mine, v);
-              if (ccv[u] != 0.f) v = fmaf(-fast_exp2(fmaf(sv[e], c2, -lcv[u])), ccv[u], v);  // warp-uniform branch
-              d[u] = (tail && j0 + e >= ncols) ? 0.f : v;
-            }
-            pw[e4 * 2] = pack_bf16(d[0], d[1]);
-            pw[e4 * 2 + 1] = pack_bf16(d[2], d[3]);
-          }
-          // dsim (bf16, two columns per 32-bit word) over the first 16 columns of this warp's own 32 S columns
-          tmem_st16(t_lane + s * AT_C + cq * 32, pw);
-          tmem_st_wait();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&s_done[s]);
         }
-      }
-
-      // ---- end of item: merge the four column quarters (LSE / STATS) or drain the accumulator (BWD)
-      if (MODE == AT_LSE) {
-        if (cq) { sMerge[(cq - 1) * 256 + r] = m_run; sMerge[(cq - 1) * 256 + 128 + r] = l_run; }
-        bar_epi();
-        if (cq == 0) {
-          float mn = m_run;
-#pragma unroll
-          for (int k = 0; k < 3; ++k) mn = fmaxf(mn, sMerge[k * 256 + r]);
-          float l = l_run * fast_exp2(m_run - mn);
-#pragma unroll
-          for (int k = 0; k < 3; ++k) l += sMerge[k * 256 + 128 + r] * fast_exp2(sMerge[k * 256 + r] - mn);
-          if (rok) (dir ? a.lse_col : a.lse_row)[ro] = (mn + log2f(l)) * 0.6931471805599453f;
-        }
-        bar_epi();
       } else if (MODE == AT_STATS) {
-        if (cq) {
-          sMerge[(cq - 1) * 384 + r] = best;
-          reinterpret_cast<int*>(sMerge)[(cq - 1) * 384 + 128 + r] = besti;
-          sMerge[(cq - 1) * 384 + 256 + r] = psum;
-        }
-        bar_epi();
-        if (cq == 0 && rok) {
+        // score_ij = (2 alpha S_ij + [lsig - lse]_other(j)) + [lsig - lse]_mine: the second bracket is constant along
+        // the row, so the running max / first argmax is taken over the first term only and the constant is added
+        // when the result is written.  (assign_scores in assign.cu keeps the reference's association order for the
+        // fp32 parity path; the two agree to fp32 rounding.)
+        const float a2 = 2.f * a.alpha;
 #pragma unroll
-          for (int k = 0; k < 3; ++k) {  // ascending column quarters: on equal values the earlier (lower) index stays
-            const float b2 = sMerge[k * 384 + r];
-            if (b2 > best) { best = b2; besti = reinterpret_cast<int*>(sMerge)[k * 384 + 128 + r]; }
-            psum += sMerge[k * 384 + 256 + r];
-          }
-          (dir ? a.colmax : a.rowmax)[ro] = best + (ls_mine - lse_mine);
-          (dir ? a.colarg : a.rowarg)[ro] = besti;
-          if (!dir && a.pos_row_sum) a.pos_row_sum[ro] = psum;
-        }
-        bar_epi();
-      } else {
-        mbar_wait(acc_full, it & 1);
-        tc_fence_after();
-        __nv_bfloat16* out = (dir ? a.dmd1 : a.dmd0) + ro * D;
-        const int cpw = D / 4;  // channels per column quarter
-#pragma unroll 1
-        for (int c = 0; c < cpw; c += 16) {
-          float v[16];
-          tmem_ld16(t_lane + AT_ACC_COL + cq * cpw + c, v);
-          tmem_ld_wait();
-          if (rok) {
+        for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
-            for (int e8 = 0; e8 < 2; ++e8) {
-              uint4 u;
-              u.x = pack_bf16(v[e8 * 8], v[e8 * 8 + 1]); u.y = pack_bf16(v[e8 * 8 + 2], v[e8 * 8 + 3]);
-              u.z = pack_bf16(v[e8 * 8 + 4], v[e8 * 8 + 5]); u.w = pack_bf16(v[e8 * 8 + 6], v[e8 * 8 + 7]);
-              *reinterpret_cast<uint4*>(out + cq * cpw + c + e8 * 8) = u;
+          for (int e = 0; e < 2; ++e) {
+            const int j = j0 + 8 * jj + e;
+            const bool cok = j < ncols;
+            const float lc = cok ? __ldg(cvec_lse + j) : 0.f;
+            const float cv = cok ? __ldg(cvec_b + j) - lc : -INFINITY;  // -inf masks the tail
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const float x = fmaf(sv[4 * jj + 2 * i + e], a2, cv);
+              if (x > best[i]) {  // columns are visited in increasing order: the first maximum stays
+                best[i] = x;
+                besti[i] = j;
+              }
+              if (grow[i] && cok && grow[i][j]) psum[i] += (x - cv) - lse_mine[i] - lc;
             }
           }
+      } else {  // AT_BWD
+        const float two_gc = 2.f * gc;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int j = j0 + 8 * jj + e;
+            const bool cok = j < ncols;
+            const float lc = cok ? __ldg(cvec_lse + j) * kLog2e_at : INFINITY;  // exp2(x - inf) = 0 past the end
+            const float cc = cok ? __ldg(cvec_b + j) * gc : 0.f;
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              float& x = sv[4 * jj + 2 * i + e];
+              float v = (cok && grow[i][j]) ? two_gc : 0.f;
+              v = fmaf(-fast_exp2(fmaf(x, c2, -lse_mine[i])), coef_mine[i], v);
+              if (cc != 0.f) v = fmaf(-fast_exp2(fmaf(x, c2, -lc)), cc, v);
+              x = cok ? v : 0.f;
+            }
+          }
+        uint32_t da[4][4];
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) acc_to_afrag(sv, kk, da[kk]);
+        wgmma_fence();
+#pragma unroll
+        for (int c = 0; c < AT_MAXKB; ++c) {
+          if (c < KB) {
+#pragma unroll
+            for (int kk = 0; kk < AT_C / 16; ++kk)  // 16 columns per step; block c holds channels [64c, 64c + 64)
+              wgmma_m64n64_rs<1>(acc[c], da[kk], sb + (uint64_t)((c * AT_BBLK) >> 4) + kk * 128, 1);
+          }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(acc_empty);
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int c = 0; c < AT_MAXKB; ++c) wgmma_hold(acc[c]);
+        if (signal) mbar_arrive(&b_empty[s]);
+      }
+    }
+    if (signal) mbar_arrive(a_empty);  // every MMA that reads the panel has retired
+
+    // ---- end of item: merge the four lanes of each row (LSE / STATS) or store the panel gradient (BWD)
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      if (MODE == AT_LSE) {
+        float m = m_run[i], l = l_run[i];
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {  // (max, sum exp2) of two lanes, log2 domain; -inf partials add nothing
+          const float m2 = __shfl_xor_sync(0xffffffffu, m, o), l2 = __shfl_xor_sync(0xffffffffu, l, o);
+          const float mn = fmaxf(m, m2);
+          l = (m == mn ? l : l * fast_exp2(m - mn)) + (m2 == mn ? l2 : l2 * fast_exp2(m2 - mn));
+          m = mn;
+        }
+        if (t4 == 0 && rok[i]) (dir ? a.lse_col : a.lse_row)[ro[i]] = (m + log2f(l)) * 0.6931471805599453f;
+      } else if (MODE == AT_STATS) {
+        float bv = best[i], ps = psum[i];
+        int bi = besti[i];
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {
+          const float b2 = __shfl_xor_sync(0xffffffffu, bv, o);
+          const int i2 = __shfl_xor_sync(0xffffffffu, bi, o);
+          if (b2 > bv || (b2 == bv && i2 < bi)) { bv = b2; bi = i2; }  // on equal values the lower index stays
+          ps += __shfl_xor_sync(0xffffffffu, ps, o);
+        }
+        if (t4 == 0 && rok[i]) {
+          (dir ? a.colmax : a.rowmax)[ro[i]] = bv + (ls_mine[i] - lse_mine[i]);
+          (dir ? a.colarg : a.rowarg)[ro[i]] = bi;
+          if (!dir && a.pos_row_sum) a.pos_row_sum[ro[i]] = ps;
+        }
+      } else if (rok[i]) {
+        __nv_bfloat16* out = (dir ? a.dmd1 : a.dmd0) + ro[i] * D + 2 * t4;
+#pragma unroll
+        for (int c = 0; c < AT_MAXKB; ++c) {
+          if (c < KB) {
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+              *reinterpret_cast<__nv_bfloat162*>(out + c * 64 + 8 * jj) =
+                  __floats2bfloat162_rn(acc[c][4 * jj + 2 * i], acc[c][4 * jj + 2 * i + 1]);
+          }
+        }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == AT_EWARPS + 1) tmem_dealloc(tmem_base, 512);
 }
 
 static int make_md_map(CUtensorMap* tm, const void* base, int B, int rows, int D) {
   const uint64_t dims[3] = {(uint64_t)D, (uint64_t)rows, (uint64_t)B};
   const uint64_t str[2] = {(uint64_t)D * 2, (uint64_t)rows * D * 2};
-  const uint32_t box[3] = {AT_KBLK, AT_R, 1};
+  const uint32_t box[3] = {AT_KBLK, AT_C, 1};
   return make_tmap_bf16(tm, base, 3, dims, str, box);
 }
 

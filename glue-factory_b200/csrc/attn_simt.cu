@@ -1,5 +1,5 @@
 // fp32 CUDA-core attention (forward + backward) -- the full-precision parity path
-// (`precision="fp32"`) and the on-device cross-check for the tcgen05 kernels.
+// (`precision="fp32"`) and the on-device cross-check for the wgmma kernels.
 //
 //   out = softmax(scale * q k^T) v       per (batch, head), head_dim = 64
 // (reference: gluefactory/models/matchers/lightglue.py:118-121 self-attention,

@@ -1,16 +1,18 @@
-// Flash attention on the 5th-generation tensor cores (sm_100a): out = softmax(scale * q k^T) v
+// Flash attention on the Hopper tensor cores (sm_90a): out = softmax(scale * q k^T) v
 // for head_dim 64, bf16 operands, fp32 accumulation, never materialising the N x N similarity.
 // (reference: lightglue.py:118-121 self-attention; :207-216 cross-attention.)
 //
-// FORWARD.  One CTA = one (batch, head, 128-query tile), two CTAs per SM.  Q/K/V tiles are brought in by TMA
-// (4-D tensor map over the token-major [B,N,H,64] layout, 128-byte swizzle) and consumed straight
-// from shared memory by tcgen05.mma:
-//     S_j (128 x 64 fp32, TMEM, double-buffered) = Q K_j^T      4 MMAs  (M128 N64 K16, SS)
-//     O  (128 x 64 fp32, TMEM, accumulated)     += P_j V_j      4 MMAs  (M128 N64 K16, TS: P_j read from TMEM)
-// Warps 0-3 are the softmax warpgroup (thread == query row == TMEM lane): one sweep over S_j with
-// tcgen05.ld (row max, exp2 / row sum / bf16 pack), P_j written to its own TMEM columns, O rescaled in
-// TMEM only when the lazy reference maximum moves.  Warp 4 = TMA producer, warp 5 = MMA issuer + TMEM owner.
-// BACKWARD: one fused kernel (dK, dV, dQ in a single pass; see attn_bwd_fused_kernel) + the round-1 two-kernel pair.
+// FORWARD.  One CTA = one (batch, head, 128-query tile): two consumer warpgroups of 64 query rows each and one TMA
+// producer warp.  Q/K/V tiles are brought in by TMA (4-D tensor map over the token-major [B,N,H,64] layout, 128-byte
+// swizzle) and consumed straight from shared memory by wgmma:
+//     S_j (64 x 64 fp32, registers) = Q K_j^T      4 wgmma m64n64k16 (both operands K-major in smem)
+//     O   (64 x 64 fp32, registers) += P_j V_j     4 wgmma m64n64k16 (P_j from registers, V_j MN-major in smem)
+// The softmax runs on the S_j accumulators in place (online maximum, rows shared by the four lanes of a quad) and
+// P_j is re-packed to bf16 A fragments without leaving the registers.
+// BACKWARD: one CTA owns 128 keys (K, V resident in smem) and walks the queries in tiles of 64 (dK, dV accumulated in
+// registers); dQ comes from a second kernel that owns the queries (the default: deterministic, so eager steps and
+// CUDA-graph replays of a training step agree bit for bit) or, with LGB200_ATTN_BWD_FUSED=1, from the same pass (dS
+// through shared memory, fp32 atomics into an accumulator: no recomputation of S / dP, run-dependent summation order).
 #include <math.h>
 
 #include "common.cuh"
@@ -26,63 +28,40 @@ constexpr int FA_STAGES = 4;
 constexpr int FA_QBYTES = FA_BM * FA_D * 2;   // 16 KiB
 constexpr int FA_KBYTES = FA_BN * FA_D * 2;   // 8 KiB
 constexpr int FA_SMEM = FA_QBYTES + FA_STAGES * 2 * FA_KBYTES + 256;
-constexpr int FA_TMEM_COLS = 256;             // S0 [0,64) S1 [64,128), O [128,192), P0 [192,224) P1 [224,256)
-constexpr int FA_S_COL = 0, FA_O_COL = 128;
-// P_j (bf16, two keys per column) has its own columns, so S(j+2) -- issued right behind P V(j) -- never writes a
-// buffer the tensor pipe may still be reading.
-#define FA_P_COL(j) (192 + ((j) & 1) * 32)
+constexpr int FA_THREADS = 2 * 128 + 32;      // two consumer warpgroups + the producer warp
+constexpr int FA_PRODUCER = 8;
+constexpr float kLn2 = 0.6931471805599453f, kLog2e = 1.4426950408889634f;
 
-// Optional clock64 pipeline trace of CTA (0,0,0) (read back with lgb200_debug_read_trace / scripts/trace_attn.py):
-// -DLGB_TRACE=1 traces the dKV kernel, -DLGB_TRACE=3 the forward kernel.
-// role 0 = producer, 1 = MMA issuer, 2 / 3 = two softmax warps; 4 time stamps per tile.
-#ifdef LGB_TRACE
-__device__ long long g_trace[4 * 64 * 4];
-#define LGB_TR_(role, i, k)                                                                        \
-  do {                                                                                             \
-    if (blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && (i) < 64) g_trace[((role) * 64 + (i)) * 4 + (k)] = clock64(); \
-  } while (0)
-// whole-CTA life time (clock64 + globaltimer at entry / exit) of CTAs 0 and 300 of the grid, in role 0 rows 40, 41
-#define LGB_TR_LIFE_(k)                                                                             \
-  do {                                                                                              \
-    const int lin_ = blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z);               \
-    if (threadIdx.x == 0 && (lin_ == 0 || lin_ == 300)) {                                           \
-      unsigned long long gt_;                                                                       \
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt_));                                       \
-      g_trace[(40 + (lin_ == 300)) * 4 + (k)] = clock64();                                          \
-      g_trace[(40 + (lin_ == 300)) * 4 + (k) + 2] = (long long)gt_;                                 \
-    }                                                                                               \
-  } while (0)
-#endif
-#if defined(LGB_TRACE) && LGB_TRACE == 3
-#define LGB_TRF(role, i, k) LGB_TR_(role, i, k)
-#define LGB_TRF_LIFE(k) LGB_TR_LIFE_(k)
-#else
-#define LGB_TRF(role, i, k) do {} while (0)
-#define LGB_TRF_LIFE(k) do {} while (0)
-#endif
-#if defined(LGB_TRACE) && LGB_TRACE != 3
-#define LGB_TR(role, i, k) LGB_TR_(role, i, k)
-#define LGB_TR_LIFE(k) LGB_TR_LIFE_(k)
-#else
-#define LGB_TR(role, i, k) do {} while (0)
-#define LGB_TR_LIFE(k) do {} while (0)
-#endif
+// max / sum over the four lanes of a quad (they share the rows of an accumulator fragment)
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
 
-// token-major [B, N, H, 64] bf16 -> 4-D tensor map {64, H, N, B}, box {64, 1, rows, 1}
-// ---------------------------------------------------------------------------------------------
-// FORWARD kernel (round 2: the round-1 kernel handed P to the second MMA through shared memory and folded O into 64
-// registers per thread every tile; 226 -> 188 us at 32 sequences, profiles/r02_stage_check.md):
-//   * P never goes through shared memory: the softmax warps write it (bf16, two keys per 32-bit column) into 32 TMEM
-//     columns of its own, and P V is a TS-form MMA (A operand in TMEM) exactly like the accumulating MMAs of the
-//     backward kernels -- no st.shared, no fence.proxy.async;
-//   * O accumulates in TMEM across key tiles (accumulate flag); a softmax warp rescales its O rows in TMEM only when
-//     one of its 32 rows outgrew the reference maximum by more than 2^8 (lazy rescaling: exponentials relative to a
-//     stale maximum, bounded by 256, so after the first few tiles O is never touched again).
-// ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(192, 2)
+// bf16 store of a 64 x 64 accumulator (the warpgroup's rows row_base.., valid while < nrows) into the token-major
+// [.., N, H, 64] layout at (batch, head)
+__device__ __forceinline__ void store_acc_rows(const float (&d)[32], __nv_bfloat16* __restrict__ dst, int bat, int N,
+                                               int H, int h, int row_base, float mul) {
+  const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int row = row_base + wq * 16 + (lane >> 2) + 8 * i;
+    if (row >= N) continue;
+    __nv_bfloat16* o = dst + (((int64_t)bat * N + row) * H + h) * FA_D + 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      *reinterpret_cast<__nv_bfloat162*>(o + 8 * j) = __floats2bfloat162_rn(d[4 * j + 2 * i] * mul, d[4 * j + 2 * i + 1] * mul);
+  }
+}
+
+__global__ void __launch_bounds__(FA_THREADS, 1)
     attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                          const __grid_constant__ CUtensorMap tmV, __nv_bfloat16* __restrict__ out,
-                          float* __restrict__ lse, int B, int Nq, int Nk, int H, int kv_shift, float scale_log2) {
+                       const __grid_constant__ CUtensorMap tmV, __nv_bfloat16* __restrict__ out,
+                       float* __restrict__ lse, int B, int Nq, int Nk, int H, int kv_shift, float scale_log2) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + FA_QBYTES;
@@ -91,46 +70,29 @@ __global__ void __launch_bounds__(192, 2)
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;               // [FA_STAGES]
   uint64_t* kv_empty = kv_full + FA_STAGES;   // [FA_STAGES]
-  uint64_t* s_full = kv_empty + FA_STAGES;    // [2]
-  uint64_t* p_full = s_full + 2;              // [2]
-  uint64_t* o_done = p_full + 2;              // one barrier, one phase per key tile (P V of tile j complete)
-  uint64_t* o_final = o_done + 1;             // P V of the LAST tile complete (see the epilogue)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_final + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * FA_BM, h = blockIdx.y, b = blockIdx.z;
   const int kb = (b + kv_shift) % B;
   const int ntiles = (Nk + FA_BN - 1) / FA_BN;
-  LGB_TRF_LIFE(0);
 
   if (threadIdx.x == 0) {
     if (smem_u32(smem) & 1023u) __trap();
     mbar_init(q_full, 1);
     for (int s = 0; s < FA_STAGES; ++s) {
       mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
+      mbar_init(&kv_empty[s], 2);
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&s_full[s], 1);
-      mbar_init(&p_full[s], 4);
-    }
-    mbar_init(o_done, 1);
-    mbar_init(o_final, 1);
     mbar_fence_init();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == FA_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
   }
-  if (warp == 5) tmem_alloc(tmem_slot, FA_TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 4) {
-    // ------------------------------------------------------------------ TMA producer
+  if (warp == FA_PRODUCER) {
     if (lane == 0) {
       mbar_expect_tx(q_full, FA_QBYTES);
       tma_load_4d(sQ, &tmQ, q_full, 0, h, q0, b);
@@ -142,154 +104,80 @@ __global__ void __launch_bounds__(192, 2)
         tma_load_4d(sV + s * FA_KBYTES, &tmV, &kv_full[s], 0, h, j * FA_BN, kb);
       }
     }
-  } else if (warp == 5) {
-    // ------------------------------------------------------------------ MMA issuer (warp-convergent, elected lane)
-    constexpr uint32_t idesc_s = make_idesc_bf16(FA_BM, FA_BN, 0, 0);  // Q (K-major) x K_j (K-major)
-    constexpr uint32_t idesc_o = make_idesc_bf16(FA_BM, FA_D, 0, 1);   // P (TMEM) x V_j (MN-major)
-    const uint64_t dQ0 = make_smem_desc(smem_u32(sQ), 16, 1024), dK0 = make_smem_desc(smem_u32(sK), 16, 1024);
-    const uint64_t dV0 = make_smem_desc(smem_u32(sV), 8192, 1024);
-    const bool leader = elect_one();
-    auto issue_s = [&](int j) {
-      const int s = j % FA_STAGES;
-      mbar_wait(&kv_full[s], (j / FA_STAGES) & 1);
-      tc_fence_after();
-      if (leader) {
-        const uint64_t dk = dK0 + (uint64_t)((s * FA_KBYTES) >> 4);
-        const uint32_t d = tmem_base + FA_S_COL + (j & 1) * FA_BN;
-#pragma unroll
-        for (int kk = 0; kk < FA_D / 16; ++kk)
-          umma_bf16(d, dQ0 + (uint64_t)(kk * 2), dk + (uint64_t)(kk * 2), idesc_s, kk != 0 ? 1u : 0u);
-        umma_commit(&s_full[j & 1]);
-      }
-      __syncwarp();
-    };
-    mbar_wait(q_full, 0);
-    issue_s(0);
-    if (ntiles > 1) issue_s(1);
-    for (int j = 0; j < ntiles; ++j) {
-      const int s = j % FA_STAGES;
-      mbar_wait(&p_full[j & 1], (j >> 1) & 1);  // P_j written (and, if it was needed, O rescaled) by all 4 warps
-      tc_fence_after();
-      if (leader) LGB_TRF(1, j, 0);
-      if (leader) {
-        const uint64_t dv = dV0 + (uint64_t)((s * FA_KBYTES) >> 4);
-        const uint32_t pcol = tmem_base + FA_P_COL(j);  // keys [kk*16, +16) at P columns kk*8
-#pragma unroll
-        for (int kk = 0; kk < FA_BN / 16; ++kk)
-          umma_bf16_ts(tmem_base + FA_O_COL, pcol + kk * 8, dv + (uint64_t)(kk * 128), idesc_o,
-                       (j | kk) != 0 ? 1u : 0u);
-        umma_commit(&kv_empty[s]);
-        umma_commit(o_done);
-        if (j == ntiles - 1) umma_commit(o_final);
-      }
-      if (leader) LGB_TRF(1, j, 1);
-      __syncwarp();
-      if (j + 2 < ntiles) issue_s(j + 2);  // overwrites the S buffer of tile j (already read by the softmax warps)
-      if (leader) LGB_TRF(1, j, 2);
-    }
-  } else {
-    // ------------------------------------------------------------------ softmax warpgroup
-    const int r = warp * 32 + lane;  // query row within the tile == TMEM lane
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
-    float m = -INFINITY, l = 0.f;
-    for (int j = 0; j < ntiles; ++j) {
-      const int kbase = j * FA_BN;
-      const bool tail = kbase + FA_BN > Nk;
-      const uint32_t sbuf = t_lane + FA_S_COL + (j & 1) * FA_BN;
-      mbar_wait(&s_full[j & 1], (j >> 1) & 1);
-      tc_fence_after();
-      if (lane == 0 && (warp == 0 || warp == 3)) LGB_TRF(2 + (warp == 3), j, 0);
-      float sv[FA_BN];
-      tmem_ld32(sbuf, sv);
-      tmem_ld32(sbuf + 32, sv + 32);
-      tmem_ld_wait();
-      if (lane == 0 && (warp == 0 || warp == 3)) LGB_TRF(2 + (warp == 3), j, 1);
-      if (tail) {
-#pragma unroll
-        for (int e = 0; e < FA_BN; ++e)
-          if (kbase + e >= Nk) sv[e] = -INFINITY;
-      }
-      float mx = sv[0];
-#pragma unroll
-      for (int e = 1; e < FA_BN; ++e) mx = fmaxf(mx, sv[e]);
-      // Lazy reference maximum: the exponentials are taken relative to m, which is only raised (and O, l rescaled)
-      // when some row of this warp outgrew it by more than 2^8 -- p <= 256 stays harmless in bf16 / fp32, the result
-      // O / l does not depend on the reference, and after the first few tiles no rescaling happens at all.  (With the
-      // exact running maximum, one of a warp's 32 rows moves in most tiles and the skip would rarely trigger.)
-      const float m_cand = fmaxf(m, mx * scale_log2);
-      float alpha = 1.f, m_new = m;
-      if (__any_sync(0xffffffffu, m_cand - m > 8.f)) {  // first tile: m = -inf, always taken
-        m_new = m_cand;
-        alpha = fast_exp2(m - m_new);  // first tile: exp2(-inf) = 0 (O is overwritten by its P V anyway)
-        if (j > 0) {                   // the P V of tile j-1 must have landed before its result is rescaled
-          // parity wait on a barrier nobody else polls: safe because S(j) is complete here, hence P V(j-2) is, so
-          // o_done is in phase j-1 or j -- never two phases away from the one awaited
-          mbar_wait(o_done, (j - 1) & 1);
-          tc_fence_after();
-#pragma unroll
-          for (int c = 0; c < FA_D / 32; ++c) {
-            float v[32];
-            uint32_t w[32];
-            tmem_ld32(t_lane + FA_O_COL + c * 32, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 32; ++e) w[e] = __float_as_uint(v[e] * alpha);
-            tmem_st16(t_lane + FA_O_COL + c * 32, w);
-            tmem_st16(t_lane + FA_O_COL + c * 32 + 16, w + 16);
-          }
-        }
-      }
-      float lsum = 0.f;
-      uint32_t pw[FA_BN / 2];
-#pragma unroll
-      for (int e = 0; e < FA_BN; e += 2) {
-        const float x0 = fmaf(sv[e], scale_log2, -m_new), x1 = fmaf(sv[e + 1], scale_log2, -m_new);
-        const float p0 = fast_exp2(x0), p1 = fast_exp2(x1);  // masked keys: exp2(-inf) = 0
-        lsum += p0 + p1;
-        pw[e >> 1] = pack_bf16(p0, p1);
-      }
-      if (lane == 0 && (warp == 0 || warp == 3)) LGB_TRF(2 + (warp == 3), j, 2);
-      tmem_st16(t_lane + FA_P_COL(j), pw);  // P_j (bf16, two keys per column) into its own 32 TMEM columns
-      tmem_st16(t_lane + FA_P_COL(j) + 16, pw + 16);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_full[j & 1]);
-      if (lane == 0 && (warp == 0 || warp == 3)) LGB_TRF(2 + (warp == 3), j, 3);
-      l = l * alpha + lsum;
-      m = m_new;
-    }
-    // NOT o_done: a warp that has just handed over P(ntiles-1) may find o_done still in phase ntiles-2 (only
-    // P V(ntiles-3) is known complete), whose parity test for phase ntiles-1 passes at once -- the output would be
-    // read before the last two P V products landed (run-to-run differences of `out`, scripts/stress_attn.py).
-    mbar_wait(o_final, 0);
-    tc_fence_after();
-    const int row = q0 + r;
-    const float inv = 1.f / l;
-    __nv_bfloat16* orow = out + (((int64_t)b * Nq + (row < Nq ? row : 0)) * H + h) * FA_D;
-#pragma unroll
-    for (int c = 0; c < FA_D / 32; ++c) {
-      float v[32];
-      tmem_ld32(t_lane + FA_O_COL + c * 32, v);
-      tmem_ld_wait();
-      if (row < Nq) {
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 u;
-          u.x = pack_bf16(v[g * 8 + 0] * inv, v[g * 8 + 1] * inv);
-          u.y = pack_bf16(v[g * 8 + 2] * inv, v[g * 8 + 3] * inv);
-          u.z = pack_bf16(v[g * 8 + 4] * inv, v[g * 8 + 5] * inv);
-          u.w = pack_bf16(v[g * 8 + 6] * inv, v[g * 8 + 7] * inv);
-          *reinterpret_cast<uint4*>(orow + c * 32 + g * 8) = u;
-        }
-      }
-    }
-    if (row < Nq) lse[((int64_t)b * H + h) * Nq + row] = (m + log2f(l)) * 0.6931471805599453f;
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc(tmem_base, FA_TMEM_COLS);
-  LGB_TRF_LIFE(1);
+  const int wg = threadIdx.x >> 7, t4 = lane & 3;
+  const bool signal = (threadIdx.x & 127) == 0;
+  const uint64_t dQ0 = make_smem_desc(smem_u32(sQ) + wg * 8192, 8192, 1024);
+  const uint64_t dK0 = make_smem_desc(smem_u32(sK), 8192, 1024), dV0 = make_smem_desc(smem_u32(sV), 8192, 1024);
+  float o[32], m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+#pragma unroll
+  for (int e = 0; e < 32; ++e) o[e] = 0.f;
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < ntiles; ++j) {
+    const int s = j % FA_STAGES;
+    const uint64_t so = (uint64_t)((s * FA_KBYTES) >> 4);
+    mbar_wait(&kv_full[s], (j / FA_STAGES) & 1);
+    float sv[32];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(sv, dQ0 + kk * 2, dK0 + so + kk * 2, kk != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_hold(sv);
+    const int kbase = j * FA_BN;
+    if (kbase + FA_BN > Nk) {
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (kbase + 8 * jj + 2 * t4 + e >= Nk) sv[4 * jj + e] = sv[4 * jj + 2 + e] = -INFINITY;
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) mx = fmaxf(mx, fmaxf(sv[4 * jj + 2 * i], sv[4 * jj + 2 * i + 1]));
+      const float m_new = fmaxf(m[i], quad_max(mx) * scale_log2);  // every key tile holds at least one valid key
+      const float alpha = fast_exp2(m[i] - m_new);                // first tile: exp2(-inf) = 0
+      float rs = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int x = 4 * jj + 2 * i + e;
+          sv[x] = fast_exp2(fmaf(sv[x], scale_log2, -m_new));  // masked keys: exp2(-inf) = 0
+          rs += sv[x];
+          o[x] *= alpha;
+        }
+      l[i] = l[i] * alpha + rs;  // this lane's partial row sum; the quad is summed at the end
+      m[i] = m_new;
+    }
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) acc_to_afrag(sv, kk, pa[kk]);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < FA_BN / 16; ++kk) wgmma_m64n64_rs<1>(o, pa[kk], dV0 + so + kk * 128, 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_hold(o);
+    if (signal) mbar_arrive(&kv_empty[s]);
+  }
+  const int rbase = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    l[i] = quad_sum(l[i]);
+    const float inv = 1.f / l[i];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      o[4 * jj + 2 * i] *= inv;
+      o[4 * jj + 2 * i + 1] *= inv;
+    }
+    const int row = rbase + 8 * i;
+    if (t4 == 0 && row < Nq) lse[((int64_t)b * H + h) * Nq + row] = (m[i] + log2f(l[i])) * kLn2;
+  }
+  store_acc_rows(o, out, b, Nq, H, h, q0 + wg * 64, 1.f);
 }
 
 static int make_qkv_tmap(CUtensorMap* tm, const void* base, int B, int N, int H, int box_rows) {
@@ -308,515 +196,37 @@ int attn_fwd_tc(const void* q, const void* k, const void* v, void* out, float* l
   if ((rc = make_qkv_tmap(&tv, v, B, Nk, H, FA_BN))) return rc;
   if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_fwd_tc_kernel), FA_SMEM))) return rc;
   dim3 grid((Nq + FA_BM - 1) / FA_BM, H, B);
-  attn_fwd_tc_kernel<<<grid, 192, FA_SMEM, stream>>>(tq, tk, tv, static_cast<__nv_bfloat16*>(out), lse, B, Nq, Nk, H,
-                                                     kv_shift, scale * 1.4426950408889634f);
+  attn_fwd_tc_kernel<<<grid, FA_THREADS, FA_SMEM, stream>>>(tq, tk, tv, static_cast<__nv_bfloat16*>(out), lse, B, Nq, Nk,
+                                                            H, kv_shift, scale * kLog2e);
   return check_launch("attn_fwd_tc");
 }
 
 // ---------------------------------------------------------------------------------------------
-// BACKWARD.  Two kernels, both deterministic (no atomics), both with the forward's structure
-// (TMA producer warp, MMA issuer warp, softmax warps with thread == TMEM lane == row):
-//
-//   dKV kernel: CTA owns 128 keys (rows), walks the queries in tiles of 64:
-//       S^T  = K  Q_i^T   (128 x 64)      dP^T = V dO_i^T   (128 x 64)
-//       P^T  = exp2(S^T c - lse_i)        dS^T = P^T (dP^T - delta_i) scale
-//       dV  += P^T dO_i                   dK  += dS^T Q_i         (accumulated in TMEM)
-//   dQ kernel : CTA owns 128 queries (rows), walks the keys in tiles of 64:
-//       S    = Q K_j^T    (128 x 64)      dP   = dO V_j^T   (128 x 64)
-//       dS   = exp2(S c - lse) (dP - delta) scale
-//       dQ  += dS K_j                                        (accumulated in TMEM)
-//
-// S and dP are recomputed in both kernels (7 GEMMs instead of 5 per tile pair) in exchange for a
-// race-free dQ.  P^T / dS^T / dS are rounded to bf16 and handed to the second MMA through shared
-// memory in the K-major 128B-swizzled layout; the 64-row operand tiles (Q_i, dO_i, K_j) are used both
-// as K-major B operands (first GEMMs) and as MN-major B operands (accumulating GEMMs) of the same
-// shared-memory bytes.  One CTA per SM: S / dP are double-buffered in TMEM (the MMA thread runs one
-// tile ahead of the softmax warps), two softmax warpgroups split the 64 columns of a tile.
+// BACKWARD.  dKV kernel: a CTA owns 128 keys (K, V resident in smem; warpgroup w owns keys 64w..64w+63) and walks the
+// queries in tiles of 64:
+//     S^T  = K Q_i^T,  dP^T = V dO_i^T            (64 x 64 per warpgroup, wgmma from smem)
+//     P^T  = exp2(c S^T - lse2_i),  dS^T = P^T (dP^T scale - delta_i scale)   (in registers; lse2 / delta are
+//            per-COLUMN values here and come as two 64-float vectors with every query tile)
+//     dV  += P^T dO_i,   dK += dS^T Q_i           (P^T / dS^T as register A operands, dO_i / Q_i MN-major from smem)
+// With the dQ fusion, dS^T also goes to shared memory ([key][query], 128-byte swizzled: read with M = query it is an
+// MN-major A operand) and dQ_i (64 x 64) += dS K is formed per warpgroup and added into an fp32 accumulator with
+// atomics (the key-tile CTAs of one (batch, head) meet there; summation order is not fixed), converted to bf16 by
+// a last small kernel.
+// dQ kernel (default path): a CTA owns 128 queries (Q, dO resident) and walks the keys in tiles of 64:
+//     S = Q K_j^T, dP = dO V_j^T, dS = exp2(c S - lse2) (dP scale - delta scale), dQ += dS K_j.
+// Queries past Nq load as zeros and carry lse2 = +inf (p = 0); keys past Nk load as zeros, so their dS meets a zero
+// row of K and adds nothing to dQ, and their dK / dV rows are not stored.
 // ---------------------------------------------------------------------------------------------
 constexpr int FB_R = 128;            // rows owned by the CTA
 constexpr int FB_C = 64;             // inner tile
 constexpr int FB_CBYTES = FB_C * FA_D * 2;  // 8 KiB
-constexpr int FB_TMEM_COLS = 512;
-
-// ---------------------------------------------------------------------------------------------
-// BACKWARD v3: every A operand lives in tensor memory.
-//   * the CTA's resident 128-row operands (K,V for dKV; Q,dO for dQ) are written once into TMEM
-//     (bf16, two K-elements per 32-bit column) and feed the S / dP MMAs as TMEM A operands;
-//   * P^T / dS^T (dKV) and dS (dQ) are written by the softmax warps with tcgen05.st IN PLACE over
-//     the S / dP columns they were computed from (each warpgroup over its own 32-column half), and
-//     feed the accumulating MMAs as TMEM A operands.
-// Shared memory then carries only the streamed 64-row B tiles: ~3x less smem traffic per tile than
-// v2 (the v2 kernels were shared-memory-bandwidth bound: 6 KB of operand reads per 32-cycle MMA),
-// and the generic->async proxy fence of the P hand-off disappears.
-// TMEM columns: A0 [0,32) A1 [32,64) | buffer b: S at 64+b*128, dP at 128+b*128 | accumulators at 320, 384.
-// ---------------------------------------------------------------------------------------------
-constexpr int F3_A0 = 0, F3_A1 = 32, F3_BUF0 = 64, F3_ACC0 = 320, F3_ACC1 = 384;
-constexpr int F3_NWG = 4;                    // softmax warpgroups; each owns 64 / F3_NWG columns of a tile
-constexpr int F3_CW = FB_C / F3_NWG;         // 16 columns per warpgroup
-constexpr int F3_SWARPS = 4 * F3_NWG;        // 16 softmax warps: latency hiding for the exp / pack chain
-constexpr int F3_THREADS = (F3_SWARPS + 2) * 32;
-constexpr int F3_STAGES = 8;  // 128 KiB of staging: deep TMA prefetch, and forces one CTA per SM (TMEM = 512 columns)
-constexpr int F3_SMEM = F3_STAGES * 2 * FB_CBYTES + 256;
-
-__device__ __forceinline__ void store_out_cols16(__nv_bfloat16* dst, uint32_t taddr, bool valid) {
-  float v[16];
-  tmem_ld16(taddr, v);
-  tmem_ld_wait();
-  if (!valid) return;
-#pragma unroll
-  for (int g = 0; g < 2; ++g) {
-    uint4 u;
-    u.x = pack_bf16(v[g * 8 + 0], v[g * 8 + 1]); u.y = pack_bf16(v[g * 8 + 2], v[g * 8 + 3]);
-    u.z = pack_bf16(v[g * 8 + 4], v[g * 8 + 5]); u.w = pack_bf16(v[g * 8 + 6], v[g * 8 + 7]);
-    *reinterpret_cast<uint4*>(dst + g * 8) = u;
-  }
-}
-
-__device__ __forceinline__ void load_row_part_to_tmem(const __nv_bfloat16* row_ptr, bool valid, uint32_t taddr) {
-  // 16 bf16 (32 B) of this thread's row -> 8 packed TMEM columns
-  uint32_t w[8];
-  if (valid) {
-    const uint4* src = reinterpret_cast<const uint4*>(row_ptr);
-#pragma unroll
-    for (int g = 0; g < 2; ++g) {
-      const uint4 u = src[g];
-      w[g * 4 + 0] = u.x; w[g * 4 + 1] = u.y; w[g * 4 + 2] = u.z; w[g * 4 + 3] = u.w;
-    }
-  } else {
-#pragma unroll
-    for (int g = 0; g < 8; ++g) w[g] = 0u;
-  }
-  tmem_st8(taddr, w);
-}
-static_assert(F3_NWG == 4, "the v3 backward kernels are written for 4 softmax warpgroups of 16 columns");
-
-// dKV kernel: the per-QUERY softmax statistics are per-COLUMN quantities of S^T / dP^T (thread == key row), so
-// every thread would need all of them.  Instead they are folded into the contraction: the K and V rows held in
-// TMEM get 16 extra K-elements [1, 1, 0, ...] and every streamed Q / dO tile gets a 16-column side tile
-//     Q' extra = [-(lse/scale)_hi, -(lse/scale)_lo, 0...]      dO' extra = [-delta_hi, -delta_lo, 0...]
-// (hi/lo = bf16 split, ~2^-17 relative), so one more K-step of the same MMAs yields directly
-//     S'^T = K Q^T - lse/scale          dP'^T = V dO^T - delta
-// and the softmax warps are left with p = exp2(c S'), ds = p dP' scale: no broadcasts, no FFMA/FSUB per element.
-// The side tiles are written once per backward by attn_bwd_prep_kernel ([B,H,Nq,16] bf16, next to delta) and
-// arrive by TMA (SWIZZLE_32B) with the Q / dO tile.  Queries past Nq load as zeros: p = 1 there, but their dO row
-// and dP' are zero, so they add nothing to dV or dK.
-constexpr int F4_A0 = 0, F4_A1 = 40, F4_BUF0 = 80, F4_ACC0 = 336, F4_ACC1 = 400;  // TMEM columns (464 used)
-constexpr int F4_STAGES = 8;
-constexpr int F4_XBYTES = FB_C * 32;                             // side tile: 64 rows x 16 bf16
-constexpr int F4_STAGE_BYTES = 2 * FB_CBYTES + 2 * F4_XBYTES;    // Q, dO, Q-side, dO-side
-constexpr int F4_SMEM = F4_STAGES * F4_STAGE_BYTES + 256;
-
-__device__ __forceinline__ uint4 neg_hi_lo_row(float x) {
-  // bf16 (-hi, -lo, 0, ...) with hi = bf16(x), lo = bf16(x - hi)
-  const __nv_bfloat16 hi = __float2bfloat16(x);
-  return make_uint4(pack_bf16(-__bfloat162float(hi), -(x - __bfloat162float(hi))), 0u, 0u, 0u);
-}
-
-// delta[b,h,i] = sum_d dout[b,i,h,d] * out[b,i,h,d] (8 lanes per row) and the two side arrays of the dKV kernel.
-__global__ void __launch_bounds__(256)
-    attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __restrict__ dout,
-                         const float* __restrict__ lse, float* __restrict__ delta, uint4* __restrict__ qx,
-                         uint4* __restrict__ dox, int64_t nrows /*B*N*H*/, int N, int H, float inv_scale) {
-  const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t r = gid >> 3;  // (b, n, h) flattened token-major
-  const int sub = (int)(gid & 7);
-  float acc = 0.f;
-  if (r < nrows) {
-    const uint4 a = *reinterpret_cast<const uint4*>(out + r * FA_D + sub * 8);
-    const uint4 g = *reinterpret_cast<const uint4*>(dout + r * FA_D + sub * 8);
-    const __nv_bfloat162* pa = reinterpret_cast<const __nv_bfloat162*>(&a);
-    const __nv_bfloat162* pg = reinterpret_cast<const __nv_bfloat162*>(&g);
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float2 fa = __bfloat1622float2(pa[e]), fg = __bfloat1622float2(pg[e]);
-      acc = fmaf(fa.x, fg.x, acc);
-      acc = fmaf(fa.y, fg.y, acc);
-    }
-  }
-  acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-  acc += __shfl_xor_sync(0xffffffffu, acc, 2);
-  acc += __shfl_xor_sync(0xffffffffu, acc, 4);
-  if (r < nrows && sub < 4) {
-    const int h = (int)(r % H);
-    const int64_t bn = r / H;
-    const int n = (int)(bn % N);
-    const int64_t o = ((bn / N) * H + h) * N + n;
-    const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
-    if (sub == 0) {
-      delta[o] = acc;
-      dox[o * 2] = neg_hi_lo_row(acc);
-    } else if (sub == 1) {
-      dox[o * 2 + 1] = zero;
-    } else if (sub == 2) {
-      qx[o * 2] = neg_hi_lo_row(lse[o] * inv_scale);
-    } else {
-      qx[o * 2 + 1] = zero;
-    }
-  }
-}
-
-__global__ void __launch_bounds__(F3_THREADS, 1)
-    attn_bwd_dkv_v3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
-                           const __grid_constant__ CUtensorMap tmQx, const __grid_constant__ CUtensorMap tmDOx,
-                           const __nv_bfloat16* __restrict__ kg, const __nv_bfloat16* __restrict__ vg,
-                           __nv_bfloat16* __restrict__ dk, __nv_bfloat16* __restrict__ dv, int B, int Nq, int Nk,
-                           int H, int kv_shift, float scale, float scale_log2) {
-  LGB_TR_LIFE(0);
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F4_STAGES * F4_STAGE_BYTES);
-  uint64_t* a_ready = bars;
-  uint64_t* in_full = bars + 1;               // [F4_STAGES]
-  uint64_t* in_empty = in_full + F4_STAGES;   // [F4_STAGES]
-  uint64_t* sp_full = in_empty + F4_STAGES;   // [2]
-  uint64_t* pds_full = sp_full + 2;           // [2]
-  uint64_t* acc_done = pds_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_done + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int k0 = blockIdx.x * FB_R, h = blockIdx.y, kb = blockIdx.z;
-  const int qb = ((kb - kv_shift) % B + B) % B;
-  const int ntiles = (Nq + FB_C - 1) / FB_C;
-
-  if (threadIdx.x == 0) {
-    if (smem_u32(smem) & 1023u) __trap();
-    mbar_init(a_ready, F3_SWARPS);
-    for (int s = 0; s < F4_STAGES; ++s) {
-      mbar_init(&in_full[s], 1);
-      mbar_init(&in_empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&sp_full[s], 1);
-      mbar_init(&pds_full[s], F3_SWARPS);
-    }
-    mbar_init(acc_done, 1);
-    mbar_fence_init();
-  }
-  if (warp == F3_SWARPS && lane == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmDO);
-    tma_prefetch_desc(&tmQx);
-    tma_prefetch_desc(&tmDOx);
-  }
-  if (warp == F3_SWARPS + 1) tmem_alloc(tmem_slot, FB_TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == F3_SWARPS) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
-      for (int i = 0; i < ntiles; ++i) {
-        const int s = i % F4_STAGES;
-        uint8_t* st = smem + s * F4_STAGE_BYTES;
-        mbar_wait(&in_empty[s], ((i / F4_STAGES) & 1) ^ 1);
-        LGB_TR(0, i, 0);
-        mbar_expect_tx(&in_full[s], F4_STAGE_BYTES);
-        tma_load_4d(st, &tmQ, &in_full[s], 0, h, i * FB_C, qb);
-        tma_load_4d(st + FB_CBYTES, &tmDO, &in_full[s], 0, h, i * FB_C, qb);
-        tma_load_3d(st + 2 * FB_CBYTES, &tmQx, &in_full[s], 0, i * FB_C, qb * H + h);
-        tma_load_3d(st + 2 * FB_CBYTES + F4_XBYTES, &tmDOx, &in_full[s], 0, i * FB_C, qb * H + h);
-        LGB_TR(0, i, 1);
-      }
-    }
-  } else if (warp == F3_SWARPS + 1) {
-    // ------------------------------------------------------------------ MMA issuer (warp-convergent, elected lane)
-    constexpr uint32_t idesc_s = make_idesc_bf16(FB_R, FB_C, 0, 0);    // (K'|V') in TMEM x (Q'|dO') K-major
-    constexpr uint32_t idesc_acc = make_idesc_bf16(FB_R, FA_D, 0, 1);  // (P^T|dS^T) in TMEM x (dO|Q) MN-major
-    const uint64_t dk0 = make_smem_desc(smem_u32(smem), 16, 1024);     // K-major view of a stage's tiles
-    const uint64_t dm0 = make_smem_desc(smem_u32(smem), 8192, 1024);   // MN-major view
-    const uint64_t dx0 = make_smem_desc(smem_u32(smem) + 2 * FB_CBYTES, 16, 256, 6);  // side tiles (SWIZZLE_32B)
-    const bool leader = elect_one();
-    auto issue_sp = [&](int i) {  // S'^T and dP'^T of query tile i into TMEM buffer i&1 (5 K-steps each)
-      const int s = i % F4_STAGES;
-      mbar_wait(&in_full[s], (i / F4_STAGES) & 1);
-      tc_fence_after();
-      if (leader) {
-        const uint32_t tb = tmem_base + F4_BUF0 + (i & 1) * 128;
-        const uint64_t so = (uint64_t)((s * F4_STAGE_BYTES) >> 4);
-        const uint64_t tq = dk0 + so, tdo = dk0 + so + (FB_CBYTES >> 4);
-        const uint64_t tqx = dx0 + so, tdox = dx0 + so + (F4_XBYTES >> 4);
-#pragma unroll
-        for (int kk = 0; kk < FA_D / 16; ++kk)
-          umma_bf16_ts(tb, tmem_base + F4_A0 + kk * 8, tq + (uint64_t)(kk * 2), idesc_s, kk != 0 ? 1u : 0u);
-        umma_bf16_ts(tb, tmem_base + F4_A0 + 32, tqx, idesc_s, 1u);
-#pragma unroll
-        for (int kk = 0; kk < FA_D / 16; ++kk)
-          umma_bf16_ts(tb + 64, tmem_base + F4_A1 + kk * 8, tdo + (uint64_t)(kk * 2), idesc_s, kk != 0 ? 1u : 0u);
-        umma_bf16_ts(tb + 64, tmem_base + F4_A1 + 32, tdox, idesc_s, 1u);
-        umma_commit(&sp_full[i & 1]);
-      }
-      __syncwarp();
-    };
-    mbar_wait(a_ready, 0);
-    tc_fence_after();
-    issue_sp(0);
-    if (ntiles > 1) issue_sp(1);
-    for (int i = 0; i < ntiles; ++i) {
-      const int s = i % F4_STAGES;
-      mbar_wait(&pds_full[i & 1], (i >> 1) & 1);
-      tc_fence_after();
-      if (leader) LGB_TR(1, i, 0);
-      if (leader) {
-        const uint32_t tb = tmem_base + F4_BUF0 + (i & 1) * 128;
-        const uint64_t so = (uint64_t)((s * F4_STAGE_BYTES) >> 4);
-        const uint64_t mq = dm0 + so, mdo = dm0 + so + (FB_CBYTES >> 4);
-#pragma unroll
-        for (int kk = 0; kk < FB_C / 16; ++kk)  // warpgroup kk wrote P^T of queries [kk*16, kk*16+16) at S col kk*16
-          umma_bf16_ts(tmem_base + F4_ACC0, tb + kk * F3_CW, mdo + (uint64_t)(kk * 128), idesc_acc,
-                       (i | kk) != 0 ? 1u : 0u);
-#pragma unroll
-        for (int kk = 0; kk < FB_C / 16; ++kk)
-          umma_bf16_ts(tmem_base + F4_ACC1, tb + 64 + kk * F3_CW, mq + (uint64_t)(kk * 128), idesc_acc,
-                       (i | kk) != 0 ? 1u : 0u);
-        umma_commit(&in_empty[s]);
-      }
-      if (leader) LGB_TR(1, i, 1);
-      __syncwarp();
-      if (i + 2 < ntiles) issue_sp(i + 2);
-      if (leader) LGB_TR(1, i, 2);
-    }
-    if (leader) umma_commit(acc_done);
-    __syncwarp();
-  } else {
-    // ------------------------------------------------------------------ softmax warps
-    const int c = warp >> 2;                 // 16-query column slice handled by this warpgroup
-    const int r = (warp & 3) * 32 + lane;    // key row within the tile == TMEM lane
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>((warp & 3) * 32) << 16);
-    const int row = k0 + r;
-    {  // resident A operands: this thread's 16-channel slice of its K and V rows (+ the [1,1,0..] extension) -> TMEM
-      const int64_t o = (((int64_t)kb * Nk + (row < Nk ? row : 0)) * H + h) * FA_D + c * F3_CW;
-      load_row_part_to_tmem(kg + o, row < Nk, t_lane + F4_A0 + c * (F3_CW / 2));
-      load_row_part_to_tmem(vg + o, row < Nk, t_lane + F4_A1 + c * (F3_CW / 2));
-      if (c == 0) {
-        const uint32_t ext[8] = {0x3F803F80u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};  // bf16 (1, 1) then zeros
-        tmem_st8(t_lane + F4_A0 + 32, ext);
-        tmem_st8(t_lane + F4_A1 + 32, ext);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(a_ready);
-    }
-    for (int i = 0; i < ntiles; ++i) {
-      const int buf = i & 1;
-      const uint32_t tb = t_lane + F4_BUF0 + buf * 128;
-      mbar_wait(&sp_full[buf], (i >> 1) & 1);
-      tc_fence_after();
-      if (lane == 0 && (warp == 0 || warp == 15)) LGB_TR(2 + (warp == 15), i, 0);
-      float sv[F3_CW], dp[F3_CW];
-      tmem_ld16(tb + c * F3_CW, sv);
-      tmem_ld16(tb + 64 + c * F3_CW, dp);
-      tmem_ld_wait();
-      if (lane == 0 && (warp == 0 || warp == 15)) LGB_TR(2 + (warp == 15), i, 1);
-      uint32_t pw[F3_CW / 2], dw[F3_CW / 2];
-#pragma unroll
-      for (int e = 0; e < F3_CW; e += 2) {
-        const float p0 = fast_exp2(sv[e] * scale_log2), p1 = fast_exp2(sv[e + 1] * scale_log2);
-        pw[e >> 1] = pack_bf16(p0, p1);
-        dw[e >> 1] = pack_bf16(p0 * dp[e] * scale, p1 * dp[e + 1] * scale);
-      }
-      if (lane == 0 && (warp == 0 || warp == 15)) LGB_TR(2 + (warp == 15), i, 2);
-      tmem_st8(tb + c * F3_CW, pw);        // P^T over the S columns this warpgroup just consumed
-      tmem_st8(tb + 64 + c * F3_CW, dw);   // dS^T over the dP columns
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&pds_full[buf]);
-      if (lane == 0 && (warp == 0 || warp == 15)) LGB_TR(2 + (warp == 15), i, 3);
-    }
-    mbar_wait(acc_done, 0);
-    tc_fence_after();
-    const int64_t o = (((int64_t)kb * Nk + (row < Nk ? row : 0)) * H + h) * FA_D + c * F3_CW;
-    store_out_cols16(dv + o, t_lane + F4_ACC0 + c * F3_CW, row < Nk);
-    store_out_cols16(dk + o, t_lane + F4_ACC1 + c * F3_CW, row < Nk);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == F3_SWARPS + 1) tmem_dealloc(tmem_base, FB_TMEM_COLS);
-  LGB_TR_LIFE(1);
-}
-
-__global__ void __launch_bounds__(F3_THREADS, 1)
-    attn_bwd_dq_v3_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                          const __nv_bfloat16* __restrict__ qg, const __nv_bfloat16* __restrict__ dog,
-                          const float* __restrict__ lse, const float* __restrict__ delta,
-                          __nv_bfloat16* __restrict__ dq, int B, int Nq, int Nk, int H, int kv_shift, float scale,
-                          float scale_log2) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sK = smem;                                // [F3_STAGES]
-  uint8_t* sV = sK + F3_STAGES * FB_CBYTES;          // [F3_STAGES]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + F3_STAGES * FB_CBYTES);
-  uint64_t* a_ready = bars;
-  uint64_t* in_full = bars + 1;
-  uint64_t* in_empty = in_full + F3_STAGES;
-  uint64_t* sp_full = in_empty + F3_STAGES;   // [2]
-  uint64_t* ds_full = sp_full + 2;            // [2]
-  uint64_t* acc_done = ds_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_done + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * FB_R, h = blockIdx.y, b = blockIdx.z;
-  const int kb = (b + kv_shift) % B;
-  const int ntiles = (Nk + FB_C - 1) / FB_C;
-
-  if (threadIdx.x == 0) {
-    if (smem_u32(smem) & 1023u) __trap();
-    mbar_init(a_ready, F3_SWARPS);
-    for (int s = 0; s < F3_STAGES; ++s) {
-      mbar_init(&in_full[s], 1);
-      mbar_init(&in_empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&sp_full[s], 1);
-      mbar_init(&ds_full[s], F3_SWARPS);
-    }
-    mbar_init(acc_done, 1);
-    mbar_fence_init();
-  }
-  if (warp == F3_SWARPS && lane == 0) {
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-  }
-  if (warp == F3_SWARPS + 1) tmem_alloc(tmem_slot, FB_TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == F3_SWARPS) {
-    if (lane == 0) {
-      for (int j = 0; j < ntiles; ++j) {
-        const int s = j % F3_STAGES;
-        mbar_wait(&in_empty[s], ((j / F3_STAGES) & 1) ^ 1);
-        mbar_expect_tx(&in_full[s], 2 * FB_CBYTES);
-        tma_load_4d(sK + s * FB_CBYTES, &tmK, &in_full[s], 0, h, j * FB_C, kb);
-        tma_load_4d(sV + s * FB_CBYTES, &tmV, &in_full[s], 0, h, j * FB_C, kb);
-      }
-    }
-  } else if (warp == F3_SWARPS + 1) {
-    constexpr uint32_t idesc_s = make_idesc_bf16(FB_R, FB_C, 0, 0);    // (Q|dO) in TMEM x (K|V) K-major
-    constexpr uint32_t idesc_acc = make_idesc_bf16(FB_R, FA_D, 0, 1);  // dS in TMEM x K_j MN-major
-    const uint64_t dKk = make_smem_desc(smem_u32(sK), 16, 1024), dVk = make_smem_desc(smem_u32(sV), 16, 1024);
-    const uint64_t dKm = make_smem_desc(smem_u32(sK), 8192, 1024);
-    const bool leader = elect_one();
-    auto issue_sp = [&](int j) {
-      const int s = j % F3_STAGES;
-      mbar_wait(&in_full[s], (j / F3_STAGES) & 1);
-      tc_fence_after();
-      if (leader) {
-        const uint32_t tb = tmem_base + F3_BUF0 + (j & 1) * 128;
-        const uint64_t so = (uint64_t)((s * FB_CBYTES) >> 4);
-#pragma unroll
-        for (int kk = 0; kk < FA_D / 16; ++kk)
-          umma_bf16_ts(tb, tmem_base + F3_A0 + kk * 8, dKk + so + (uint64_t)(kk * 2), idesc_s, kk != 0 ? 1u : 0u);
-#pragma unroll
-        for (int kk = 0; kk < FA_D / 16; ++kk)
-          umma_bf16_ts(tb + 64, tmem_base + F3_A1 + kk * 8, dVk + so + (uint64_t)(kk * 2), idesc_s, kk != 0 ? 1u : 0u);
-        umma_commit(&sp_full[j & 1]);
-      }
-      __syncwarp();
-    };
-    mbar_wait(a_ready, 0);
-    tc_fence_after();
-    issue_sp(0);
-    if (ntiles > 1) issue_sp(1);
-    for (int j = 0; j < ntiles; ++j) {
-      const int s = j % F3_STAGES;
-      mbar_wait(&ds_full[j & 1], (j >> 1) & 1);
-      tc_fence_after();
-      if (leader) {
-        const uint32_t tb = tmem_base + F3_BUF0 + (j & 1) * 128;
-        const uint64_t so = (uint64_t)((s * FB_CBYTES) >> 4);
-#pragma unroll
-        for (int kk = 0; kk < FB_C / 16; ++kk)  // dS of keys [kk*16, kk*16+16) sits at dP column kk*16
-          umma_bf16_ts(tmem_base + F3_ACC0, tb + 64 + kk * F3_CW, dKm + so + (uint64_t)(kk * 128), idesc_acc,
-                       (j | kk) != 0 ? 1u : 0u);
-        umma_commit(&in_empty[s]);
-      }
-      __syncwarp();
-      if (j + 2 < ntiles) issue_sp(j + 2);
-    }
-    if (leader) umma_commit(acc_done);
-    __syncwarp();
-  } else {
-    const int c = warp >> 2;
-    const int r = (warp & 3) * 32 + lane;
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>((warp & 3) * 32) << 16);
-    const int row = q0 + r;
-    {
-      const int64_t o = (((int64_t)b * Nq + (row < Nq ? row : 0)) * H + h) * FA_D + c * F3_CW;
-      load_row_part_to_tmem(qg + o, row < Nq, t_lane + F3_A0 + c * (F3_CW / 2));
-      load_row_part_to_tmem(dog + o, row < Nq, t_lane + F3_A1 + c * (F3_CW / 2));
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(a_ready);
-    }
-    const int64_t lo = ((int64_t)b * H + h) * Nq + (row < Nq ? row : 0);
-    const float lse2 = row < Nq ? lse[lo] * 1.4426950408889634f : INFINITY;
-    const float dl = row < Nq ? delta[lo] : 0.f;
-    for (int j = 0; j < ntiles; ++j) {
-      const int buf = j & 1;
-      const uint32_t tb = t_lane + F3_BUF0 + buf * 128;
-      mbar_wait(&sp_full[buf], (j >> 1) & 1);
-      tc_fence_after();
-      float sv[F3_CW], dp[F3_CW];
-      tmem_ld16(tb + c * F3_CW, sv);
-      tmem_ld16(tb + 64 + c * F3_CW, dp);
-      tmem_ld_wait();
-      uint32_t dw[F3_CW / 2];
-#pragma unroll
-      for (int e = 0; e < F3_CW; e += 2) {
-        const float p0 = fast_exp2(fmaf(sv[e], scale_log2, -lse2));
-        const float p1 = fast_exp2(fmaf(sv[e + 1], scale_log2, -lse2));
-        dw[e >> 1] = pack_bf16(p0 * (dp[e] - dl) * scale, p1 * (dp[e + 1] - dl) * scale);
-      }
-      tmem_st8(tb + 64 + c * F3_CW, dw);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&ds_full[buf]);
-    }
-    mbar_wait(acc_done, 0);
-    tc_fence_after();
-    store_out_cols16(dq + (((int64_t)b * Nq + (row < Nq ? row : 0)) * H + h) * FA_D + c * F3_CW,
-                     t_lane + F3_ACC0 + c * F3_CW, row < Nq);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == F3_SWARPS + 1) tmem_dealloc(tmem_base, FB_TMEM_COLS);
-}
-
-// ---------------------------------------------------------------------------------------------
-// BACKWARD, fused single pass (round 2).  The two-kernel backward above recomputes S and dP in both kernels
-// (14 GEMM-units for 10 algorithmic) and evaluates every exponential twice.  Here one CTA owns 128 keys (K, V rows
-// resident in TMEM exactly as in the dKV kernel) and walks the queries in tiles of 64:
-//     S^T  = K Q_i^T,  dP^T = V dO_i^T            (128 x 64, TS MMAs, double-buffered in TMEM)
-//     P^T  = exp2(c S^T - lse_i),  dS^T = P^T (dP^T - delta_i) scale       (softmax warps, thread == key row)
-//     dV  += P^T dO_i,   dK += dS^T Q_i           (TS MMAs, P^T / dS^T written in place over S^T / dP^T)
-// and additionally, once per PAIR of query tiles,
-//     dQ_pair (128 queries x 64) = dS_pair K      (M = 128: both operands MN-major from shared memory)
-// where dS_pair is the bf16 copy of dS^T the softmax warps also leave in shared memory ([key][query], 128-byte
-// swizzled: read with M = query it is the MN-major A operand).  dQ_pair is drained TMEM -> swizzled smem -> global by a
-// TMA REDUCE-ADD into an fp32 accumulation buffer (the 16 key-tile CTAs of one (batch, head) add into the same rows; they
-// are adjacent in the grid, so the buffer lives in L2), converted to bf16 by a last small kernel.
-// Per 128 x 128 block: 2 x (5+5) S/dP + 2 x (4+4) dV/dK + 8 dQ MMAs and ONE exponential per element, against
-// 2 x (5+5+4+4) + 2 x (4+4+4) MMAs and two exponentials in the two-kernel version.  lse / delta per query are per-COLUMN
-// values here; they come as two 64-float vectors with every query tile (bulk copies into the stage) and are read as
-// shared-memory broadcasts (the dKV kernel folds them into the contraction instead, which costs 16 more TMEM columns
-// than this kernel has left).  Summation order of dQ across key tiles is not fixed (fp32 adds in L2).
-// TMEM: K [0,32) V [32,64) | buffer b: S^T at 64+b*128, dP^T at 128+b*128 | dV [320,384) dK [384,448) dQ [448,512).
-// ---------------------------------------------------------------------------------------------
-constexpr int FF_STAGES = 4;
+constexpr int FF_STAGES = 3;
 constexpr int FF_STAGE_BYTES = 17 * 1024;                 // Q 8 KiB | dO 8 KiB | lse2 256 B | delta 256 B (| pad)
-constexpr int FF_DSBYTES = 2 * FB_R * 128;                // one pair of 64-query chunks: 128 key rows x 128 B each
-constexpr int FF_DQBYTES = FB_R * FA_D * 4;               // fp32 staging of a dQ pair (two 32-float halves)
-constexpr int FF_OFF_STAGE = FB_R * FA_D * 2;             // after the resident K tile (16 KiB)
+constexpr int FF_OFF_STAGE = 2 * FB_R * FA_D * 2;         // after the resident K and V tiles (16 KiB each)
 constexpr int FF_OFF_DS = FF_OFF_STAGE + FF_STAGES * FF_STAGE_BYTES;
-constexpr int FF_OFF_DQ = FF_OFF_DS + 2 * FF_DSBYTES;
-constexpr int FF_SMEM = FF_OFF_DQ + FF_DQBYTES + 256;
-constexpr int FF_A0 = 0, FF_A1 = 32, FF_BUF0 = 64, FF_DV = 320, FF_DK = 384, FF_DQ = 448;
+constexpr int FF_SMEM = FF_OFF_DS + 2 * FB_C * 128 + 256; // + one 64 x 64 bf16 dS^T tile per warpgroup
+constexpr int FQ_STAGES = 4;
+constexpr int FQ_SMEM = 2 * FB_R * FA_D * 2 + FQ_STAGES * 2 * FB_CBYTES + 256;
 
 __device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
@@ -824,16 +234,6 @@ __device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_
                "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-__device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-constexpr int FF_DWARPS = 4;                               // dedicated dQ-drain warpgroup (warps 16..19)
-constexpr int FF_THREADS = (F3_SWARPS + FF_DWARPS + 2) * 32;
-__device__ __forceinline__ void bar_drain() { asm volatile("bar.sync 2, %0;" ::"n"(FF_DWARPS * 32) : "memory"); }
-
 // delta = rowsum(dout * out) * scale; lse2 = lse * log2(e); both written token-tile padded: [B*H][nq_pad] with +inf / 0 in the pad
 __global__ void __launch_bounds__(256)
     attn_bwd_prep_fused_kernel(const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __restrict__ dout,
@@ -882,79 +282,55 @@ __global__ void __launch_bounds__(256) dq_convert_kernel(const float* __restrict
   reinterpret_cast<uint4*>(dq)[i] = u;
 }
 
-__global__ void __launch_bounds__(FF_THREADS, 1)
-    attn_bwd_fused_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
-                          const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmDQ,
-                          const __nv_bfloat16* __restrict__ kg, const __nv_bfloat16* __restrict__ vg,
-                          const float* __restrict__ lse2p, const float* __restrict__ deltap,
-                          __nv_bfloat16* __restrict__ dk, __nv_bfloat16* __restrict__ dv, int B, int Nq, int nq_pad, int Nk,
-                          int H, int kv_shift, float scale, float scale_log2) {
+template <bool WITH_DQ>
+__global__ void __launch_bounds__(FA_THREADS, 1)
+    attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
+                        const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                        const float* __restrict__ lse2p, const float* __restrict__ deltap,
+                        __nv_bfloat16* __restrict__ dk, __nv_bfloat16* __restrict__ dv, float* __restrict__ dqacc, int B,
+                        int Nq, int nq_pad, int Nk, int H, int kv_shift, float scale, float scale_log2) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sK = smem;
+  uint8_t* sV = smem + FB_R * FA_D * 2;
   uint8_t* sStage = smem + FF_OFF_STAGE;
-  uint8_t* sDS = smem + FF_OFF_DS;
-  uint8_t* sDQ = smem + FF_OFF_DQ;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + FF_OFF_DQ + FF_DQBYTES);
-  uint64_t* k_full = bars;
-  uint64_t* a_ready = bars + 1;
-  uint64_t* in_full = bars + 2;               // [FF_STAGES]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + FF_SMEM - 256);
+  uint64_t* kv_full = bars;
+  uint64_t* in_full = bars + 1;               // [FF_STAGES]
   uint64_t* in_empty = in_full + FF_STAGES;   // [FF_STAGES]
-  uint64_t* sp_full = in_empty + FF_STAGES;   // [2]
-  uint64_t* pds_full = sp_full + 2;           // [2]
-  uint64_t* ds_free = pds_full + 2;           // [2]  MMA 5 of the pair that used sDS[b] has read it
-  uint64_t* dq_full = ds_free + 2;
-  uint64_t* dq_empty = dq_full + 1;
-  uint64_t* acc_done = dq_empty + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_done + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int k0 = blockIdx.x * FB_R, h = blockIdx.y, kb = blockIdx.z;
   const int qb = ((kb - kv_shift) % B + B) % B;
   const int ntiles = (Nq + FB_C - 1) / FB_C;
-  const int npairs = (ntiles + 1) >> 1;
 
   if (threadIdx.x == 0) {
     if (smem_u32(smem) & 1023u) __trap();
-    mbar_init(k_full, 1);
-    mbar_init(a_ready, F3_SWARPS);
+    mbar_init(kv_full, 1);
     for (int s = 0; s < FF_STAGES; ++s) {
       mbar_init(&in_full[s], 1);
-      mbar_init(&in_empty[s], 1);
+      mbar_init(&in_empty[s], 2);
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&sp_full[s], 1);
-      mbar_init(&pds_full[s], F3_SWARPS);
-      mbar_init(&ds_free[s], 1);
-    }
-    mbar_init(dq_full, 1);
-    mbar_init(dq_empty, FF_DWARPS);
-    mbar_init(acc_done, 1);
     mbar_fence_init();
   }
-  if (warp == F3_SWARPS + FF_DWARPS && lane == 0) {
+  if (warp == FA_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmDO);
     tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmDQ);
+    tma_prefetch_desc(&tmV);
   }
-  if (warp == F3_SWARPS + FF_DWARPS + 1) tmem_alloc(tmem_slot, FB_TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == F3_SWARPS + FF_DWARPS) {
-    // ------------------------------------------------------------------ TMA producer
+  if (warp == FA_PRODUCER) {
     if (lane == 0) {
-      mbar_expect_tx(k_full, FB_R * FA_D * 2);
-      tma_load_4d(sK, &tmK, k_full, 0, h, k0, kb);
+      mbar_expect_tx(kv_full, 2 * FB_R * FA_D * 2);
+      tma_load_4d(sK, &tmK, kv_full, 0, h, k0, kb);
+      tma_load_4d(sV, &tmV, kv_full, 0, h, k0, kb);
       const float* l2 = lse2p + ((int64_t)qb * H + h) * nq_pad;
       const float* dl = deltap + ((int64_t)qb * H + h) * nq_pad;
       for (int i = 0; i < ntiles; ++i) {
         const int s = i % FF_STAGES;
         uint8_t* st = sStage + s * FF_STAGE_BYTES;
         mbar_wait(&in_empty[s], ((i / FF_STAGES) & 1) ^ 1);
-        LGB_TR(0, i, 0);
         mbar_expect_tx(&in_full[s], 2 * FB_CBYTES + 512);
         tma_load_4d(st, &tmQ, &in_full[s], 0, h, i * FB_C, qb);
         tma_load_4d(st + FB_CBYTES, &tmDO, &in_full[s], 0, h, i * FB_C, qb);
@@ -962,200 +338,212 @@ __global__ void __launch_bounds__(FF_THREADS, 1)
         bulk_load_1d(st + 2 * FB_CBYTES + 256, dl + i * FB_C, 256, &in_full[s]);
       }
     }
-  } else if (warp == F3_SWARPS + FF_DWARPS + 1) {
-    // ------------------------------------------------------------------ MMA issuer (warp-convergent, elected lane)
-    constexpr uint32_t idesc_s = make_idesc_bf16(FB_R, FB_C, 0, 0);    // (K|V) in TMEM x (Q|dO) K-major
-    constexpr uint32_t idesc_acc = make_idesc_bf16(FB_R, FA_D, 0, 1);  // (P^T|dS^T) in TMEM x (dO|Q) MN-major
-    constexpr uint32_t idesc_dq = make_idesc_bf16(FB_R, FA_D, 1, 1);   // dS_pair (smem, MN-major) x K (smem, MN-major)
-    const uint64_t dstK = make_smem_desc(smem_u32(sStage), 16, 1024);    // K-major view of a stage's tiles
-    const uint64_t dstM = make_smem_desc(smem_u32(sStage), 8192, 1024);  // MN-major view
-    const uint64_t dDS = make_smem_desc(smem_u32(sDS), FB_R * 128, 1024);  // two 64-query chunks 16 KiB apart
-    const uint64_t dKm = make_smem_desc(smem_u32(sK), 8192, 1024);
-    const bool leader = elect_one();
-    auto issue_sp = [&](int i) {
-      const int s = i % FF_STAGES;
-      mbar_wait(&in_full[s], (i / FF_STAGES) & 1);
-      tc_fence_after();
-      if (leader) {
-        const uint32_t tb = tmem_base + FF_BUF0 + (i & 1) * 128;
-        const uint64_t so = (uint64_t)((s * FF_STAGE_BYTES) >> 4);
-        const uint64_t tq = dstK + so, tdo = dstK + so + (FB_CBYTES >> 4);
-#pragma unroll
-        for (int kk = 0; kk < FA_D / 16; ++kk)
-          umma_bf16_ts(tb, tmem_base + FF_A0 + kk * 8, tq + (uint64_t)(kk * 2), idesc_s, kk != 0 ? 1u : 0u);
-#pragma unroll
-        for (int kk = 0; kk < FA_D / 16; ++kk)
-          umma_bf16_ts(tb + 64, tmem_base + FF_A1 + kk * 8, tdo + (uint64_t)(kk * 2), idesc_s, kk != 0 ? 1u : 0u);
-        umma_commit(&sp_full[i & 1]);
-      }
-      __syncwarp();
-    };
-    mbar_wait(a_ready, 0);
-    mbar_wait(k_full, 0);
-    tc_fence_after();
-    issue_sp(0);
-    if (ntiles > 1) issue_sp(1);
-    for (int i = 0; i < ntiles; ++i) {
-      const int s = i % FF_STAGES;
-      mbar_wait(&pds_full[i & 1], (i >> 1) & 1);
-      tc_fence_after();
-      if (leader) LGB_TR(1, i, 0);
-      if (leader) {
-        const uint32_t tb = tmem_base + FF_BUF0 + (i & 1) * 128;
-        const uint64_t so = (uint64_t)((s * FF_STAGE_BYTES) >> 4);
-        const uint64_t mq = dstM + so, mdo = dstM + so + (FB_CBYTES >> 4);
-#pragma unroll
-        for (int kk = 0; kk < FB_C / 16; ++kk)  // warpgroup kk wrote P^T of queries [kk*16, +16) at S^T column kk*16
-          umma_bf16_ts(tmem_base + FF_DV, tb + kk * F3_CW, mdo + (uint64_t)(kk * 128), idesc_acc, (i | kk) != 0 ? 1u : 0u);
-#pragma unroll
-        for (int kk = 0; kk < FB_C / 16; ++kk)
-          umma_bf16_ts(tmem_base + FF_DK, tb + 64 + kk * F3_CW, mq + (uint64_t)(kk * 128), idesc_acc,
-                       (i | kk) != 0 ? 1u : 0u);
-        umma_commit(&in_empty[s]);
-      }
-      if (leader) LGB_TR(1, i, 1);
-      __syncwarp();
-      // S/dP of tile i+2 go in AHEAD of the pair's dQ product (8 SS MMAs, ~700 clk): nothing waits for dQ but the drain
-      // warps, while the softmax of tile i+2 is on the loop's critical path (fused backward 462 -> 437 us at 32 sequences)
-      if (i + 2 < ntiles) issue_sp(i + 2);
-      if ((i & 1) || i == ntiles - 1) {  // the pair is complete: dQ_pair = dS_pair K
-        const int pr = i >> 1;
-        mbar_wait(dq_empty, (pr & 1) ^ 1);  // the softmax warps drained the previous pair's dQ
-        tc_fence_after();
-        if (leader) {
-          const uint64_t da = dDS + (uint64_t)(((pr & 1) * FF_DSBYTES) >> 4);
-#pragma unroll
-          for (int kk = 0; kk < FB_R / 16; ++kk)  // 16 keys per step: 16 rows of 128 B in both operands
-            umma_bf16(tmem_base + FF_DQ, da + (uint64_t)(kk * 128), dKm + (uint64_t)(kk * 128), idesc_dq, kk != 0 ? 1u : 0u);
-          umma_commit(dq_full);
-          umma_commit(&ds_free[pr & 1]);
-        }
-        __syncwarp();
-      }
-      if (leader) LGB_TR(1, i, 2);
-      if (leader) LGB_TR(1, i, 3);
-    }
-    if (leader) umma_commit(acc_done);
-    __syncwarp();
-  } else if (warp >= F3_SWARPS) {
-    // ------------------------------------------------------------------ dQ drain warpgroup
-    // One pair of query tiles at a time: dQ_pair (128 queries x 64 channels fp32, TMEM) -> registers -> swizzled
-    // staging -> TMA reduce-add into the fp32 accumulator.  Kept off the softmax warps: in the first version they did
-    // this between two tiles (two 512-thread barriers + the TMEM read + the staging stores = 840 clk every other tile,
-    // the longest item of their per-pair critical path in the clock64 trace).
-    const int r = (warp & 3) * 32 + lane;    // query row of the pair == TMEM lane (warps 16..19 -> lane quarters 0..3)
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>((warp & 3) * 32) << 16);
-    const bool issuer = warp == F3_SWARPS && lane == 0;
-    for (int pr = 0; pr < npairs; ++pr) {
-      mbar_wait(dq_full, pr & 1);
-      tc_fence_after();
-      float v[FA_D];
-#pragma unroll
-      for (int q4 = 0; q4 < 4; ++q4) tmem_ld16(t_lane + FF_DQ + q4 * 16, v + q4 * 16);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(dq_empty);          // dQ columns are free for the next pair's MMAs
-      if (issuer) tma_store_wait_read<0>();          // the previous pair's reduce has read the staging block
-      bar_drain();
-      // staging: two halves (channels 0-31 / 32-63), each 128 rows x 128 B, 16-byte chunks XOR-swizzled by the row
-#pragma unroll
-      for (int hf = 0; hf < 2; ++hf) {
-        uint8_t* half = sDQ + hf * (FB_R * 128) + r * 128;
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          *reinterpret_cast<float4*>(half + ((j ^ (r & 7)) << 4)) =
-              make_float4(v[hf * 32 + 4 * j], v[hf * 32 + 4 * j + 1], v[hf * 32 + 4 * j + 2], v[hf * 32 + 4 * j + 3]);
-      }
-      fence_proxy_async_smem();
-      bar_drain();
-      if (issuer) {
-        tma_reduce_add_4d(&tmDQ, sDQ, 0, h, pr * FB_R, qb);
-        tma_reduce_add_4d(&tmDQ, sDQ + FB_R * 128, 32, h, pr * FB_R, qb);
-        tma_store_commit();
-      }
-    }
-    if (issuer) tma_store_wait_all();  // the last reduce must have left shared memory before the CTA exits
-  } else {
-    // ------------------------------------------------------------------ softmax warps
-    const int c = warp >> 2;                 // 16-query column slice handled by this warpgroup
-    const int r = (warp & 3) * 32 + lane;    // key row within the tile == TMEM lane
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>((warp & 3) * 32) << 16);
-    const int row = k0 + r;
-    {  // resident A operands: this thread's 16-channel slice of its K and V rows -> TMEM
-      const int64_t o = (((int64_t)kb * Nk + (row < Nk ? row : 0)) * H + h) * FA_D + c * F3_CW;
-      load_row_part_to_tmem(kg + o, row < Nk, t_lane + FF_A0 + c * (F3_CW / 2));
-      load_row_part_to_tmem(vg + o, row < Nk, t_lane + FF_A1 + c * (F3_CW / 2));
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(a_ready);
-    }
-    for (int i = 0; i < ntiles; ++i) {
-      const int buf = i & 1, pr = i >> 1, s = i % FF_STAGES;
-      const uint32_t tb = t_lane + FF_BUF0 + buf * 128;
-      const float* sl = reinterpret_cast<const float*>(sStage + s * FF_STAGE_BYTES + 2 * FB_CBYTES) + c * F3_CW;
-      mbar_wait(&in_full[s], (i / FF_STAGES) & 1);  // the side vectors of this tile (bulk copies) are visible to this thread
-      mbar_wait(&sp_full[buf], (i >> 1) & 1);
-      tc_fence_after();
-      if (lane == 0 && (warp == 0 || warp == 15)) LGB_TR(2 + (warp == 15), i, 0);
-      float sv[F3_CW], dp[F3_CW];
-      tmem_ld16(tb + c * F3_CW, sv);
-      tmem_ld16(tb + 64 + c * F3_CW, dp);
-      float l2[F3_CW], dl[F3_CW];
-#pragma unroll
-      for (int e4 = 0; e4 < F3_CW / 4; ++e4) {  // same addresses in every lane: shared-memory broadcasts
-        const float4 a = *reinterpret_cast<const float4*>(sl + e4 * 4);
-        const float4 b = *reinterpret_cast<const float4*>(sl + 64 + e4 * 4);
-        l2[e4 * 4] = a.x; l2[e4 * 4 + 1] = a.y; l2[e4 * 4 + 2] = a.z; l2[e4 * 4 + 3] = a.w;
-        dl[e4 * 4] = b.x; dl[e4 * 4 + 1] = b.y; dl[e4 * 4 + 2] = b.z; dl[e4 * 4 + 3] = b.w;
-      }
-      tmem_ld_wait();
-      uint32_t pw[F3_CW / 2], dw[F3_CW / 2];
-#pragma unroll
-      for (int e = 0; e < F3_CW; e += 2) {
-        const float p0 = fast_exp2(fmaf(sv[e], scale_log2, -l2[e]));
-        const float p1 = fast_exp2(fmaf(sv[e + 1], scale_log2, -l2[e + 1]));
-        pw[e >> 1] = pack_bf16(p0, p1);
-        dw[e >> 1] = pack_bf16(p0 * fmaf(dp[e], scale, -dl[e]), p1 * fmaf(dp[e + 1], scale, -dl[e + 1]));  // dl = delta * scale
-      }
-      if (lane == 0 && (warp == 0 || warp == 15)) LGB_TR(2 + (warp == 15), i, 1);
-      tmem_st8(tb + c * F3_CW, pw);        // P^T over the S^T columns this warpgroup just consumed
-      tmem_st8(tb + 64 + c * F3_CW, dw);   // dS^T over the dP^T columns
-      // bf16 dS also goes to shared memory, [key][query] (row = this thread's key), for the dQ MMA of the pair
-      if (buf == 0 && pr >= 2) mbar_wait(&ds_free[pr & 1], ((pr >> 1) & 1) ^ 1);  // pair pr-2 has been consumed
-      {
-        uint8_t* rowp = sDS + (pr & 1) * FF_DSBYTES + buf * (FB_R * 128) + r * 128;
-        *reinterpret_cast<uint4*>(rowp + (((2 * c) ^ (r & 7)) << 4)) = make_uint4(dw[0], dw[1], dw[2], dw[3]);
-        *reinterpret_cast<uint4*>(rowp + (((2 * c + 1) ^ (r & 7)) << 4)) = make_uint4(dw[4], dw[5], dw[6], dw[7]);
-      }
-      fence_proxy_async_smem();
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&pds_full[buf]);
-      if (lane == 0 && (warp == 0 || warp == 15)) LGB_TR(2 + (warp == 15), i, 2);
-    }
-    mbar_wait(acc_done, 0);
-    tc_fence_after();
-    const int64_t o = (((int64_t)kb * Nk + (row < Nk ? row : 0)) * H + h) * FA_D + c * F3_CW;
-    store_out_cols16(dv + o, t_lane + FF_DV + c * F3_CW, row < Nk);
-    store_out_cols16(dk + o, t_lane + FF_DK + c * F3_CW, row < Nk);
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == F3_SWARPS + FF_DWARPS + 1) tmem_dealloc(tmem_base, FB_TMEM_COLS);
+  const int wg = threadIdx.x >> 7, wq = warp & 3, g = lane >> 2, t4 = lane & 3;
+  const bool signal = (threadIdx.x & 127) == 0;
+  uint8_t* sDS = smem + FF_OFF_DS + wg * (FB_C * 128);
+  const uint64_t dK0 = make_smem_desc(smem_u32(sK) + wg * 8192, 8192, 1024);
+  const uint64_t dV0 = make_smem_desc(smem_u32(sV) + wg * 8192, 8192, 1024);
+  const uint64_t dSt0 = make_smem_desc(smem_u32(sStage), 8192, 1024);
+  const uint64_t dDS = make_smem_desc(smem_u32(sDS), 8192, 1024);
+  float acc_v[32], acc_k[32];
+#pragma unroll
+  for (int e = 0; e < 32; ++e) acc_v[e] = acc_k[e] = 0.f;
+  mbar_wait(kv_full, 0);
+  for (int i = 0; i < ntiles; ++i) {
+    const int s = i % FF_STAGES;
+    const uint64_t so = (uint64_t)((s * FF_STAGE_BYTES) >> 4), so_do = so + (FB_CBYTES >> 4);
+    const float* sl = reinterpret_cast<const float*>(sStage + s * FF_STAGE_BYTES + 2 * FB_CBYTES);
+    mbar_wait(&in_full[s], (i / FF_STAGES) & 1);
+    float st[32], dp[32];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(st, dK0 + kk * 2, dSt0 + so + kk * 2, kk != 0);
+#pragma unroll
+    for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(dp, dV0 + kk * 2, dSt0 + so_do + kk * 2, kk != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_hold(st);
+    wgmma_hold(dp);
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const float2 l2 = *reinterpret_cast<const float2*>(sl + 8 * jj + 2 * t4);       // columns = queries
+      const float2 dl = *reinterpret_cast<const float2*>(sl + 64 + 8 * jj + 2 * t4);  // delta * scale
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int x = 4 * jj + 2 * r;
+        st[x] = fast_exp2(fmaf(st[x], scale_log2, -l2.x));
+        st[x + 1] = fast_exp2(fmaf(st[x + 1], scale_log2, -l2.y));
+        dp[x] = st[x] * fmaf(dp[x], scale, -dl.x);
+        dp[x + 1] = st[x + 1] * fmaf(dp[x + 1], scale, -dl.y);
+      }
+    }
+    uint32_t pa[4][4], da[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      acc_to_afrag(st, kk, pa[kk]);
+      acc_to_afrag(dp, kk, da[kk]);
+    }
+    if constexpr (WITH_DQ) {
+      // dS^T (bf16) -> this warpgroup's [key][query] tile; the previous tile's dQ product has retired in every warp
+      named_bar(1 + wg, 128);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int key = wq * 16 + g + 8 * r;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+          *reinterpret_cast<uint32_t*>(sDS + key * 128 + ((jj ^ (key & 7)) << 4) + 4 * t4) =
+              pack_bf16(dp[4 * jj + 2 * r], dp[4 * jj + 2 * r + 1]);
+      }
+      fence_proxy_async_smem();
+      named_bar(1 + wg, 128);
+    }
+    float dq[32];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < FB_C / 16; ++kk) wgmma_m64n64_rs<1>(acc_v, pa[kk], dSt0 + so_do + kk * 128, 1);
+#pragma unroll
+    for (int kk = 0; kk < FB_C / 16; ++kk) wgmma_m64n64_rs<1>(acc_k, da[kk], dSt0 + so + kk * 128, 1);
+    if constexpr (WITH_DQ) {
+#pragma unroll
+      for (int kk = 0; kk < FB_C / 16; ++kk)  // dQ_i = dS K_w: 16 keys per step, both operands MN-major
+        wgmma_m64n64_ss<1, 1>(dq, dDS + kk * 128, dK0 + kk * 128, kk != 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_hold(acc_v);
+    wgmma_hold(acc_k);
+    if (signal) mbar_arrive(&in_empty[s]);
+    if constexpr (WITH_DQ) {
+      wgmma_hold(dq);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int q = i * FB_C + wq * 16 + g + 8 * r;
+        if (q >= Nq) continue;
+        float* dst = dqacc + (((int64_t)qb * Nq + q) * H + h) * FA_D + 2 * t4;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+          atomicAdd(reinterpret_cast<float2*>(dst + 8 * jj), make_float2(dq[4 * jj + 2 * r], dq[4 * jj + 2 * r + 1]));
+      }
+    }
+  }
+  store_acc_rows(acc_v, dv, kb, Nk, H, h, k0 + wg * 64, 1.f);
+  store_acc_rows(acc_k, dk, kb, Nk, H, h, k0 + wg * 64, 1.f);
 }
 
-// workspace of the fused backward, in floats: lse2 / delta padded to whole query tiles + the fp32 dQ accumulator
-static int64_t attn_bwd_fused_ws_floats(int B, int Nq, int H) {
+__global__ void __launch_bounds__(FA_THREADS, 1)
+    attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
+                       const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                       const float* __restrict__ lse2p, const float* __restrict__ deltap, __nv_bfloat16* __restrict__ dq,
+                       int B, int Nq, int nq_pad, int Nk, int H, int kv_shift, float scale, float scale_log2) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* sQ = smem;
+  uint8_t* sDO = smem + FB_R * FA_D * 2;
+  uint8_t* sK = smem + 2 * FB_R * FA_D * 2;       // [FQ_STAGES]
+  uint8_t* sV = sK + FQ_STAGES * FB_CBYTES;       // [FQ_STAGES]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + FQ_STAGES * FB_CBYTES);
+  uint64_t* qd_full = bars;
+  uint64_t* in_full = bars + 1;
+  uint64_t* in_empty = in_full + FQ_STAGES;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q0 = blockIdx.x * FB_R, h = blockIdx.y, b = blockIdx.z;
+  const int kb = (b + kv_shift) % B;
+  const int ntiles = (Nk + FB_C - 1) / FB_C;
+
+  if (threadIdx.x == 0) {
+    if (smem_u32(smem) & 1023u) __trap();
+    mbar_init(qd_full, 1);
+    for (int s = 0; s < FQ_STAGES; ++s) {
+      mbar_init(&in_full[s], 1);
+      mbar_init(&in_empty[s], 2);
+    }
+    mbar_fence_init();
+  }
+  if (warp == FA_PRODUCER && lane == 0) {
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmDO);
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+  }
+  __syncthreads();
+
+  if (warp == FA_PRODUCER) {
+    if (lane == 0) {
+      mbar_expect_tx(qd_full, 2 * FB_R * FA_D * 2);
+      tma_load_4d(sQ, &tmQ, qd_full, 0, h, q0, b);
+      tma_load_4d(sDO, &tmDO, qd_full, 0, h, q0, b);
+      for (int j = 0; j < ntiles; ++j) {
+        const int s = j % FQ_STAGES;
+        mbar_wait(&in_empty[s], ((j / FQ_STAGES) & 1) ^ 1);
+        mbar_expect_tx(&in_full[s], 2 * FB_CBYTES);
+        tma_load_4d(sK + s * FB_CBYTES, &tmK, &in_full[s], 0, h, j * FB_C, kb);
+        tma_load_4d(sV + s * FB_CBYTES, &tmV, &in_full[s], 0, h, j * FB_C, kb);
+      }
+    }
+    return;
+  }
+  const int wg = threadIdx.x >> 7;
+  const bool signal = (threadIdx.x & 127) == 0;
+  const uint64_t dQ0 = make_smem_desc(smem_u32(sQ) + wg * 8192, 8192, 1024);
+  const uint64_t dDO0 = make_smem_desc(smem_u32(sDO) + wg * 8192, 8192, 1024);
+  const uint64_t dK0 = make_smem_desc(smem_u32(sK), 8192, 1024), dV0 = make_smem_desc(smem_u32(sV), 8192, 1024);
+  float l2[2], dl[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;
+    const int64_t o = ((int64_t)b * H + h) * nq_pad + row;
+    l2[r] = row < Nq ? lse2p[o] : INFINITY;
+    dl[r] = row < Nq ? deltap[o] : 0.f;
+  }
+  float acc[32];
+#pragma unroll
+  for (int e = 0; e < 32; ++e) acc[e] = 0.f;
+  mbar_wait(qd_full, 0);
+  for (int j = 0; j < ntiles; ++j) {
+    const int s = j % FQ_STAGES;
+    const uint64_t so = (uint64_t)((s * FB_CBYTES) >> 4);
+    mbar_wait(&in_full[s], (j / FQ_STAGES) & 1);
+    float sv[32], dp[32];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(sv, dQ0 + kk * 2, dK0 + so + kk * 2, kk != 0);
+#pragma unroll
+    for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(dp, dDO0 + kk * 2, dV0 + so + kk * 2, kk != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_hold(sv);
+    wgmma_hold(dp);
+#pragma unroll
+    for (int x = 0; x < 32; ++x) {
+      const int r = (x >> 1) & 1;
+      dp[x] = fast_exp2(fmaf(sv[x], scale_log2, -l2[r])) * fmaf(dp[x], scale, -dl[r]);
+    }
+    uint32_t da[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) acc_to_afrag(dp, kk, da[kk]);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < FB_C / 16; ++kk) wgmma_m64n64_rs<1>(acc, da[kk], dK0 + so + kk * 128, 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_hold(acc);
+    if (signal) mbar_arrive(&in_empty[s]);
+  }
+  store_acc_rows(acc, dq, b, Nq, H, h, q0 + wg * 64, 1.f);
+}
+
+int64_t attn_bwd_ws_floats(int B, int Nq, int Nk, int H) {
+  // lse2 / delta padded to whole query tiles + the fp32 dQ accumulator of the fused path
   const int64_t nq_pad = (int64_t)((Nq + FB_C - 1) / FB_C) * FB_C;
   return 2 * (int64_t)B * H * nq_pad + (int64_t)B * Nq * H * FA_D + 64;
 }
 
-static int attn_bwd_fused(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
-                          void* dq, void* dk, void* dv, float* ws, int B, int Nq, int Nk, int H, int kv_shift, float scale,
-                          cudaStream_t stream) {
+int attn_bwd_tc(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
+                void* dq, void* dk, void* dv, float* ws, int B, int Nq, int Nk, int H, int kv_shift, float scale,
+                cudaStream_t stream) {
+  const bool fused = env_flag("LGB200_ATTN_BWD_FUSED");  // default: the deterministic dQ kernel
   const int nq_pad = (Nq + FB_C - 1) / FB_C * FB_C;
   float* lse2p = ws;
   float* deltap = lse2p + (int64_t)B * H * nq_pad;
@@ -1168,84 +556,37 @@ static int attn_bwd_fused(const void* q, const void* k, const void* v, const voi
         static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), lse, lse2p, deltap, nrows, Nq,
         nq_pad, H, scale);
   }
-  const size_t acc_bytes = (size_t)B * Nq * H * FA_D * 4;
-  cudaError_t e = cudaMemsetAsync(dqacc, 0, acc_bytes, stream);
-  LGB_REQUIRE(e == cudaSuccess, kErrCuda, "attn_bwd(fused): memset: %s", cudaGetErrorString(e));
-  if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_fused_kernel), FF_SMEM))) return rc;
-  CUtensorMap tq, tdo, tk, tdq;
+  if (fused) {
+    const size_t acc_bytes = (size_t)B * Nq * H * FA_D * 4;
+    cudaError_t e = cudaMemsetAsync(dqacc, 0, acc_bytes, stream);
+    LGB_REQUIRE(e == cudaSuccess, kErrCuda, "attn_bwd(fused): memset: %s", cudaGetErrorString(e));
+  }
+  const float sl2 = scale * kLog2e;
+  CUtensorMap tq, tdo, tk, tv;
+  if (!fused) {  // dQ kernel: 128-query resident tiles, 64-key streamed tiles
+    if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_dq_kernel), FQ_SMEM))) return rc;
+    if ((rc = make_qkv_tmap(&tq, q, B, Nq, H, FB_R))) return rc;
+    if ((rc = make_qkv_tmap(&tdo, dout, B, Nq, H, FB_R))) return rc;
+    if ((rc = make_qkv_tmap(&tk, k, B, Nk, H, FB_C))) return rc;
+    if ((rc = make_qkv_tmap(&tv, v, B, Nk, H, FB_C))) return rc;
+    attn_bwd_dq_kernel<<<dim3((Nq + FB_R - 1) / FB_R, H, B), FA_THREADS, FQ_SMEM, stream>>>(
+        tq, tdo, tk, tv, lse2p, deltap, static_cast<__nv_bfloat16*>(dq), B, Nq, nq_pad, Nk, H, kv_shift, scale, sl2);
+    if ((rc = check_launch("attn_bwd_dq"))) return rc;
+  }
   if ((rc = make_qkv_tmap(&tq, q, B, Nq, H, FB_C))) return rc;
   if ((rc = make_qkv_tmap(&tdo, dout, B, Nq, H, FB_C))) return rc;
   if ((rc = make_qkv_tmap(&tk, k, B, Nk, H, FB_R))) return rc;
-  {
-    const uint64_t dims[4] = {64, (uint64_t)H, (uint64_t)Nq, (uint64_t)B};
-    const uint64_t str[3] = {64 * 4, (uint64_t)H * 64 * 4, (uint64_t)Nq * H * 64 * 4};
-    const uint32_t box[4] = {32, 1, (uint32_t)FB_R, 1};
-    if ((rc = make_tmap(&tdq, dqacc, /*fp32=*/true, 4, dims, str, box))) return rc;
-  }
-  const float sl2 = scale * 1.4426950408889634f;
-  attn_bwd_fused_kernel<<<dim3((Nk + FB_R - 1) / FB_R, H, B), FF_THREADS, FF_SMEM, stream>>>(
-      tq, tdo, tk, tdq, static_cast<const __nv_bfloat16*>(k), static_cast<const __nv_bfloat16*>(v), lse2p, deltap,
-      static_cast<__nv_bfloat16*>(dk), static_cast<__nv_bfloat16*>(dv), B, Nq, nq_pad, Nk, H, kv_shift, scale, sl2);
-  if ((rc = check_launch("attn_bwd_fused"))) return rc;
+  if ((rc = make_qkv_tmap(&tv, v, B, Nk, H, FB_R))) return rc;
+  auto kern = fused ? attn_bwd_dkv_kernel<true> : attn_bwd_dkv_kernel<false>;
+  if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), FF_SMEM))) return rc;
+  kern<<<dim3((Nk + FB_R - 1) / FB_R, H, B), FA_THREADS, FF_SMEM, stream>>>(
+      tq, tdo, tk, tv, lse2p, deltap, static_cast<__nv_bfloat16*>(dk), static_cast<__nv_bfloat16*>(dv), dqacc, B, Nq,
+      nq_pad, Nk, H, kv_shift, scale, sl2);
+  if ((rc = check_launch("attn_bwd_dkv"))) return rc;
+  if (!fused) return 0;
   const int64_t n8 = (int64_t)B * Nq * H * FA_D / 8;
   dq_convert_kernel<<<(unsigned)((n8 + 255) / 256), 256, 0, stream>>>(dqacc, static_cast<__nv_bfloat16*>(dq), n8);
-  return check_launch("attn_bwd_fused(convert)");
-}
-
-int64_t attn_bwd_ws_floats(int B, int Nq, int Nk, int H) {
-  const int64_t two_kernel = 17 * (((int64_t)B * H * Nq + 3) / 4 * 4);
-  const int64_t fused = attn_bwd_fused_ws_floats(B, Nq, H);
-  return two_kernel > fused ? two_kernel : fused;
-}
-
-int attn_bwd_tc(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
-                void* dq, void* dk, void* dv, float* delta, int B, int Nq, int Nk, int H, int kv_shift, float scale,
-                cudaStream_t stream) {
-  const bool fused = !env_flag("LGB200_ATTN_BWD_TWO_KERNEL");  // default: the fused single-pass backward
-  if (fused) return attn_bwd_fused(q, k, v, out, lse, dout, dq, dk, dv, delta, B, Nq, Nk, H, kv_shift, scale, stream);
-  // workspace: delta [B*H*Nq] fp32, then the dKV side arrays qx, dox [B*H*Nq, 16] bf16 (16-byte aligned)
-  const int64_t nq_all = ((int64_t)B * H * Nq + 3) & ~(int64_t)3;
-  __nv_bfloat16* qx = reinterpret_cast<__nv_bfloat16*>(delta + nq_all);
-  __nv_bfloat16* dox = qx + nq_all * 16;
-  int rc = 0;
-  {
-    const int64_t nrows = (int64_t)B * Nq * H;
-    attn_bwd_prep_kernel<<<(unsigned)((nrows * 8 + 255) / 256), 256, 0, stream>>>(
-        static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), lse, delta,
-        reinterpret_cast<uint4*>(qx), reinterpret_cast<uint4*>(dox), nrows, Nq, H, 1.f / scale);
-  }
-  const float sl2 = scale * 1.4426950408889634f;
-  {
-    if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_dkv_v3_kernel), F4_SMEM))) return rc;
-    if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_dq_v3_kernel), F3_SMEM))) return rc;
-    CUtensorMap tq, tk, tv, tdo, tqx, tdox;
-    if ((rc = make_qkv_tmap(&tk, k, B, Nk, H, FB_C))) return rc;
-    if ((rc = make_qkv_tmap(&tv, v, B, Nk, H, FB_C))) return rc;
-    attn_bwd_dq_v3_kernel<<<dim3((Nq + FB_R - 1) / FB_R, H, B), F3_THREADS, F3_SMEM, stream>>>(
-        tk, tv, static_cast<const __nv_bfloat16*>(q), static_cast<const __nv_bfloat16*>(dout), lse, delta,
-        static_cast<__nv_bfloat16*>(dq), B, Nq, Nk, H, kv_shift, scale, sl2);
-    if ((rc = make_qkv_tmap(&tq, q, B, Nq, H, FB_C))) return rc;
-    if ((rc = make_qkv_tmap(&tdo, dout, B, Nq, H, FB_C))) return rc;
-    {
-      const uint64_t dims[3] = {16, (uint64_t)Nq, (uint64_t)B * H};
-      const uint64_t str[2] = {32, (uint64_t)Nq * 32};
-      const uint32_t box[3] = {16, (uint32_t)FB_C, 1};
-      if ((rc = make_tmap_bf16(&tqx, qx, 3, dims, str, box, 32))) return rc;
-      if ((rc = make_tmap_bf16(&tdox, dox, 3, dims, str, box, 32))) return rc;
-    }
-    attn_bwd_dkv_v3_kernel<<<dim3((Nk + FB_R - 1) / FB_R, H, B), F3_THREADS, F4_SMEM, stream>>>(
-        tq, tdo, tqx, tdox, static_cast<const __nv_bfloat16*>(k), static_cast<const __nv_bfloat16*>(v),
-        static_cast<__nv_bfloat16*>(dk), static_cast<__nv_bfloat16*>(dv), B, Nq, Nk, H, kv_shift, scale, sl2);
-    return check_launch("attn_bwd_tc(v3)");
-  }
-  return check_launch("attn_bwd_tc");
+  return check_launch("attn_bwd(convert)");
 }
 
 }  // namespace lgb
-
-#ifdef LGB_TRACE
-extern "C" int lgb200_debug_read_trace(long long* host, int n) {
-  return (int)cudaMemcpyFromSymbol(host, lgb::g_trace, sizeof(long long) * (n < 1024 ? n : 1024));
-}
-#endif
-

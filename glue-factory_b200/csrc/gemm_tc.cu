@@ -1,13 +1,13 @@
-// Batched bf16 GEMM on the 5th-generation tensor cores (tcgen05.mma, accumulator in TMEM, operands
-// staged by TMA into 128-byte-swizzled shared memory).  Used for the assignment similarity
-// sim = mdesc0 . mdesc1^T (lightglue.py:283) and its two backward contractions, which need every
-// combination of K-major / MN-major operands.
+// Batched bf16 GEMM on the Hopper tensor cores (wgmma, fp32 accumulators in registers, operands staged by TMA
+// into 128-byte-swizzled shared memory).  Used for the assignment similarity sim = mdesc0 . mdesc1^T
+// (lightglue.py:283), its two backward contractions and the layer's projections, which need every combination of
+// K-major / MN-major operands (wgmma reads both layouts straight from shared memory).
 //
 // Persistent CTAs (one per SM) walk 128x128 tiles of C, n fastest so neighbouring CTAs share the A tile in L2.
-// Warp roles: warps 0-3 epilogue, warp 4 TMA producer (one elected lane), warp 5 MMA issuer (warp-convergent, one
-// elected lane) + TMEM owner.  6-stage smem ring of 64-wide K blocks (one 128-byte swizzle atom per operand row)
-// that runs ahead across tile boundaries; TWO accumulators in TMEM, so the MMAs of tile i+1 overlap the epilogue
-// of tile i; the epilogue stages 32-row x 128-byte blocks in swizzled smem and stores them with TMA.
+// Warp roles: warpgroups 0 and 1 each own 64 rows of the tile (m64n128k16 wgmma, 64 accumulators per thread) and
+// write their rows straight from registers; warp 8 is the TMA producer (one lane).  A 4-stage smem ring of 64-wide
+// K blocks (one 128-byte swizzle atom per operand row) runs ahead across tile boundaries, so the loads of tile i+1
+// overlap the epilogue of tile i.
 #include <string.h>
 
 #include "common.cuh"
@@ -16,33 +16,75 @@
 
 namespace lgb {
 
-#ifndef LGB_G_STAGES
-#define LGB_G_STAGES 6  // 192 KiB of operand tiles in flight per SM: 629 vs 691 us over the layer's GEMM shapes (4 stages)
-#endif
-constexpr int GB_M = 128, GB_N = 128, GB_K = 64, G_STAGES = LGB_G_STAGES;
+constexpr int GB_M = 128, GB_N = 128, GB_K = 64, G_STAGES = 4;
 constexpr int G_TILE = GB_M * GB_K * 2;  // 16 KiB per operand per stage
-constexpr int G_EPI = 4 * 2 * 4096;      // per-warp staging: two 32-row x 128-byte blocks
-constexpr int G_BIAS = 4 * GB_N * 4;     // per-warp copy of the tile's 128 bias values
-constexpr int G_SMEM = G_STAGES * 2 * G_TILE + G_EPI + G_BIAS + 256;
+constexpr int G_THREADS = 2 * 128 + 32;  // two consumer warpgroups + the producer warp
+constexpr int G_PRODUCER = 8;            // warp index of the producer
+constexpr int G_SMEM = G_STAGES * 2 * G_TILE + 256;
+
+// Epilogue of one warpgroup's 64 x 128 accumulator: C (+)= alpha * acc (+ bias[col]).  Each thread owns two
+// adjacent columns of 16 column groups in two rows; pairs are stored as one 8-byte (fp32) / 4-byte (bf16) word
+// when `vec` (C and its pitches even-aligned), element by element otherwise.  reduce_add (fp32 C only) adds into C.
+template <typename OutT>
+__device__ __forceinline__ void gemm_store_tile(const float (&d)[64], OutT* __restrict__ C, int M, int N, int64_t ldc,
+                                                int m_base, int n0, float alpha, const float* __restrict__ bias,
+                                                int reduce_add, int vec) {
+  const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+  const int r0 = m_base + wq * 16 + (lane >> 2);
+#pragma unroll
+  for (int j = 0; j < GB_N / 8; ++j) {
+    const int col = n0 + 8 * j + 2 * (lane & 3);
+    if (col >= N) continue;
+    const bool two = col + 1 < N;
+    float b0 = 0.f, b1 = 0.f;
+    if (bias) {
+      b0 = bias[col];
+      if (two) b1 = bias[col + 1];
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int row = r0 + 8 * i;
+      if (row >= M) continue;
+      float v0 = fmaf(d[4 * j + 2 * i], alpha, b0), v1 = fmaf(d[4 * j + 2 * i + 1], alpha, b1);
+      OutT* dst = C + (int64_t)row * ldc + col;
+      if constexpr (sizeof(OutT) == 4) {
+        if (vec && two) {
+          float2* p2 = reinterpret_cast<float2*>(dst);
+          if (reduce_add) {
+            const float2 o = *p2;
+            v0 += o.x;
+            v1 += o.y;
+          }
+          *p2 = make_float2(v0, v1);
+        } else {
+          dst[0] = reduce_add ? dst[0] + v0 : v0;
+          if (two) dst[1] = reduce_add ? dst[1] + v1 : v1;
+        }
+      } else {
+        if (vec && two) {
+          *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(v0, v1);
+        } else {
+          dst[0] = __float2bfloat16(v0);
+          if (two) dst[1] = __float2bfloat16(v1);
+        }
+      }
+    }
+  }
+}
 
 template <bool A_MN, bool B_MN, typename OutT>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(G_THREADS, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                     const __grid_constant__ CUtensorMap tmC, OutT* __restrict__ C, int M, int N, int K, int64_t ldc,
-                     int64_t strideC, float alpha, int tiles_m, int tiles_n, int ntiles, int use_tma_store,
+                     OutT* __restrict__ C, int M, int N, int K, int64_t ldc, int64_t strideC, float alpha, int tiles_m,
+                     int tiles_n, int ntiles,
                      int kps /* split-K: k-blocks per split (0 = off); the tile's batch index is then the split */,
                      const float* __restrict__ bias /* [N] added to every row, or null */,
-                     int reduce_add /* fp32 C only: C += alpha A B (+ bias) through TMA reduce-add */) {
+                     int reduce_add /* fp32 C only: C += alpha A B (+ bias) */, int vec) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sA = smem;
   uint8_t* sB = smem + G_STAGES * G_TILE;
-  float* sE = reinterpret_cast<float*>(smem + 2 * G_STAGES * G_TILE);
-  float* sBias = reinterpret_cast<float*>(smem + 2 * G_STAGES * G_TILE + G_EPI);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + 2 * G_STAGES * G_TILE + G_EPI + G_BIAS);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + 2 * G_STAGES * G_TILE);
   uint64_t* empty = full + G_STAGES;
-  uint64_t* acc_full = empty + G_STAGES;  // [2]
-  uint64_t* acc_empty = acc_full + 2;     // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nk = (K + GB_K - 1) / GB_K;
@@ -51,26 +93,17 @@ __global__ void __launch_bounds__(192, 1)
     if (smem_u32(smem) & 1023u) __trap();
     for (int s = 0; s < G_STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&acc_full[s], 1);
-      mbar_init(&acc_empty[s], 4);
+      mbar_init(&empty[s], 2);  // one arrival per consumer warpgroup
     }
     mbar_fence_init();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == G_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    if (use_tma_store) tma_prefetch_desc(&tmC);
   }
-  if (warp == 5) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 4) {
+  if (warp == G_PRODUCER) {
     if (lane == 0) {
       int it = 0;  // running k-block count across tiles (ring position)
       for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
@@ -98,174 +131,69 @@ __global__ void __launch_bounds__(192, 1)
         }
       }
     }
-  } else if (warp == 5) {
-    constexpr uint32_t idesc = make_idesc_bf16(GB_M, GB_N, A_MN ? 1 : 0, B_MN ? 1 : 0);
-    const uint64_t ad0 = A_MN ? make_smem_desc(smem_u32(sA), 8192, 1024) : make_smem_desc(smem_u32(sA), 16, 1024);
-    const uint64_t bd0 = B_MN ? make_smem_desc(smem_u32(sB), 8192, 1024) : make_smem_desc(smem_u32(sB), 16, 1024);
+  } else {
+    const int wg = threadIdx.x >> 7;
+    const bool signal = (threadIdx.x & 127) == 0;
+    // the warpgroup's 64 rows of A start 8 KiB into the block in both layouts (K-major: 64 rows of 128 B further;
+    // MN-major: the second 64-wide TMA box)
+    const uint64_t ad0 = make_smem_desc(smem_u32(sA) + wg * 8192, 8192, 1024);
+    const uint64_t bd0 = make_smem_desc(smem_u32(sB), 8192, 1024);
     constexpr uint64_t a_step = (A_MN ? 2048 : 32) >> 4, b_step = (B_MN ? 2048 : 32) >> 4;
-    const bool leader = elect_one();
-    int it = 0, lt = 0;
-    for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++lt) {
-      const int acc = lt & 1;
-      mbar_wait(&acc_empty[acc], ((lt >> 1) & 1) ^ 1);  // epilogue drained this accumulator (2 tiles ago)
-      tc_fence_after();
-      const int bo = t / (tiles_n * tiles_m);
+    int it = 0;
+    for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+      const int n0 = (t % tiles_n) * GB_N, m0 = ((t / tiles_n) % tiles_m) * GB_M, bo = t / (tiles_n * tiles_m);
       const int nk_item = kps ? min(nk, (bo + 1) * kps) - bo * kps : nk;
+      float d[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) d[i] = 0.f;
       for (int kb = 0; kb < nk_item; ++kb, ++it) {
         const int s = it % G_STAGES;
         mbar_wait(&full[s], (it / G_STAGES) & 1);
-        tc_fence_after();
-        if (leader) {
-          const uint64_t so = (uint64_t)((s * G_TILE) >> 4);
+        wgmma_fence();
+        const uint64_t so = (uint64_t)((s * G_TILE) >> 4);
 #pragma unroll
-          for (int kk = 0; kk < GB_K / 16; ++kk)
-            umma_bf16(tmem_base + acc * GB_N, ad0 + so + kk * a_step, bd0 + so + kk * b_step, idesc,
-                      (kb | kk) != 0 ? 1u : 0u);
-          umma_commit(&empty[s]);
-        }
-        __syncwarp();
+        for (int kk = 0; kk < GB_K / 16; ++kk)
+          wgmma_m64n128_ss<A_MN, B_MN>(d, ad0 + so + kk * a_step, bd0 + so + kk * b_step, (kb | kk) != 0);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous block's MMAs have retired: its stage goes back to the producer
+        if (kb > 0 && signal) mbar_arrive(&empty[(it - 1) % G_STAGES]);
       }
-      if (leader) umma_commit(&acc_full[acc]);
-      __syncwarp();
+      wgmma_wait<0>();
+      wgmma_hold(d);
+      if (signal) mbar_arrive(&empty[(it - 1) % G_STAGES]);
+      gemm_store_tile<OutT>(d, C + (int64_t)bo * strideC, M, N, ldc, m0 + wg * 64, n0, alpha, bias,
+                            reduce_add, vec);
     }
-  } else {
-    // Epilogue.  Fast path: each warp stages its 32 rows x 128 bytes (32 fp32 / 64 bf16 columns) in 128B-swizzled
-    // smem and one lane hands the block to TMA (asynchronous, clips the tile at M / N); two blocks per warp so that
-    // the TMEM read-out of the next chunk overlaps the store of the previous one.  Fallback (C not 16-byte
-    // aligned): scalar / vector stores from the same staging block.
-    constexpr int CW = 128 / (int)sizeof(OutT);  // columns per staging block
-    uint8_t* stage = reinterpret_cast<uint8_t*>(sE) + warp * 8192;
-    int lt = 0, nblk = 0;
-    for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++lt) {
-      const int n0 = (t % tiles_n) * GB_N, m0 = ((t / tiles_n) % tiles_m) * GB_M, b = t / (tiles_n * tiles_m);
-      const int acc = lt & 1;
-      float* sb = sBias + warp * GB_N;
-      if (bias) {  // this warp's copy of the tile's bias slice (lane l holds columns 4l .. 4l+3)
-        __syncwarp();
-        const int col = n0 + lane * 4;
-        float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (col + 3 < N && (reinterpret_cast<uintptr_t>(bias + col) & 15) == 0) {
-          bv = *reinterpret_cast<const float4*>(bias + col);
-        } else {
-          if (col < N) bv.x = bias[col];
-          if (col + 1 < N) bv.y = bias[col + 1];
-          if (col + 2 < N) bv.z = bias[col + 2];
-          if (col + 3 < N) bv.w = bias[col + 3];
-        }
-        *reinterpret_cast<float4*>(sb + lane * 4) = bv;
-        __syncwarp();
-      }
-      mbar_wait(&acc_full[acc], (lt >> 1) & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < GB_N / CW; ++c, ++nblk) {
-        uint8_t* blk = stage + (nblk & 1) * 4096;
-        float v[CW];
-#pragma unroll
-        for (int q = 0; q < CW / 32; ++q)
-          tmem_ld32(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + acc * GB_N + c * CW + q * 32, v + q * 32);
-        if (use_tma_store) {
-          if (lane == 0) tma_store_wait_read<1>();  // the store that used this block two chunks ago has read it
-          __syncwarp();
-        }
-        tmem_ld_wait();
-        if (c == GB_N / CW - 1) {  // accumulator fully read: hand it back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&acc_empty[acc]);
-        }
-        if (bias) {
-#pragma unroll
-          for (int q4 = 0; q4 < CW / 4; ++q4) {
-            const float4 bq = *reinterpret_cast<const float4*>(sb + c * CW + q4 * 4);  // same address in every lane
-            v[4 * q4] = fmaf(v[4 * q4], alpha, bq.x); v[4 * q4 + 1] = fmaf(v[4 * q4 + 1], alpha, bq.y);
-            v[4 * q4 + 2] = fmaf(v[4 * q4 + 2], alpha, bq.z); v[4 * q4 + 3] = fmaf(v[4 * q4 + 3], alpha, bq.w);
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < CW; ++i) v[i] *= alpha;
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {  // 16-byte chunk j of this thread's row, XOR-swizzled by the row (== SWIZZLE_128B)
-          uint4 u;
-          if constexpr (sizeof(OutT) == 4) {
-            u.x = __float_as_uint(v[4 * j]); u.y = __float_as_uint(v[4 * j + 1]);
-            u.z = __float_as_uint(v[4 * j + 2]); u.w = __float_as_uint(v[4 * j + 3]);
-          } else {
-            u.x = pack_bf16(v[8 * j], v[8 * j + 1]);
-            u.y = pack_bf16(v[8 * j + 2], v[8 * j + 3]);
-            u.z = pack_bf16(v[8 * j + 4], v[8 * j + 5]);
-            u.w = pack_bf16(v[8 * j + 6], v[8 * j + 7]);
-          }
-          *reinterpret_cast<uint4*>(blk + lane * 128 + ((j ^ (lane & 7)) << 4)) = u;
-        }
-        if (use_tma_store) {
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            if (reduce_add) tma_reduce_add_3d(&tmC, blk, n0 + c * CW, m0 + warp * 32, b);
-            else tma_store_3d(&tmC, blk, n0 + c * CW, m0 + warp * 32, b);
-            tma_store_commit();
-          }
-        } else {
-          __syncwarp();
-          constexpr int EPC = 16 / (int)sizeof(OutT);  // elements per 16-byte chunk
-#pragma unroll 1
-          for (int i = 0; i < 8; ++i) {
-            const int r = i * 4 + (lane >> 3), row = m0 + warp * 32 + r;
-            const uint4 o = *reinterpret_cast<const uint4*>(blk + r * 128 + (((lane & 7) ^ (r & 7)) << 4));
-            const OutT* ov = reinterpret_cast<const OutT*>(&o);
-            const int col = n0 + c * CW + (lane & 7) * EPC;
-            if (row < M) {
-              OutT* dst = C + (int64_t)b * strideC + (int64_t)row * ldc + col;
-              for (int e = 0; e < EPC; ++e)
-                if (col + e < N) dst[e] = ov[e];
-            }
-          }
-          __syncwarp();
-        }
-      }
-    }
-    if (use_tma_store && lane == 0) tma_store_wait_all();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc(tmem_base, 256);
 }
 
 // ---------------------------------------------------------------------------------------------
 // A-panel-resident variant for the layer's K <= 256 GEMMs (y = x W^T and dx = dy W with a 256-wide contraction: 6 of the
 // 10 forward projections and 5 of the 9 input-gradient GEMMs of a layer).  The generic kernel above re-loads the A tile
-// for every n-tile and is bound by the L2 -> SM path (128 KiB of operands per 128 x 128 output tile, ncu: DRAM 50 %,
-// tensor 37 %, nothing saturated).  Here a work item is one 128-row panel of A: the panel (KB x 16 KiB) is loaded ONCE
-// into one of two resident buffers (the next item's panel is prefetched while this one is multiplied), only the B
-// blocks stream through a ring, and the CTA walks all n-tiles of the panel.  Operand bytes per panel for N = 256:
-// 64 + 128 KiB instead of 256 KiB; for N = 768: 64 + 384 instead of 768.  A is K-major (rows of x / dy).
-// Same TMEM double-buffered accumulators and the same epilogue (bias, bf16 / fp32, TMA store or reduce-add).
+// for every n-tile (128 KiB of operands per 128 x 128 output tile).  Here a work item is one 128-row panel of A: the
+// panel (KB x 16 KiB) is loaded ONCE into one of two resident buffers (the next item's panel is prefetched while this
+// one is multiplied), only the B blocks stream through a ring, and the CTA walks all n-tiles of the panel.  Operand
+// bytes per panel for N = 256: 64 + 128 KiB instead of 256 KiB; for N = 768: 64 + 384 instead of 768.  A is K-major
+// (rows of x / dy).  Same warpgroup split and epilogue (bias, bf16 / fp32, accumulate) as the generic kernel.
 // ---------------------------------------------------------------------------------------------
 constexpr int GP_KB = 4;                      // K <= 256
 constexpr int GP_BSTAGES = 4;                 // 16 KiB B blocks in flight
 constexpr int GP_BBLK = GB_N * GB_K * 2;      // 16 KiB
-constexpr int GP_SMEM = 2 * GP_KB * G_TILE + GP_BSTAGES * GP_BBLK + G_EPI + G_BIAS + 256;
+constexpr int GP_SMEM = 2 * GP_KB * G_TILE + GP_BSTAGES * GP_BBLK + 256;
 
 template <bool B_MN, typename OutT>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(G_THREADS, 1)
     gemm_apanel_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                       const __grid_constant__ CUtensorMap tmC, int M, int N, int K, float alpha, int tiles_m, int tiles_n,
-                       const float* __restrict__ bias, int reduce_add) {
+                       OutT* __restrict__ C, int M, int N, int K, int64_t ldc, float alpha, int tiles_m, int tiles_n,
+                       const float* __restrict__ bias, int reduce_add, int vec) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sA = smem;                                   // [2 panels][GP_KB blocks]
   uint8_t* sB = smem + 2 * GP_KB * G_TILE;              // [GP_BSTAGES]
-  uint8_t* sEp = sB + GP_BSTAGES * GP_BBLK;
-  float* sBias = reinterpret_cast<float*>(sEp + G_EPI);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sEp + G_EPI + G_BIAS);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + GP_BSTAGES * GP_BBLK);
   uint64_t* a_full = bars;                 // [2]
   uint64_t* a_empty = bars + 2;            // [2]
   uint64_t* b_full = bars + 4;             // [GP_BSTAGES]
   uint64_t* b_empty = b_full + GP_BSTAGES; // [GP_BSTAGES]
-  uint64_t* acc_full = b_empty + GP_BSTAGES;  // [2]
-  uint64_t* acc_empty = acc_full + 2;         // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int KB = (K + GB_K - 1) / GB_K;
@@ -275,28 +203,21 @@ __global__ void __launch_bounds__(192, 1)
     if (smem_u32(smem) & 1023u) __trap();
     for (int s = 0; s < 2; ++s) {
       mbar_init(&a_full[s], 1);
-      mbar_init(&a_empty[s], 1);
-      mbar_init(&acc_full[s], 1);
-      mbar_init(&acc_empty[s], 4);
+      mbar_init(&a_empty[s], 2);
     }
     for (int s = 0; s < GP_BSTAGES; ++s) {
       mbar_init(&b_full[s], 1);
-      mbar_init(&b_empty[s], 1);
+      mbar_init(&b_empty[s], 2);
     }
     mbar_fence_init();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == G_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmC);
   }
-  if (warp == 5) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 4) {
+  if (warp == G_PRODUCER) {
     if (lane == 0) {
       auto load_panel = [&](int item, int li) {  // li: this CTA's running item index -> panel buffer li & 1
         const int pa = li & 1;
@@ -328,139 +249,56 @@ __global__ void __launch_bounds__(192, 1)
         if (tiles_n == 1 && item + (int)gridDim.x < nitems) load_panel(item + gridDim.x, li + 1);
       }
     }
-  } else if (warp == 5) {
-    constexpr uint32_t idesc = make_idesc_bf16(GB_M, GB_N, 0, B_MN ? 1 : 0);
-    const uint64_t ad0 = make_smem_desc(smem_u32(sA), 16, 1024);
-    const uint64_t bd0 = B_MN ? make_smem_desc(smem_u32(sB), 8192, 1024) : make_smem_desc(smem_u32(sB), 16, 1024);
+  } else {
+    const int wg = threadIdx.x >> 7;
+    const bool signal = (threadIdx.x & 127) == 0;
+    const uint64_t ad0 = make_smem_desc(smem_u32(sA) + wg * 8192, 8192, 1024);
+    const uint64_t bd0 = make_smem_desc(smem_u32(sB), 8192, 1024);
     constexpr uint64_t a_step = 32 >> 4, b_step = (B_MN ? 2048 : 32) >> 4;
-    const bool leader = elect_one();
-    int li = 0, bi = 0, lt = 0;
+    int li = 0, bi = 0;
     for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++li) {
       const int pa = li & 1;
       mbar_wait(&a_full[pa], (li >> 1) & 1);
-      for (int nt = 0; nt < tiles_n; ++nt, ++lt) {
-        const int acc = lt & 1;
-        mbar_wait(&acc_empty[acc], ((lt >> 1) & 1) ^ 1);
-        tc_fence_after();
+      for (int nt = 0; nt < tiles_n; ++nt) {
+        float d[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) d[i] = 0.f;
         for (int kb = 0; kb < KB; ++kb, ++bi) {
           const int s = bi % GP_BSTAGES;
           mbar_wait(&b_full[s], (bi / GP_BSTAGES) & 1);
-          tc_fence_after();
-          if (leader) {
-            const uint64_t ao = (uint64_t)(((pa * GP_KB + kb) * G_TILE) >> 4), bo = (uint64_t)((s * GP_BBLK) >> 4);
+          wgmma_fence();
+          const uint64_t ao = (uint64_t)(((pa * GP_KB + kb) * G_TILE) >> 4), bo = (uint64_t)((s * GP_BBLK) >> 4);
 #pragma unroll
-            for (int kk = 0; kk < GB_K / 16; ++kk)
-              umma_bf16(tmem_base + acc * GB_N, ad0 + ao + kk * a_step, bd0 + bo + kk * b_step, idesc, (kb | kk) != 0 ? 1u : 0u);
-            umma_commit(&b_empty[s]);
-          }
-          __syncwarp();
+          for (int kk = 0; kk < GB_K / 16; ++kk)
+            wgmma_m64n128_ss<false, B_MN>(d, ad0 + ao + kk * a_step, bd0 + bo + kk * b_step, (kb | kk) != 0);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (kb > 0 && signal) mbar_arrive(&b_empty[(bi - 1) % GP_BSTAGES]);
         }
-        if (leader) {
-          umma_commit(&acc_full[acc]);
-          if (nt == tiles_n - 1) umma_commit(&a_empty[pa]);  // every MMA that reads this panel has been issued
+        wgmma_wait<0>();
+        wgmma_hold(d);
+        if (signal) {
+          mbar_arrive(&b_empty[(bi - 1) % GP_BSTAGES]);
+          if (nt == tiles_n - 1) mbar_arrive(&a_empty[pa]);  // every MMA that reads this panel has retired
         }
-        __syncwarp();
+        gemm_store_tile<OutT>(d, C, M, N, ldc, item * GB_M + wg * 64, nt * GB_N, alpha, bias, reduce_add, vec);
       }
     }
-  } else {
-    constexpr int CW = 128 / (int)sizeof(OutT);
-    uint8_t* stage = sEp + warp * 8192;
-    int lt = 0, nblk = 0;
-    for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
-      const int m0 = item * GB_M;
-      for (int nt = 0; nt < tiles_n; ++nt, ++lt) {
-        const int n0 = nt * GB_N, acc = lt & 1;
-        float* sb = sBias + warp * GB_N;
-        if (bias) {
-          __syncwarp();
-          const int col = n0 + lane * 4;
-          float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (col + 3 < N && (reinterpret_cast<uintptr_t>(bias + col) & 15) == 0) {
-            bv = *reinterpret_cast<const float4*>(bias + col);
-          } else {
-            if (col < N) bv.x = bias[col];
-            if (col + 1 < N) bv.y = bias[col + 1];
-            if (col + 2 < N) bv.z = bias[col + 2];
-            if (col + 3 < N) bv.w = bias[col + 3];
-          }
-          *reinterpret_cast<float4*>(sb + lane * 4) = bv;
-          __syncwarp();
-        }
-        mbar_wait(&acc_full[acc], (lt >> 1) & 1);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c = 0; c < GB_N / CW; ++c, ++nblk) {
-          uint8_t* blk = stage + (nblk & 1) * 4096;
-          float v[CW];
-#pragma unroll
-          for (int q = 0; q < CW / 32; ++q)
-            tmem_ld32(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + acc * GB_N + c * CW + q * 32, v + q * 32);
-          if (lane == 0) tma_store_wait_read<1>();
-          __syncwarp();
-          tmem_ld_wait();
-          if (c == GB_N / CW - 1) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[acc]);
-          }
-          if (bias) {
-#pragma unroll
-            for (int q4 = 0; q4 < CW / 4; ++q4) {
-              const float4 bq = *reinterpret_cast<const float4*>(sb + c * CW + q4 * 4);
-              v[4 * q4] = fmaf(v[4 * q4], alpha, bq.x); v[4 * q4 + 1] = fmaf(v[4 * q4 + 1], alpha, bq.y);
-              v[4 * q4 + 2] = fmaf(v[4 * q4 + 2], alpha, bq.z); v[4 * q4 + 3] = fmaf(v[4 * q4 + 3], alpha, bq.w);
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < CW; ++i) v[i] *= alpha;
-          }
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            uint4 u;
-            if constexpr (sizeof(OutT) == 4) {
-              u.x = __float_as_uint(v[4 * j]); u.y = __float_as_uint(v[4 * j + 1]);
-              u.z = __float_as_uint(v[4 * j + 2]); u.w = __float_as_uint(v[4 * j + 3]);
-            } else {
-              u.x = pack_bf16(v[8 * j], v[8 * j + 1]); u.y = pack_bf16(v[8 * j + 2], v[8 * j + 3]);
-              u.z = pack_bf16(v[8 * j + 4], v[8 * j + 5]); u.w = pack_bf16(v[8 * j + 6], v[8 * j + 7]);
-            }
-            *reinterpret_cast<uint4*>(blk + lane * 128 + ((j ^ (lane & 7)) << 4)) = u;
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            if (reduce_add) tma_reduce_add_3d(&tmC, blk, n0 + c * CW, m0 + warp * 32, 0);
-            else tma_store_3d(&tmC, blk, n0 + c * CW, m0 + warp * 32, 0);
-            tma_store_commit();
-          }
-        }
-      }
-    }
-    if (lane == 0) tma_store_wait_all();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc(tmem_base, 256);
+}
+
+// C and its pitches allow the paired (two-column) stores of the epilogue
+template <typename OutT>
+static int pair_aligned(const void* C, int64_t ldc, int batch, int64_t strideC) {
+  constexpr int ES = (int)sizeof(OutT);
+  return (reinterpret_cast<uintptr_t>(C) % (2 * ES)) == 0 && ldc % 2 == 0 && (batch == 1 || strideC % 2 == 0);
 }
 
 template <bool A_MN, bool B_MN, typename OutT>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int batch, int M, int N, int K,
                        int64_t ldc, int64_t strideC, float alpha, cudaStream_t stream, int kps = 0,
                        const float* bias = nullptr, int reduce_add = 0) {
-  constexpr int ES = (int)sizeof(OutT);
-  CUtensorMap tc;
-  memset(&tc, 0, sizeof(tc));
-  const bool tma_ok = (reinterpret_cast<uintptr_t>(C) & 15) == 0 && (ldc * ES) % 16 == 0 &&
-                      (batch == 1 || (strideC * ES) % 16 == 0);
-  if (tma_ok) {
-    const uint64_t dims[3] = {(uint64_t)N, (uint64_t)M, (uint64_t)batch};
-    const uint64_t str[2] = {(uint64_t)ldc * ES, (uint64_t)(batch > 1 ? strideC : (int64_t)M * ldc) * ES};
-    const uint32_t box[3] = {128u / ES, 32u, 1u};
-    int rc = make_tmap(&tc, C, ES == 4, 3, dims, str, box);
-    if (rc) return rc;
-  }
-  LGB_REQUIRE(!reduce_add || (tma_ok && ES == 4), kErrInvalid,
-              "gemm: accumulate-into-C needs an fp32 C with 16-byte aligned base / row pitch");
+  LGB_REQUIRE(!reduce_add || sizeof(OutT) == 4, kErrInvalid, "gemm: accumulate-into-C needs an fp32 C");
   auto kern = gemm_bf16_kernel<A_MN, B_MN, OutT>;
   {
     int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), G_SMEM);
@@ -471,8 +309,9 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, void* C, in
   const int64_t ntiles = (int64_t)tiles_m * tiles_n * batch;
   LGB_REQUIRE(ntiles < (1ll << 31), kErrUnsupported, "gemm: too many tiles");
   const unsigned grid = (unsigned)(ntiles < num_sms ? ntiles : num_sms);
-  kern<<<grid, 192, G_SMEM, stream>>>(ta, tb, tc, static_cast<OutT*>(C), M, N, K, ldc, strideC, alpha, tiles_m, tiles_n,
-                                      (int)ntiles, tma_ok ? 1 : 0, kps, bias, reduce_add);
+  kern<<<grid, G_THREADS, G_SMEM, stream>>>(ta, tb, static_cast<OutT*>(C), M, N, K, ldc, strideC, alpha, tiles_m, tiles_n,
+                                            (int)ntiles, kps, bias, reduce_add,
+                                            pair_aligned<OutT>(C, ldc, batch, strideC));
   return check_launch("gemm_bf16");
 }
 
@@ -606,16 +445,9 @@ extern "C" int lgb200_linear(const void* A, const void* B, void* C, const float*
   CUtensorMap ta, tb;
   int rc = make_ab_maps(&ta, &tb, A, B, 1, M, N, K, a_mn_major, b_mn_major, lda, ldb, 0, 0);
   if (rc) return rc;
-  {  // A-panel-resident kernel: K <= 256, K-major A, C reachable by TMA
-    const int es = c_dtype == LGB200_F32 ? 4 : 2;
+  {  // A-panel-resident kernel: K <= 256, K-major A
     const bool off = env_flag("LGB200_GEMM_NO_APANEL");
-    const bool c_ok = (reinterpret_cast<uintptr_t>(C) & 15) == 0 && (ldc * es) % 16 == 0;
-    if (!off && !a_mn_major && K <= GP_KB * GB_K && c_ok && (c_dtype == LGB200_F32 || c_dtype == LGB200_BF16)) {
-      CUtensorMap tc;
-      const uint64_t dims[3] = {(uint64_t)N, (uint64_t)M, 1};
-      const uint64_t str[2] = {(uint64_t)ldc * es, (uint64_t)M * ldc * es};
-      const uint32_t box[3] = {128u / es, 32u, 1u};
-      if ((rc = make_tmap(&tc, C, es == 4, 3, dims, str, box))) return rc;
+    if (!off && !a_mn_major && K <= GP_KB * GB_K && (c_dtype == LGB200_F32 || c_dtype == LGB200_BF16)) {
       const int tiles_m = (M + GB_M - 1) / GB_M, tiles_n = (N + GB_N - 1) / GB_N;
       const int sms = device_sm_count();
       const unsigned grid = (unsigned)(tiles_m < sms ? tiles_m : sms);
@@ -623,7 +455,8 @@ extern "C" int lgb200_linear(const void* A, const void* B, void* C, const float*
   {                                                                                                              \
     auto kern = gemm_apanel_kernel<BMJ, T>;                                                                      \
     if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), GP_SMEM))) return rc;                        \
-    kern<<<grid, 192, GP_SMEM, stream>>>(ta, tb, tc, M, N, K, alpha, tiles_m, tiles_n, bias, accumulate ? 1 : 0); \
+    kern<<<grid, G_THREADS, GP_SMEM, stream>>>(ta, tb, static_cast<T*>(C), M, N, K, ldc, alpha, tiles_m, tiles_n, \
+                                               bias, accumulate ? 1 : 0, pair_aligned<T>(C, ldc, 1, 0));         \
     return check_launch("linear(apanel)");                                                                       \
   }
       if (c_dtype == LGB200_F32) {

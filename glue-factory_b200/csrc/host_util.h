@@ -29,14 +29,14 @@ int attn_bwd_simt(const void* q, const void* k, const void* v, const void* out, 
 template <typename T>
 int attn_delta(const void* out, const void* dout, float* delta, int B, int N, int H, cudaStream_t stream);
 
-// tcgen05 attention (attn_tc.cu)
+// wgmma attention (attn_tc.cu)
 int attn_fwd_tc(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk, int H,
                 int kv_shift, float scale, cudaStream_t stream);
 int attn_bwd_tc(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
                 void* dq, void* dk, void* dv, float* delta, int B, int Nq, int Nk, int H, int kv_shift, float scale,
                 cudaStream_t stream);
 
-// scratch (floats) lgb200_attn_bwd needs for the bf16 path: max over the two-kernel and the fused backward
+// scratch (floats) lgb200_attn_bwd needs for the bf16 path (padded softmax statistics + the fused dQ accumulator)
 int64_t attn_bwd_ws_floats(int B, int Nq, int Nk, int H);
 
 }  // namespace lgb

@@ -13,10 +13,10 @@ shadow refreshed once per step, weight gradients are produced in fp32 directly b
 N x N is ever kept besides `sim`.
 
 In `precision: bf16` every GEMM of the layer and of the head -- the nine nn.Linear projections, their input-gradient
-and weight-gradient contractions -- runs on the library's own persistent tcgen05 GEMM (`ops.linear`: bias and
+and weight-gradient contractions -- runs on the library's own persistent wgmma GEMM (`ops.linear`: bias and
 fp32 accumulate-into-dx epilogues; `ops.wgrad_bf16`: split-K, fp32 out); no cuBLAS kernel is launched.  The fp32
 parity mode keeps fp32 cuBLAS (`torch.addmm/mm`) for the projections; `precision: bf16x3` runs the same fp32 data flow with
-every GEMM on the tcgen05 kernel through split bf16 operands (see FP32_GEMM).
+every GEMM on the wgmma kernel through split bf16 operands (see FP32_GEMM).
 """
 import torch
 import torch.nn.functional as F
@@ -29,10 +29,10 @@ FUSED_ASSIGN = True
 
 
 # How the fp32 parity mode multiplies matrices: "cublas" (torch.addmm / mm) or "x3" -- every fp32 operand split into
-# bf16 hi + lo, and  A B ~= Ah Bh + Ah Bl + Al Bh  evaluated as ONE tcgen05 GEMM over the 3x longer contraction
+# bf16 hi + lo, and  A B ~= Ah Bh + Ah Bl + Al Bh  evaluated as ONE wgmma GEMM over the 3x longer contraction
 # [Ah | Ah | Al] x [Bh | Bl | Bh] (fp32 accumulation in tensor memory; the dropped Al Bl term is 2^-16 relative).  This is
 # `precision: bf16x3`: the fp32 goldens (1e-3, bit-exact match indices) are then met with every GEMM of the path on the
-# same persistent tcgen05 kernel, TMA pipeline and epilogues the bf16 mode uses.
+# same persistent wgmma kernel, TMA pipeline and epilogues the bf16 mode uses.
 FP32_GEMM = "cublas"
 
 
@@ -61,8 +61,8 @@ def split3(x, dim, pattern):
 
 
 def _lin(x, W, b, out=None):
-    """y = x W^T + b.  bf16: own tcgen05 GEMM with the fp32 bias added in the epilogue (W = bf16 shadow, b = the fp32
-    parameter); fp32 parity mode: cuBLAS, or the split-operand tcgen05 GEMM (FP32_GEMM)."""
+    """y = x W^T + b.  bf16: own wgmma GEMM with the fp32 bias added in the epilogue (W = bf16 shadow, b = the fp32
+    parameter); fp32 parity mode: cuBLAS, or the split-operand wgmma GEMM (FP32_GEMM)."""
     if x.dtype == torch.bfloat16:
         return ops.linear(x, W, b, out=out)
     if FP32_GEMM == "x3":
@@ -92,7 +92,7 @@ def _wgrad(dy, a, out=None):
 
 class LinearX3Fn(torch.autograd.Function):
     """nn.Linear in the `bf16x3` mode for the callers outside LayerFn / HeadFn (input_proj, the dense evaluation
-    head): fp32 in / out, forward, dgrad and wgrad on the split-operand tcgen05 GEMM."""
+    head): fp32 in / out, forward, dgrad and wgrad on the split-operand wgmma GEMM."""
 
     @staticmethod
     def forward(ctx, x, weight, bias):

@@ -69,7 +69,7 @@ class DepthMatcher(nn.Module):
         "overlap_th": 0.2,
         "min_visibility_th": 0.5,
         "dense_assignment": True,  # plugin-only: materialise the boolean [B,M,N] assignment (the reference always does)
-        # plugin-only: also emit `assignment_t`, the [B,N,M] transpose, in the same pass (saves the B200 matcher's loss a
+        # plugin-only: also emit `assignment_t`, the [B,N,M] transpose, in the same pass (saves the plugin matcher's loss a
         # 0.5 ms transpose per step: its fused assignment backward walks the mask by columns too)
         "transposed_assignment": False,
     }

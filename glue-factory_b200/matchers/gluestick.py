@@ -1,4 +1,4 @@
-"""B200-native GlueStick matcher (points + lines) -- drop-in for gluefactory's in-tree `matchers.gluestick`
+"""H100-native GlueStick matcher (points + lines) -- drop-in for gluefactory's in-tree `matchers.gluestick`
 (BASELINE.json configs[4]: SP + LSD + GlueStick; SURVEY.md section 8a row a15).
 
 Select it with `model.matcher.name: gluefactory_b200.matchers.gluestick`.  Same constructor, `forward(data) -> pred`,
@@ -8,13 +8,13 @@ checkpoints are interchangeable (gluestick.py:68-141).
 
 Layout and kernels.  The reference keeps channels first ([B, D, N], Conv1d with kernel 1, gluestick.py:158); here the
 node features are token-major [B*N, D] like in the LightGlue plugin, so
-  * every Conv1d(k=1) with a tensor-core-sized input is the library's tcgen05 GEMM (`ops.LinearFn`: bias in the
+  * every Conv1d(k=1) with a tensor-core-sized input is the library's wgmma GEMM (`ops.LinearFn`: bias in the
     epilogue, split-K weight gradient); the tiny encoder layers (3 / 5 / 32 input channels) are plain fp32 linears;
-  * the attention core (gluestick.py:524-529) is the same tcgen05 flash-attention pair as LightGlue's.  GlueStick splits
+  * the attention core (gluestick.py:524-529) is the same wgmma flash-attention pair as LightGlue's.  GlueStick splits
     heads as channel = d * H + h; instead of permuting activations, the rows of the q / k / v projection weights and the
     columns of the merge weight are permuted once per call so the projections emit head-major [B, N, H, 64] directly;
   * the assignment is `log_double_softmax` with a learnt bin (gluestick.py:772-783) on the similarity produced by the
-    batched tcgen05 GEMM: forward kernels + closed-form backward (`ops.log_double_softmax`, heads_grad.py);
+    batched wgmma GEMM: forward kernels + closed-form backward (`ops.log_double_softmax`, heads_grad.py);
   * match filtering (`_get_matches`, gluestick.py:318-331) is `filter_matches_kernel`;
   * BatchNorm1d (training-mode batch statistics, running-stat update), the LineLayer's gather / scatter-mean over
     junctions and the O(lines^2) line-score gathers are torch ops.
@@ -97,7 +97,7 @@ class AttentionalGNN(nn.Module):
 
 
 class _BmmNT(torch.autograd.Function):
-    """sim [B,M,N] fp32 = alpha * a [B,M,D] . b [B,N,D]^T on the batched tcgen05 GEMM, with its two backward
+    """sim [B,M,N] fp32 = alpha * a [B,M,D] . b [B,N,D]^T on the batched wgmma GEMM, with its two backward
     contractions (gluestick.py:248-249 `einsum("bdn,bdm->bnm")`)."""
 
     @staticmethod
@@ -273,7 +273,7 @@ class GlueStick(nn.Module):
     def _forward(self, data):
         for key in self.required_data_keys:
             assert key in data, f"Missing key {key} in data"
-        _lib.load()  # raises unless the CUDA library is built and the device is a B200 (no CPU fallback)
+        _lib.load()  # raises unless the CUDA library is built and the device is an H100 (no CPU fallback)
         kp0, kp1 = data["keypoints0"].float(), data["keypoints1"].float()
         B, n0 = kp0.shape[:2]
         n1 = kp1.shape[1]

@@ -1,4 +1,4 @@
-"""Drop-in ground-truth "matcher" for homography pairs, computed on the B200.
+"""Drop-in ground-truth "matcher" for homography pairs, computed on the GPU.
 
 Mirrors gluefactory/models/matchers/homography_matcher.py:8-66 (the `ground_truth` component of TwoViewPipeline,
 two_view_pipeline.py:54-56, 83-86, 98-100): same constructor, `default_conf`, `required_data_keys`, output keys and
@@ -33,7 +33,7 @@ class HomographyMatcher(nn.Module):
         "min_visibility_th": 0.5,
         # plugin-only: also materialise the boolean [B,M,N] assignment (the reference always does)
         "dense_assignment": True,
-        # plugin-only: also emit `assignment_t`, the [B,N,M] transpose, in the same pass (saves the B200 matcher's loss a
+        # plugin-only: also emit `assignment_t`, the [B,N,M] transpose, in the same pass (saves the plugin matcher's loss a
         # 0.5 ms transpose per step: its fused assignment backward walks the mask by columns too)
         "transposed_assignment": False,
     }

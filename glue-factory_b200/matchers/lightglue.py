@@ -1,4 +1,4 @@
-"""B200-native LightGlue matcher -- drop-in for gluefactory's in-tree matcher.
+"""H100-native LightGlue matcher -- drop-in for gluefactory's in-tree matcher.
 
 Select it from a glue-factory config with
 
@@ -15,15 +15,15 @@ Same constructor (`cls(conf_dict)`), same `forward(data) -> pred`, same
 checkpoints are interchangeable, SURVEY.md Appendix B.2).  The arithmetic of
 the N x N path -- rotary split, self / cross attention, LayerNorm+GELU, the
 assignment head, its NLL terms, argmax and match filtering, and all of their
-backward passes -- runs in the hand-written sm_100a kernels behind the C ABI
+backward passes -- runs in the hand-written sm_90a kernels behind the C ABI
 of include/lgb200.h.  The small dense projections (nn.Linear) go through
-cuBLAS via torch.  There is no CPU path: without the built library and a B200
+cuBLAS via torch.  There is no CPU path: without the built library and an H100
 `forward` raises.
 
 conf additions over the reference's default_conf:
-    precision: "bf16" -> bf16 operands / fp32 accumulation on the tcgen05 tensor cores (default)
+    precision: "bf16" -> bf16 operands / fp32 accumulation on the Hopper tensor cores (default)
                "fp32" -> full-precision parity path (CUDA cores + fp32 cuBLAS)
-               "bf16x3" -> the fp32 data flow with every GEMM on the tcgen05 kernel: fp32 operands split into bf16
+               "bf16x3" -> the fp32 data flow with every GEMM on the wgmma kernel: fp32 operands split into bf16
                          hi + lo parts, three partial products accumulated in fp32 tensor memory (engine.FP32_GEMM);
                          attention on the fp32 CUDA-core kernel.  Meets the fp32 goldens like "fp32" does.
 """
@@ -222,7 +222,7 @@ class LightGlue(nn.Module):
         return w, params
 
     def _lin(self, x, layer):
-        """nn.Linear: bf16 mode -> the library's tcgen05 GEMM (bf16 operands, fp32 accumulate, fp32 bias epilogue);
+        """nn.Linear: bf16 mode -> the library's wgmma GEMM (bf16 operands, fp32 accumulate, fp32 bias epilogue);
         fp32 parity mode -> fp32 cuBLAS."""
         if self._bf16:
             shp = x.shape
@@ -298,7 +298,7 @@ class LightGlue(nn.Module):
     def _forward(self, data):
         for key in self.required_data_keys:
             assert key in data, f"Missing key {key} in data"
-        _lib.load()  # raises unless the CUDA library is built and the device is a B200 (no CPU fallback)
+        _lib.load()  # raises unless the CUDA library is built and the device is an H100 (no CPU fallback)
         conf = self.conf
         adaptive = not self.training and (conf.depth_confidence > 0 or conf.width_confidence > 0)
         kpts0, kpts1 = data["keypoints0"], data["keypoints1"]
@@ -535,7 +535,7 @@ class LightGlue(nn.Module):
         gt = data["gt_assignment"]
         gt_u8 = gt.contiguous().view(torch.uint8) if gt.dtype == torch.bool else gt.to(torch.uint8).contiguous()
         # both counts in one pass over the 4.2 MB/pair mask (`gt.sum(2)` / `gt.sum(1)` each widen it first: int64 by
-        # default -- 1.1 ms per step at 32 pairs, profiles/r01_roofline_table.md -- fp32 with dtype=, still 0.9 ms)
+        # default, fp32 with dtype=)
         rowcnt, colcnt = ops.mask_counts(gt_u8)
         neg0 = (data["gt_matches0"] == -1).float()
         neg1 = (data["gt_matches1"] == -1).float()

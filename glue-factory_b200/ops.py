@@ -3,7 +3,7 @@
 PyTorch is used here only as plumbing: it owns the device buffers, the stream
 and the autograd tape; every numerical step of the N x N path is one of the
 C-ABI entry points of include/lgb200.h.  Nothing in this file has a CPU
-branch: on a machine without the built library or without a B200 the first
+branch: on a machine without the built library or without an H100 the first
 call raises `Lgb200Error`.
 """
 import torch
@@ -249,7 +249,7 @@ def add_f32_cast_(x, y, cdt):
 def gluestick_attention(query, key, value):
     """GlueStick's attention core (models/matchers/gluestick.py:524-529) on the same kernels: query [B, 64, H, N],
     key/value [B, 64, H, M] (channels first, channel = d * H + h) -> [B, 64, H, N].  The reference forces fp32 here
-    (AMP_CUSTOM_FWD_F32): fp32 inputs run the full-precision kernels, bf16 inputs the tcgen05 ones."""
+    (AMP_CUSTOM_FWD_F32): fp32 inputs run the full-precision kernels, bf16 inputs the wgmma ones."""
     assert query.shape[1] == 64, "head dimension 64 only"
     tm = lambda t: t.permute(0, 3, 2, 1).contiguous()  # noqa: E731  -> token-major [B, N, H, 64]
     out = Attention.apply(tm(query), tm(key), tm(value), 0, 0.125)
@@ -257,7 +257,7 @@ def gluestick_attention(query, key, value):
 
 
 # ------------------------------------------------------------------------------------------------
-# batched GEMM on tcgen05 (lightglue.py:283)
+# batched GEMM on wgmma (lightglue.py:283)
 # ------------------------------------------------------------------------------------------------
 def gemm_bf16(a, b, a_mn_major=False, b_mn_major=False, out_dtype=torch.float32, alpha=1.0):
     """C[i] = opA(a[i]) @ opB(b[i])^T-style contraction on the tensor cores (see lgb200.h).
@@ -275,7 +275,7 @@ def gemm_bf16(a, b, a_mn_major=False, b_mn_major=False, out_dtype=torch.float32,
 
 
 def linear(a, w, bias=None, out=None, out_dtype=torch.bfloat16, w_is_kn=False, accumulate=False, alpha=1.0):
-    """The nn.Linear-shaped GEMMs of the layer on the persistent tcgen05 kernel (lgb200_linear, include/lgb200.h):
+    """The nn.Linear-shaped GEMMs of the layer on the persistent wgmma kernel (lgb200_linear, include/lgb200.h):
         out[M, N] (=|+=) alpha * a[M, K] @ W^T + bias,   W = w[N, K]  (forward: y = x W^T + b)
                                                      or  W^T = w[K, N] when w_is_kn (dgrad: dx = dy W, w = the [out, in] weight)
     a, w bf16 2-D with unit inner stride (row-strided views are fine: column blocks of wider matrices);
@@ -326,7 +326,7 @@ def _similarity(md0, md1, bf16):
         return gemm_bf16(md0.to(torch.bfloat16).contiguous(), md1.to(torch.bfloat16).contiguous())
     from . import engine
 
-    if engine.FP32_GEMM == "x3":  # split-operand tcgen05 GEMM (precision: bf16x3)
+    if engine.FP32_GEMM == "x3":  # split-operand wgmma GEMM (precision: bf16x3)
         return gemm_bf16(engine.split3(md0.float(), 2, "hhl"), engine.split3(md1.float(), 2, "hlh"))
     return torch.bmm(md0, md1.transpose(1, 2))
 
@@ -364,7 +364,7 @@ def assign_fused_ok(md, D):
 def assign_fused_stats(md0, md1, alpha, ls0, ls1, gt_u8=None):
     """md0 [B,M,D], md1 [B,N,D] bf16 -> the same dict as assign_stats(dense=False) (lse_row/lse_col, rowmax/rowarg,
     colmax/colarg, pos_row_sum) without ever writing sim = alpha md0 md1^T (csrc/assign_tc.cu: two passes, each a
-    tcgen05 GEMM whose accumulator tiles are reduced in the epilogue)."""
+    wgmma GEMM whose accumulator tiles are reduced in the epilogue)."""
     _chk(md0, torch.bfloat16), _chk(md1, torch.bfloat16)
     B, M, D = md0.shape
     N = md1.shape[1]
@@ -443,7 +443,7 @@ def head_logsig(zt):
 
 def wgrad_bf16(dy, a, out=None):
     """dW [out, in] fp32 = dy^T a for bf16 dy [T, out], a [T, in] (rows may be strided views with unit inner stride):
-    split-K tcgen05 GEMM with both operands consumed MN-major, i.e. exactly as they lie in memory."""
+    split-K wgmma GEMM with both operands consumed MN-major, i.e. exactly as they lie in memory."""
     _chk(dy, torch.bfloat16, strided_rows=True), _chk(a, torch.bfloat16, strided_rows=True)
     T, M = dy.shape
     N = a.shape[1]

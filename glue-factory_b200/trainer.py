@@ -2,7 +2,7 @@
 
 Restates the per-iteration body of the reference trainer
 (/root/reference/gluefactory/train.py:456-517: zero_grad -> forward -> loss ->
-mean -> backward -> gradient exchange -> Adam) with the two B200-specific
+mean -> backward -> gradient exchange -> Adam) with the two H100-specific
 changes SURVEY.md section 2.2 (C1) calls for:
 
   * every parameter lives in ONE flat fp32 buffer and every gradient in one flat
@@ -27,9 +27,8 @@ _ALIGN = 64  # elements; keeps every parameter view 256-byte aligned
 # Gradient-exchange schedule (FlatParams.exchange): "end" (default) = ONE sum-all-reduce of the flat gradient buffer
 # behind backward, issued in its synchronous form so that it runs on the step's own stream (a captured step stays a
 # linear chain of graph nodes); "chunked" = each layer's slice as soon as its backward wrote it, the rest at the end.
-# Measured on 2 B200s (scripts/diag_allreduce.py, diag_lockstep.py, DESIGN.md section 6): the 47.4 MB all-reduce takes
-# 0.12 ms, the lock-step wait for the slower GPU ~0.4 ms, and the two schedules are within noise of each other -- there
-# is nothing left to hide, so the default is the simple one.  "none" is a DIAGNOSTIC (ranks train independently).
+# The default is the simple one; scripts/diag_allreduce.py and diag_lockstep.py time the all-reduce and the lock-step
+# wait of the two schedules.  "none" is a DIAGNOSTIC (ranks train independently).
 _EXCHANGE = os.environ.get("LGB200_EXCHANGE", "end")
 assert _EXCHANGE in ("chunked", "end", "none"), _EXCHANGE
 

@@ -1,4 +1,4 @@
-/* lgb200 -- C ABI of the B200-native LightGlue matcher hot path.
+/* lgb200 -- C ABI of the H100-native LightGlue matcher hot path.
  *
  * The reference (cvg/glue-factory) is pure Python/PyTorch: its "FFI" for this
  * path is the set of PyTorch operator calls inside
@@ -16,7 +16,7 @@
  *  - activations are token-major: [batch, tokens, heads, 64] for q/k/v/ctx,
  *    [batch, rows, cols] row-major for similarity/score matrices.
  *  - `dtype` is LGB200_F32 (full-precision parity path, CUDA cores) or
- *    LGB200_BF16 (bf16 operands, fp32 accumulation, tcgen05 tensor cores).
+ *    LGB200_BF16 (bf16 operands, fp32 accumulation, Hopper tensor cores).
  *  - head dimension is fixed to 64 (descriptor_dim / num_heads in every
  *    LightGlue configuration, lightglue.py:349).
  */
@@ -46,7 +46,7 @@ typedef struct CUstream_st* cudaStream_t;
 
 int lgb200_abi_version(void);
 const char* lgb200_last_error(void);
-/* 0 when the current device is sm_100 (B200); LGB200_ERR_UNSUPPORTED otherwise. */
+/* 0 when the current device is sm_90 (H100); LGB200_ERR_UNSUPPORTED otherwise. */
 int lgb200_check_device(void);
 
 /* ---- rotary encoding + QKV de-interleave ------------------------------------------------------
@@ -89,7 +89,7 @@ int lgb200_ln_gelu_bwd(const void* dy, const void* x, const float* gamma, const 
                        const float* rstd, void* dx, float* dgamma_part, float* dbeta_part, float* dxsum_part,
                        int64_t ntok, int W, int dtype, cudaStream_t stream);
 
-/* ---- batched bf16 tensor-core GEMM (tcgen05, fp32 accumulate) ---------------------------------------
+/* ---- batched bf16 tensor-core GEMM (wgmma, fp32 accumulate) ---------------------------------------
  * replaces torch.einsum("bmd,bnd->bmn") of MatchAssignment (lightglue.py:283) and its two backward
  * contractions.  C[b] (M x N) = opA(A[b]) * opB(B[b]):
  *   a_mn_major = 0: A is [M,K] row-major (lda);  1: A is stored [K,M] row-major (lda)
@@ -106,10 +106,10 @@ int lgb200_gemm_bf16(const void* A, const void* B, void* C, int batch, int M, in
 int64_t lgb200_gemm_splitk_ws_floats(int M, int N, int K);
 int lgb200_gemm_bf16_splitk(const void* A, const void* B, float* C, int M, int N, int K, int a_mn_major,
                             int b_mn_major, int64_t lda, int64_t ldb, int64_t ldc, float* ws, cudaStream_t stream);
-/* One nn.Linear-shaped GEMM on the same persistent tcgen05 kernel, with the epilogues the layer needs
+/* One nn.Linear-shaped GEMM on the same persistent wgmma kernel, with the epilogues the layer needs
  * (replaces F.linear / its autograd, lightglue.py:139-148, 156-163, 174-183, 195-221, 280):
  *   C[M,N] (c_dtype, row pitch ldc) = alpha * op(A) op(B)^T + bias[N]          (accumulate == 0)
- *   C[M,N] (fp32)                  += alpha * op(A) op(B)^T + bias[N]          (accumulate != 0; TMA reduce-add in L2)
+ *   C[M,N] (fp32)                  += alpha * op(A) op(B)^T + bias[N]          (accumulate != 0; read-modify-write in the epilogue)
  * A: [M,K] row pitch lda (or [K,M] when a_mn_major), B: [N,K] row pitch ldb (or [K,N] when b_mn_major), bf16;
  * bias: fp32 [N] or NULL.  forward: A = x, B = W;  dgrad: A = dy, B = W (b_mn_major);  row pitches let C be a column
  * block of a wider matrix (the [x | msg] FFN input, lightglue.py:162). */

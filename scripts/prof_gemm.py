@@ -1,4 +1,4 @@
-"""Event timing of the tcgen05 GEMM at the assignment-head shapes (32 pairs, N=M=2048, d=256)."""
+"""Event timing of the wgmma GEMM at the assignment-head shapes (32 pairs, N=M=2048, d=256)."""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from gluefactory_b200 import ops

@@ -1,4 +1,4 @@
-"""Event timing of the layer's GEMM shapes on the library's persistent tcgen05 kernel (lgb200_linear / split-K wgrad)
+"""Event timing of the layer's GEMM shapes on the library's persistent wgmma kernel (lgb200_linear / split-K wgrad)
 at the bench token count (T = 131072 = 32 pairs x 2 images x 2048), with the HBM bytes each one has to move."""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

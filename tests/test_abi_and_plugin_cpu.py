@@ -1,5 +1,6 @@
 """CPU: the C-ABI library loads and exports every symbol of include/lgb200.h; the plugin honours
 the reference's plugin surface (construction, names, state_dict) and fails loudly without a GPU."""
+import json
 import os
 import re
 import sys
@@ -8,7 +9,7 @@ import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+GOLDEN_SURFACE = os.path.join(ROOT, "tests", "golden", "reference_plugin_surface.json")
 
 
 @pytest.fixture(scope="module")
@@ -62,15 +63,36 @@ def test_no_cpu_fallback():
         model(data)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not present on this machine")
 def test_dropin_through_reference_get_model():
-    """gluefactory.models.get_model must discover the plugin the way it discovers the reference
-    matcher (models/__init__.py:7-30) and both must expose the same state_dict."""
+    """The plugin must expose the reference's surface: the LightGlue state_dict layout and confidence thresholds, and the
+    homography ground-truth component's required keys and defaults, as recorded from the unmodified reference in
+    tests/golden/reference_plugin_surface.json (oracle/make_surface_golden.py).  Where the build staged the reference
+    under oracle/_ref, gluefactory.models.get_model must also discover the plugin the way it discovers the reference
+    matcher (models/__init__.py:7-30)."""
+    from gluefactory_b200.matchers.homography_matcher import HomographyMatcher
+    from gluefactory_b200.matchers.lightglue import LightGlue
+
+    with open(GOLDEN_SURFACE) as f:
+        g = json.load(f)
+    lg = g["lightglue_n_layers2"]
+    mine = LightGlue({"n_layers": 2})
+    sd = mine.state_dict()
+    assert list(sd.keys()) == lg["keys"]
+    for k, shape in zip(lg["keys"], lg["shapes"]):
+        assert list(sd[k].shape) == shape, k
+    mine.load_state_dict({k: torch.zeros(shape) for k, shape in zip(lg["keys"], lg["shapes"])})  # strict
+    assert torch.allclose(LightGlue({"n_layers": 2}).confidence_thresholds, torch.tensor(lg["confidence_thresholds"]))
+    hm = g["homography_matcher"]
+    assert sorted(HomographyMatcher({}).required_data_keys) == hm["required_data_keys"]
+    for k, v in hm["default_conf"].items():
+        assert HomographyMatcher.default_conf[k] == v, k
+
     saved = list(sys.path)
-    sys.path.insert(0, os.path.join(ROOT, "oracle", "_shim"))
-    sys.path.insert(0, REF)
     try:
-        _dropin_checks()
+        from oracle import stage_reference
+
+        if stage_reference.import_reference() is not None:
+            _dropin_checks()
     finally:
         sys.path[:] = saved
 
@@ -101,8 +123,9 @@ def _dropin_checks():
         assert gt_cls.default_conf[k] == v, k
     with pytest.raises(NotImplementedError):
         gt_cls({}).loss({}, {})
-    with pytest.raises(Exception):  # no CUDA device here: the op refuses instead of falling back to the CPU
-        gt_cls({})({"H_0to1": torch.eye(3)[None], "keypoints0": torch.zeros(1, 4, 2), "keypoints1": torch.zeros(1, 4, 2)})
+    if not torch.cuda.is_available():
+        with pytest.raises(Exception):  # no CUDA device: the op refuses instead of falling back to the CPU
+            gt_cls({})({"H_0to1": torch.eye(3)[None], "keypoints0": torch.zeros(1, 4, 2), "keypoints1": torch.zeros(1, 4, 2)})
 
 
 def test_split_operand_host_logic():

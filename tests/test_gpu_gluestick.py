@@ -3,7 +3,7 @@ unmodified reference (tests/golden/gluestick_l4_n160.npz: forward + loss + backw
 and, at a larger ragged size, against the CPU oracle (oracle/gluestick_oracle.py, pinned to the same fixture).
 
 precision="fp32" (fp32 cuBLAS linears, CUDA-core attention: the reference also forces its attention to fp32) meets the
-north-star bar: match indices bit-exact, log-scores / losses / gradients within 1e-3.  precision="bf16" (tcgen05
+north-star bar: match indices bit-exact, log-scores / losses / gradients within 1e-3.  precision="bf16" (wgmma
 GEMMs and attention) is held to bf16-operand tolerances."""
 import ast
 import os

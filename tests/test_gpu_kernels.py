@@ -43,7 +43,7 @@ def test_gemm_bf16_tcgen05(a_mn, b_mn, shape):
 
 @pytest.mark.parametrize("T,M,N", [(4096, 256, 256), (10000, 512, 256), (777, 768, 256), (300, 256, 512), (64, 128, 72)])
 def test_wgrad_splitk(T, M, N):
-    """dW = dy^T a (autograd of F.linear) through the split-K tcgen05 GEMM, both operands MN-major as stored."""
+    """dW = dy^T a (autograd of F.linear) through the split-K wgmma GEMM, both operands MN-major as stored."""
     dy = _rand(T, M, seed=1, dtype=torch.bfloat16)
     a = _rand(T, N, seed=2, dtype=torch.bfloat16)
     ref = dy.double().t() @ a.double()
@@ -58,7 +58,7 @@ def test_wgrad_splitk(T, M, N):
 @pytest.mark.parametrize("T,K,N", [(4096, 256, 768), (1000, 512, 512), (777, 512, 256), (130, 256, 256), (64, 128, 72)])
 def test_linear_epilogues(T, K, N):
     """lgb200_linear: y = x W^T + b with the fp32 bias added in the epilogue, into a column block of a wider matrix;
-    dx = dy W (W read as stored); fp32 accumulate-into-dx through the TMA reduce."""
+    dx = dy W (W read as stored); fp32 accumulate-into-dx in the epilogue."""
     wide = _rand(T, 2 * K, seed=1, dtype=torch.bfloat16)
     x = wide[:, K:]                                   # row-strided A (the [x | msg] FFN input halves)
     w = _rand(N, K, seed=2, dtype=torch.bfloat16, scale=K ** -0.5)
@@ -154,7 +154,7 @@ def test_assign_fused_matches_unfused_and_fp64(B, M, N, D):
 
 
 def test_gemm_unaligned_output_uses_fallback_epilogue():
-    """N = 130: C rows are not 16-byte multiples, so the TMA-store epilogue is replaced by plain stores."""
+    """N = 130: C rows are not 8-byte multiples, so the paired-column stores of the epilogue fall back to single ones."""
     a = _rand(2, 100, 64, seed=1, dtype=torch.bfloat16)
     b = _rand(2, 130, 64, seed=2, dtype=torch.bfloat16)
     ref = a.double() @ b.double().transpose(1, 2)
@@ -198,7 +198,7 @@ def test_attention_forward_backward(dtype, tol, B, Nq, Nk, H, shift):
 
 @pytest.mark.parametrize("B,Nq,Nk,H,shift", ATTN_SHAPES)
 def test_attention_tc_matches_simt_lse(B, Nq, Nk, H, shift):
-    """the tcgen05 forward and the CUDA-core forward must agree on out and on the saved log-sum-exp"""
+    """the wgmma forward and the CUDA-core forward must agree on out and on the saved log-sum-exp"""
     from gluefactory_b200._lib import BF16, call, ptr, stream_ptr
 
     if shift and Nq != Nk:
@@ -216,17 +216,17 @@ def test_attention_tc_matches_simt_lse(B, Nq, Nk, H, shift):
 
 @pytest.mark.parametrize("B,Nq,Nk,H,shift", [(2, 512, 512, 4, 1), (2, 300, 200, 4, 0)])
 def test_attention_two_kernel_backward_agrees_with_fused(B, Nq, Nk, H, shift, monkeypatch):
-    """The round-1 pair of backward kernels (dQ, dK/dV; deterministic summation order) stays selectable with
-    LGB200_ATTN_BWD_TWO_KERNEL=1 as an independent cross-check of the fused single-pass backward."""
+    """The default pair of backward kernels (dQ, dK/dV; deterministic summation order) and the single-pass backward
+    with dQ accumulated by atomics (LGB200_ATTN_BWD_FUSED=1) cross-check each other."""
     q = _rand(B, Nq, H, 64, seed=1, dtype=torch.bfloat16, scale=1.5)
     k = _rand(B, Nk, H, 64, seed=2, dtype=torch.bfloat16, scale=1.5)
     v = _rand(B, Nk, H, 64, seed=3, dtype=torch.bfloat16)
     go = _rand(B, Nq, H, 64, seed=4, dtype=torch.bfloat16)
     out, lse = ops.attn_fwd(q, k, v, shift, 0.125)
-    fused = ops.attn_bwd(q, k, v, out, lse, go, shift, 0.125)
-    monkeypatch.setenv("LGB200_ATTN_BWD_TWO_KERNEL", "1")
     two = ops.attn_bwd(q, k, v, out, lse, go, shift, 0.125)
-    monkeypatch.delenv("LGB200_ATTN_BWD_TWO_KERNEL")
+    monkeypatch.setenv("LGB200_ATTN_BWD_FUSED", "1")
+    fused = ops.attn_bwd(q, k, v, out, lse, go, shift, 0.125)
+    monkeypatch.delenv("LGB200_ATTN_BWD_FUSED")
     for a, b, name in zip(fused, two, ("dq", "dk", "dv")):
         assert rel_err(a, b.double()) < 6e-3, name
 

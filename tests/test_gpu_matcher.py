@@ -57,7 +57,7 @@ def test_fp32_path_matches_reference_golden(name, engine):
 def test_bf16x3_tensor_core_parity_mode_matches_reference_golden(name):
     """`precision: bf16x3`: the fp32 goldens -- bit-exact match indices, 1e-3 on log-scores, losses and every
     gradient -- with EVERY GEMM of the path (projections, their dgrad / wgrad, the similarity and its two backward
-    contractions) on the persistent tcgen05 kernel through split bf16 operands (engine.FP32_GEMM == "x3")."""
+    contractions) on the persistent wgmma kernel through split bf16 operands (engine.FP32_GEMM == "x3")."""
     g, conf, w, data = load_case(name)
     model = _build(conf, w, "bf16x3")
     d = _f32(data)

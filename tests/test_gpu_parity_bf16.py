@@ -1,5 +1,5 @@
-"""GPU: parity of the MEASURED path (precision = bf16: tcgen05 attention / GEMM kernels) at the shapes it is
-benchmarked on, under the two contracts DESIGN.md section 2 states for it:
+"""GPU: parity of the MEASURED path (precision = bf16: wgmma attention / GEMM kernels) at the shapes it is
+benchmarked on, under two contracts:
 
 (A) "same autocast dtype" contract (SURVEY.md section 7, hard part 1b).  tests/golden/ac_*.npz hold, per output /
     loss entry / parameter gradient, how far the UNMODIFIED reference moves from its own fp64 result when it is
@@ -147,7 +147,7 @@ def _margin_safe(la, dim, margin):
 def test_bf16_path_at_bench_shape_against_rounding_model(N, seed):
     """Full matcher at the benchmark shapes.  bf16 rounding noise is amplified by nine residual layers to a floor of
     ~1.5e-3 relative on the log-scores REGARDLESS of which (valid) set of rounding points is used -- two CPU rounding
-    models differ from each other by as much as each differs from fp64 (DESIGN.md section 2) -- so the tolerances below
+    models differ from each other by as much as each differs from fp64 -- so the tolerances below
     are that floor with ~2x head-room; an indexing / pipeline bug at N = 2048 shows up as O(1) errors.  At N = 1024 the
     floor is measured in the test itself and the CUDA path must be no further from the model than a second model is."""
     conf = dict(synthetic.DEFAULT_CONF)  # L = 9, H = 4, d = 256
@@ -202,7 +202,7 @@ def _attn_ref64(q, k, v, shift):
 
 @pytest.mark.parametrize("shift", [0, 2])
 def test_attention_kernels_at_bench_shape(shift):
-    """4 sequences (2 pairs) x 4 heads x N = 2048: forward, lse, dQ, dK, dV of the tcgen05 kernels against fp64 on the
+    """4 sequences (2 pairs) x 4 heads x N = 2048: forward, lse, dQ, dK, dV of the wgmma kernels against fp64 on the
     same bf16 operands (self attention: shift 0; cross attention: keys of sequence (b + 2) % 4)."""
     B, N, H = 4, 2048, 4
     g = torch.Generator().manual_seed(5 + shift)

@@ -63,7 +63,7 @@ def rel_err(a, b):
 
 def report(tag, **vals):
     """Append measured error figures to gpurun_out/parity_report.txt (when that directory exists): the numbers behind
-    the tolerance table in DESIGN.md.  Never fails a test."""
+    the tolerances of the parity tests.  Never fails a test."""
     try:
         root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
         d = os.path.join(root, "gpurun_out")
