@@ -107,7 +107,7 @@ def load(check_device=True):
 
 # kernels launched per entry point (for bench.py's gpu_launches accounting)
 KERNELS_PER_CALL = {
-    "lgb200_rope_split_fwd": 1, "lgb200_rope_split_bwd": 1, "lgb200_attn_fwd": 1, "lgb200_attn_bwd": 3,  # prep + fused + dQ convert (or prep + dQ + dKV)
+    "lgb200_rope_split_fwd": 1, "lgb200_rope_split_bwd": 1, "lgb200_attn_fwd": 1, "lgb200_attn_bwd": 3,  # prep + fused + dQ convert (or prep + dQ + dKV; shared-qk cross: 2, passed by the caller)
     "lgb200_ln_gelu_fwd": 1, "lgb200_ln_gelu_bwd": 1, "lgb200_gemm_bf16": 1, "lgb200_assign_lse": 2,
     "lgb200_assign_scores": 2, "lgb200_assign_bwd": 1, "lgb200_filter_matches": 1, "lgb200_log_double_softmax": 3,
     "lgb200_adam_flat": 1, "lgb200_cast_bf16": 1, "lgb200_colsum": 1, "lgb200_residual_add_cast": 1,
@@ -120,9 +120,10 @@ timed_tag = None
 timed_tagger = None       # optional callable (name, args) -> hashable, e.g. to tell self- from cross-attention launches
 
 
-def call(name, *args):
+def call(name, *args, launches=None):
     """Invoke an entry point; a negative return code becomes a Python exception carrying the
-    library's message (reference convention: Python exceptions / asserts, lightglue.py:413-414)."""
+    library's message (reference convention: Python exceptions / asserts, lightglue.py:413-414).
+    launches: kernels this call launches, when it differs from KERNELS_PER_CALL[name]."""
     global launch_count
     lib = load()
     if timed_entry is not None and (timed_entry == name or (isinstance(timed_entry, (set, frozenset)) and name in timed_entry)):
@@ -137,7 +138,7 @@ def call(name, *args):
         rc = getattr(lib, name)(*args)
     if rc != 0:
         raise Lgb200Error(f"{name} failed ({rc}): {lib.lgb200_last_error().decode()}")
-    launch_count += KERNELS_PER_CALL.get(name, 1)
+    launch_count += launches if launches is not None else KERNELS_PER_CALL.get(name, 1)
 
 
 def stream_ptr():

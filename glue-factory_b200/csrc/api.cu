@@ -171,6 +171,9 @@ int lgb200_attn_bwd(const void* q, const void* k, const void* v, const void* out
   LGB_REQUIRE(q && k && v && out && lse && dout && dq && dk && dv && delta_ws, kErrInvalid, "attn_bwd: null pointer");
   LGB_REQUIRE(B > 0 && Nq > 0 && Nk > 0 && H > 0, kErrInvalid, "attn_bwd: empty input");
   LGB_REQUIRE(kv_shift >= 0 && kv_shift < B, kErrInvalid, "attn_bwd: kv_shift %d out of range", kv_shift);
+  const bool shared_qk = attn_bwd_is_shared_qk(q, k, dq, dk, B, Nq, Nk, kv_shift);
+  LGB_REQUIRE(!shared_qk || (dtype == LGB200_BF16 && !env_flag("LGB200_ATTN_SIMT")), kErrUnsupported,
+              "attn_bwd: dq == dk (shared-qk cross-attention) runs on the bf16 tensor-core path only");
   if (dtype == LGB200_F32)
     return attn_bwd_simt<float>(q, k, v, out, lse, dout, dq, dk, dv, delta_ws, B, Nq, Nk, H, kv_shift, scale, stream);
   LGB_REQUIRE(dtype == LGB200_BF16, kErrInvalid, "attn_bwd: bad dtype %d", dtype);

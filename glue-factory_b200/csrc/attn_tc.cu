@@ -8,11 +8,18 @@
 //     S_j (64 x 64 fp32, registers) = Q K_j^T      4 wgmma m64n64k16 (both operands K-major in smem)
 //     O   (64 x 64 fp32, registers) += P_j V_j     4 wgmma m64n64k16 (P_j from registers, V_j MN-major in smem)
 // The softmax runs on the S_j accumulators in place (online maximum, rows shared by the four lanes of a quad) and
-// P_j is re-packed to bf16 A fragments without leaving the registers.
+// P_j is re-packed to bf16 A fragments without leaving the registers.  For one 64 x 64 tile the wgmma work and the
+// 4096 exponentials cost about the same SM time, so they are overlapped: a warpgroup issues S_{j+1} with P_j V_j and
+// runs the softmax of S_{j+1} while P_j V_j executes.  106 registers, so two CTAs (four consumer warpgroups) share an
+// SM and fill each other's gaps; making the two warpgroups of a CTA take turns (named-barrier ping-pong) measured
+// slower at that occupancy.  Tile order and per-element arithmetic are those of the unpipelined loop, so out and lse
+// do not depend on the overlap.
 // BACKWARD: one CTA owns 128 keys (K, V resident in smem) and walks the queries in tiles of 64 (dK, dV accumulated in
 // registers); dQ comes from a second kernel that owns the queries (the default: deterministic, so eager steps and
 // CUDA-graph replays of a training step agree bit for bit) or, with LGB200_ATTN_BWD_FUSED=1, from the same pass (dS
 // through shared memory, fp32 atomics into an accumulator: no recomputation of S / dP, run-dependent summation order).
+// Cross-attention with one shared q = k projection (LightGlue's to_qk) has its own kernel: both directions share the
+// similarity, so one sweep per image yields dV and dq + dk (attn_bwd_shared_qk_kernel, below).
 #include <math.h>
 
 #include "common.cuh"
@@ -110,21 +117,18 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
   const bool signal = (threadIdx.x & 127) == 0;
   const uint64_t dQ0 = make_smem_desc(smem_u32(sQ) + wg * 8192, 8192, 1024);
   const uint64_t dK0 = make_smem_desc(smem_u32(sK), 8192, 1024), dV0 = make_smem_desc(smem_u32(sV), 8192, 1024);
-  float o[32], m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float o[32], sv[32], m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, alpha[2];
+  uint32_t pa[4][4];
 #pragma unroll
   for (int e = 0; e < 32; ++e) o[e] = 0.f;
-  mbar_wait(q_full, 0);
-  for (int j = 0; j < ntiles; ++j) {
-    const int s = j % FA_STAGES;
+  auto issue_s = [&](int s) {  // S = Q K^T of stage s into sv (the caller waits for the stage, fences and commits)
     const uint64_t so = (uint64_t)((s * FA_KBYTES) >> 4);
-    mbar_wait(&kv_full[s], (j / FA_STAGES) & 1);
-    float sv[32];
-    wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(sv, dQ0 + kk * 2, dK0 + so + kk * 2, kk != 0);
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_hold(sv);
+  };
+  // online softmax of S_j in place (sv becomes P_j); O is not touched: its rescale by alpha waits until the P V
+  // product that is in flight meanwhile has retired
+  auto softmax = [&](int j) {
     const int kbase = j * FA_BN;
     if (kbase + FA_BN > Nk) {
 #pragma unroll
@@ -139,7 +143,7 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj) mx = fmaxf(mx, fmaxf(sv[4 * jj + 2 * i], sv[4 * jj + 2 * i + 1]));
       const float m_new = fmaxf(m[i], quad_max(mx) * scale_log2);  // every key tile holds at least one valid key
-      const float alpha = fast_exp2(m[i] - m_new);                // first tile: exp2(-inf) = 0
+      alpha[i] = fast_exp2(m[i] - m_new);                          // first tile: exp2(-inf) = 0
       float rs = 0.f;
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj)
@@ -148,21 +152,56 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
           const int x = 4 * jj + 2 * i + e;
           sv[x] = fast_exp2(fmaf(sv[x], scale_log2, -m_new));  // masked keys: exp2(-inf) = 0
           rs += sv[x];
-          o[x] *= alpha;
         }
-      l[i] = l[i] * alpha + rs;  // this lane's partial row sum; the quad is summed at the end
+      l[i] = l[i] * alpha[i] + rs;  // this lane's partial row sum; the quad is summed at the end
       m[i] = m_new;
     }
-    uint32_t pa[4][4];
+  };
+  auto rescale_pack = [&]() {  // O *= alpha, P_j -> bf16 A fragments
+#pragma unroll
+    for (int x = 0; x < 32; ++x) o[x] *= alpha[(x >> 1) & 1];
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) acc_to_afrag(sv, kk, pa[kk]);
+  };
+  // Pipeline per warpgroup: S_{j+1} is issued together with P_j V_j, and its softmax runs while P_j V_j is still on
+  // the tensor cores.  K/V stage j is released once P_j V_j has retired.
+  mbar_wait(q_full, 0);
+  mbar_wait(&kv_full[0], 0);
+  wgmma_fence();
+  issue_s(0);
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_hold(sv);
+  softmax(0);
+  rescale_pack();
+  for (int j = 0; j + 1 < ntiles; ++j) {
+    const int s = j % FA_STAGES;
+    const uint64_t so = (uint64_t)((s * FA_KBYTES) >> 4);
+    const int s1 = (j + 1) % FA_STAGES;
+    mbar_wait(&kv_full[s1], ((j + 1) / FA_STAGES) & 1);
     wgmma_fence();
+    issue_s(s1);
+    wgmma_commit();
 #pragma unroll
     for (int kk = 0; kk < FA_BN / 16; ++kk) wgmma_m64n64_rs<1>(o, pa[kk], dV0 + so + kk * 128, 1);
     wgmma_commit();
+    wgmma_wait<1>();
+    wgmma_hold(sv);
+    softmax(j + 1);
     wgmma_wait<0>();
     wgmma_hold(o);
     if (signal) mbar_arrive(&kv_empty[s]);
+    rescale_pack();
+  }
+  {  // last tile: P V only
+    const int s = (ntiles - 1) % FA_STAGES;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < FA_BN / 16; ++kk)
+      wgmma_m64n64_rs<1>(o, pa[kk], dV0 + (uint64_t)((s * FA_KBYTES) >> 4) + kk * 128, 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_hold(o);
   }
   const int rbase = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
@@ -534,6 +573,167 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
   store_acc_rows(acc, dq, b, Nq, H, h, q0 + wg * 64, 1.f);
 }
 
+// Shared-qk cross-attention (reference: lightglue.py:207-216): sequence b attends to its partner p = (b + B/2) mod B
+// and p to b with the same projection qk, so both directions share one similarity S = qk_b qk_p^T.  A CTA owns 128
+// rows of b (qk_b, v_b, dO_b resident in smem, lse2 / delta of its rows in registers) and streams 64-row tiles of p
+// (qk_p, v_p, dO_p, lse2_p, delta_p) through the TMA ring.  Per tile and warpgroup:
+//     S = qk_b qk_p^T,  dP = dO_b v_p^T,  dP' = v_b dO_p^T                    (wgmma from smem)
+//     P = exp2(c S - lse2_b[row])     (b -> p: rows are the queries)
+//     P' = exp2(c S - lse2_p[col])    (p -> b, transposed: columns are the queries)
+//     dS = P (dP scale - delta_b scale) + P' (dP' scale - delta_p scale)
+//     dV_b += P' dO_p,   dqk_b += dS qk_p                                     (register A operands)
+// so dqk_b = dQ_b + dK_b comes out of one sweep: 5 contractions per tile instead of the 7 of a dQ kernel plus a
+// dK / dV kernel per direction.  The summation order is fixed (no atomics).  Padding follows the generic kernels: rows
+// of p past N load as zeros with lse2 = +inf, so they meet a zero qk_p / dO_p row and P' = 0; rows of b past N are not
+// stored.
+constexpr int FX_STAGES = 4;
+constexpr int FX_STAGE_BYTES = 25 * 1024;                 // qk_p 8 KiB | v_p 8 KiB | dO_p 8 KiB | lse2 256 B | delta 256 B
+constexpr int FX_OFF_STAGE = 3 * FB_R * FA_D * 2;         // after the resident qk_b, v_b, dO_b tiles (16 KiB each)
+constexpr int FX_SMEM = FX_OFF_STAGE + FX_STAGES * FX_STAGE_BYTES + 256;
+// a whole producer warpgroup, so that setmaxnreg can move registers from it to the two consumer warpgroups: S, dP,
+// dP', the two accumulators and the in-flight A fragments do not fit in the 168 registers a thread gets at 288 or
+// 384 threads per CTA
+constexpr int FX_THREADS = 3 * 128;
+constexpr int FX_PRODUCER_REGS = 40, FX_CONSUMER_REGS = 232;
+
+__global__ void __launch_bounds__(FX_THREADS, 1)
+    attn_bwd_shared_qk_kernel(const __grid_constant__ CUtensorMap tmQKr, const __grid_constant__ CUtensorMap tmVr,
+                              const __grid_constant__ CUtensorMap tmDOr, const __grid_constant__ CUtensorMap tmQKs,
+                              const __grid_constant__ CUtensorMap tmVs, const __grid_constant__ CUtensorMap tmDOs,
+                              const float* __restrict__ lse2p, const float* __restrict__ deltap,
+                              __nv_bfloat16* __restrict__ dqk, __nv_bfloat16* __restrict__ dv, int B, int N, int n_pad,
+                              int H, int kv_shift, float scale, float scale_log2) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* sQK = smem;
+  uint8_t* sV = smem + FB_R * FA_D * 2;
+  uint8_t* sDO = smem + 2 * FB_R * FA_D * 2;
+  uint8_t* sStage = smem + FX_OFF_STAGE;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + FX_SMEM - 256);
+  uint64_t* res_full = bars;
+  uint64_t* in_full = bars + 1;               // [FX_STAGES]
+  uint64_t* in_empty = in_full + FX_STAGES;   // [FX_STAGES]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r0 = blockIdx.x * FB_R, h = blockIdx.y, b = blockIdx.z;
+  const int p = (b + kv_shift) % B;
+  const int ntiles = (N + FB_C - 1) / FB_C;
+
+  if (threadIdx.x == 0) {
+    if (smem_u32(smem) & 1023u) __trap();
+    mbar_init(res_full, 1);
+    for (int s = 0; s < FX_STAGES; ++s) {
+      mbar_init(&in_full[s], 1);
+      mbar_init(&in_empty[s], 2);
+    }
+    mbar_fence_init();
+  }
+  if (warp == FA_PRODUCER && lane == 0) {
+    tma_prefetch_desc(&tmQKr);
+    tma_prefetch_desc(&tmVr);
+    tma_prefetch_desc(&tmDOr);
+    tma_prefetch_desc(&tmQKs);
+    tma_prefetch_desc(&tmVs);
+    tma_prefetch_desc(&tmDOs);
+  }
+  __syncthreads();
+
+  if (warp >= FA_PRODUCER) {
+    setmaxnreg_dec<FX_PRODUCER_REGS>();
+    if (warp == FA_PRODUCER && lane == 0) {
+      mbar_expect_tx(res_full, 3 * FB_R * FA_D * 2);
+      tma_load_4d(sQK, &tmQKr, res_full, 0, h, r0, b);
+      tma_load_4d(sV, &tmVr, res_full, 0, h, r0, b);
+      tma_load_4d(sDO, &tmDOr, res_full, 0, h, r0, b);
+      const float* l2 = lse2p + ((int64_t)p * H + h) * n_pad;
+      const float* dl = deltap + ((int64_t)p * H + h) * n_pad;
+      for (int i = 0; i < ntiles; ++i) {
+        const int s = i % FX_STAGES;
+        uint8_t* st = sStage + s * FX_STAGE_BYTES;
+        mbar_wait(&in_empty[s], ((i / FX_STAGES) & 1) ^ 1);
+        mbar_expect_tx(&in_full[s], 3 * FB_CBYTES + 512);
+        tma_load_4d(st, &tmQKs, &in_full[s], 0, h, i * FB_C, p);
+        tma_load_4d(st + FB_CBYTES, &tmVs, &in_full[s], 0, h, i * FB_C, p);
+        tma_load_4d(st + 2 * FB_CBYTES, &tmDOs, &in_full[s], 0, h, i * FB_C, p);
+        bulk_load_1d(st + 3 * FB_CBYTES, l2 + i * FB_C, 256, &in_full[s]);
+        bulk_load_1d(st + 3 * FB_CBYTES + 256, dl + i * FB_C, 256, &in_full[s]);
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<FX_CONSUMER_REGS>();
+  const int wg = threadIdx.x >> 7, t4 = lane & 3;
+  const bool signal = (threadIdx.x & 127) == 0;
+  const uint64_t dQK0 = make_smem_desc(smem_u32(sQK) + wg * 8192, 8192, 1024);
+  const uint64_t dV0 = make_smem_desc(smem_u32(sV) + wg * 8192, 8192, 1024);
+  const uint64_t dDO0 = make_smem_desc(smem_u32(sDO) + wg * 8192, 8192, 1024);
+  const uint64_t dSt0 = make_smem_desc(smem_u32(sStage), 8192, 1024);
+  float l2r[2], dlr[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = r0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;
+    const int64_t o = ((int64_t)b * H + h) * n_pad + row;
+    l2r[r] = row < N ? lse2p[o] : INFINITY;
+    dlr[r] = row < N ? deltap[o] : 0.f;
+  }
+  float acc_v[32], acc_q[32];
+#pragma unroll
+  for (int e = 0; e < 32; ++e) acc_v[e] = acc_q[e] = 0.f;
+  mbar_wait(res_full, 0);
+  for (int i = 0; i < ntiles; ++i) {
+    const int s = i % FX_STAGES;
+    const uint64_t so = (uint64_t)((s * FX_STAGE_BYTES) >> 4);
+    const uint64_t so_v = so + (FB_CBYTES >> 4), so_do = so + ((2 * FB_CBYTES) >> 4);
+    const float* sl = reinterpret_cast<const float*>(sStage + s * FX_STAGE_BYTES + 3 * FB_CBYTES);
+    mbar_wait(&in_full[s], (i / FX_STAGES) & 1);
+    float sv[32], dp[32], dpt[32];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(sv, dQK0 + kk * 2, dSt0 + so + kk * 2, kk != 0);
+#pragma unroll
+    for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(dp, dDO0 + kk * 2, dSt0 + so_v + kk * 2, kk != 0);
+#pragma unroll
+    for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(dpt, dV0 + kk * 2, dSt0 + so_do + kk * 2, kk != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_hold(sv);
+    wgmma_hold(dp);
+    wgmma_hold(dpt);
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const float2 l2c = *reinterpret_cast<const float2*>(sl + 8 * jj + 2 * t4);       // columns = rows of p
+      const float2 dlc = *reinterpret_cast<const float2*>(sl + 64 + 8 * jj + 2 * t4);  // delta_p * scale
+#pragma unroll
+      for (int r = 0; r < 2; ++r)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int x = 4 * jj + 2 * r + e;
+          const float pr = fast_exp2(fmaf(sv[x], scale_log2, -l2r[r]));
+          const float pc = fast_exp2(fmaf(sv[x], scale_log2, -(e ? l2c.y : l2c.x)));
+          dp[x] = fmaf(pr, fmaf(dp[x], scale, -dlr[r]), pc * fmaf(dpt[x], scale, -(e ? dlc.y : dlc.x)));
+          sv[x] = pc;
+        }
+    }
+    uint32_t pa[4][4], da[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      acc_to_afrag(sv, kk, pa[kk]);
+      acc_to_afrag(dp, kk, da[kk]);
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < FB_C / 16; ++kk) wgmma_m64n64_rs<1>(acc_v, pa[kk], dSt0 + so_do + kk * 128, 1);
+#pragma unroll
+    for (int kk = 0; kk < FB_C / 16; ++kk) wgmma_m64n64_rs<1>(acc_q, da[kk], dSt0 + so + kk * 128, 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_hold(acc_v);
+    wgmma_hold(acc_q);
+    if (signal) mbar_arrive(&in_empty[s]);
+  }
+  store_acc_rows(acc_v, dv, b, N, H, h, r0 + wg * 64, 1.f);
+  store_acc_rows(acc_q, dqk, b, N, H, h, r0 + wg * 64, 1.f);
+}
+
 int64_t attn_bwd_ws_floats(int B, int Nq, int Nk, int H) {
   // lse2 / delta padded to whole query tiles + the fp32 dQ accumulator of the fused path
   const int64_t nq_pad = (int64_t)((Nq + FB_C - 1) / FB_C) * FB_C;
@@ -556,12 +756,26 @@ int attn_bwd_tc(const void* q, const void* k, const void* v, const void* out, co
         static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), lse, lse2p, deltap, nrows, Nq,
         nq_pad, H, scale);
   }
+  const float sl2 = scale * kLog2e;
+  if (attn_bwd_is_shared_qk(q, k, dq, dk, B, Nq, Nk, kv_shift)) {  // dq (= dk) receives dq + dk
+    CUtensorMap tqr, tvr, tdor, tqs, tvs, tdos;
+    if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_shared_qk_kernel), FX_SMEM))) return rc;
+    if ((rc = make_qkv_tmap(&tqr, q, B, Nq, H, FB_R))) return rc;
+    if ((rc = make_qkv_tmap(&tvr, v, B, Nq, H, FB_R))) return rc;
+    if ((rc = make_qkv_tmap(&tdor, dout, B, Nq, H, FB_R))) return rc;
+    if ((rc = make_qkv_tmap(&tqs, q, B, Nq, H, FB_C))) return rc;
+    if ((rc = make_qkv_tmap(&tvs, v, B, Nq, H, FB_C))) return rc;
+    if ((rc = make_qkv_tmap(&tdos, dout, B, Nq, H, FB_C))) return rc;
+    attn_bwd_shared_qk_kernel<<<dim3((Nq + FB_R - 1) / FB_R, H, B), FX_THREADS, FX_SMEM, stream>>>(
+        tqr, tvr, tdor, tqs, tvs, tdos, lse2p, deltap, static_cast<__nv_bfloat16*>(dq), static_cast<__nv_bfloat16*>(dv),
+        B, Nq, nq_pad, H, kv_shift, scale, sl2);
+    return check_launch("attn_bwd_shared_qk");
+  }
   if (fused) {
     const size_t acc_bytes = (size_t)B * Nq * H * FA_D * 4;
     cudaError_t e = cudaMemsetAsync(dqacc, 0, acc_bytes, stream);
     LGB_REQUIRE(e == cudaSuccess, kErrCuda, "attn_bwd(fused): memset: %s", cudaGetErrorString(e));
   }
-  const float sl2 = scale * kLog2e;
   CUtensorMap tq, tdo, tk, tv;
   if (!fused) {  // dQ kernel: 128-query resident tiles, 64-key streamed tiles
     if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_dq_kernel), FQ_SMEM))) return rc;

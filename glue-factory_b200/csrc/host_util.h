@@ -36,6 +36,12 @@ int attn_bwd_tc(const void* q, const void* k, const void* v, const void* out, co
                 void* dq, void* dk, void* dv, float* delta, int B, int Nq, int Nk, int H, int kv_shift, float scale,
                 cudaStream_t stream);
 
+// lgb200_attn_bwd's shared-qk cross-attention case (q == k, dq == dk, both directions in one batch)
+inline bool attn_bwd_is_shared_qk(const void* q, const void* k, const void* dq, const void* dk, int B, int Nq, int Nk,
+                                  int kv_shift) {
+  return q == k && dq == dk && Nq == Nk && 2 * kv_shift == B;
+}
+
 // scratch (floats) lgb200_attn_bwd needs for the bf16 path (padded softmax statistics + the fused dQ accumulator)
 int64_t attn_bwd_ws_floats(int B, int Nq, int Nk, int H);
 

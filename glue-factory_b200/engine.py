@@ -166,6 +166,18 @@ def _attend_bwd(q, k, v, out, lses, dout, sizes, H, cross):
     return cat(dq0, dq1), cat(dk0, dk1), cat(dv0, dv1)
 
 
+def _attend_bwd_shared_qk(qk, v, out, lses, dout, sizes, H):
+    """Cross-attention backward with one to_qk projection as query in one direction and key in the other
+    (lightglue.py:207-216) -> (dqk = dq + dk, dv)."""
+    B, M, N = sizes
+    if M != N:
+        dq, dk, dv = _attend_bwd(qk, qk, v, out, lses, dout, sizes, H, cross=True)
+        return dq.add_(dk), dv
+    shp = (2 * B, M, H, 64)
+    dqk, dv = ops.attn_bwd_shared_qk(qk.view(shp), v.view(shp), out.view(shp), lses[0], dout.view(shp), 0.125)
+    return dqk.view(qk.shape), dv.view(qk.shape)
+
+
 # order of the per-layer tensors (reference names, lightglue.py:139-148, 174-183)
 LAYER_PARAMS = [
     "self_attn.Wqkv.weight", "self_attn.Wqkv.bias", "self_attn.out_proj.weight", "self_attn.out_proj.bias",
@@ -275,8 +287,7 @@ class LayerFn(torch.autograd.Function):
         del dh2
         dWout, dbout = _wgrad(dmsg2, m, gv[14]), _bgrad(dmsg2)
         dm = _dgrad(dmsg2, Wout)
-        dq_, dk_, dvv = _attend_bwd(qk, qk, vv, m, lse2, dm, sizes, H, cross=True)
-        dqk = dq_.add_(dk_)  # the shared to_qk projection is query in one direction and key in the other
+        dqk, dvv = _attend_bwd_shared_qk(qk, vv, m, lse2, dm, sizes, H)
         dWqk, dbqk = _wgrad(dqk, x1_16, gv[10]), _bgrad(dqk)
         dWv, dbv = _wgrad(dvv, x1_16, gv[12]), _bgrad(dvv)
         dx1 = _dgrad_acc(dx1, dqk, Wqk)

@@ -100,6 +100,23 @@ def attn_bwd(q, k, v, out, lse, dout, kv_shift, scale):
     return dq, dk, dv
 
 
+def attn_bwd_shared_qk(qk, v, out, lse, dout, scale):
+    """Backward of the cross-attention whose query and key are the same tensor qk [2B,N,H,64] (batch b attends to
+    batch (b + B) % 2B, lightglue.py:207-216).  Returns (dqk, dv) with dqk the total gradient dq + dk of qk.
+    bf16: one pass over the shared similarity (lgb200_attn_bwd with q == k and dq == dk)."""
+    B2 = qk.shape[0]
+    if qk.dtype != torch.bfloat16:
+        dq, dk, dv = attn_bwd(qk, qk, v, out, lse, dout, B2 // 2, scale)
+        return dq.add_(dk), dv
+    _, N, H, _ = qk.shape
+    dout = dout.contiguous()
+    dqk, dv = torch.empty_like(qk), torch.empty_like(v)
+    delta = torch.empty(_lib.load().lgb200_attn_bwd_ws_floats(B2, N, N, H), device=qk.device, dtype=torch.float32)
+    call("lgb200_attn_bwd", ptr(qk), ptr(qk), ptr(v), ptr(out), ptr(lse), ptr(dout), ptr(dqk), ptr(dqk), ptr(dv),
+         ptr(delta), B2, N, N, H, B2 // 2, float(scale), _code(qk.dtype), stream_ptr(), launches=2)  # prep + sweep
+    return dqk, dv
+
+
 class Attention(torch.autograd.Function):
     """q [B,Nq,H,64], k,v [B,Nk,H,64] -> softmax(q k^T / 8) v, keys of batch b taken from batch
     (b + kv_shift) % B."""
