@@ -7,9 +7,12 @@
 //   Running both directions doubles the (cheap, tensor-core) contraction but makes every reduction a per-row running
 //   value: no column partials, no merge kernels, no atomics, deterministic.
 //   The panel (A, 128 x D bf16) stays resident in shared memory for the item; 64-column tiles of the other image
-//   (B, 64 x D) stream through a 3-stage TMA ring.  Two consumer warpgroups own 64 panel rows each and form
+//   (B, 64 x D) stream through a 3-stage ring.  Two consumer warpgroups own 64 panel rows each and form
 //   S = A B^T (64 x 64 per warpgroup, D/16 wgmma m64n64k16) in registers; a row is shared by the four lanes of a
 //   quad (16 of the tile's columns each), whose running values are merged at the end of the item.
+//   A producer warpgroup fills each stage: the B tile by TMA and, for STATS / BWD, the tile's side data next to it --
+//   the 128 x 64 mask tile (gt for direction 0, gt_t for direction 1) and the two per-column fp32 vectors the
+//   elementwise work reads -- so the consumers' inner loop makes no global loads.
 //
 //   LSE  : running (max, sum exp2) per row -> lse_row [B,M] (dir 0), lse_col [B,N] (dir 1).
 //   STATS: scores in the reference's association order ((s - lse_r) + (s - lse_c)) + (lsig0 + lsig1); running
@@ -33,10 +36,18 @@ constexpr int AT_ABLK = AT_R * AT_KBLK * 2; // 16 KiB
 constexpr int AT_BBLK = AT_C * AT_KBLK * 2; // 8 KiB
 constexpr int AT_MAXKB = 4;                // D <= 256
 constexpr int AT_STAGES = 3;
-constexpr int AT_THREADS = 2 * 128 + 32;   // two consumer warpgroups + the producer warp
-constexpr int AT_PRODUCER = 8;
+constexpr int AT_GBLK = AT_R * AT_C;       // 8 KiB: a stage's mask tile, one 64-byte row per panel row
+constexpr int AT_VBLK = 2 * AT_C;          // a stage's two per-column fp32 vectors (512 B)
+// A whole producer warpgroup, so that setmaxnreg can move registers from it to the two consumer warpgroups: a BWD
+// consumer holds its 64 x 256 fp32 d(mdesc) panel (128 registers) next to S and the dsim fragments, which does not fit
+// in the 168 registers a thread gets at 288 or 384 threads per CTA.  Its 128 threads also copy the side data.
+constexpr int AT_THREADS = 3 * 128;
+constexpr int AT_PRODUCER_WG = 2;
+constexpr int AT_PRODUCER_REGS = 56, AT_CONSUMER_REGS = 224;
 constexpr float kLog2e_at = 1.4426950408889634f;
-constexpr int AT_SMEM = AT_MAXKB * AT_ABLK + AT_STAGES * AT_MAXKB * AT_BBLK + 256;
+constexpr int AT_OFF_G = AT_MAXKB * AT_ABLK + AT_STAGES * AT_MAXKB * AT_BBLK;
+constexpr int AT_OFF_V = AT_OFF_G + AT_STAGES * AT_GBLK;
+constexpr int AT_SMEM = AT_OFF_V + AT_STAGES * AT_VBLK * 4 + 256;
 
 enum { AT_LSE = 0, AT_STATS = 1, AT_BWD = 2 };
 
@@ -53,19 +64,35 @@ struct AssignTcArgs {
   __nv_bfloat16* dmd0; __nv_bfloat16* dmd1;  // BWD out: [B*M, D], [B*N, D]
 };
 
+// cp.async (generic proxy, read by ordinary shared loads): src_size 0 writes zeros and reads nothing
+__device__ __forceinline__ void cp_async_16(void* dst, const void* src, bool ok) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(ok ? 16 : 0)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_4(void* dst, const void* src, bool ok) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(ok ? 4 : 0)
+               : "memory");
+}
+// one arrival on `bar` once every cp.async this thread has issued so far has landed (counted in the barrier's init)
+__device__ __forceinline__ void cp_async_mbar_arrive(uint64_t* bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+
 template <int MODE>
 __global__ void __launch_bounds__(AT_THREADS, 1)
     assign_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1, AssignTcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sA = smem;
   uint8_t* sB = smem + AT_MAXKB * AT_ABLK;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + AT_STAGES * AT_MAXKB * AT_BBLK);
+  uint8_t* sG = smem + AT_OFF_G;
+  float* sV = reinterpret_cast<float*>(smem + AT_OFF_V);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + AT_SMEM - 256);
   uint64_t* a_full = bars;                   // 1
   uint64_t* a_empty = bars + 1;              // 1
   uint64_t* b_full = bars + 2;               // [AT_STAGES]
   uint64_t* b_empty = b_full + AT_STAGES;    // [AT_STAGES]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   const int B = a.B, M = a.M, N = a.N, D = a.D;
   const int KB = D / AT_KBLK;
   const int PM = (M + AT_R - 1) / AT_R, PN = (N + AT_R - 1) / AT_R;
@@ -76,12 +103,12 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
     mbar_init(a_full, 1);
     mbar_init(a_empty, 2);
     for (int s = 0; s < AT_STAGES; ++s) {
-      mbar_init(&b_full[s], 1);
-      mbar_init(&b_empty[s], 2);
+      mbar_init(&b_full[s], MODE == AT_LSE ? 1 : 1 + 128);  // the TMA bytes + each producer thread's side data
+      mbar_init(&b_empty[s], 8);                           // every consumer warp has read the stage
     }
     mbar_fence_init();
   }
-  if (warp == AT_PRODUCER && lane == 0) {
+  if (threadIdx.x == AT_PRODUCER_WG * 128) {
     tma_prefetch_desc(&tm0);
     tma_prefetch_desc(&tm1);
   }
@@ -94,55 +121,109 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
     dir = r >= PM;
     p = dir ? r - PM : r;
   };
+  // the mask an item reads, rows = its panel's rows (null: none)
+  auto mask_of = [&](int dir) -> const uint8_t* {
+    return MODE == AT_BWD ? (dir ? a.gt_t : a.gt) : (MODE == AT_STATS && !dir) ? a.gt : nullptr;
+  };
 
-  if (warp == AT_PRODUCER) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
-      int it = 0, g = 0;
-      for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++it) {
-        int dir, b, p;
-        decode(item, dir, b, p);
-        const CUtensorMap* tA = dir ? &tm1 : &tm0;
-        const CUtensorMap* tB = dir ? &tm0 : &tm1;
-        const int ncols = dir ? M : N;
-        const int ntiles = (ncols + AT_C - 1) / AT_C;
+  if (wg == AT_PRODUCER_WG) {
+    // ------------------------------------------------------------------ producer: TMA (thread 0) + side data
+    setmaxnreg_dec<AT_PRODUCER_REGS>();
+    const int pt = threadIdx.x & 127;
+    if (MODE == AT_LSE && pt != 0) return;
+    int it = 0, g = 0;
+    for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++it) {
+      int dir, b, p;
+      decode(item, dir, b, p);
+      const CUtensorMap* tA = dir ? &tm1 : &tm0;
+      const CUtensorMap* tB = dir ? &tm0 : &tm1;
+      const int nrows = dir ? N : M, ncols = dir ? M : N;
+      const int ntiles = (ncols + AT_C - 1) / AT_C;
+      if (pt == 0) {
         mbar_wait(a_empty, (it & 1) ^ 1);
         mbar_expect_tx(a_full, KB * AT_ABLK);
         for (int kb = 0; kb < KB; ++kb)
           for (int hf = 0; hf < 2; ++hf)  // two 64-row boxes per block: the same bytes as one 128-row box
             tma_load_3d(sA + kb * AT_ABLK + hf * AT_BBLK, tA, a_full, kb * AT_KBLK, p * AT_R + hf * AT_C, b);
-        for (int t = 0; t < ntiles; ++t, ++g) {
-          const int s = g % AT_STAGES;
-          mbar_wait(&b_empty[s], ((g / AT_STAGES) & 1) ^ 1);
+      }
+      const uint8_t* gm = mask_of(dir);
+      const uint8_t* gpanel = gm ? gm + ((int64_t)b * nrows + p * AT_R) * ncols : nullptr;
+      // 16-byte copies need 16-byte aligned rows; ragged widths take the byte-wise path
+      const bool direct = !gm || (ncols % 16 == 0 && (reinterpret_cast<uintptr_t>(gm) & 15) == 0);
+      const int prows = min(AT_R, nrows - p * AT_R);
+      const float* va = nullptr;
+      const float* vb = nullptr;
+      if (MODE != AT_LSE) {  // STATS: lse_other, ls_other; BWD: lse_other, cnt_other
+        va = (dir ? a.lse_row : a.lse_col) + (int64_t)b * ncols;
+        vb = (MODE == AT_STATS ? (dir ? a.ls0 : a.ls1) : (dir ? a.rowcnt : a.colcnt)) + (int64_t)b * ncols;
+      }
+      for (int t = 0; t < ntiles; ++t, ++g) {
+        const int s = g % AT_STAGES;
+        mbar_wait(&b_empty[s], ((g / AT_STAGES) & 1) ^ 1);
+        if (pt == 0) {
           mbar_expect_tx(&b_full[s], KB * AT_BBLK);
           for (int kb = 0; kb < KB; ++kb)
             tma_load_3d(sB + (s * AT_MAXKB + kb) * AT_BBLK, tB, &b_full[s], kb * AT_KBLK, t * AT_C, b);
+        }
+        if (MODE != AT_LSE) {
+          const int c0 = t * AT_C;
+          const int jv = c0 + (pt & 63);  // thread pt copies entry pt % 64 of vector pt / 64; zeros past the end
+          const float* vsrc = (pt < 64 ? va : vb) + (jv < ncols ? jv : 0);
+          float* vdst = sV + s * AT_VBLK + pt;
+          uint8_t* gdst = sG + s * AT_GBLK;
+          if (direct) {
+            cp_async_4(vdst, vsrc, jv < ncols);
+            if (gpanel) {
+#pragma unroll
+              for (int u = 0; u < 4; ++u) {  // 16-byte piece q: panel row q / 4, columns c0 + 16 (q % 4) + [0, 16)
+                const int q = pt + 128 * u, r = q >> 2, c = c0 + 16 * (q & 3);
+                const bool ok = r < prows && c < ncols;
+                cp_async_16(gdst + 16 * q, gpanel + (ok ? (int64_t)r * ncols + c : 0), ok);
+              }
+            }
+            cp_async_mbar_arrive(&b_full[s]);
+          } else {
+            *vdst = jv < ncols ? *vsrc : 0.f;
+#pragma unroll 1
+            for (int u = 0; u < 4; ++u) {
+              const int q = pt + 128 * u, r = q >> 2, c = c0 + 16 * (q & 3);
+              const uint8_t* src = gpanel + (int64_t)r * ncols + c;
+              const int n = r < prows ? min(16, ncols - c) : 0;
+#pragma unroll 1
+              for (int k = 0; k < 16; ++k) gdst[16 * q + k] = k < n ? src[k] : 0;
+            }
+            mbar_arrive(&b_full[s]);
+          }
         }
       }
     }
     return;
   }
   // ------------------------------------------------------------------ consumer warpgroups
-  const int wg = threadIdx.x >> 7, t4 = lane & 3;
+  setmaxnreg_inc<AT_CONSUMER_REGS>();
+  const int t4 = lane & 3;
   const bool signal = (threadIdx.x & 127) == 0;
   const uint64_t dA = make_smem_desc(smem_u32(sA) + wg * 8192, 8192, 1024);
   const uint64_t dB = make_smem_desc(smem_u32(sB), 8192, 1024);
   const float c2 = a.alpha * kLog2e_at;
+  int rl[2];  // this thread's two rows within the panel
+#pragma unroll
+  for (int i = 0; i < 2; ++i) rl[i] = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
   int it = 0, g = 0;
   for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++it) {
     int dir, b, p;
     decode(item, dir, b, p);
     const int nrows = dir ? N : M, ncols = dir ? M : N;
     const int ntiles = (ncols + AT_C - 1) / AT_C;
+    const bool has_mask = mask_of(dir) != nullptr;
     // per-row constants of this thread's two rows
     bool rok[2];
     int64_t ro[2];
     float lse_mine[2] = {0.f, 0.f}, ls_mine[2] = {0.f, 0.f}, coef_mine[2] = {0.f, 0.f};
-    const uint8_t* grow[2] = {nullptr, nullptr};  // the rows of the boolean assignment (or of its transpose)
     const float gc = MODE == AT_BWD ? a.gcoef[b] : 0.f;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-      const int row = p * AT_R + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+      const int row = p * AT_R + rl[i];
       rok[i] = row < nrows;
       ro[i] = (int64_t)b * nrows + (rok[i] ? row : 0);
       if (MODE != AT_LSE) lse_mine[i] = (dir ? a.lse_col : a.lse_row)[ro[i]];
@@ -150,13 +231,8 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
       if (MODE == AT_BWD) {
         coef_mine[i] = rok[i] ? gc * (dir ? a.colcnt : a.rowcnt)[ro[i]] : 0.f;
         lse_mine[i] *= kLog2e_at;
-        grow[i] = (dir ? a.gt_t : a.gt) + ro[i] * ncols;
       }
-      if (MODE == AT_STATS && !dir && a.gt) grow[i] = a.gt + ro[i] * ncols;
     }
-    const float* cvec_lse = (dir ? a.lse_row : a.lse_col) + (int64_t)b * ncols;  // per-column vectors of the tile
-    const float* cvec_b = MODE == AT_STATS ? (dir ? a.ls0 : a.ls1) + (int64_t)b * ncols
-                          : MODE == AT_BWD ? (dir ? a.rowcnt : a.colcnt) + (int64_t)b * ncols : nullptr;
     // running values (this lane's 16 columns of every tile)
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // LSE (log2 domain)
     float best[2] = {-INFINITY, -INFINITY}, psum[2] = {0.f, 0.f};    // STATS
@@ -172,6 +248,8 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
     for (int t = 0; t < ntiles; ++t, ++g) {
       const int s = g % AT_STAGES;
       const uint64_t sb = dB + (uint64_t)((s * AT_MAXKB * AT_BBLK) >> 4);
+      const uint8_t* sg = sG + s * AT_GBLK;  // mask tile: row r at sg + 64 r
+      const float* sv_a = sV + s * AT_VBLK;  // lse_other[64] | ls_other or cnt_other[64]
       mbar_wait(&b_full[s], (g / AT_STAGES) & 1);
       float sv[32];
       wgmma_fence();
@@ -182,9 +260,22 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
                                 sb + (uint64_t)((kb * AT_BBLK) >> 4) + kk * 2, (kb | kk) != 0);
       }
       wgmma_commit();
+      // does this row hold a positive in the tile?  Each lane of the quad tests 16 of the row's 64 bytes (a warp
+      // reads 512 contiguous bytes: no bank conflicts); nearly every row is all zero and skips the positive term.
+      bool pos[2] = {false, false};
+      if (MODE != AT_LSE && has_mask) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const uint4 w = *reinterpret_cast<const uint4*>(sg + 64 * rl[i] + 16 * t4);
+          uint32_t u = w.x | w.y | w.z | w.w;
+          u |= __shfl_xor_sync(0xffffffffu, u, 1);
+          u |= __shfl_xor_sync(0xffffffffu, u, 2);
+          pos[i] = u != 0u;
+        }
+      }
       wgmma_wait<0>();
       wgmma_hold(sv);
-      if (MODE != AT_BWD && signal) mbar_arrive(&b_empty[s]);  // S is in registers: the tile's stage is free
+      if (MODE == AT_LSE && lane == 0) mbar_arrive(&b_empty[s]);  // S is in registers: the tile's stage is free
       const int j0 = t * AT_C + 2 * t4;  // column of sv[0]; sv[4jj + 2i + e] is column j0 + 8jj + e of row i
       if (MODE == AT_LSE) {
 #pragma unroll
@@ -217,13 +308,15 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
         // fp32 parity path; the two agree to fp32 rounding.)
         const float a2 = 2.f * a.alpha;
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj)
+        for (int jj = 0; jj < 8; ++jj) {
+          const float2 lc2 = *reinterpret_cast<const float2*>(sv_a + 8 * jj + 2 * t4);
+          const float2 ls2 = *reinterpret_cast<const float2*>(sv_a + AT_C + 8 * jj + 2 * t4);
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const int j = j0 + 8 * jj + e;
+            const int c = 8 * jj + 2 * t4 + e, j = t * AT_C + c;
             const bool cok = j < ncols;
-            const float lc = cok ? __ldg(cvec_lse + j) : 0.f;
-            const float cv = cok ? __ldg(cvec_b + j) - lc : -INFINITY;  // -inf masks the tail
+            const float lc = cok ? (e ? lc2.y : lc2.x) : 0.f;
+            const float cv = cok ? (e ? ls2.y : ls2.x) - lc : -INFINITY;  // -inf masks the tail
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
               const float x = fmaf(sv[4 * jj + 2 * i + e], a2, cv);
@@ -231,31 +324,38 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
                 best[i] = x;
                 besti[i] = j;
               }
-              if (grow[i] && cok && grow[i][j]) psum[i] += (x - cv) - lse_mine[i] - lc;
+              if (pos[i] && sg[64 * rl[i] + c]) psum[i] += (x - cv) - lse_mine[i] - lc;  // zeros past the end
             }
           }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&b_empty[s]);
       } else {  // AT_BWD
         const float two_gc = 2.f * gc;
+        float ds[32];  // dsim, in S's layout (written apart from S: S's registers belong to the MMA pipeline)
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj)
+        for (int jj = 0; jj < 8; ++jj) {
+          const float2 lc2 = *reinterpret_cast<const float2*>(sv_a + 8 * jj + 2 * t4);
+          const float2 cn2 = *reinterpret_cast<const float2*>(sv_a + AT_C + 8 * jj + 2 * t4);
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const int j = j0 + 8 * jj + e;
+            const int c = 8 * jj + 2 * t4 + e, j = t * AT_C + c;
             const bool cok = j < ncols;
-            const float lc = cok ? __ldg(cvec_lse + j) * kLog2e_at : INFINITY;  // exp2(x - inf) = 0 past the end
-            const float cc = cok ? __ldg(cvec_b + j) * gc : 0.f;
+            const float lc = cok ? (e ? lc2.y : lc2.x) * kLog2e_at : INFINITY;  // exp2(x - inf) = 0 past the end
+            const float cc = cok ? (e ? cn2.y : cn2.x) * gc : 0.f;
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
-              float& x = sv[4 * jj + 2 * i + e];
-              float v = (cok && grow[i][j]) ? two_gc : 0.f;
+              const float x = sv[4 * jj + 2 * i + e];
+              float v = (pos[i] && sg[64 * rl[i] + c]) ? two_gc : 0.f;  // zeros past the end
               v = fmaf(-fast_exp2(fmaf(x, c2, -lse_mine[i])), coef_mine[i], v);
               if (cc != 0.f) v = fmaf(-fast_exp2(fmaf(x, c2, -lc)), cc, v);
-              x = cok ? v : 0.f;
+              ds[4 * jj + 2 * i + e] = cok ? v : 0.f;
             }
           }
+        }
         uint32_t da[4][4];
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) acc_to_afrag(sv, kk, da[kk]);
+        for (int kk = 0; kk < 4; ++kk) acc_to_afrag(ds, kk, da[kk]);
         wgmma_fence();
 #pragma unroll
         for (int c = 0; c < AT_MAXKB; ++c) {
@@ -269,7 +369,8 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
         wgmma_wait<0>();
 #pragma unroll
         for (int c = 0; c < AT_MAXKB; ++c) wgmma_hold(acc[c]);
-        if (signal) mbar_arrive(&b_empty[s]);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&b_empty[s]);
       }
     }
     if (signal) mbar_arrive(a_empty);  // every MMA that reads the panel has retired
