@@ -4,10 +4,15 @@
 // K-major / MN-major operands (wgmma reads both layouts straight from shared memory).
 //
 // Persistent CTAs (one per SM) walk 128x128 tiles of C, n fastest so neighbouring CTAs share the A tile in L2.
-// Warp roles: warpgroups 0 and 1 each own 64 rows of the tile (m64n128k16 wgmma, 64 accumulators per thread) and
-// write their rows straight from registers; warp 8 is the TMA producer (one lane).  A 4-stage smem ring of 64-wide
-// K blocks (one 128-byte swizzle atom per operand row) runs ahead across tile boundaries, so the loads of tile i+1
-// overlap the epilogue of tile i.
+// Warp roles: warpgroups 0 and 1 each own 64 rows of the tile (m64n128k16 wgmma, 64 accumulators per thread); warp 8
+// is the TMA producer (one lane).  A 4-stage smem ring of 64-wide K blocks (one 128-byte swizzle atom per operand row)
+// runs ahead across tile boundaries, so the loads of tile i+1 overlap the epilogue of tile i.
+//
+// Epilogue: each warpgroup writes alpha * acc (+ bias) into its own 128-byte-swizzled staging buffer in shared memory,
+// and one thread hands the buffer to the TMA unit: a tensor store, or for an accumulating fp32 C a tensor reduce-add
+// (C += tile, done at L2: the SM never reads C).  The warpgroup goes straight on to the next tile's MMAs while the
+// stores drain; it waits for the TMA unit to have read the buffer only before it fills it again.  A C that TMA cannot
+// address (base or pitch not 16-byte aligned) is written straight from the accumulator registers instead.
 #include <string.h>
 
 #include "common.cuh"
@@ -20,11 +25,84 @@ constexpr int GB_M = 128, GB_N = 128, GB_K = 64, G_STAGES = 4;
 constexpr int G_TILE = GB_M * GB_K * 2;  // 16 KiB per operand per stage
 constexpr int G_THREADS = 2 * 128 + 32;  // two consumer warpgroups + the producer warp
 constexpr int G_PRODUCER = 8;            // warp index of the producer
-constexpr int G_SMEM = G_STAGES * 2 * G_TILE + 256;
+constexpr int G_BOX = 64 * 128;          // one TMA box of C: 64 rows x 128 bytes (32 fp32 / 64 bf16 columns), 8 KiB
+// staging per consumer warpgroup in the generic kernel: its whole 64 x 128 slice of the tile
+template <typename OutT>
+__host__ __device__ constexpr int g_stage_bytes() { return 64 * GB_N * (int)sizeof(OutT); }
+template <typename OutT>
+__host__ __device__ constexpr int g_smem() { return G_STAGES * 2 * G_TILE + 2 * g_stage_bytes<OutT>() + 256; }
 
-// Epilogue of one warpgroup's 64 x 128 accumulator: C (+)= alpha * acc (+ bias[col]).  Each thread owns two
-// adjacent columns of 16 column groups in two rows; pairs are stored as one 8-byte (fp32) / 4-byte (bf16) word
-// when `vec` (C and its pitches even-aligned), element by element otherwise.  reduce_add (fp32 C only) adds into C.
+__device__ __forceinline__ void st_shared_pair(uint32_t addr, float v0, float v1) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v0), "f"(v1) : "memory");
+}
+__device__ __forceinline__ void st_shared_pair(uint32_t addr, uint32_t packed) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(packed) : "memory");
+}
+
+// Staged epilogue of one warpgroup's 64 x 128 accumulator: C (+)= alpha * acc (+ bias[col]) through `stage`
+// (SB bytes, 1024-aligned, SB / 8 KiB boxes of 64 rows x 128 bytes in the 128-byte swizzle of tmC).  An fp32 tile
+// that does not fit (SB = 16 KiB in the A-panel kernel) goes out in column passes of SB / 256 columns.  Same per-element
+// arithmetic as gemm_store_tile; TMA clips the rows >= M and columns >= N of ragged tiles.  Called by all 128 threads
+// of the warpgroup; `leader` (one of them) issues and tracks the bulk stores.
+template <typename OutT, int SB>
+__device__ __forceinline__ void gemm_store_tile_tma(const float (&d)[64], uint8_t* stage, const CUtensorMap* tmC,
+                                                    int M, int N, int m_base, int n0, int bo, float alpha,
+                                                    const float* __restrict__ bias, int reduce_add, int wg,
+                                                    bool leader) {
+  constexpr int ES = (int)sizeof(OutT);
+  constexpr int PASS_COLS = SB / (64 * ES), PASSES = GB_N / PASS_COLS, BOXES = SB / G_BOX, BOX_COLS = 128 / ES;
+  static_assert(SB % G_BOX == 0 && GB_N % PASS_COLS == 0, "staging holds whole boxes");
+  const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+  const int r0 = wq * 16 + (lane >> 2);  // row within the slice; (r0 + 8i) & 7 == lane >> 2
+  const uint32_t sbase = smem_u32(stage);
+#pragma unroll
+  for (int p = 0; p < PASSES; ++p) {
+    if (leader) bulk_wait_read<0>();  // the previous stores out of this buffer have read it
+    named_bar(1 + wg, 128);
+#pragma unroll
+    for (int jj = 0; jj < PASS_COLS / 8; ++jj) {
+      const int j = p * (PASS_COLS / 8) + jj;
+      const int c = 8 * jj + 2 * (lane & 3);  // column within the pass
+      const int col = n0 + 8 * j + 2 * (lane & 3);
+      float b0 = 0.f, b1 = 0.f;
+      if (bias) {
+        if (col < N) b0 = bias[col];
+        if (col + 1 < N) b1 = bias[col + 1];
+      }
+      const uint32_t cb = (uint32_t)(c * ES);  // byte offset of the pair within the pass's rows
+      const uint32_t box = cb >> 7, chunk = (cb >> 4) & 7;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const uint32_t row = (uint32_t)(r0 + 8 * i);
+        const float v0 = fmaf(d[4 * j + 2 * i], alpha, b0), v1 = fmaf(d[4 * j + 2 * i + 1], alpha, b1);
+        const uint32_t addr = sbase + box * G_BOX + row * 128 + ((chunk ^ (uint32_t)(lane >> 2)) << 4) + (cb & 15);
+        if constexpr (ES == 4)
+          st_shared_pair(addr, v0, v1);
+        else
+          st_shared_pair(addr, pack_bf16(v0, v1));
+      }
+    }
+    fence_proxy_async_smem();  // the st.shared above -> visible to the TMA unit
+    named_bar(1 + wg, 128);
+    if (leader && m_base < M) {
+#pragma unroll
+      for (int b = 0; b < BOXES; ++b) {
+        const int cx = n0 + p * PASS_COLS + b * BOX_COLS;
+        if (cx >= N) break;
+        if (reduce_add)
+          tma_reduce_add_3d(tmC, stage + b * G_BOX, cx, m_base, bo);
+        else
+          tma_store_3d(tmC, stage + b * G_BOX, cx, m_base, bo);
+      }
+      bulk_commit();
+    }
+  }
+}
+
+// Register epilogue for a C that TMA cannot address: C (+)= alpha * acc (+ bias[col]) straight from the accumulators.
+// Each thread owns two adjacent columns of 16 column groups in two rows; pairs are stored as one 8-byte (fp32) /
+// 4-byte (bf16) word when `vec` (C and its pitches even-aligned), element by element otherwise.  reduce_add (fp32 C
+// only) adds into C.
 template <typename OutT>
 __device__ __forceinline__ void gemm_store_tile(const float (&d)[64], OutT* __restrict__ C, int M, int N, int64_t ldc,
                                                 int m_base, int n0, float alpha, const float* __restrict__ bias,
@@ -75,15 +153,18 @@ __device__ __forceinline__ void gemm_store_tile(const float (&d)[64], OutT* __re
 template <bool A_MN, bool B_MN, typename OutT>
 __global__ void __launch_bounds__(G_THREADS, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                     const __grid_constant__ CUtensorMap tmC /* {N, M, batch} over C, used when tma_out */,
                      OutT* __restrict__ C, int M, int N, int K, int64_t ldc, int64_t strideC, float alpha, int tiles_m,
                      int tiles_n, int ntiles,
                      int kps /* split-K: k-blocks per split (0 = off); the tile's batch index is then the split */,
                      const float* __restrict__ bias /* [N] added to every row, or null */,
-                     int reduce_add /* fp32 C only: C += alpha A B (+ bias) */, int vec) {
+                     int reduce_add /* fp32 C only: C += alpha A B (+ bias) */, int tma_out, int vec) {
+  constexpr int SB = g_stage_bytes<OutT>();
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sA = smem;
   uint8_t* sB = smem + G_STAGES * G_TILE;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + 2 * G_STAGES * G_TILE);
+  uint8_t* sC = smem + 2 * G_STAGES * G_TILE;  // [2 warpgroups][SB]
+  uint64_t* full = reinterpret_cast<uint64_t*>(sC + 2 * SB);
   uint64_t* empty = full + G_STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -100,6 +181,7 @@ __global__ void __launch_bounds__(G_THREADS, 1)
   if (warp == G_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (tma_out) tma_prefetch_desc(&tmC);
   }
   __syncthreads();
 
@@ -161,9 +243,14 @@ __global__ void __launch_bounds__(G_THREADS, 1)
       wgmma_wait<0>();
       wgmma_hold(d);
       if (signal) mbar_arrive(&empty[(it - 1) % G_STAGES]);
-      gemm_store_tile<OutT>(d, C + (int64_t)bo * strideC, M, N, ldc, m0 + wg * 64, n0, alpha, bias,
-                            reduce_add, vec);
+      if (tma_out)
+        gemm_store_tile_tma<OutT, SB>(d, sC + wg * SB, &tmC, M, N, m0 + wg * 64, n0, bo, alpha, bias, reduce_add, wg,
+                                      signal);
+      else
+        gemm_store_tile<OutT>(d, C + (int64_t)bo * strideC, M, N, ldc, m0 + wg * 64, n0, alpha, bias,
+                              reduce_add, vec);
     }
+    if (tma_out && signal) bulk_wait<0>();  // the CTA's last stores have landed before it exits
   }
 }
 
@@ -174,22 +261,27 @@ __global__ void __launch_bounds__(G_THREADS, 1)
 // panel (KB x 16 KiB) is loaded ONCE into one of two resident buffers (the next item's panel is prefetched while this
 // one is multiplied), only the B blocks stream through a ring, and the CTA walks all n-tiles of the panel.  Operand
 // bytes per panel for N = 256: 64 + 128 KiB instead of 256 KiB; for N = 768: 64 + 384 instead of 768.  A is K-major
-// (rows of x / dy).  Same warpgroup split and epilogue (bias, bf16 / fp32, accumulate) as the generic kernel.
+// (rows of x / dy).  Same warpgroup split and epilogue (bias, bf16 / fp32, accumulate) as the generic kernel; its
+// staging is 16 KiB per warpgroup (the panels and the B ring leave 32 KiB), which holds a bf16 slice whole and an fp32
+// slice in two column halves.
 // ---------------------------------------------------------------------------------------------
 constexpr int GP_KB = 4;                      // K <= 256
 constexpr int GP_BSTAGES = 4;                 // 16 KiB B blocks in flight
 constexpr int GP_BBLK = GB_N * GB_K * 2;      // 16 KiB
-constexpr int GP_SMEM = 2 * GP_KB * G_TILE + GP_BSTAGES * GP_BBLK + 256;
+constexpr int GP_STAGE = 2 * G_BOX;           // epilogue staging per consumer warpgroup
+constexpr int GP_SMEM = 2 * GP_KB * G_TILE + GP_BSTAGES * GP_BBLK + 2 * GP_STAGE + 256;
 
 template <bool B_MN, typename OutT>
 __global__ void __launch_bounds__(G_THREADS, 1)
     gemm_apanel_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                       OutT* __restrict__ C, int M, int N, int K, int64_t ldc, float alpha, int tiles_m, int tiles_n,
-                       const float* __restrict__ bias, int reduce_add, int vec) {
+                       const __grid_constant__ CUtensorMap tmC, OutT* __restrict__ C, int M, int N, int K, int64_t ldc,
+                       float alpha, int tiles_m, int tiles_n, const float* __restrict__ bias, int reduce_add,
+                       int tma_out, int vec) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sA = smem;                                   // [2 panels][GP_KB blocks]
   uint8_t* sB = smem + 2 * GP_KB * G_TILE;              // [GP_BSTAGES]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + GP_BSTAGES * GP_BBLK);
+  uint8_t* sC = sB + GP_BSTAGES * GP_BBLK;              // [2 warpgroups][GP_STAGE]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sC + 2 * GP_STAGE);
   uint64_t* a_full = bars;                 // [2]
   uint64_t* a_empty = bars + 2;            // [2]
   uint64_t* b_full = bars + 4;             // [GP_BSTAGES]
@@ -214,6 +306,7 @@ __global__ void __launch_bounds__(G_THREADS, 1)
   if (warp == G_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (tma_out) tma_prefetch_desc(&tmC);
   }
   __syncthreads();
 
@@ -281,9 +374,14 @@ __global__ void __launch_bounds__(G_THREADS, 1)
           mbar_arrive(&b_empty[(bi - 1) % GP_BSTAGES]);
           if (nt == tiles_n - 1) mbar_arrive(&a_empty[pa]);  // every MMA that reads this panel has retired
         }
-        gemm_store_tile<OutT>(d, C, M, N, ldc, item * GB_M + wg * 64, nt * GB_N, alpha, bias, reduce_add, vec);
+        if (tma_out)
+          gemm_store_tile_tma<OutT, GP_STAGE>(d, sC + wg * GP_STAGE, &tmC, M, N, item * GB_M + wg * 64, nt * GB_N, 0,
+                                              alpha, bias, reduce_add, wg, signal);
+        else
+          gemm_store_tile<OutT>(d, C, M, N, ldc, item * GB_M + wg * 64, nt * GB_N, alpha, bias, reduce_add, vec);
       }
     }
+    if (tma_out && signal) bulk_wait<0>();
   }
 }
 
@@ -294,14 +392,38 @@ static int pair_aligned(const void* C, int64_t ldc, int batch, int64_t strideC) 
   return (reinterpret_cast<uintptr_t>(C) % (2 * ES)) == 0 && ldc % 2 == 0 && (batch == 1 || strideC % 2 == 0);
 }
 
+// Tensor map of C for the staged epilogue: dims {N, M, batch}, 64-row x 128-byte boxes in the 128-byte swizzle.
+// *tma_out = 0 (and the map left zeroed) when TMA cannot address C: its base, row pitch or batch stride is not a
+// multiple of 16 bytes.  The kernel then writes C from registers.
+template <typename OutT>
+static int make_c_map(CUtensorMap* tc, int* tma_out, const void* C, int batch, int M, int N, int64_t ldc,
+                      int64_t strideC) {
+  constexpr int ES = (int)sizeof(OutT);
+  memset(tc, 0, sizeof(*tc));
+  *tma_out = reinterpret_cast<uintptr_t>(C) % 16 == 0 && (ldc * ES) % 16 == 0 &&
+             (batch == 1 || (strideC * ES) % 16 == 0);
+  if (!*tma_out) return 0;
+  const uint64_t dims[3] = {(uint64_t)N, (uint64_t)M, (uint64_t)batch};
+  const uint64_t str[2] = {(uint64_t)ldc * ES, (uint64_t)(batch > 1 ? strideC : (int64_t)M * ldc) * ES};
+  const uint32_t box[3] = {128 / ES, 64, 1};
+  return make_tmap(tc, C, ES == 4, 3, dims, str, box);
+}
+
 template <bool A_MN, bool B_MN, typename OutT>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int batch, int M, int N, int K,
                        int64_t ldc, int64_t strideC, float alpha, cudaStream_t stream, int kps = 0,
                        const float* bias = nullptr, int reduce_add = 0) {
   LGB_REQUIRE(!reduce_add || sizeof(OutT) == 4, kErrInvalid, "gemm: accumulate-into-C needs an fp32 C");
   auto kern = gemm_bf16_kernel<A_MN, B_MN, OutT>;
+  constexpr int smem = g_smem<OutT>();
   {
-    int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), G_SMEM);
+    int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), smem);
+    if (rc) return rc;
+  }
+  CUtensorMap tc;
+  int tma_out = 0;
+  {
+    int rc = make_c_map<OutT>(&tc, &tma_out, C, batch, M, N, ldc, strideC);
     if (rc) return rc;
   }
   const int num_sms = device_sm_count();
@@ -309,9 +431,9 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, void* C, in
   const int64_t ntiles = (int64_t)tiles_m * tiles_n * batch;
   LGB_REQUIRE(ntiles < (1ll << 31), kErrUnsupported, "gemm: too many tiles");
   const unsigned grid = (unsigned)(ntiles < num_sms ? ntiles : num_sms);
-  kern<<<grid, G_THREADS, G_SMEM, stream>>>(ta, tb, static_cast<OutT*>(C), M, N, K, ldc, strideC, alpha, tiles_m, tiles_n,
-                                            (int)ntiles, kps, bias, reduce_add,
-                                            pair_aligned<OutT>(C, ldc, batch, strideC));
+  kern<<<grid, G_THREADS, smem, stream>>>(ta, tb, tc, static_cast<OutT*>(C), M, N, K, ldc, strideC, alpha, tiles_m,
+                                          tiles_n, (int)ntiles, kps, bias, reduce_add, tma_out,
+                                          pair_aligned<OutT>(C, ldc, batch, strideC));
   return check_launch("gemm_bf16");
 }
 
@@ -455,8 +577,12 @@ extern "C" int lgb200_linear(const void* A, const void* B, void* C, const float*
   {                                                                                                              \
     auto kern = gemm_apanel_kernel<BMJ, T>;                                                                      \
     if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), GP_SMEM))) return rc;                        \
-    kern<<<grid, G_THREADS, GP_SMEM, stream>>>(ta, tb, static_cast<T*>(C), M, N, K, ldc, alpha, tiles_m, tiles_n, \
-                                               bias, accumulate ? 1 : 0, pair_aligned<T>(C, ldc, 1, 0));         \
+    CUtensorMap tc;                                                                                              \
+    int tma_out = 0;                                                                                             \
+    if ((rc = make_c_map<T>(&tc, &tma_out, C, 1, M, N, ldc, 0))) return rc;                                      \
+    kern<<<grid, G_THREADS, GP_SMEM, stream>>>(ta, tb, tc, static_cast<T*>(C), M, N, K, ldc, alpha, tiles_m,     \
+                                               tiles_n, bias, accumulate ? 1 : 0, tma_out,                       \
+                                               pair_aligned<T>(C, ldc, 1, 0));                                   \
     return check_launch("linear(apanel)");                                                                       \
   }
       if (c_dtype == LGB200_F32) {

@@ -114,9 +114,10 @@ def _bgrad(dy):
 
 
 def _dgrad_acc(acc, dy, w):
-    """acc (fp32 [T, in]) += dy (compute dtype [T, out]) @ w ([out, in]), IN PLACE: the GEMM's epilogue adds its tile
-    into acc with a TMA reduce (bf16 operands), so the residual-stream gradient is accumulated in fp32 and never
-    re-read by an SM.  Every `acc` handed in is a gradient buffer this engine owns."""
+    """acc (fp32 [T, in]) += dy (compute dtype [T, out]) @ w ([out, in]), IN PLACE: the GEMM's epilogue stages its
+    tile in shared memory and adds it into acc with a TMA reduce-add (bf16 operands), so the residual-stream gradient
+    is accumulated in fp32 and never re-read by an SM (an acc that is not 16-byte aligned is read-modify-written from
+    registers instead).  Every `acc` handed in is a gradient buffer this engine owns."""
     if dy.dtype == torch.float32:
         if FP32_GEMM == "x3":
             return ops.linear(split3(dy, 1, "hhl"), split3(w, 0, "hlh"), out=acc, w_is_kn=True, accumulate=True)
