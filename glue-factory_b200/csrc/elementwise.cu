@@ -6,6 +6,7 @@
 // All use 128-bit loads/stores; row reductions are warp shuffles.
 #include <math.h>
 
+#include <initializer_list>
 #include "common.cuh"
 #include "host_util.h"
 #include "lgb200.h"
@@ -780,6 +781,14 @@ __global__ void __launch_bounds__(256) head_token_bwd_kernel(const float* __rest
   }
 }
 
+// The kernels above read and write whole rows with 16-byte vector accesses: every such pointer must be 16-byte aligned
+// (null pointers pass).  Checked on the host so a misaligned view is an LGB200_ERR_INVALID, not a device fault.
+static bool aligned16(std::initializer_list<const void*> ps) {
+  for (const void* p : ps)
+    if (reinterpret_cast<uintptr_t>(p) & 15) return false;
+  return true;
+}
+
 }  // namespace lgb
 
 using namespace lgb;
@@ -835,6 +844,7 @@ int lgb200_residual_add_cast_pitched(const float* x, const void* y, float* x_out
               (long long)cols);
   LGB_REQUIRE(cast_pitch == cols || (cols % 8 == 0 && cast_pitch % 8 == 0), kErrInvalid,
               "residual_add_cast: a pitched cast output needs cols and pitch to be multiples of 8");
+  LGB_REQUIRE(aligned16({x, y, x_out, x_cast}), kErrInvalid, "residual_add_cast: misaligned pointer (16 bytes needed)");
   const int64_t n = rows * cols;
   const unsigned grid = (unsigned)(((n + 7) / 8 + 255) / 256);
   if (dtype == LGB200_F32)
@@ -851,6 +861,7 @@ int lgb200_residual_add_cast_pitched(const float* x, const void* y, float* x_out
 int lgb200_add_f32_cast(const float* x, const float* y, float* x_out, void* x_cast, int64_t n, int dtype,
                         cudaStream_t stream) {
   LGB_REQUIRE(x && y && (x_out || x_cast) && n > 0, kErrInvalid, "add_f32_cast: bad arguments");
+  LGB_REQUIRE(aligned16({x, y, x_out, x_cast}), kErrInvalid, "add_f32_cast: misaligned pointer (16 bytes needed)");
   const unsigned grid = (unsigned)(((n + 7) / 8 + 255) / 256);
   if (dtype == LGB200_F32)
     residual_add_cast_kernel<float, float><<<grid, 256, 0, stream>>>(x, y, x_out, (float*)x_cast, n, n, n);
@@ -871,6 +882,7 @@ int lgb200_rope_split_fwd(const void* qkv, const float* theta, void* q, void* k,
                           int dtype, cudaStream_t stream) {
   LGB_REQUIRE(qkv && theta && q && k && v, kErrInvalid, "rope_split_fwd: null pointer");
   LGB_REQUIRE(ntok > 0 && H > 0, kErrInvalid, "rope_split_fwd: empty input");
+  LGB_REQUIRE(aligned16({qkv, theta, q, k, v}), kErrInvalid, "rope_split_fwd: misaligned pointer (16 bytes needed)");
   const int64_t nthr = ntok * 8;
   const unsigned grid = (unsigned)((nthr + 255) / 256);
   if (dtype == LGB200_F32)
@@ -889,6 +901,8 @@ int lgb200_rope_split_bwd(const void* dq, const void* dk, const void* dv, const 
                           cudaStream_t stream) {
   LGB_REQUIRE(dq && dk && dv && q && k && theta && dqkv && dtheta, kErrInvalid, "rope_split_bwd: null pointer");
   LGB_REQUIRE(ntok > 0 && H > 0, kErrInvalid, "rope_split_bwd: empty input");
+  LGB_REQUIRE(aligned16({dq, dk, dv, q, k, theta, dqkv, dtheta}), kErrInvalid,
+              "rope_split_bwd: misaligned pointer (16 bytes needed)");
   const int64_t nthr = ntok * 8;
   const unsigned grid = (unsigned)((nthr + 255) / 256);
   if (dtype == LGB200_F32)
@@ -925,6 +939,7 @@ int lgb200_ln_gelu_fwd(const void* x, const float* gamma, const float* beta, voi
                        int64_t ntok, int W, float eps, int dtype, cudaStream_t stream) {
   LGB_REQUIRE(x && gamma && beta && y && mean && rstd, kErrInvalid, "ln_gelu_fwd: null pointer");
   LGB_REQUIRE(ntok > 0, kErrInvalid, "ln_gelu_fwd: empty input");
+  LGB_REQUIRE(aligned16({x, gamma, beta, y}), kErrInvalid, "ln_gelu_fwd: misaligned pointer (16 bytes needed)");
   if (dtype == LGB200_F32) return ln_gelu_fwd_dispatch<float>(x, gamma, beta, y, mean, rstd, ntok, W, eps, stream);
   if (dtype == LGB200_BF16) return ln_gelu_fwd_dispatch<__nv_bfloat16>(x, gamma, beta, y, mean, rstd, ntok, W, eps, stream);
   LGB_REQUIRE(false, kErrInvalid, "ln_gelu_fwd: bad dtype %d", dtype);
@@ -959,6 +974,7 @@ int lgb200_ln_gelu_bwd(const void* dy, const void* x, const float* gamma, const 
   LGB_REQUIRE(dy && x && gamma && beta && mean && rstd && dx && dgamma_part && dbeta_part && dxsum_part, kErrInvalid,
               "ln_gelu_bwd: null pointer");
   LGB_REQUIRE(ntok > 0, kErrInvalid, "ln_gelu_bwd: empty input");
+  LGB_REQUIRE(aligned16({dy, x, gamma, beta, dx}), kErrInvalid, "ln_gelu_bwd: misaligned pointer (16 bytes needed)");
   if (dtype == LGB200_F32)
     return ln_gelu_bwd_dispatch<float>(dy, x, gamma, beta, mean, rstd, dx, dgamma_part, dbeta_part, dxsum_part, ntok, W,
                                        stream);
@@ -1007,6 +1023,7 @@ int lgb200_amp_update(const float* found_inf, int* step_dev, float* loss_scale, 
 
 int lgb200_cast_bf16(const float* src, void* dst, int64_t n, cudaStream_t stream) {
   LGB_REQUIRE(src && dst && n > 0, kErrInvalid, "cast_bf16: bad arguments");
+  LGB_REQUIRE(aligned16({src, dst}), kErrInvalid, "cast_bf16: misaligned pointer (16 bytes needed)");
   const unsigned grid = (unsigned)(((n + 7) / 8 + 255) / 256);
   cast_bf16_kernel<<<grid, 256, 0, stream>>>(src, (__nv_bfloat16*)dst, n);
   return check_launch("cast_bf16");

@@ -52,7 +52,8 @@ int lgb200_check_device(void);
 /* ---- rotary encoding + QKV de-interleave ------------------------------------------------------
  * replaces lightglue.py:157-160 (unflatten(H,-1,3), q/k/v slices, apply_cached_rotary_emb) and
  * lightglue.py:42-49.  qkv [ntok, H*192] with feature = h*192 + d*3 + {q,k,v};
- * theta [ntok, 32] fp32 = posenc.Wr(kpts) (lightglue.py:62); q,k,v [ntok, H*64].           */
+ * theta [ntok, 32] fp32 = posenc.Wr(kpts) (lightglue.py:62); q,k,v [ntok, H*64].
+ * Every pointer of both rope entry points must be 16-byte aligned.                          */
 int lgb200_rope_split_fwd(const void* qkv, const float* theta, void* q, void* k, void* v, int64_t ntok, int H,
                           int dtype, cudaStream_t stream);
 /* dq,dk are gradients w.r.t. the rotated q,k (saved by forward as q,k); writes dqkv [ntok, H*192]
@@ -82,7 +83,8 @@ int lgb200_attn_bwd(const void* q, const void* k, const void* v, const void* out
 
 /* ---- FFN LayerNorm + GELU -------------------------------------------------------------------------
  * replaces nn.LayerNorm(2D) + nn.GELU() of the ffn Sequential (lightglue.py:143-148, 178-183).
- * x,y [ntok, W], W in {256,512,1024}; mean,rstd [ntok] saved for backward.                       */
+ * x,y [ntok, W], W in {256,512,1024}; mean,rstd [ntok] saved for backward.
+ * x, y, dy, dx, gamma and beta must be 16-byte aligned.                                          */
 int lgb200_ln_gelu_fwd(const void* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd,
                        int64_t ntok, int W, float eps, int dtype, cudaStream_t stream);
 /* number of partial rows written to dgamma_part / dbeta_part / dxsum_part [parts, W] (caller sums over
@@ -265,7 +267,9 @@ int lgb200_add_f32_cast(const float* x, const float* y, float* x_out, void* x_ca
 int lgb200_residual_add_cast(const float* x, const void* y, float* x_out, void* x_cast, int64_t n, int dtype,
                              cudaStream_t stream);
 /* same over [rows, cols] with the cast copy written at row pitch cast_pitch >= cols (elements): the copy lands
- * directly in the left / right half of the [x | msg] operand of ffn.0 (lightglue.py:162, 219), no torch.cat.   */
+ * directly in the left / right half of the [x | msg] operand of ffn.0 (lightglue.py:162, 219), no torch.cat.
+ * lgb200_add_f32_cast, lgb200_residual_add_cast and lgb200_residual_add_cast_pitched need 16-byte aligned x, y,
+ * x_out and x_cast; lgb200_cast_bf16 needs 16-byte aligned src and dst.                                        */
 int lgb200_residual_add_cast_pitched(const float* x, const void* y, float* x_out, void* x_cast, int64_t rows,
                                      int64_t cols, int64_t cast_pitch, int dtype, cudaStream_t stream);
 
