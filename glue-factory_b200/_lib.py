@@ -64,6 +64,10 @@ SIGNATURES = {
     "lgb200_cast_bf16": (_i, [_vp, _vp, _i64, _vp]),
     "lgb200_colsum_slabs": (_i, [_i64, _i]),
     "lgb200_colsum": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _i, _vp]),
+    "lgb200_bn_stats": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _i, _vp]),
+    "lgb200_bn_relu_fwd": (_i, [_vp] * 6 + [_f, _f] + [_vp] * 3 + [_i64, _i, _i, _vp]),
+    "lgb200_bn_relu_bwd_reduce": (_i, [_vp] * 9 + [_i64, _i, _i, _vp]),
+    "lgb200_bn_relu_bwd": (_i, [_vp] * 9 + [_i64, _i, _i, _vp]),
     "lgb200_posenc_wgrad_blocks": (_i, []),
     "lgb200_posenc_wgrad": (_i, [_vp, _vp, _vp, _i64, _i, _i, _vp]),
     "lgb200_mask_counts": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),

@@ -551,42 +551,132 @@ __global__ void __launch_bounds__(256) mask_counts_kernel(const uint8_t* __restr
 }
 
 // ---------------------------------------------------------------------------------------------
-// column sums of a tall [rows, cols] matrix (bias gradients): block = 32 row-lanes x 8 column-vectors
-// (8 elements = one 128-bit load for bf16), row slabs across blockIdx.y, deterministic two-stage sum.
+// column sums of a tall [rows, cols] matrix: block = 32 row-lanes x 8 column-vectors (8 elements = one 128-bit load
+// for bf16), row slabs across blockIdx.y, deterministic two-stage sum.  `Op` says what is summed: Op::K per-element
+// terms of the row data it loads, accumulated in Op::Acc; out = [K, cols].
+//   ColsumPlain  : the column sums themselves (bias gradients), fp32
+//   BnStats      : sum x, sum x^2 (BatchNorm statistics), fp64, and the row count behind them
+//   BnReluBwdSums: sum dy', sum dy' xhat with dy' = dy [relu output > 0] (BatchNorm + ReLU backward), fp64
 // ---------------------------------------------------------------------------------------------
 template <typename T>
-__global__ void __launch_bounds__(256) colsum_kernel(const T* __restrict__ a, float* __restrict__ part,
-                                                    float* __restrict__ out, unsigned* __restrict__ counter,
-                                                    int64_t rows, int cols, int rows_per_slab) {
-  __shared__ float s_red[32][65];
+struct ColsumPlain {
+  using Acc = float;
+  static constexpr int K = 1;
+  const T* a;
+  struct Ctx {};
+  using Raw = Vec8<T>;
+  __device__ Ctx ctx(int) const { return {}; }
+  __device__ Raw load(int64_t r, int cols, int col0) const { return Vec8<T>::load(a + r * cols + col0); }
+  __device__ Acc term(const Ctx&, const Raw& v, int, int e) const { return v.v[e]; }
+  __device__ void finish(Acc*, int64_t, int) const {}
+};
+
+template <typename T>
+struct BnStats {
+  using Acc = double;  // exact enough for sum x^2 - n mean^2 when |mean| >> std
+  static constexpr int K = 2;
+  const T* x;
+  struct Ctx {};
+  using Raw = Vec8<T>;
+  __device__ Ctx ctx(int) const { return {}; }
+  __device__ Raw load(int64_t r, int cols, int col0) const { return Vec8<T>::load(x + r * cols + col0); }
+  __device__ Acc term(const Ctx&, const Raw& v, int k, int e) const {
+    const double d = v.v[e];
+    return k == 0 ? d : d * d;
+  }
+  __device__ void finish(Acc* out, int64_t rows, int cols) const { out[2 * cols] = (double)rows; }
+};
+
+// normalised input and pre-activation of BatchNorm + ReLU; forward and backward evaluate the same expressions, so the
+// backward's ReLU mask equals the forward's
+__device__ __forceinline__ float bn_xhat(float v, float mu, float rs) { return (v - mu) * rs; }
+__device__ __forceinline__ float bn_pre(float xh, float g, float b) { return fmaf(xh, g, b); }
+
+template <typename T>
+struct BnReluBwdSums {
+  using Acc = double;
+  static constexpr int K = 2;
+  const T* dy;
+  const T* x;
+  const float *mean, *rstd, *gamma, *beta;
+  struct Ctx {
+    float mu[8], rs[8], g[8], b[8];
+  };
+  struct Raw {
+    Vec8<T> x, g;
+  };
+  __device__ Ctx ctx(int col0) const {
+    Ctx c;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      c.mu[e] = mean[col0 + e];
+      c.rs[e] = rstd[col0 + e];
+      c.g[e] = gamma[col0 + e];
+      c.b[e] = beta[col0 + e];
+    }
+    return c;
+  }
+  __device__ Raw load(int64_t r, int cols, int col0) const {
+    return {Vec8<T>::load(x + r * cols + col0), Vec8<T>::load(dy + r * cols + col0)};
+  }
+  __device__ Acc term(const Ctx& c, const Raw& v, int k, int e) const {
+    const float xh = bn_xhat(v.x.v[e], c.mu[e], c.rs[e]);
+    const float d = bn_pre(xh, c.g[e], c.b[e]) > 0.f ? v.g.v[e] : 0.f;
+    return k == 0 ? (double)d : (double)d * (double)xh;
+  }
+  __device__ void finish(Acc*, int64_t, int) const {}
+};
+
+template <typename Op>
+__global__ void __launch_bounds__(256) colsum_kernel(Op op, typename Op::Acc* __restrict__ part,
+                                                    typename Op::Acc* __restrict__ out,
+                                                    unsigned* __restrict__ counter, int64_t rows, int cols,
+                                                    int rows_per_slab) {
+  using Acc = typename Op::Acc;
+  constexpr int K = Op::K;
+  __shared__ Acc s_red[32][65];
   __shared__ bool s_last;
   const int cx = threadIdx.x & 7, ry = threadIdx.x >> 3;
   const int col0 = blockIdx.x * 64 + cx * 8;
   const int64_t r0 = (int64_t)blockIdx.y * rows_per_slab;
   const int64_t r1 = min(rows, r0 + rows_per_slab);
-  float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  Acc acc[K][8];
+#pragma unroll
+  for (int k = 0; k < K; ++k)
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[k][e] = Acc(0);
   if (col0 < cols) {
+    const typename Op::Ctx c = op.ctx(col0);
     int64_t r = r0 + ry;
     for (; r + 96 < r1; r += 128) {  // four independent 16-byte loads in flight per thread
-      Vec8<T> v0 = Vec8<T>::load(a + r * cols + col0), v1 = Vec8<T>::load(a + (r + 32) * cols + col0);
-      Vec8<T> v2 = Vec8<T>::load(a + (r + 64) * cols + col0), v3 = Vec8<T>::load(a + (r + 96) * cols + col0);
+      const typename Op::Raw v0 = op.load(r, cols, col0), v1 = op.load(r + 32, cols, col0);
+      const typename Op::Raw v2 = op.load(r + 64, cols, col0), v3 = op.load(r + 96, cols, col0);
 #pragma unroll
-      for (int e = 0; e < 8; ++e) acc[e] += (v0.v[e] + v1.v[e]) + (v2.v[e] + v3.v[e]);
+      for (int k = 0; k < K; ++k)
+#pragma unroll
+        for (int e = 0; e < 8; ++e)
+          acc[k][e] += (op.term(c, v0, k, e) + op.term(c, v1, k, e)) + (op.term(c, v2, k, e) + op.term(c, v3, k, e));
     }
     for (; r < r1; r += 32) {
-      Vec8<T> v = Vec8<T>::load(a + r * cols + col0);
+      const typename Op::Raw v = op.load(r, cols, col0);
 #pragma unroll
-      for (int e = 0; e < 8; ++e) acc[e] += v.v[e];
+      for (int k = 0; k < K; ++k)
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc[k][e] += op.term(c, v, k, e);
     }
   }
 #pragma unroll
-  for (int e = 0; e < 8; ++e) s_red[ry][cx * 8 + e] = acc[e];
-  __syncthreads();
-  if (threadIdx.x < 64 && blockIdx.x * 64 + threadIdx.x < cols) {
-    float t = 0.f;
+  for (int k = 0; k < K; ++k) {
+    if (k > 0) __syncthreads();  // the previous term's slab sums have been read out of s_red
 #pragma unroll
-    for (int r = 0; r < 32; ++r) t += s_red[r][threadIdx.x];
-    part[(int64_t)blockIdx.y * cols + blockIdx.x * 64 + threadIdx.x] = t;
+    for (int e = 0; e < 8; ++e) s_red[ry][cx * 8 + e] = acc[k][e];
+    __syncthreads();
+    if (threadIdx.x < 64 && blockIdx.x * 64 + threadIdx.x < cols) {
+      Acc t = Acc(0);
+#pragma unroll
+      for (int r = 0; r < 32; ++r) t += s_red[r][threadIdx.x];
+      part[((int64_t)blockIdx.y * K + k) * cols + blockIdx.x * 64 + threadIdx.x] = t;
+    }
   }
   // the last CTA of this column block to finish sums the slab partials in slab order (deterministic)
   __threadfence();
@@ -601,10 +691,136 @@ __global__ void __launch_bounds__(256) colsum_kernel(const T* __restrict__ a, fl
     __threadfence();
     const int c = blockIdx.x * 64 + (threadIdx.x & 63);
     if (threadIdx.x < 64 && c < cols) {
-      float t = 0.f;
-      for (unsigned sidx = 0; sidx < gridDim.y; ++sidx) t += __ldcg(&part[(int64_t)sidx * cols + c]);
-      out[c] = t;
+#pragma unroll
+      for (int k = 0; k < K; ++k) {
+        Acc t = Acc(0);
+        for (unsigned sidx = 0; sidx < gridDim.y; ++sidx) t += __ldcg(&part[((int64_t)sidx * K + k) * cols + c]);
+        out[k * cols + c] = t;
+      }
     }
+    if (blockIdx.x == 0 && threadIdx.x == 0) op.finish(out, rows, cols);
+  }
+}
+
+template <typename Op>
+static int colsum_launch(const Op& op, typename Op::Acc* out, typename Op::Acc* ws, unsigned* counters, int64_t rows,
+                         int cols, cudaStream_t stream) {
+  const int nslabs = lgb200_colsum_slabs(rows, cols);
+  const int rps = (int)((rows + nslabs - 1) / nslabs);
+  colsum_kernel<Op><<<dim3((cols + 63) / 64, nslabs), 256, 0, stream>>>(op, ws, out, counters, rows, cols, rps);
+  return check_launch("colsum");
+}
+
+// ---------------------------------------------------------------------------------------------
+// BatchNorm + ReLU, token-major x [ntok, C], C a power of two in [8, 512].  Thread <-> 8 consecutive channels of a
+// row; the grid stride is a multiple of C / 8, so a thread keeps its channels.  Each CTA turns the per-channel
+// statistics into scale / shift in shared memory first (every CTA evaluates the same expressions: identical values).
+// ---------------------------------------------------------------------------------------------
+constexpr int kBnMaxC = 512;
+
+__device__ __forceinline__ int64_t bn_grid_stride() { return (int64_t)gridDim.x * blockDim.x; }
+
+// sums = [sum x (C) | sum x^2 (C) | count] (fp64, possibly summed over ranks): training mode; NULL: eval mode with the
+// running statistics.  Block 0 writes the saved mean / rstd and, in training mode, updates the running statistics
+// (momentum, unbiased variance with the count in `sums`).
+template <typename T>
+__global__ void __launch_bounds__(256) bn_relu_fwd_kernel(const T* __restrict__ x, const double* __restrict__ sums,
+                                                         const float* __restrict__ gamma,
+                                                         const float* __restrict__ beta, float* __restrict__ rmean,
+                                                         float* __restrict__ rvar, float momentum, float eps,
+                                                         T* __restrict__ y, float* __restrict__ save_mean,
+                                                         float* __restrict__ save_rstd, int64_t ntok, int C) {
+  __shared__ float s_mu[kBnMaxC], s_rs[kBnMaxC];
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    float mu, rs;
+    if (sums) {
+      const double n = sums[2 * C];
+      const double m = sums[c] / n;
+      const double var = fmax(sums[C + c] / n - m * m, 0.0);
+      mu = (float)m;
+      rs = 1.f / sqrtf((float)var + eps);
+      if (blockIdx.x == 0 && rmean) {
+        rmean[c] = (1.f - momentum) * rmean[c] + momentum * mu;
+        rvar[c] = (1.f - momentum) * rvar[c] + momentum * (float)(var * n / (n - 1.0));
+      }
+    } else {
+      mu = rmean[c];
+      rs = 1.f / sqrtf(rvar[c] + eps);
+    }
+    s_mu[c] = mu;
+    s_rs[c] = rs;
+    if (blockIdx.x == 0) {
+      save_mean[c] = mu;
+      save_rstd[c] = rs;
+    }
+  }
+  __syncthreads();
+  const int cv = C / 8;
+  const int64_t start = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int c0 = (int)(start % cv) * 8;
+  float mu[8], rs[8], g[8], b[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    mu[e] = s_mu[c0 + e];
+    rs[e] = s_rs[c0 + e];
+    g[e] = gamma[c0 + e];
+    b[e] = beta[c0 + e];
+  }
+  const int64_t n8 = ntok * cv;
+  for (int64_t i = start; i < n8; i += bn_grid_stride()) {
+    float v[8];
+    Raw8<T>::load(x + i * 8).unpack(v);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const float z = bn_pre(bn_xhat(v[e], mu[e], rs[e]), g[e], b[e]);
+      v[e] = z < 0.f ? 0.f : z;  // NaN propagates like torch.relu
+    }
+    store8<T>(y + i * 8, v);
+  }
+}
+
+// dx = gamma rstd (dy' - gsums[0:C] / n - xhat gsums[C:2C] / n), dy' = dy [pre-activation > 0], n = *count.
+// gsums NULL: eval mode (the statistics are constants), dx = gamma rstd dy'.
+template <typename T>
+__global__ void __launch_bounds__(256) bn_relu_bwd_kernel(const T* __restrict__ dy, const T* __restrict__ x,
+                                                         const float* __restrict__ gamma,
+                                                         const float* __restrict__ beta,
+                                                         const float* __restrict__ mean,
+                                                         const float* __restrict__ rstd,
+                                                         const double* __restrict__ gsums,
+                                                         const double* __restrict__ count, T* __restrict__ dx,
+                                                         int64_t ntok, int C) {
+  __shared__ float s_k1[kBnMaxC], s_k2[kBnMaxC];
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    s_k1[c] = gsums ? (float)(gsums[c] / *count) : 0.f;
+    s_k2[c] = gsums ? (float)(gsums[C + c] / *count) : 0.f;
+  }
+  __syncthreads();
+  const int cv = C / 8;
+  const int64_t start = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int c0 = (int)(start % cv) * 8;
+  float mu[8], rs[8], g[8], b[8], k1[8], k2[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    mu[e] = mean[c0 + e];
+    rs[e] = rstd[c0 + e];
+    g[e] = gamma[c0 + e];
+    b[e] = beta[c0 + e];
+    k1[e] = s_k1[c0 + e];
+    k2[e] = s_k2[c0 + e];
+  }
+  const int64_t n8 = ntok * cv;
+  for (int64_t i = start; i < n8; i += bn_grid_stride()) {
+    float v[8], d[8];
+    Raw8<T>::load(x + i * 8).unpack(v);
+    Raw8<T>::load(dy + i * 8).unpack(d);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const float xh = bn_xhat(v[e], mu[e], rs[e]);
+      const float dd = bn_pre(xh, g[e], b[e]) > 0.f ? d[e] : 0.f;
+      d[e] = (dd - k1[e] - xh * k2[e]) * (g[e] * rs[e]);
+    }
+    store8<T>(dx + i * 8, d);
   }
 }
 
@@ -825,16 +1041,89 @@ int lgb200_colsum(const void* a, float* out, float* ws, unsigned* counters, int6
                   cudaStream_t stream) {
   LGB_REQUIRE(a && out && ws && counters && rows > 0 && cols > 0, kErrInvalid, "colsum: bad arguments");
   LGB_REQUIRE(cols % 8 == 0, kErrInvalid, "colsum: cols must be a multiple of 8");
-  const int nslabs = lgb200_colsum_slabs(rows, cols);
-  const int rps = (int)((rows + nslabs - 1) / nslabs);
-  dim3 grid((cols + 63) / 64, nslabs);
   if (dtype == LGB200_F32)
-    colsum_kernel<float><<<grid, 256, 0, stream>>>((const float*)a, ws, out, counters, rows, cols, rps);
+    return colsum_launch(ColsumPlain<float>{(const float*)a}, out, ws, counters, rows, cols, stream);
+  if (dtype == LGB200_BF16)
+    return colsum_launch(ColsumPlain<__nv_bfloat16>{(const __nv_bfloat16*)a}, out, ws, counters, rows, cols, stream);
+  LGB_REQUIRE(false, kErrInvalid, "colsum: bad dtype %d", dtype);
+}
+
+static bool bn_channels_ok(int C) { return C >= 8 && C <= kBnMaxC && (C & (C - 1)) == 0; }
+
+static unsigned bn_apply_grid(int64_t ntok, int C) {
+  const int64_t blocks = (ntok * (C / 8) + 255) / 256, cap = 8 * (int64_t)device_sm_count();
+  return (unsigned)(blocks < cap ? blocks : cap);
+}
+
+int lgb200_bn_stats(const void* x, double* sums, double* ws, unsigned* counters, int64_t ntok, int C, int dtype,
+                    cudaStream_t stream) {
+  LGB_REQUIRE(x && sums && ws && counters && ntok > 0, kErrInvalid, "bn_stats: bad arguments");
+  LGB_REQUIRE(bn_channels_ok(C), kErrUnsupported, "bn_stats: C=%d is not a power of two in [8, %d]", C, kBnMaxC);
+  LGB_REQUIRE(aligned16({x}), kErrInvalid, "bn_stats: misaligned pointer (16 bytes needed)");
+  if (dtype == LGB200_F32) return colsum_launch(BnStats<float>{(const float*)x}, sums, ws, counters, ntok, C, stream);
+  if (dtype == LGB200_BF16)
+    return colsum_launch(BnStats<__nv_bfloat16>{(const __nv_bfloat16*)x}, sums, ws, counters, ntok, C, stream);
+  LGB_REQUIRE(false, kErrInvalid, "bn_stats: bad dtype %d", dtype);
+}
+
+int lgb200_bn_relu_fwd(const void* x, const double* sums, const float* gamma, const float* beta, float* running_mean,
+                       float* running_var, float momentum, float eps, void* y, float* save_mean, float* save_rstd,
+                       int64_t ntok, int C, int dtype, cudaStream_t stream) {
+  LGB_REQUIRE(x && gamma && beta && y && save_mean && save_rstd && ntok > 0, kErrInvalid, "bn_relu_fwd: bad arguments");
+  LGB_REQUIRE((running_mean == nullptr) == (running_var == nullptr), kErrInvalid,
+              "bn_relu_fwd: running_mean / running_var must both be set or both be null");
+  LGB_REQUIRE(sums || running_mean, kErrInvalid, "bn_relu_fwd: eval mode needs the running statistics");
+  LGB_REQUIRE(bn_channels_ok(C), kErrUnsupported, "bn_relu_fwd: C=%d is not a power of two in [8, %d]", C, kBnMaxC);
+  LGB_REQUIRE(aligned16({x, y}), kErrInvalid, "bn_relu_fwd: misaligned pointer (16 bytes needed)");
+  const unsigned grid = bn_apply_grid(ntok, C);
+  if (dtype == LGB200_F32)
+    bn_relu_fwd_kernel<float><<<grid, 256, 0, stream>>>((const float*)x, sums, gamma, beta, running_mean, running_var,
+                                                        momentum, eps, (float*)y, save_mean, save_rstd, ntok, C);
   else if (dtype == LGB200_BF16)
-    colsum_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16*)a, ws, out, counters, rows, cols, rps);
+    bn_relu_fwd_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16*)x, sums, gamma, beta,
+                                                                running_mean, running_var, momentum, eps,
+                                                                (__nv_bfloat16*)y, save_mean, save_rstd, ntok, C);
   else
-    LGB_REQUIRE(false, kErrInvalid, "colsum: bad dtype %d", dtype);
-  return check_launch("colsum");
+    LGB_REQUIRE(false, kErrInvalid, "bn_relu_fwd: bad dtype %d", dtype);
+  return check_launch("bn_relu_fwd");
+}
+
+int lgb200_bn_relu_bwd_reduce(const void* dy, const void* x, const float* gamma, const float* beta, const float* mean,
+                              const float* rstd, double* sums, double* ws, unsigned* counters, int64_t ntok, int C,
+                              int dtype, cudaStream_t stream) {
+  LGB_REQUIRE(dy && x && gamma && beta && mean && rstd && sums && ws && counters && ntok > 0, kErrInvalid,
+              "bn_relu_bwd_reduce: bad arguments");
+  LGB_REQUIRE(bn_channels_ok(C), kErrUnsupported, "bn_relu_bwd_reduce: C=%d is not a power of two in [8, %d]", C,
+              kBnMaxC);
+  LGB_REQUIRE(aligned16({dy, x}), kErrInvalid, "bn_relu_bwd_reduce: misaligned pointer (16 bytes needed)");
+  if (dtype == LGB200_F32)
+    return colsum_launch(BnReluBwdSums<float>{(const float*)dy, (const float*)x, mean, rstd, gamma, beta}, sums, ws,
+                         counters, ntok, C, stream);
+  if (dtype == LGB200_BF16)
+    return colsum_launch(BnReluBwdSums<__nv_bfloat16>{(const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, mean, rstd,
+                                                      gamma, beta},
+                         sums, ws, counters, ntok, C, stream);
+  LGB_REQUIRE(false, kErrInvalid, "bn_relu_bwd_reduce: bad dtype %d", dtype);
+}
+
+int lgb200_bn_relu_bwd(const void* dy, const void* x, const float* gamma, const float* beta, const float* mean,
+                       const float* rstd, const double* sums, const double* count, void* dx, int64_t ntok, int C,
+                       int dtype, cudaStream_t stream) {
+  LGB_REQUIRE(dy && x && gamma && beta && mean && rstd && dx && ntok > 0, kErrInvalid, "bn_relu_bwd: bad arguments");
+  LGB_REQUIRE((sums == nullptr) == (count == nullptr), kErrInvalid, "bn_relu_bwd: sums / count must both be set or null");
+  LGB_REQUIRE(bn_channels_ok(C), kErrUnsupported, "bn_relu_bwd: C=%d is not a power of two in [8, %d]", C, kBnMaxC);
+  LGB_REQUIRE(aligned16({dy, x, dx}), kErrInvalid, "bn_relu_bwd: misaligned pointer (16 bytes needed)");
+  const unsigned grid = bn_apply_grid(ntok, C);
+  if (dtype == LGB200_F32)
+    bn_relu_bwd_kernel<float><<<grid, 256, 0, stream>>>((const float*)dy, (const float*)x, gamma, beta, mean, rstd,
+                                                        sums, count, (float*)dx, ntok, C);
+  else if (dtype == LGB200_BF16)
+    bn_relu_bwd_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x,
+                                                                gamma, beta, mean, rstd, sums, count,
+                                                                (__nv_bfloat16*)dx, ntok, C);
+  else
+    LGB_REQUIRE(false, kErrInvalid, "bn_relu_bwd: bad dtype %d", dtype);
+  return check_launch("bn_relu_bwd");
 }
 
 int lgb200_residual_add_cast_pitched(const float* x, const void* y, float* x_out, void* x_cast, int64_t rows,

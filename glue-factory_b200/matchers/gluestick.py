@@ -16,8 +16,12 @@ node features are token-major [B*N, D] like in the LightGlue plugin, so
   * the assignment is `log_double_softmax` with a learnt bin (gluestick.py:772-783) on the similarity produced by the
     batched wgmma GEMM: forward kernels + closed-form backward (`ops.log_double_softmax`, heads_grad.py);
   * match filtering (`_get_matches`, gluestick.py:318-331) is `filter_matches_kernel`;
-  * BatchNorm1d (training-mode batch statistics, running-stat update), the LineLayer's gather / scatter-mean over
-    junctions and the O(lines^2) line-score gathers are torch ops.
+  * every BatchNorm1d and the ReLU behind it are one fused pair of kernels (`ops.batchnorm_relu`): a deterministic fp64
+    statistics pass, then normalisation + ReLU + the running-stat update on the device; the backward likewise.  Under
+    glue-factory's distributed trainer the BatchNorms are `nn.SyncBatchNorm` (train.py:337-339, convert_sync_batchnorm
+    before the DDP wrap): their statistics and backward sums are then all-reduced over the module's process group
+    between the two passes, so every rank normalises with the global batch's statistics like the reference;
+  * the LineLayer's gather / scatter-mean over junctions and the O(lines^2) line-score gathers are torch ops.
 `precision: "bf16"` (default) rounds GEMM / attention operands to bf16 (the reference forces its attention to fp32,
 gluestick.py:17-22; the fp32 mode reproduces that); `precision: "fp32"` is the parity path (fp32 cuBLAS linears,
 CUDA-core attention).  No CPU fallback.
@@ -27,6 +31,7 @@ Not built (raise NotImplementedError): `line_attention`, `inter_supervision`, in
 import torch
 import torch.nn.functional as F
 from torch import nn
+from torch.nn.modules.batchnorm import _BatchNorm
 
 from .. import _lib, ops
 from .lightglue import _Conf, _merge, _to_plain, matcher_metrics
@@ -193,11 +198,14 @@ class GlueStick(nn.Module):
         for i, m in enumerate(mods):
             if isinstance(m, nn.Conv1d):
                 # an inner layer's output only feeds BatchNorm / ReLU and the next GEMM, which rounds it to bf16 at the
-                # same point either way: keep it bf16 (BatchNorm still accumulates its statistics in fp32)
+                # same point either way: keep it bf16 (BatchNorm still accumulates its statistics in fp64)
                 x = self._conv(x, m, keep_bf16=self._bf16 and i < len(mods) - 1)
-            elif isinstance(m, nn.BatchNorm1d):
-                x = m(x if x.dtype == torch.bfloat16 else x.float())  # [T, C]: statistics over all tokens of this call
-            else:
+            elif isinstance(m, _BatchNorm):
+                # BatchNorm1d, or SyncBatchNorm after convert_sync_batchnorm (statistics summed over its process
+                # group), fused with the ReLU that MLP() puts behind it; [T, C]: statistics over all tokens of this call
+                assert isinstance(mods[i + 1], nn.ReLU), mods[i + 1]
+                x = ops.batchnorm_relu(x if x.dtype == torch.bfloat16 else x.float(), m, ops.bn_exchange(m))
+            elif not isinstance(mods[i - 1], _BatchNorm):
                 x = torch.relu(x)
         return x
 

@@ -218,6 +218,15 @@ def mask_counts(mask_u8):
     return rowcnt, colcnt
 
 
+def _colsum_counter(dev, cols):
+    """Self-resetting arrival counters of the column-sum kernels, zeroed once per device."""
+    cnt = _colsum_counters.get(dev)
+    if cnt is None:
+        cnt = _colsum_counters[dev] = torch.zeros(64, device=dev, dtype=torch.int32)
+    assert cols <= 64 * 64
+    return cnt
+
+
 def colsum(a):
     """[rows, cols] (fp32 / bf16) -> fp32 [cols] column sums (bias gradients); one launch."""
     _chk(a)
@@ -225,14 +234,130 @@ def colsum(a):
     if cols % 8:
         return a.sum(0, dtype=torch.float32)
     dev = a.device
-    cnt = _colsum_counters.get(dev)
-    if cnt is None:  # self-resetting arrival counters, zeroed once per device
-        cnt = _colsum_counters[dev] = torch.zeros(64, device=dev, dtype=torch.int32)
-    assert cols <= 64 * 64
+    cnt = _colsum_counter(dev, cols)
     out = torch.empty(cols, device=dev, dtype=torch.float32)
     ws = torch.empty(_lib.load().lgb200_colsum_slabs(rows, cols) * cols, device=dev, dtype=torch.float32)
     call("lgb200_colsum", ptr(a), ptr(out), ptr(ws), ptr(cnt), rows, cols, _code(a.dtype), stream_ptr())
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# BatchNorm1d + ReLU (GlueStick MLPs, gluestick.py:465-475), statistics optionally summed across ranks
+# ------------------------------------------------------------------------------------------------
+def _bn_ws(T, C, dev):
+    return torch.empty(_lib.load().lgb200_colsum_slabs(T, C) * 2 * C, device=dev, dtype=torch.float64)
+
+
+def bn_stats(x):
+    """x [T, C] -> fp64 [2C+1] = [sum x | sum x^2 | T] per channel (lgb200_bn_stats)."""
+    _chk(x)
+    T, C = x.shape
+    sums = torch.empty(2 * C + 1, device=x.device, dtype=torch.float64)
+    # both held until the launch: a temporary freed inside the argument list could be handed to the other
+    cnt, ws = _colsum_counter(x.device, C), _bn_ws(T, C, x.device)
+    call("lgb200_bn_stats", ptr(x), ptr(sums), ptr(ws), ptr(cnt), T, C, _code(x.dtype), stream_ptr())
+    return sums
+
+
+def bn_relu_fwd(x, sums, weight, bias, running_mean, running_var, momentum, eps):
+    """y = relu(batch_norm(x)) with the statistics in `sums` (bn_stats, possibly summed across ranks; the running
+    statistics are updated in place) or, when sums is None, the running statistics.  Returns y, mean, rstd [C]."""
+    _chk(x), _chk(weight, torch.float32), _chk(bias, torch.float32)
+    for t in (running_mean, running_var):
+        if t is not None:
+            _chk(t, torch.float32)
+    T, C = x.shape
+    y = torch.empty_like(x)
+    mean = torch.empty(C, device=x.device, dtype=torch.float32)
+    rstd = torch.empty_like(mean)
+    call("lgb200_bn_relu_fwd", ptr(x), ptr(sums), ptr(weight), ptr(bias), ptr(running_mean), ptr(running_var),
+         float(momentum), float(eps), ptr(y), ptr(mean), ptr(rstd), T, C, _code(x.dtype), stream_ptr())
+    return y, mean, rstd
+
+
+def bn_relu_bwd_reduce(dy, x, weight, bias, mean, rstd):
+    """fp64 [2C] = [sum dy' | sum dy' xhat] with dy' = dy [relu output > 0]: dbeta and dgamma of these rows."""
+    _chk(dy, x.dtype), _chk(x)
+    T, C = x.shape
+    sums = torch.empty(2 * C, device=x.device, dtype=torch.float64)
+    cnt, ws = _colsum_counter(x.device, C), _bn_ws(T, C, x.device)
+    call("lgb200_bn_relu_bwd_reduce", ptr(dy), ptr(x), ptr(weight), ptr(bias), ptr(mean), ptr(rstd), ptr(sums), ptr(ws),
+         ptr(cnt), T, C, _code(x.dtype), stream_ptr())
+    return sums
+
+
+def bn_relu_bwd(dy, x, weight, bias, mean, rstd, sums, count):
+    """dx from the (possibly summed across ranks) backward sums and the count behind the forward statistics (a 1-element
+    fp64 view); sums = count = None: eval mode."""
+    _chk(dy, x.dtype), _chk(x)
+    T, C = x.shape
+    dx = torch.empty_like(x)
+    call("lgb200_bn_relu_bwd", ptr(dy), ptr(x), ptr(weight), ptr(bias), ptr(mean), ptr(rstd), ptr(sums), ptr(count),
+         ptr(dx), T, C, _code(x.dtype), stream_ptr())
+    return dx
+
+
+class BnRelu(torch.autograd.Function):
+    """relu(batch_norm(x)) on token-major x [T, C] (fp32 or bf16, C a power of two <= 512), statistics over all T rows.
+    `exchange`: None, or a callable that sums an fp64 vector in place over the ranks that share the statistics; it is
+    called once in forward on [sum x | sum x^2 | count] and once in backward on [sum dy' | sum dy' xhat].  dgamma and
+    dbeta come from this rank's sums (the gradient all-reduce adds the other ranks'), dx from the exchanged ones."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, running_mean, running_var, training, momentum, eps, exchange):
+        x = x.contiguous()
+        w, b = weight.detach().float().contiguous(), bias.detach().float().contiguous()
+        sums = None
+        if training:
+            if exchange is None and x.shape[0] < 2:
+                raise ValueError(f"Expected more than 1 value per channel when training, got input size {tuple(x.shape)}")
+            sums = bn_stats(x)
+            if exchange is not None:
+                exchange(sums)
+        y, mean, rstd = bn_relu_fwd(x, sums, w, b, running_mean, running_var, momentum, eps)
+        ctx.save_for_backward(x, w, b, mean, rstd, sums)
+        ctx.exchange = exchange
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w, b, mean, rstd, sums = ctx.saved_tensors
+        dy = dy.to(x.dtype).contiguous()
+        C = x.shape[1]
+        red = bn_relu_bwd_reduce(dy, x, w, b, mean, rstd)
+        dbeta, dgamma = red[:C].float(), red[C:].float()  # copies: taken before the exchange
+        count = None
+        if sums is not None:
+            if ctx.exchange is not None:
+                ctx.exchange(red)
+            count = sums[2 * C:]
+        dx = bn_relu_bwd(dy, x, w, b, mean, rstd, red if sums is not None else None, count)
+        return dx, dgamma, dbeta, None, None, None, None, None, None
+
+
+def bn_exchange(bn):
+    """The cross-rank sum for the statistics of BatchNorm module `bn`: an in-place all_reduce over its process group
+    (WORLD when unset) when it is a training nn.SyncBatchNorm and that group has more than one rank, else None."""
+    import torch.distributed as dist
+
+    if not (isinstance(bn, torch.nn.SyncBatchNorm) and bn.training and dist.is_available() and dist.is_initialized()):
+        return None
+    group = bn.process_group if bn.process_group is not None else dist.group.WORLD
+    if dist.get_world_size(group) < 2:
+        return None
+    return lambda t: dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
+
+
+def batchnorm_relu(x, bn, exchange=None):
+    """relu(bn(x)) for an nn.BatchNorm1d / nn.SyncBatchNorm `bn` on token-major x [T, C], with the module's semantics:
+    batch statistics in training mode (or without running statistics), running statistics in eval mode; a training call
+    updates running_mean / running_var and num_batches_tracked.  `exchange` as in BnRelu (see bn_exchange)."""
+    if bn.momentum is None or not bn.affine:
+        raise NotImplementedError("gluefactory_b200 batchnorm_relu: momentum=None and affine=False are not built")
+    rm, rv = (bn.running_mean, bn.running_var) if bn.track_running_stats else (None, None)
+    if bn.training and bn.track_running_stats:
+        bn.num_batches_tracked.add_(1)
+    return BnRelu.apply(x, bn.weight, bn.bias, rm, rv, bn.training or rm is None, bn.momentum, bn.eps, exchange)
 
 
 def residual_add_cast(x, y, cdt, want_sum=True, out_cast=None):

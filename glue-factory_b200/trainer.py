@@ -166,11 +166,18 @@ class MatcherTrainer:
     `loss_scale`: None (default; bf16 needs no loss scaling) or an initial GradScaler scale (train.py:456, 490):
     the loss is multiplied by the device-resident scale, the gradients are un-scaled inside the Adam kernel and the
     scale follows torch.amp.GradScaler.update.  `lr_scaling`: the reference's LR groups (train.py:353-361).
-    `ground_truth`: device label generator (SURVEY 8f row 1), so a batch needs only keypoints, descriptors and H."""
+    `ground_truth`: device label generator (SURVEY 8f row 1), so a batch needs only keypoints, descriptors and H.
+    `sync_batchnorm`: at world size > 1, convert the model's BatchNorms to nn.SyncBatchNorm over `process_group` (as
+    train.py:337-339 does before the DDP wrap), so that they normalise with the statistics of the global batch;
+    `self.model` is the converted module."""
 
     def __init__(self, model, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, process_group=None,
                  loss_scale=None, growth_factor=2.0, backoff_factor=0.5, growth_interval=2000, lr_scaling=None,
-                 ground_truth=None):
+                 ground_truth=None, sync_batchnorm=False):
+        self.group = process_group
+        self.world = dist.get_world_size(process_group) if dist.is_available() and dist.is_initialized() else 1
+        if sync_batchnorm and self.world > 1:  # before FlatParams: the converted modules keep the same Parameters
+            model = torch.nn.SyncBatchNorm.convert_sync_batchnorm(model, process_group)
         self.model = model.train()
         # optional label generator run at the top of every step on the device (two_view_pipeline.py:98-100 runs the
         # `ground_truth` component inside loss()): a module data -> {matches0, matches1, assignment, ...}, e.g.
@@ -181,8 +188,6 @@ class MatcherTrainer:
         self.m = torch.zeros_like(self.fp.flat)
         self.v = torch.zeros_like(self.fp.flat)
         self.betas, self.eps, self.wd = betas, eps, weight_decay
-        self.group = process_group
-        self.world = dist.get_world_size(process_group) if dist.is_available() and dist.is_initialized() else 1
         self.fp.world, self.fp.group = self.world, process_group
         layers = getattr(model, "transformers", None)
         if layers is not None and getattr(getattr(model, "conf", None), "engine", None) == "fused":

@@ -237,6 +237,32 @@ int lgb200_mask_counts(const uint8_t* mask, float* rowcnt, float* colcnt, int B,
 int lgb200_colsum(const void* a, float* out, float* ws, unsigned* counters, int64_t rows, int cols, int dtype,
                   cudaStream_t stream);
 
+/* ---- BatchNorm1d + ReLU (GlueStick MLPs, gluestick.py:465-475; nn.SyncBatchNorm under data parallelism) ----------
+ * x, y, dy, dx token-major [ntok, C] in `dtype`, C a power of two in [8, 512]; gamma, beta, mean, rstd, running
+ * statistics fp32 [C].  The statistics pass and the normalisation pass are separate calls so that the fp64 sum vectors
+ * can be summed across ranks in between.  ws: lgb200_colsum_slabs(ntok, C) * 2 * C doubles, counters as for
+ * lgb200_colsum (both may be shared with it on one stream).  Deterministic: fixed summation order, no float atomics.
+ *   bn_stats          : sums [2C+1] = [sum x | sum x^2 | ntok] (fp64)
+ *   bn_relu_fwd       : y = relu((x - mean) rstd gamma + beta) with mean / biased variance from `sums` (training mode;
+ *                       the count is sums[2C]) or, when sums is NULL, from running_mean / running_var (eval mode).
+ *                       save_mean / save_rstd [C] receive the mean and rstd used.  Training mode also updates
+ *                       running_mean / running_var (may be NULL) with `momentum`, the variance unbiased by the count.
+ *   bn_relu_bwd_reduce: sums [2C] = [sum dy' | sum dy' xhat], dy' = dy [pre-activation > 0]: dbeta and dgamma.
+ *   bn_relu_bwd       : dx = gamma rstd (dy' - sums[0:C] / n - xhat sums[C:2C] / n), n = *count (the forward sums'
+ *                       last element); sums = count = NULL (eval mode): dx = gamma rstd dy'.
+ * x, y, dy and dx must be 16-byte aligned. */
+int lgb200_bn_stats(const void* x, double* sums, double* ws, unsigned* counters, int64_t ntok, int C, int dtype,
+                    cudaStream_t stream);
+int lgb200_bn_relu_fwd(const void* x, const double* sums, const float* gamma, const float* beta, float* running_mean,
+                       float* running_var, float momentum, float eps, void* y, float* save_mean, float* save_rstd,
+                       int64_t ntok, int C, int dtype, cudaStream_t stream);
+int lgb200_bn_relu_bwd_reduce(const void* dy, const void* x, const float* gamma, const float* beta, const float* mean,
+                              const float* rstd, double* sums, double* ws, unsigned* counters, int64_t ntok, int C,
+                              int dtype, cudaStream_t stream);
+int lgb200_bn_relu_bwd(const void* dy, const void* x, const float* gamma, const float* beta, const float* mean,
+                       const float* rstd, const double* sums, const double* count, void* dx, int64_t ntok, int C,
+                       int dtype, cudaStream_t stream);
+
 /* ---- flat-buffer optimiser (train.py:358-361, 513) and casts --------------------------------------- */
 /* Adam over the flat buffers, one launch.  g is multiplied by grad_scale (1/world for the summed all-reduce).
  * step: 1-based step count for the bias correction; the four *_dev pointers (each may be NULL) move the per-step

@@ -106,3 +106,19 @@ if os.environ.get("PROF"):
     print(f"plugin bf16: total device time {tot / 1e3:.2f} ms over {sum(e.count for e in evs)} launches")
     for e in evs[:32]:
         print(f"  {e.device_time_total:9.0f} us {100 * e.device_time_total / tot:5.1f}% x{e.count:4d}  {e.key[:110]}")
+    # BatchNorm + ReLU: the library's fused kernels, or torch's batch_norm + relu (clamp) + relu backward (threshold).
+    # Bytes the fused two-pass scheme needs per call: forward reads x twice and writes y, backward reads x and dy twice
+    # and writes dx: 8 T C element sizes.  Calls per image (bf16 mode): keypoint / line-endpoint encoders at C = 32, 64
+    # (fp32 linears in front) and 128, 256 (bf16), one C = 512 BatchNorm per GNN layer (B N tokens) and per line layer
+    # (B 2L tokens).
+    n_gnn = len(conf["GNN_layers"])
+    calls = [(T, C, 4 if C <= 64 else 2) for T in (B * N, B * 2 * L) for C in conf["keypoint_encoder"]]
+    calls += [(B * N, 2 * conf["descriptor_dim"], 2)] * n_gnn + [(B * 2 * L, 2 * conf["descriptor_dim"], 2)] * (n_gnn // 2)
+    bn_bytes = 2 * sum(8 * T * C * s for T, C, s in calls)  # both images
+    pat = ("BnStats", "BnReluBwdSums", "bn_relu_", "batch_norm", "clamp_scalar", "threshold")
+    bn = [e for e in evs if any(p in e.key for p in pat)]
+    t_bn = sum(e.device_time_total for e in bn)
+    print(f"BatchNorm+ReLU: {t_bn / 1e3:.3f} ms device time over {sum(e.count for e in bn)} launches "
+          f"({2 * len(calls)} BatchNorm calls), {bn_bytes / 1e9:.3f} GB needed -> {bn_bytes / (t_bn * 1e-6) / 1e9:.0f} GB/s")
+    for e in bn:
+        print(f"  {e.device_time_total:9.0f} us x{e.count:4d}  {e.key[:110]}")
