@@ -16,6 +16,7 @@ _lib = None
 _device_checked = False
 
 _vp, _i, _i64, _f, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_size_t
+_d = ctypes.c_double
 
 # name -> (restype, argtypes); mirrors include/lgb200.h one to one
 SIGNATURES = {
@@ -58,6 +59,10 @@ SIGNATURES = {
     "lgb200_gt_from_homography": (_i, [_vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "lgb200_gt_from_reprojection": (_i, [_vp] * 8 + [_f, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "lgb200_gt_epipolar_unmatched": (_i, [_vp] * 5 + [_f, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "lgb200_gt_line_sample": (_i, [_vp, _vp, _i, _i, _i, _vp]),
+    "lgb200_lsap": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
+    "lgb200_gt_lines_ws_bytes": (_sz, [_i, _i, _i]),
+    "lgb200_gt_line_matches": (_i, [_vp] * 10 + [_i] * 5 + [_d] * 3 + [_vp] * 4 + [_i, _i, _i, _vp]),
     "lgb200_adam_flat": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _i, _vp, _f, _vp, _vp, _vp, _vp]),
     "lgb200_flat_grad_check": (_i, [_vp, _i64, _vp, _vp]),
     "lgb200_amp_update": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _vp]),
@@ -115,7 +120,7 @@ KERNELS_PER_CALL = {
     "lgb200_ln_gelu_fwd": 1, "lgb200_ln_gelu_bwd": 1, "lgb200_gemm_bf16": 1, "lgb200_assign_lse": 2,
     "lgb200_assign_scores": 2, "lgb200_assign_bwd": 1, "lgb200_filter_matches": 1, "lgb200_log_double_softmax": 3,
     "lgb200_adam_flat": 1, "lgb200_cast_bf16": 1, "lgb200_colsum": 1, "lgb200_residual_add_cast": 1,
-    "lgb200_gemm_bf16_splitk": 2, "lgb200_gt_from_homography": 3, "lgb200_gt_from_reprojection": 3, "lgb200_gt_epipolar_unmatched": 2, "lgb200_flat_grad_check": 1, "lgb200_amp_update": 1,
+    "lgb200_gemm_bf16_splitk": 2, "lgb200_gt_from_homography": 3, "lgb200_gt_from_reprojection": 3, "lgb200_gt_epipolar_unmatched": 2, "lgb200_gt_line_matches": 5, "lgb200_flat_grad_check": 1, "lgb200_amp_update": 1,
 }
 launch_count = 0          # running total of kernels launched through `call`
 timed_entry = None        # entry-point name or a set of names: every call of them is bracketed by CUDA events

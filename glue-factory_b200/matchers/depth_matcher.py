@@ -12,6 +12,12 @@ duck-typed: `.image2cam`, `.cam2image`, `.calibration_matrix`, `.transform`, `.i
 geometry/depth.py:21-85.  The distance matrix, mutual nearest neighbours, thresholds and the epipolar exclusion --
 everything the reference builds ~15 dense [B, M, N] temporaries for -- run in `lgb200_gt_from_reprojection` /
 `lgb200_gt_epipolar_unmatched` without any dense temporary.
+
+With `use_lines` the line labels (`line_matches0/1`, `line_assignment`) of `gt_line_matches_from_pose_depth`
+(gt_generation.py:207-406) are added: the sampled line points go through the same `sample_depth` / `project` as the
+keypoints, and the point-segment counting, the per-pair linear assignment (scipy's, on the host, in the reference)
+and the labels run in csrc/gt_lines.cu without a host synchronisation.  Segments are clamped to `view*["depth"]`, the
+"outside" test uses `view*["image"]`, and the reverse projection uses `T_0to1.inv()`, as in the reference (:286).
 """
 import torch
 import torch.nn.functional as F
@@ -82,16 +88,17 @@ class DepthMatcher(nn.Module):
         if conf.use_points:
             self.required_data_keys += ["keypoints0", "keypoints1"]
         if conf.use_lines:
-            raise NotImplementedError("gluefactory_b200 depth_matcher: line ground truth is not implemented")
+            self.required_data_keys += ["lines0", "lines1", "valid_lines0", "valid_lines1"]
 
     @torch.no_grad()
     def forward(self, data):
         for key in self.required_data_keys:
             assert key in data, f"Missing key {key} in data"
-        if not self.conf.use_points:
-            return {}
         with torch.autocast(device_type="cuda", enabled=False):  # reference: custom_fwd(cast_inputs=float32)
-            return self._labels(data)
+            result = self._labels(data) if self.conf.use_points else {}
+            if self.conf.use_lines:
+                result.update(self._line_labels(data))
+        return result
 
     def _labels(self, data):
         conf = self.conf
@@ -124,6 +131,22 @@ class DepthMatcher(nn.Module):
                     "depth_keypoints0": d0, "depth_keypoints1": d1, "proj_0to1": kp0_1, "proj_1to0": kp1_0,
                     "visible0": visible0, "visible1": visible1})
         return out
+
+    def _line_labels(self, data):
+        conf, npts = self.conf, self.conf.n_line_sampled_pts
+        v0, v1 = data["view0"], data["view1"]
+        segs0 = ops.line_segments(data["lines0"], *v0["depth"].shape[-2:])
+        segs1 = ops.line_segments(data["lines1"], *v1["depth"].shape[-2:])
+        pts0, pts1 = ops.sample_line_points(segs0, npts), ops.sample_line_points(segs1, npts)
+        d0, valid0 = sample_depth(pts0, v0["depth"])
+        d1, valid1 = sample_depth(pts1, v1["depth"])
+        T_0to1 = data["T_0to1"]
+        pts0_1, visible0 = project(pts0, d0, v1["depth"], v0["camera"], v1["camera"], T_0to1, valid0)
+        pts1_0, visible1 = project(pts1, d1, v0["depth"], v1["camera"], v0["camera"], T_0to1.inv(), valid1)
+        return ops.gt_line_matches_from_projection(
+            segs0, segs1, pts0_1, pts1_0, v0["image"].shape[-2:], v1["image"].shape[-2:], data["valid_lines0"],
+            data["valid_lines1"], visible0, visible1, valid0, valid1, npts=npts, dist_th=conf.line_perp_dist_th,
+            overlap_th=conf.overlap_th, min_visibility_th=conf.min_visibility_th)
 
     def loss(self, pred, data):
         raise NotImplementedError

@@ -657,6 +657,92 @@ def gt_epipolar_unmatched_(kp0, kp1, F, valid0, valid1, m0, m1, th):
          B, M, N, stream_ptr())
 
 
+def line_segments(lines, h, w):
+    """Lines [B,L,2,2], [B,L,4] or [B,L,K,2] (first and last point) -> [B,L,4] fp32 segments clamped to [0, w-1] x
+    [0, h-1] (geometry/gt_generation.py:430-448)."""
+    if lines.shape[-2:] == (2, 2):
+        lines = lines.flatten(-2)
+    elif lines.dim() == 4:
+        lines = torch.cat([lines[:, :, 0], lines[:, :, -1]], dim=2)
+    if lines.shape[1] == 0:
+        raise ValueError("line ground truth needs at least one line per view")
+    x, y = lines.float()[..., 0::2].clamp(0, w - 1), lines.float()[..., 1::2].clamp(0, h - 1)  # no host tensor: capturable
+    return torch.stack([x[..., 0], y[..., 0], x[..., 1], y[..., 1]], -1).contiguous()
+
+
+def sample_line_points(segs, npts):
+    """segs [B,L,4] -> [B, L*npts, 2]: npts points evenly spaced from start to end (sample_pts, :164-170)."""
+    _chk(segs, torch.float32)
+    B, L = segs.shape[:2]
+    pts = torch.empty(B, L * npts, 2, device=segs.device, dtype=torch.float32)
+    call("lgb200_gt_line_sample", ptr(segs), ptr(pts), B, L, int(npts), stream_ptr())
+    return pts
+
+
+def linear_sum_assignment(cost):
+    """cost [B,rows,cols] float64 (finite) -> (row2col [B,rows], col2row [B,cols]) int32, -1 where unassigned: the
+    minimum-cost assignment scipy.optimize.linear_sum_assignment returns for each matrix, ties included."""
+    cost = _chk(cost.contiguous(), torch.float64)
+    B, R, C = cost.shape
+    row2col = torch.empty(B, R, device=cost.device, dtype=torch.int32)
+    col2row = torch.empty(B, C, device=cost.device, dtype=torch.int32)
+    call("lgb200_lsap", ptr(cost), ptr(row2col), ptr(col2row), B, R, C, stream_ptr())
+    return row2col, col2row
+
+
+def gt_line_matches_from_projection(segs0, segs1, pts0_1, pts1_0, size0, size1, valid_lines0, valid_lines1,
+                                    visible0=None, visible1=None, valid_pts0=None, valid_pts1=None, npts=50, dist_th=5,
+                                    overlap_th=0.2, min_visibility_th=0.5, return_cost=False):
+    """The O(L0 L1 npts) label pass and the assignment of the line ground truth (gt_generation.py:173-204, 290-406,
+    460-558) for given projections.  segs0/1 [B,L,4]: clamped segments (line_segments); pts0_1 [B,L0*npts,2]: the
+    sampled points of segs0 projected into view 1, whose image is size1 = (h1, w1) (pts1_0, size0 likewise).
+    visible0/1, valid_pts0/1 [B,L*npts] bool: visibility in the other view and valid depth of each point, all None in
+    the homography variant.  Returns {line_assignment bool [B,L0,L1], line_matches0/1 int64 (partner, -1 unmatched, -2
+    ignored)}, plus `cost` (the float64 matrix given to the assignment) when return_cost."""
+    segs0, segs1 = _chk(segs0.contiguous(), torch.float32), _chk(segs1.contiguous(), torch.float32)
+    pts0_1, pts1_0 = pts0_1.float().contiguous(), pts1_0.float().contiguous()
+    B, L0, L1 = segs0.shape[0], segs0.shape[1], segs1.shape[1]
+    if L0 == 0 or L1 == 0:
+        raise ValueError("line ground truth needs at least one line per view")
+    assert pts0_1.numel() == B * L0 * npts * 2 and pts1_0.numel() == B * L1 * npts * 2, "points: [B, L*npts, 2]"
+    dev = segs0.device
+    u8 = lambda t: None if t is None else t.to(torch.uint8).contiguous()  # noqa: E731
+    m0 = torch.empty(B, L0, device=dev, dtype=torch.int64)
+    m1 = torch.empty(B, L1, device=dev, dtype=torch.int64)
+    asg = torch.empty(B, L0, L1, device=dev, dtype=torch.bool)
+    ws = torch.empty(_lib.load().lgb200_gt_lines_ws_bytes(B, L0, L1), device=dev, dtype=torch.uint8)
+    (h0, w0), (h1, w1) = (int(s) for s in size0), (int(s) for s in size1)
+    # byte copies held until the launch is queued (a temporary would go back to the allocator before it)
+    vis0, vis1, vp0, vp1, vl0, vl1 = (u8(t) for t in (visible0, visible1, valid_pts0, valid_pts1, valid_lines0,
+                                                      valid_lines1))
+    call("lgb200_gt_line_matches", ptr(segs0), ptr(segs1), ptr(pts0_1), ptr(pts1_0), ptr(vis0), ptr(vis1), ptr(vp0),
+         ptr(vp1), ptr(vl0), ptr(vl1), w0, h0, w1, h1, int(npts),
+         float(dist_th), float(overlap_th), float(min_visibility_th), ptr(m0), ptr(m1), ptr(asg), ptr(ws), B, L0, L1,
+         stream_ptr())
+    out = {"line_assignment": asg, "line_matches0": m0, "line_matches1": m1}
+    if return_cost:
+        out["cost"] = ws[:B * L0 * L1 * 8].view(torch.float64).view(B, L0, L1)
+    return out
+
+
+def gt_line_matches_from_homography(lines0, lines1, valid_lines0, valid_lines1, shape0, shape1, H, npts=50, dist_th=5,
+                                    overlap_th=0.2, min_visibility_th=0.2):
+    """Device-side gt_line_matches_from_homography (geometry/gt_generation.py:409-558; defaults as the reference's).
+    lines [B,L,2,2] / [B,L,4] / [B,L,K,2] in pixels, valid_lines [B,L] bool, shape0/1 (..., h, w) of the images, H
+    [B,3,3] -> {line_assignment, line_matches0, line_matches1}, with no host synchronisation."""
+    from .geometry import inv3x3, warp_points
+
+    (h0, w0), (h1, w1) = tuple(shape0[-2:]), tuple(shape1[-2:])
+    segs0, segs1 = line_segments(lines0, h0, w0), line_segments(lines1, h1, w1)
+    B = segs0.shape[0]
+    Hm = H.float().expand(B, 3, 3) if H.dim() == 2 else H.float()
+    pts0_1 = warp_points(sample_line_points(segs0, npts), Hm)  # O(L npts): homography.py:161-180
+    pts1_0 = warp_points(sample_line_points(segs1, npts), inv3x3(Hm))
+    return gt_line_matches_from_projection(segs0, segs1, pts0_1, pts1_0, (h0, w0), (h1, w1), valid_lines0,
+                                           valid_lines1, npts=npts, dist_th=dist_th, overlap_th=overlap_th,
+                                           min_visibility_th=min_visibility_th)
+
+
 _head_token_counters = {}
 
 

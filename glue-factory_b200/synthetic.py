@@ -341,3 +341,73 @@ class RigidPose:
     def inv(self):
         Rt = self.R.transpose(-1, -2)
         return RigidPose(Rt, -(Rt @ self.t.unsqueeze(-1)).squeeze(-1))
+
+
+# ----------------------------------------------------------------------------
+# line ground truth (use_lines of matchers/homography_matcher.py and matchers/depth_matcher.py)
+# ----------------------------------------------------------------------------
+def _line_pairs(rs, to1, L0, L1, W, H):
+    """View-0 segments and view-1 segments built from them: `to1` maps [n,2] view-0 points into view 1.  View 1 holds
+    the mapped segments with 0.6 px endpoint noise (some shortened, so that they overlap partly), exact and near
+    duplicates (tied costs), distractors, all permuted; 10 % of the segments of each view are flagged invalid.  Some
+    view-0 segments start near the border and run out of the image (clamped), some map outside image 1."""
+    ang = rs.uniform(0, np.pi, L0)
+    length = rs.uniform(15, 160, L0)
+    start = np.stack([rs.uniform(-20, W + 20, L0), rs.uniform(-20, H + 20, L0)], -1)
+    end = start + length[:, None] * np.stack([np.cos(ang), np.sin(ang)], -1)
+    l0 = np.stack([start, end], 1)                                   # [L0, 2, 2]
+    K = min(int(0.6 * L0), L1 - 4)
+    src = l0[:K].copy()
+    cut = rs.uniform(size=K) < 0.3                                   # shortened copies: partial overlap
+    f = rs.uniform(0.5, 0.9, size=(K, 1))
+    src[cut, 1] = src[cut, 0] + f[cut] * (src[cut, 1] - src[cut, 0])
+    m = to1(src.reshape(-1, 2)).reshape(K, 2, 2) + 0.6 * rs.standard_normal((K, 2, 2))
+    nd = min(4, K)
+    dups = m[:nd].copy()
+    dups[nd // 2:] += 0.3 * rs.standard_normal((nd - nd // 2, 2, 2))  # near duplicates; the first half exact
+    nrand = L1 - K - nd
+    a1 = rs.uniform(0, np.pi, nrand)
+    s1 = np.stack([rs.uniform(0, W, nrand), rs.uniform(0, H, nrand)], -1)
+    r1 = np.stack([s1, s1 + rs.uniform(15, 160, (nrand, 1)) * np.stack([np.cos(a1), np.sin(a1)], -1)], 1)
+    l1 = np.concatenate([m, dups, r1])[rs.permutation(L1)]
+    v0, v1 = rs.uniform(size=L0) > 0.1, rs.uniform(size=L1) > 0.1
+    return l0, l1, v0, v1
+
+
+def line_gt_scene(kind, B, L0, L1, seed, W=640, H=480):
+    """Seeded two-view line scene for the line ground truth.  kind "homography": lines0/1 [B,L,2,2], valid_lines0/1,
+    H_0to1 [B,3,3], image_size (H, W).  kind "pose_depth": the camera / plane scene of `pose_depth_scene` (K0, K1, R,
+    t, depth0, depth1) with view-1 segments reprojected through the plane."""
+    rs = np.random.RandomState(seed)
+    out = {k: [] for k in ("lines0", "lines1", "valid_lines0", "valid_lines1")}
+    if kind == "homography":
+        Hs = []
+        for _ in range(B):
+            Hm = _random_homography(rs, 512.0, difficulty=0.5)
+            Hs.append(Hm)
+            to1 = lambda p, Hm=Hm: (lambda q: q[:, :2] / q[:, 2:])(np.concatenate([p, np.ones((len(p), 1))], 1) @ Hm.T)  # noqa: E731
+            for k, v in zip(out, _line_pairs(rs, to1, L0, L1, W, H)):
+                out[k].append(v)
+        extra = {"H_0to1": torch.from_numpy(np.stack(Hs)).float()}
+    elif kind == "pose_depth":
+        extra = pose_depth_scene(B, 1, 1, seed, W=W, H=H)
+        del extra["kp0"], extra["kp1"]
+        n0 = np.array([0.15, -0.1, 1.0]); n0 /= np.linalg.norm(n0)  # the plane of pose_depth_scene
+        for b in range(B):
+            Km, R, t = (extra[k][b].double().numpy() for k in ("K0", "R", "t"))
+            Kinv = np.linalg.inv(Km)
+
+            def to1(p, Kinv=Kinv, Km=Km, R=R, t=t):
+                r0 = np.concatenate([p, np.ones((len(p), 1))], 1) @ Kinv.T
+                X1 = (r0 * (5.0 / (r0 @ n0))[:, None]) @ R.T + t
+                return ((X1 / X1[:, 2:]) @ Km.T)[:, :2]
+            for k, v in zip(out, _line_pairs(rs, to1, L0, L1, W, H)):
+                out[k].append(v)
+    else:
+        raise ValueError(kind)
+    res = {k: torch.from_numpy(np.stack(v)) for k, v in out.items()}
+    for k in ("lines0", "lines1"):
+        res[k] = res[k].float()
+    res.update(extra)
+    res["image_size"] = (H, W)
+    return res

@@ -327,6 +327,32 @@ int lgb200_gt_epipolar_unmatched(const float* kp0, const float* kp1, const float
                                  const uint8_t* valid1, float th, int64_t* m0, int64_t* m1, uint8_t* ws, int B, int M,
                                  int N, cudaStream_t stream);
 
+/* ---- ground-truth line correspondences (gt_line_matches_from_homography / _from_pose_depth,
+ * geometry/gt_generation.py:164-558) -------------------------------------------------------------------------
+ * lgb200_gt_line_sample: lines [B,L,4] (x0, y0, x1, y1; 16-byte aligned) -> pts [B,L,npts,2], point k =
+ * start + ((end - start) / (npts - 1)) * k (sample_pts, :164-170), npts >= 2.                                 */
+int lgb200_gt_line_sample(const float* lines, float* pts, int B, int L, int npts, cudaStream_t stream);
+/* Exact rectangular linear assignment (minimum cost) of B independent [rows, cols] float64 cost matrices (finite),
+ * with the shortest-augmenting-path algorithm and tie rules of scipy.optimize.linear_sum_assignment, so the same
+ * optimum is returned.  row2col [B,rows]: assigned column or -1; col2row [B,cols]: assigned row or -1.  One CTA per
+ * matrix; shared memory ~33 max(rows,cols) + 13 min(rows,cols) bytes (up to 227 KiB).                           */
+int lgb200_lsap(const double* cost, int* row2col, int* col2row, int B, int rows, int cols, cudaStream_t stream);
+/* Labels from projected line points.  lines0 [B,L0,4] / lines1 [B,L1,4]: clamped segments (16-byte aligned);
+ * pts0_1 [B,L0,npts,2]: the points of lines0 projected into view 1 (w1 x h1), pts1_0 the converse.  visible0/1
+ * [B,L*npts] (projected point visible), valid_pts0/1 [B,L*npts] (valid depth at the point): all four NULL for the
+ * homography variant, all four given for the depth variant.  valid_lines0/1 [B,L] bytes.  dist_th, overlap_th,
+ * min_visibility_th as the reference's arguments.  Writes matches0/1 (int64: partner, -1 unmatched, -2 ignored) and,
+ * when assignment is not NULL, the [B,L0,L1] bool positives.  ws: lgb200_gt_lines_ws_bytes(B, L0, L1); on return its
+ * first B*L0*L1 float64 hold the cost matrix handed to the assignment (-close0*close1, 1e6 on unmatched / ignored
+ * rows and columns).  No host synchronisation.                                                                   */
+size_t lgb200_gt_lines_ws_bytes(int B, int L0, int L1);
+int lgb200_gt_line_matches(const float* lines0, const float* lines1, const float* pts0_1, const float* pts1_0,
+                           const uint8_t* visible0, const uint8_t* visible1, const uint8_t* valid_pts0,
+                           const uint8_t* valid_pts1, const uint8_t* valid_lines0, const uint8_t* valid_lines1, int w0,
+                           int h0, int w1, int h1, int npts, double dist_th, double overlap_th,
+                           double min_visibility_th, int64_t* matches0, int64_t* matches1, uint8_t* assignment,
+                           void* ws, int B, int L0, int L1, cudaStream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
