@@ -2,8 +2,6 @@
 // construction (driver entry point fetched through the runtime, no link-time libcuda dependency).
 #include <stdarg.h>
 #include <stdio.h>
-#include <stdlib.h>
-#include <string.h>
 
 #include "common.cuh"
 #include "host_util.h"
@@ -124,11 +122,6 @@ int device_sm_count() {
   return n;
 }
 
-bool env_flag(const char* name) {
-  const char* v = getenv(name);
-  return v && v[0] && strcmp(v, "0") != 0;
-}
-
 }  // namespace lgb
 
 using namespace lgb;
@@ -156,10 +149,8 @@ int lgb200_attn_fwd(const void* q, const void* k, const void* v, void* out, floa
   LGB_REQUIRE(B > 0 && Nq > 0 && Nk > 0 && H > 0, kErrInvalid, "attn_fwd: empty input B=%d Nq=%d Nk=%d H=%d", B, Nq,
               Nk, H);
   LGB_REQUIRE(kv_shift >= 0 && kv_shift < B, kErrInvalid, "attn_fwd: kv_shift %d out of range", kv_shift);
-  if (dtype == LGB200_F32) return attn_fwd_simt<float>(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream);
+  if (dtype == LGB200_F32) return attn_fwd_simt(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream);
   LGB_REQUIRE(dtype == LGB200_BF16, kErrInvalid, "attn_fwd: bad dtype %d", dtype);
-  if (env_flag("LGB200_ATTN_SIMT"))
-    return attn_fwd_simt<__nv_bfloat16>(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream);
   return attn_fwd_tc(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream);
 }
 
@@ -172,14 +163,11 @@ int lgb200_attn_bwd(const void* q, const void* k, const void* v, const void* out
   LGB_REQUIRE(B > 0 && Nq > 0 && Nk > 0 && H > 0, kErrInvalid, "attn_bwd: empty input");
   LGB_REQUIRE(kv_shift >= 0 && kv_shift < B, kErrInvalid, "attn_bwd: kv_shift %d out of range", kv_shift);
   const bool shared_qk = attn_bwd_is_shared_qk(q, k, dq, dk, B, Nq, Nk, kv_shift);
-  LGB_REQUIRE(!shared_qk || (dtype == LGB200_BF16 && !env_flag("LGB200_ATTN_SIMT")), kErrUnsupported,
+  LGB_REQUIRE(!shared_qk || dtype == LGB200_BF16, kErrUnsupported,
               "attn_bwd: dq == dk (shared-qk cross-attention) runs on the bf16 tensor-core path only");
   if (dtype == LGB200_F32)
-    return attn_bwd_simt<float>(q, k, v, out, lse, dout, dq, dk, dv, delta_ws, B, Nq, Nk, H, kv_shift, scale, stream);
+    return attn_bwd_simt(q, k, v, out, lse, dout, dq, dk, dv, delta_ws, B, Nq, Nk, H, kv_shift, scale, stream);
   LGB_REQUIRE(dtype == LGB200_BF16, kErrInvalid, "attn_bwd: bad dtype %d", dtype);
-  if (env_flag("LGB200_ATTN_SIMT"))
-    return attn_bwd_simt<__nv_bfloat16>(q, k, v, out, lse, dout, dq, dk, dv, delta_ws, B, Nq, Nk, H, kv_shift, scale,
-                                        stream);
   return attn_bwd_tc(q, k, v, out, lse, dout, dq, dk, dv, delta_ws, B, Nq, Nk, H, kv_shift, scale, stream);
 }
 

@@ -1,5 +1,5 @@
-// fp32 CUDA-core attention (forward + backward) -- the full-precision parity path
-// (`precision="fp32"`) and the on-device cross-check for the wgmma kernels.
+// fp32 CUDA-core attention (forward + backward) -- the full-precision parity path (`precision="fp32"`).  The bf16
+// wgmma kernels (attn_tc.cu) are tested against fp64 torch, not against this file.
 //
 //   out = softmax(scale * q k^T) v       per (batch, head), head_dim = 64
 // (reference: gluefactory/models/matchers/lightglue.py:118-121 self-attention,
@@ -23,27 +23,18 @@ constexpr int kD = 64;
 constexpr int kHalf = 32;
 constexpr int kTile = 64;  // rows per smem tile == rows per CTA
 
-template <typename T> __device__ __forceinline__ float to_f(T v);
-template <> __device__ __forceinline__ float to_f<float>(float v) { return v; }
-template <> __device__ __forceinline__ float to_f<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
-template <typename T> __device__ __forceinline__ T from_f(float v);
-template <> __device__ __forceinline__ float from_f<float>(float v) { return v; }
-template <> __device__ __forceinline__ __nv_bfloat16 from_f<__nv_bfloat16>(float v) { return __float2bfloat16(v); }
-
 // cooperative load of `rows` x 64 (row stride ld elements) into smem [kTile][kD], zero-filled past nvalid
-template <typename T>
-__device__ __forceinline__ void load_tile(float (*dst)[kD], const T* src, int64_t ld, int nvalid) {
+__device__ __forceinline__ void load_tile(float (*dst)[kD], const float* src, int64_t ld, int nvalid) {
   for (int idx = threadIdx.x; idx < kTile * kD; idx += blockDim.x) {
     const int r = idx >> 6, c = idx & 63;
-    dst[r][c] = r < nvalid ? to_f<T>(src[(int64_t)r * ld + c]) : 0.f;
+    dst[r][c] = r < nvalid ? src[(int64_t)r * ld + c] : 0.f;
   }
 }
 
-template <typename T>
-__global__ void __launch_bounds__(128) attn_fwd_simt_kernel(const T* __restrict__ q, const T* __restrict__ k,
-                                                           const T* __restrict__ v, T* __restrict__ out,
-                                                           float* __restrict__ lse, int B, int Nq, int Nk, int H,
-                                                           int kv_shift, float scale) {
+__global__ void __launch_bounds__(128) attn_fwd_simt_kernel(const float* __restrict__ q, const float* __restrict__ k,
+                                                            const float* __restrict__ v, float* __restrict__ out,
+                                                            float* __restrict__ lse, int B, int Nq, int Nk, int H,
+                                                            int kv_shift, float scale) {
   __shared__ float sk[kTile][kD];
   __shared__ float sv[kTile][kD];
   const int b = blockIdx.z, h = blockIdx.y;
@@ -55,15 +46,15 @@ __global__ void __launch_bounds__(128) attn_fwd_simt_kernel(const T* __restrict_
   float qr[kHalf], o[kHalf];
 #pragma unroll
   for (int d = 0; d < kHalf; ++d) {
-    qr[d] = rvalid ? to_f<T>(q[((int64_t)b * Nq + row) * ld + h * kD + half * kHalf + d]) * scale : 0.f;
+    qr[d] = rvalid ? q[((int64_t)b * Nq + row) * ld + h * kD + half * kHalf + d] * scale : 0.f;
     o[d] = 0.f;
   }
   float m = -INFINITY, l = 0.f;
   for (int j0 = 0; j0 < Nk; j0 += kTile) {
     const int nv = min(kTile, Nk - j0);
     __syncthreads();
-    load_tile<T>(sk, k + ((int64_t)kb * Nk + j0) * ld + h * kD, ld, nv);
-    load_tile<T>(sv, v + ((int64_t)kb * Nk + j0) * ld + h * kD, ld, nv);
+    load_tile(sk, k + ((int64_t)kb * Nk + j0) * ld + h * kD, ld, nv);
+    load_tile(sv, v + ((int64_t)kb * Nk + j0) * ld + h * kD, ld, nv);
     __syncthreads();
     for (int j = 0; j < nv; ++j) {
       float s = 0.f;
@@ -87,23 +78,22 @@ __global__ void __launch_bounds__(128) attn_fwd_simt_kernel(const T* __restrict_
     const float inv = 1.f / l;
 #pragma unroll
     for (int d = 0; d < kHalf; ++d)
-      out[((int64_t)b * Nq + row) * ld + h * kD + half * kHalf + d] = from_f<T>(o[d] * inv);
+      out[((int64_t)b * Nq + row) * ld + h * kD + half * kHalf + d] = o[d] * inv;
     if (half == 0) lse[((int64_t)b * H + h) * Nq + row] = m + logf(l);
   }
 }
 
 // delta[b,h,i] = sum_d dout[b,i,h,d] * out[b,i,h,d]   (8 lanes per row)
-template <typename T>
-__global__ void __launch_bounds__(256) attn_delta_kernel(const T* __restrict__ out, const T* __restrict__ dout,
-                                                        float* __restrict__ delta, int64_t nrows /*B*N*H*/, int N,
-                                                        int H) {
+__global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict__ out, const float* __restrict__ dout,
+                                                         float* __restrict__ delta, int64_t nrows /*B*N*H*/, int N,
+                                                         int H) {
   const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t r = gid >> 3;  // (b, n, h) flattened token-major
   const int sub = (int)(gid & 7);
   float acc = 0.f;
   if (r < nrows) {
 #pragma unroll
-    for (int e = 0; e < 8; ++e) acc += to_f<T>(out[r * kD + sub * 8 + e]) * to_f<T>(dout[r * kD + sub * 8 + e]);
+    for (int e = 0; e < 8; ++e) acc += out[r * kD + sub * 8 + e] * dout[r * kD + sub * 8 + e];
   }
   acc += __shfl_xor_sync(0xffffffffu, acc, 1);
   acc += __shfl_xor_sync(0xffffffffu, acc, 2);
@@ -118,13 +108,11 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const T* __restrict__ o
 }
 
 // dq_i = scale * sum_j p_ij (dp_ij - delta_i) k_j
-template <typename T>
-__global__ void __launch_bounds__(128) attn_bwd_dq_simt_kernel(const T* __restrict__ q, const T* __restrict__ k,
-                                                              const T* __restrict__ v, const T* __restrict__ dout,
-                                                              const float* __restrict__ lse,
-                                                              const float* __restrict__ delta, T* __restrict__ dq,
-                                                              int B, int Nq, int Nk, int H, int kv_shift,
-                                                              float scale) {
+__global__ void __launch_bounds__(128)
+    attn_bwd_dq_simt_kernel(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
+                            const float* __restrict__ dout, const float* __restrict__ lse,
+                            const float* __restrict__ delta, float* __restrict__ dq, int B, int Nq, int Nk, int H,
+                            int kv_shift, float scale) {
   __shared__ float sk[kTile][kD];
   __shared__ float sv[kTile][kD];
   const int b = blockIdx.z, h = blockIdx.y;
@@ -137,8 +125,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_simt_kernel(const T* __restri
 #pragma unroll
   for (int d = 0; d < kHalf; ++d) {
     const int64_t off = ((int64_t)b * Nq + row) * ld + h * kD + half * kHalf + d;
-    qr[d] = rvalid ? to_f<T>(q[off]) * scale : 0.f;
-    go[d] = rvalid ? to_f<T>(dout[off]) : 0.f;
+    qr[d] = rvalid ? q[off] * scale : 0.f;
+    go[d] = rvalid ? dout[off] : 0.f;
     acc[d] = 0.f;
   }
   const float L = rvalid ? lse[((int64_t)b * H + h) * Nq + row] : 0.f;
@@ -146,8 +134,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_simt_kernel(const T* __restri
   for (int j0 = 0; j0 < Nk; j0 += kTile) {
     const int nv = min(kTile, Nk - j0);
     __syncthreads();
-    load_tile<T>(sk, k + ((int64_t)kb * Nk + j0) * ld + h * kD, ld, nv);
-    load_tile<T>(sv, v + ((int64_t)kb * Nk + j0) * ld + h * kD, ld, nv);
+    load_tile(sk, k + ((int64_t)kb * Nk + j0) * ld + h * kD, ld, nv);
+    load_tile(sv, v + ((int64_t)kb * Nk + j0) * ld + h * kD, ld, nv);
     __syncthreads();
     for (int j = 0; j < nv; ++j) {
       float s = 0.f, dp = 0.f;
@@ -166,19 +154,17 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_simt_kernel(const T* __restri
   if (rvalid) {
 #pragma unroll
     for (int d = 0; d < kHalf; ++d)
-      dq[((int64_t)b * Nq + row) * ld + h * kD + half * kHalf + d] = from_f<T>(acc[d]);
+      dq[((int64_t)b * Nq + row) * ld + h * kD + half * kHalf + d] = acc[d];
   }
 }
 
 // dv_j = sum_i p_ij do_i ;  dk_j = scale * sum_i p_ij (dp_ij - delta_i) q_i
 // launched over KEY batches kb; the query batch is qb = (kb - kv_shift) mod B.
-template <typename T>
-__global__ void __launch_bounds__(128) attn_bwd_dkv_simt_kernel(const T* __restrict__ q, const T* __restrict__ k,
-                                                               const T* __restrict__ v, const T* __restrict__ dout,
-                                                               const float* __restrict__ lse,
-                                                               const float* __restrict__ delta, T* __restrict__ dk,
-                                                               T* __restrict__ dv, int B, int Nq, int Nk, int H,
-                                                               int kv_shift, float scale) {
+__global__ void __launch_bounds__(128)
+    attn_bwd_dkv_simt_kernel(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
+                             const float* __restrict__ dout, const float* __restrict__ lse,
+                             const float* __restrict__ delta, float* __restrict__ dk, float* __restrict__ dv, int B,
+                             int Nq, int Nk, int H, int kv_shift, float scale) {
   __shared__ float sq[kTile][kD];
   __shared__ float sdo[kTile][kD];
   __shared__ float sl[kTile], sd[kTile];
@@ -192,15 +178,15 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_simt_kernel(const T* __restr
 #pragma unroll
   for (int d = 0; d < kHalf; ++d) {
     const int64_t off = ((int64_t)kb * Nk + row) * ld + h * kD + half * kHalf + d;
-    kr[d] = rvalid ? to_f<T>(k[off]) * scale : 0.f;
-    vr[d] = rvalid ? to_f<T>(v[off]) : 0.f;
+    kr[d] = rvalid ? k[off] * scale : 0.f;
+    vr[d] = rvalid ? v[off] : 0.f;
     gk[d] = gv[d] = 0.f;
   }
   for (int i0 = 0; i0 < Nq; i0 += kTile) {
     const int nv = min(kTile, Nq - i0);
     __syncthreads();
-    load_tile<T>(sq, q + ((int64_t)qb * Nq + i0) * ld + h * kD, ld, nv);
-    load_tile<T>(sdo, dout + ((int64_t)qb * Nq + i0) * ld + h * kD, ld, nv);
+    load_tile(sq, q + ((int64_t)qb * Nq + i0) * ld + h * kD, ld, nv);
+    load_tile(sdo, dout + ((int64_t)qb * Nq + i0) * ld + h * kD, ld, nv);
     if (threadIdx.x < kTile) {
       const bool ok = (int)threadIdx.x < nv;
       sl[threadIdx.x] = ok ? lse[((int64_t)qb * H + h) * Nq + i0 + threadIdx.x] : 0.f;
@@ -229,54 +215,41 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_simt_kernel(const T* __restr
 #pragma unroll
     for (int d = 0; d < kHalf; ++d) {
       const int64_t off = ((int64_t)kb * Nk + row) * ld + h * kD + half * kHalf + d;
-      dk[off] = from_f<T>(gk[d]);
-      dv[off] = from_f<T>(gv[d]);
+      dk[off] = gk[d];
+      dv[off] = gv[d];
     }
   }
 }
 
-template <typename T>
 int attn_fwd_simt(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk, int H,
                   int kv_shift, float scale, cudaStream_t stream) {
   dim3 grid((Nq + kTile - 1) / kTile, H, B);
-  attn_fwd_simt_kernel<T><<<grid, 128, 0, stream>>>((const T*)q, (const T*)k, (const T*)v, (T*)out, lse, B, Nq, Nk, H,
-                                                    kv_shift, scale);
+  attn_fwd_simt_kernel<<<grid, 128, 0, stream>>>((const float*)q, (const float*)k, (const float*)v, (float*)out, lse, B,
+                                                 Nq, Nk, H, kv_shift, scale);
   return check_launch("attn_fwd_simt");
 }
 
-template <typename T>
 int attn_delta(const void* out, const void* dout, float* delta, int B, int N, int H, cudaStream_t stream) {
   const int64_t nrows = (int64_t)B * N * H;
   const unsigned grid = (unsigned)((nrows * 8 + 255) / 256);
-  attn_delta_kernel<T><<<grid, 256, 0, stream>>>((const T*)out, (const T*)dout, delta, nrows, N, H);
+  attn_delta_kernel<<<grid, 256, 0, stream>>>((const float*)out, (const float*)dout, delta, nrows, N, H);
   return check_launch("attn_delta");
 }
 
-template <typename T>
 int attn_bwd_simt(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
                   void* dq, void* dk, void* dv, float* delta, int B, int Nq, int Nk, int H, int kv_shift, float scale,
                   cudaStream_t stream) {
-  int rc = attn_delta<T>(out, dout, delta, B, Nq, H, stream);
+  int rc = attn_delta(out, dout, delta, B, Nq, H, stream);
   if (rc) return rc;
   dim3 gq((Nq + kTile - 1) / kTile, H, B);
-  attn_bwd_dq_simt_kernel<T><<<gq, 128, 0, stream>>>((const T*)q, (const T*)k, (const T*)v, (const T*)dout, lse, delta,
-                                                     (T*)dq, B, Nq, Nk, H, kv_shift, scale);
+  attn_bwd_dq_simt_kernel<<<gq, 128, 0, stream>>>((const float*)q, (const float*)k, (const float*)v,
+                                                  (const float*)dout, lse, delta, (float*)dq, B, Nq, Nk, H, kv_shift,
+                                                  scale);
   dim3 gk((Nk + kTile - 1) / kTile, H, B);
-  attn_bwd_dkv_simt_kernel<T><<<gk, 128, 0, stream>>>((const T*)q, (const T*)k, (const T*)v, (const T*)dout, lse,
-                                                      delta, (T*)dk, (T*)dv, B, Nq, Nk, H, kv_shift, scale);
+  attn_bwd_dkv_simt_kernel<<<gk, 128, 0, stream>>>((const float*)q, (const float*)k, (const float*)v,
+                                                   (const float*)dout, lse, delta, (float*)dk, (float*)dv, B, Nq, Nk, H,
+                                                   kv_shift, scale);
   return check_launch("attn_bwd_simt");
 }
-
-template int attn_fwd_simt<float>(const void*, const void*, const void*, void*, float*, int, int, int, int, int, float,
-                                  cudaStream_t);
-template int attn_fwd_simt<__nv_bfloat16>(const void*, const void*, const void*, void*, float*, int, int, int, int, int,
-                                          float, cudaStream_t);
-template int attn_bwd_simt<float>(const void*, const void*, const void*, const void*, const float*, const void*, void*,
-                                  void*, void*, float*, int, int, int, int, int, float, cudaStream_t);
-template int attn_bwd_simt<__nv_bfloat16>(const void*, const void*, const void*, const void*, const float*,
-                                          const void*, void*, void*, void*, float*, int, int, int, int, int, float,
-                                          cudaStream_t);
-template int attn_delta<float>(const void*, const void*, float*, int, int, int, cudaStream_t);
-template int attn_delta<__nv_bfloat16>(const void*, const void*, float*, int, int, int, cudaStream_t);
 
 }  // namespace lgb

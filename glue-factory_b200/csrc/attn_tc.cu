@@ -15,9 +15,8 @@
 // slower at that occupancy.  Tile order and per-element arithmetic are those of the unpipelined loop, so out and lse
 // do not depend on the overlap.
 // BACKWARD: one CTA owns 128 keys (K, V resident in smem) and walks the queries in tiles of 64 (dK, dV accumulated in
-// registers); dQ comes from a second kernel that owns the queries (the default: deterministic, so eager steps and
-// CUDA-graph replays of a training step agree bit for bit) or, with LGB200_ATTN_BWD_FUSED=1, from the same pass (dS
-// through shared memory, fp32 atomics into an accumulator: no recomputation of S / dP, run-dependent summation order).
+// registers); dQ comes from a second kernel that owns the queries and recomputes S / dP.  No atomics: every sum has
+// a fixed order, so eager steps and CUDA-graph replays of a training step agree bit for bit.
 // Cross-attention with one shared q = k projection (LightGlue's to_qk) has its own kernel: both directions share the
 // similarity, so one sweep per image yields dV and dq + dk (attn_bwd_shared_qk_kernel, below).
 #include <math.h>
@@ -247,11 +246,7 @@ int attn_fwd_tc(const void* q, const void* k, const void* v, void* out, float* l
 //     P^T  = exp2(c S^T - lse2_i),  dS^T = P^T (dP^T scale - delta_i scale)   (in registers; lse2 / delta are
 //            per-COLUMN values here and come as two 64-float vectors with every query tile)
 //     dV  += P^T dO_i,   dK += dS^T Q_i           (P^T / dS^T as register A operands, dO_i / Q_i MN-major from smem)
-// With the dQ fusion, dS^T also goes to shared memory ([key][query], 128-byte swizzled: read with M = query it is an
-// MN-major A operand) and dQ_i (64 x 64) += dS K is formed per warpgroup and added into an fp32 accumulator with
-// atomics (the key-tile CTAs of one (batch, head) meet there; summation order is not fixed), converted to bf16 by
-// a last small kernel.
-// dQ kernel (default path): a CTA owns 128 queries (Q, dO resident) and walks the keys in tiles of 64:
+// dQ kernel: a CTA owns 128 queries (Q, dO resident) and walks the keys in tiles of 64:
 //     S = Q K_j^T, dP = dO V_j^T, dS = exp2(c S - lse2) (dP scale - delta scale), dQ += dS K_j.
 // Queries past Nq load as zeros and carry lse2 = +inf (p = 0); keys past Nk load as zeros, so their dS meets a zero
 // row of K and adds nothing to dQ, and their dK / dV rows are not stored.
@@ -262,8 +257,7 @@ constexpr int FB_CBYTES = FB_C * FA_D * 2;  // 8 KiB
 constexpr int FF_STAGES = 3;
 constexpr int FF_STAGE_BYTES = 17 * 1024;                 // Q 8 KiB | dO 8 KiB | lse2 256 B | delta 256 B (| pad)
 constexpr int FF_OFF_STAGE = 2 * FB_R * FA_D * 2;         // after the resident K and V tiles (16 KiB each)
-constexpr int FF_OFF_DS = FF_OFF_STAGE + FF_STAGES * FF_STAGE_BYTES;
-constexpr int FF_SMEM = FF_OFF_DS + 2 * FB_C * 128 + 256; // + one 64 x 64 bf16 dS^T tile per warpgroup
+constexpr int FF_SMEM = FF_OFF_STAGE + FF_STAGES * FF_STAGE_BYTES + 256;
 constexpr int FQ_STAGES = 4;
 constexpr int FQ_SMEM = 2 * FB_R * FA_D * 2 + FQ_STAGES * 2 * FB_CBYTES + 256;
 
@@ -311,23 +305,12 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-__global__ void __launch_bounds__(256) dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict__ dq,
-                                                        int64_t n8) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n8) return;
-  const float4 a = reinterpret_cast<const float4*>(acc)[2 * i], b = reinterpret_cast<const float4*>(acc)[2 * i + 1];
-  uint4 u;
-  u.x = pack_bf16(a.x, a.y); u.y = pack_bf16(a.z, a.w); u.z = pack_bf16(b.x, b.y); u.w = pack_bf16(b.z, b.w);
-  reinterpret_cast<uint4*>(dq)[i] = u;
-}
-
-template <bool WITH_DQ>
 __global__ void __launch_bounds__(FA_THREADS, 1)
     attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
                         const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                         const float* __restrict__ lse2p, const float* __restrict__ deltap,
-                        __nv_bfloat16* __restrict__ dk, __nv_bfloat16* __restrict__ dv, float* __restrict__ dqacc, int B,
-                        int Nq, int nq_pad, int Nk, int H, int kv_shift, float scale, float scale_log2) {
+                        __nv_bfloat16* __restrict__ dk, __nv_bfloat16* __restrict__ dv, int B, int Nq, int nq_pad,
+                        int Nk, int H, int kv_shift, float scale, float scale_log2) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sK = smem;
   uint8_t* sV = smem + FB_R * FA_D * 2;
@@ -379,13 +362,11 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
     }
     return;
   }
-  const int wg = threadIdx.x >> 7, wq = warp & 3, g = lane >> 2, t4 = lane & 3;
+  const int wg = threadIdx.x >> 7, t4 = lane & 3;
   const bool signal = (threadIdx.x & 127) == 0;
-  uint8_t* sDS = smem + FF_OFF_DS + wg * (FB_C * 128);
   const uint64_t dK0 = make_smem_desc(smem_u32(sK) + wg * 8192, 8192, 1024);
   const uint64_t dV0 = make_smem_desc(smem_u32(sV) + wg * 8192, 8192, 1024);
   const uint64_t dSt0 = make_smem_desc(smem_u32(sStage), 8192, 1024);
-  const uint64_t dDS = make_smem_desc(smem_u32(sDS), 8192, 1024);
   float acc_v[32], acc_k[32];
 #pragma unroll
   for (int e = 0; e < 32; ++e) acc_v[e] = acc_k[e] = 0.f;
@@ -424,48 +405,16 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
       acc_to_afrag(st, kk, pa[kk]);
       acc_to_afrag(dp, kk, da[kk]);
     }
-    if constexpr (WITH_DQ) {
-      // dS^T (bf16) -> this warpgroup's [key][query] tile; the previous tile's dQ product has retired in every warp
-      named_bar(1 + wg, 128);
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int key = wq * 16 + g + 8 * r;
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj)
-          *reinterpret_cast<uint32_t*>(sDS + key * 128 + ((jj ^ (key & 7)) << 4) + 4 * t4) =
-              pack_bf16(dp[4 * jj + 2 * r], dp[4 * jj + 2 * r + 1]);
-      }
-      fence_proxy_async_smem();
-      named_bar(1 + wg, 128);
-    }
-    float dq[32];
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < FB_C / 16; ++kk) wgmma_m64n64_rs<1>(acc_v, pa[kk], dSt0 + so_do + kk * 128, 1);
 #pragma unroll
     for (int kk = 0; kk < FB_C / 16; ++kk) wgmma_m64n64_rs<1>(acc_k, da[kk], dSt0 + so + kk * 128, 1);
-    if constexpr (WITH_DQ) {
-#pragma unroll
-      for (int kk = 0; kk < FB_C / 16; ++kk)  // dQ_i = dS K_w: 16 keys per step, both operands MN-major
-        wgmma_m64n64_ss<1, 1>(dq, dDS + kk * 128, dK0 + kk * 128, kk != 0);
-    }
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_hold(acc_v);
     wgmma_hold(acc_k);
     if (signal) mbar_arrive(&in_empty[s]);
-    if constexpr (WITH_DQ) {
-      wgmma_hold(dq);
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int q = i * FB_C + wq * 16 + g + 8 * r;
-        if (q >= Nq) continue;
-        float* dst = dqacc + (((int64_t)qb * Nq + q) * H + h) * FA_D + 2 * t4;
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj)
-          atomicAdd(reinterpret_cast<float2*>(dst + 8 * jj), make_float2(dq[4 * jj + 2 * r], dq[4 * jj + 2 * r + 1]));
-      }
-    }
   }
   store_acc_rows(acc_v, dv, kb, Nk, H, h, k0 + wg * 64, 1.f);
   store_acc_rows(acc_k, dk, kb, Nk, H, h, k0 + wg * 64, 1.f);
@@ -735,20 +684,17 @@ __global__ void __launch_bounds__(FX_THREADS, 1)
 }
 
 int64_t attn_bwd_ws_floats(int B, int Nq, int Nk, int H) {
-  // lse2 / delta padded to whole query tiles + the fp32 dQ accumulator of the fused path
+  // lse2 / delta padded to whole query tiles (also covers the fp32 path's B * Nq * H delta floats)
   const int64_t nq_pad = (int64_t)((Nq + FB_C - 1) / FB_C) * FB_C;
-  return 2 * (int64_t)B * H * nq_pad + (int64_t)B * Nq * H * FA_D + 64;
+  return 2 * (int64_t)B * H * nq_pad;
 }
 
 int attn_bwd_tc(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
                 void* dq, void* dk, void* dv, float* ws, int B, int Nq, int Nk, int H, int kv_shift, float scale,
                 cudaStream_t stream) {
-  const bool fused = env_flag("LGB200_ATTN_BWD_FUSED");  // default: the deterministic dQ kernel
   const int nq_pad = (Nq + FB_C - 1) / FB_C * FB_C;
   float* lse2p = ws;
   float* deltap = lse2p + (int64_t)B * H * nq_pad;
-  float* dqacc = deltap + (int64_t)B * H * nq_pad;
-  dqacc = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(dqacc) + 255) & ~(uintptr_t)255);
   int rc;
   {
     const int64_t nrows = (int64_t)B * nq_pad * H;
@@ -771,36 +717,26 @@ int attn_bwd_tc(const void* q, const void* k, const void* v, const void* out, co
         B, Nq, nq_pad, H, kv_shift, scale, sl2);
     return check_launch("attn_bwd_shared_qk");
   }
-  if (fused) {
-    const size_t acc_bytes = (size_t)B * Nq * H * FA_D * 4;
-    cudaError_t e = cudaMemsetAsync(dqacc, 0, acc_bytes, stream);
-    LGB_REQUIRE(e == cudaSuccess, kErrCuda, "attn_bwd(fused): memset: %s", cudaGetErrorString(e));
-  }
   CUtensorMap tq, tdo, tk, tv;
-  if (!fused) {  // dQ kernel: 128-query resident tiles, 64-key streamed tiles
-    if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_dq_kernel), FQ_SMEM))) return rc;
-    if ((rc = make_qkv_tmap(&tq, q, B, Nq, H, FB_R))) return rc;
-    if ((rc = make_qkv_tmap(&tdo, dout, B, Nq, H, FB_R))) return rc;
-    if ((rc = make_qkv_tmap(&tk, k, B, Nk, H, FB_C))) return rc;
-    if ((rc = make_qkv_tmap(&tv, v, B, Nk, H, FB_C))) return rc;
-    attn_bwd_dq_kernel<<<dim3((Nq + FB_R - 1) / FB_R, H, B), FA_THREADS, FQ_SMEM, stream>>>(
-        tq, tdo, tk, tv, lse2p, deltap, static_cast<__nv_bfloat16*>(dq), B, Nq, nq_pad, Nk, H, kv_shift, scale, sl2);
-    if ((rc = check_launch("attn_bwd_dq"))) return rc;
-  }
+  // dQ kernel: 128-query resident tiles, 64-key streamed tiles
+  if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_dq_kernel), FQ_SMEM))) return rc;
+  if ((rc = make_qkv_tmap(&tq, q, B, Nq, H, FB_R))) return rc;
+  if ((rc = make_qkv_tmap(&tdo, dout, B, Nq, H, FB_R))) return rc;
+  if ((rc = make_qkv_tmap(&tk, k, B, Nk, H, FB_C))) return rc;
+  if ((rc = make_qkv_tmap(&tv, v, B, Nk, H, FB_C))) return rc;
+  attn_bwd_dq_kernel<<<dim3((Nq + FB_R - 1) / FB_R, H, B), FA_THREADS, FQ_SMEM, stream>>>(
+      tq, tdo, tk, tv, lse2p, deltap, static_cast<__nv_bfloat16*>(dq), B, Nq, nq_pad, Nk, H, kv_shift, scale, sl2);
+  if ((rc = check_launch("attn_bwd_dq"))) return rc;
+  // dK / dV kernel: 128-key resident tiles, 64-query streamed tiles
   if ((rc = make_qkv_tmap(&tq, q, B, Nq, H, FB_C))) return rc;
   if ((rc = make_qkv_tmap(&tdo, dout, B, Nq, H, FB_C))) return rc;
   if ((rc = make_qkv_tmap(&tk, k, B, Nk, H, FB_R))) return rc;
   if ((rc = make_qkv_tmap(&tv, v, B, Nk, H, FB_R))) return rc;
-  auto kern = fused ? attn_bwd_dkv_kernel<true> : attn_bwd_dkv_kernel<false>;
-  if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), FF_SMEM))) return rc;
-  kern<<<dim3((Nk + FB_R - 1) / FB_R, H, B), FA_THREADS, FF_SMEM, stream>>>(
-      tq, tdo, tk, tv, lse2p, deltap, static_cast<__nv_bfloat16*>(dk), static_cast<__nv_bfloat16*>(dv), dqacc, B, Nq,
-      nq_pad, Nk, H, kv_shift, scale, sl2);
-  if ((rc = check_launch("attn_bwd_dkv"))) return rc;
-  if (!fused) return 0;
-  const int64_t n8 = (int64_t)B * Nq * H * FA_D / 8;
-  dq_convert_kernel<<<(unsigned)((n8 + 255) / 256), 256, 0, stream>>>(dqacc, static_cast<__nv_bfloat16*>(dq), n8);
-  return check_launch("attn_bwd(convert)");
+  if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_dkv_kernel), FF_SMEM))) return rc;
+  attn_bwd_dkv_kernel<<<dim3((Nk + FB_R - 1) / FB_R, H, B), FA_THREADS, FF_SMEM, stream>>>(
+      tq, tdo, tk, tv, lse2p, deltap, static_cast<__nv_bfloat16*>(dk), static_cast<__nv_bfloat16*>(dv), B, Nq, nq_pad,
+      Nk, H, kv_shift, scale, sl2);
+  return check_launch("attn_bwd_dkv");
 }
 
 }  // namespace lgb

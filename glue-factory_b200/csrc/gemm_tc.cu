@@ -568,8 +568,7 @@ extern "C" int lgb200_linear(const void* A, const void* B, void* C, const float*
   int rc = make_ab_maps(&ta, &tb, A, B, 1, M, N, K, a_mn_major, b_mn_major, lda, ldb, 0, 0);
   if (rc) return rc;
   {  // A-panel-resident kernel: K <= 256, K-major A
-    const bool off = env_flag("LGB200_GEMM_NO_APANEL");
-    if (!off && !a_mn_major && K <= GP_KB * GB_K && (c_dtype == LGB200_F32 || c_dtype == LGB200_BF16)) {
+    if (!a_mn_major && K <= GP_KB * GB_K && (c_dtype == LGB200_F32 || c_dtype == LGB200_BF16)) {
       const int tiles_m = (M + GB_M - 1) / GB_M, tiles_n = (N + GB_N - 1) / GB_N;
       const int sms = device_sm_count();
       const unsigned grid = (unsigned)(tiles_m < sms ? tiles_m : sms);

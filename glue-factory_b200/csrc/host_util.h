@@ -11,22 +11,18 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
 // same for fp32 (fp32 = true) or bf16 elements
 int make_tmap(CUtensorMap* out, const void* base, bool fp32, int rank, const uint64_t* dims,
               const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes = 128);
-bool env_flag(const char* name);
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device attribute: set it once per (kernel, device), not once
 // per process.  Returns 0 or kErrCuda.
 int ensure_dyn_smem(const void* func, int bytes);
 // SM count of the CURRENT device (cached per device ordinal)
 int device_sm_count();
 
-// fp32 / bf16 CUDA-core attention (attn_simt.cu)
-template <typename T>
+// fp32 CUDA-core attention (attn_simt.cu)
 int attn_fwd_simt(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk, int H,
                   int kv_shift, float scale, cudaStream_t stream);
-template <typename T>
 int attn_bwd_simt(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
                   void* dq, void* dk, void* dv, float* delta, int B, int Nq, int Nk, int H, int kv_shift, float scale,
                   cudaStream_t stream);
-template <typename T>
 int attn_delta(const void* out, const void* dout, float* delta, int B, int N, int H, cudaStream_t stream);
 
 // wgmma attention (attn_tc.cu)
@@ -42,7 +38,7 @@ inline bool attn_bwd_is_shared_qk(const void* q, const void* k, const void* dq, 
   return q == k && dq == dk && Nq == Nk && 2 * kv_shift == B;
 }
 
-// scratch (floats) lgb200_attn_bwd needs for the bf16 path (padded softmax statistics + the fused dQ accumulator)
+// scratch (floats) lgb200_attn_bwd needs for the bf16 path (padded softmax statistics)
 int64_t attn_bwd_ws_floats(int B, int Nq, int Nk, int H);
 
 }  // namespace lgb

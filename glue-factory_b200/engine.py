@@ -24,8 +24,6 @@ import torch.nn.functional as F
 from . import ops
 
 _head_counters = {}
-# fused GEMM + assignment kernels (csrc/assign_tc.cu) for bf16 descriptors; False = the round-1 path (sim written to HBM)
-FUSED_ASSIGN = True
 
 
 # How the fp32 parity mode multiplies matrices: "cublas" (torch.addmm / mm) or "x3" -- every fp32 operand split into
@@ -315,7 +313,6 @@ class LayerFn(torch.autograd.Function):
             # the nine weight gradients are already in place; the 13 vectors go in with one multi-tensor copy
             small = [i for i in range(22) if grads[i].data_ptr() != gv[i].data_ptr()]
             torch._foreach_copy_([gv[i] for i in small], [grads[i].view_as(gv[i]) for i in small])
-            fp.chunk_ready(slot)
             grads = (None,) * 22
         return (dx0, dtheta, None, None, None, None, None, None) + grads
 
@@ -342,7 +339,7 @@ class HeadFn(torch.autograd.Function):
         md0, md1 = md[:t0].view(B, M, D), md[t0:].view(B, N, D)
         alpha = float(D) ** -0.5
         ls0, ls1, du0, du1 = ls[:t0].view(B, M), ls[t0:].view(B, N), du[:t0].view(B, M), du[t0:].view(B, N)
-        fused = FUSED_ASSIGN and ops.assign_fused_ok(md, D) and gt.get("u8_t") is not None
+        fused = ops.assign_fused_ok(md, D) and gt.get("u8_t") is not None
         if fused:
             # GEMM + LSE, then GEMM + scores / argmax / positives: the similarity matrix stays in tensor memory
             sim = None

@@ -458,7 +458,7 @@ class LightGlue(nn.Module):
         L = len(layers_x)
         gtd = {"u8": gt_u8, "rowcnt": rowcnt.contiguous(), "colcnt": colcnt.contiguous(), "neg0": neg0.contiguous(),
                "neg1": neg1.contiguous(), "num_pos": num_pos.contiguous(), "num_neg": (num_neg0 + num_neg1).contiguous()}
-        if self._bf16 and engine.FUSED_ASSIGN and torch.is_grad_enabled():
+        if self._bf16 and torch.is_grad_enabled():
             # the fused backward walks the mask by columns as well: one transposed copy per step, shared by all layers
             gt_t = data.get("gt_assignment_t")  # written by the plugin's ground-truth components when asked to
             gtd["u8_t"] = (gt_t.contiguous().view(torch.uint8) if gt_t is not None and gt_t.dtype == torch.bool

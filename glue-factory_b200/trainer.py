@@ -15,8 +15,6 @@ changes SURVEY.md section 2.2 (C1) calls for:
 The matcher is per-pair, so image pairs shard across ranks with no other
 collective (SURVEY.md section 8e).
 """
-import os
-
 import torch
 import torch.distributed as dist
 
@@ -24,13 +22,6 @@ from . import ops
 from .synthetic import to_device
 
 _ALIGN = 64  # elements; keeps every parameter view 256-byte aligned
-# Gradient-exchange schedule (FlatParams.exchange): "end" (default) = ONE sum-all-reduce of the flat gradient buffer
-# behind backward, issued in its synchronous form so that it runs on the step's own stream (a captured step stays a
-# linear chain of graph nodes); "chunked" = each layer's slice as soon as its backward wrote it, the rest at the end.
-# The default is the simple one; scripts/diag_allreduce.py and diag_lockstep.py time the all-reduce and the lock-step
-# wait of the two schedules.  "none" is a DIAGNOSTIC (ranks train independently).
-_EXCHANGE = os.environ.get("LGB200_EXCHANGE", "end")
-assert _EXCHANGE in ("chunked", "end", "none"), _EXCHANGE
 
 
 class FlatParams:
@@ -62,53 +53,23 @@ class FlatParams:
         self._views16 = None
         self.grad_views = [self.grad[off:off + p.numel()].view_as(p) for p, off in zip(self.params, self.offsets)]
         # "direct" parameter groups: their gradients are written into the flat buffer by the backward kernels themselves
-        # (engine.LayerFn) and each group's slice is exchanged as soon as it is final (see enable_direct)
+        # (engine.LayerFn), so their .grad views stay attached (see enable_direct)
         self.direct_groups = []
         self._direct_ids = set()
-        self.world, self.group, self._pending = 1, None, []
-        self.exchange = _EXCHANGE
         module._b200_flat = self
 
     def enable_direct(self, groups):
-        """groups: lists of parameters, each list contiguous in the flat buffer (e.g. one transformer layer)."""
+        """groups: lists of parameters (e.g. one transformer layer) whose backward writes the flat gradient buffer."""
         index = {id(p): i for i, p in enumerate(self.params)}
         for params in groups:
-            idx = [index[id(p)] for p in params]
-            assert idx == list(range(idx[0], idx[0] + len(idx))), "a direct group must be contiguous in the flat buffer"
-            lo = self.offsets[idx[0]]
-            hi = self.offsets[idx[-1] + 1] if idx[-1] + 1 < len(self.params) else self.numel
-            self.direct_groups.append((lo, hi, [self.grad_views[i] for i in idx]))
+            self.direct_groups.append([self.grad_views[index[id(p)]] for p in params])
             self._direct_ids.update(id(p) for p in params)
         for p, v in zip(self.params, self.grad_views):
             if id(p) in self._direct_ids:
                 p.grad = v
 
     def direct_views(self, gi):
-        return self.direct_groups[gi][2]
-
-    def chunk_ready(self, gi):
-        """Called from backward when group gi's gradients are final: start its all-reduce now (it overlaps the backward
-        of the layers below); `finish_exchange` waits for all of them."""
-        if self.world > 1 and self.exchange == "chunked":
-            lo, hi, _ = self.direct_groups[gi]
-            self._pending.append((lo, hi, dist.all_reduce(self.grad[lo:hi], op=dist.ReduceOp.SUM, group=self.group,
-                                                          async_op=True)))
-
-    def finish_exchange(self):
-        """All-reduce whatever the per-group exchanges did not cover (the head / encoding parameters and the loss slot
-        behind the gradients), then wait for every outstanding chunk."""
-        if self.world > 1 and self.exchange != "none":
-            covered = sorted((lo, hi) for lo, hi, _ in self._pending)  # the slices whose exchange is already in flight
-            pos, total = 0, self.grad_ext.numel()
-            for lo, hi in covered + [(total, total)]:
-                if lo > pos:
-                    # synchronous form: the collective is enqueued on the CURRENT stream (no side stream), so a
-                    # captured step stays one linear chain of graph nodes when nothing was exchanged early
-                    dist.all_reduce(self.grad_ext[pos:lo], op=dist.ReduceOp.SUM, group=self.group)
-                pos = max(pos, hi)
-            for _, _, w in self._pending:
-                w.wait()
-        self._pending = []
+        return self.direct_groups[gi]
 
     def shadow_bf16(self):
         """name -> bf16 view of the parameter, refreshed from the fp32 master copy by ONE cast kernel."""
@@ -141,7 +102,6 @@ class FlatParams:
         (no per-parameter accumulate kernel); `gather_grads` packs them into the flat buffer."""
         for p, v in zip(self.params, self.grad_views):
             p.grad = v if id(p) in self._direct_ids else None  # direct groups are overwritten in place by backward
-        self._pending = []
 
     def gather_grads(self):
         rest = [(v, p) for v, p in zip(self.grad_views, self.params) if id(p) not in self._direct_ids]
@@ -188,7 +148,6 @@ class MatcherTrainer:
         self.m = torch.zeros_like(self.fp.flat)
         self.v = torch.zeros_like(self.fp.flat)
         self.betas, self.eps, self.wd = betas, eps, weight_decay
-        self.fp.world, self.fp.group = self.world, process_group
         layers = getattr(model, "transformers", None)
         if layers is not None and getattr(getattr(model, "conf", None), "engine", None) == "fused":
             self.fp.enable_direct([list(layer.parameters()) for layer in layers])
@@ -225,10 +184,11 @@ class MatcherTrainer:
         return None if self._scale_dev is None else float(self._scale_dev.item())
 
     def exchange_gradients(self):
-        """The path's one exchange: the sum-all-reduce of the flat gradient buffer (+ the loss slot), issued in slices --
-        each transformer layer's slice as soon as its backward has written it (FlatParams.chunk_ready), the rest here."""
-        self.fp.world, self.fp.group = self.world, self.group
-        self.fp.finish_exchange()
+        """The step's one exchange: ONE sum-all-reduce of the whole flat gradient buffer (+ the loss slot), behind
+        backward.  Issued in its synchronous form, so the collective runs on the current stream and a captured step
+        stays one linear chain of graph nodes."""
+        if self.world > 1:
+            dist.all_reduce(self.fp.grad_ext, op=dist.ReduceOp.SUM, group=self.group)
 
     # ---- CUDA-graph replay of the whole step (removes the ~2500 per-step launch calls from the host)
     def capture(self, example, device, warmup=3):

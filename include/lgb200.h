@@ -71,11 +71,11 @@ int lgb200_rope_split_bwd(const void* dq, const void* dk, const void* dv, const 
 int lgb200_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk, int H,
                     int kv_shift, float scale, int dtype, cudaStream_t stream);
 /* dq [B,Nq,H,64]; dk,dv [B,Nk,H,64] (indexed by KEY batch); delta_ws: lgb200_attn_bwd_ws_floats(B,Nq,Nk,H) floats of
- * scratch, 256-byte aligned (rowsum(dout*out), the per-query side data of the kernels and, for the fused bf16
- * backward, the fp32 dQ accumulator the key-tile CTAs reduce into).
+ * scratch, 256-byte aligned (the per-query softmax statistics the kernels read: rowsum(dout*out) and, on the bf16
+ * path, the base-2 log-sum-exp, padded to whole query tiles).
  * Shared-qk cross-attention (lightglue.py:207-216, one to_qk projection for both directions): when k == q,
  * dk == dq, Nq == Nk and 2 * kv_shift == B, dq receives the total gradient of the shared tensor (dq + dk) from one
- * pass over the shared similarity.  bf16 tensor-core path only; the fp32 / SIMT paths reject this aliasing.      */
+ * pass over the shared similarity.  bf16 tensor-core path only; the fp32 path rejects this aliasing.             */
 int64_t lgb200_attn_bwd_ws_floats(int B, int Nq, int Nk, int H);
 int lgb200_attn_bwd(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
                     void* dq, void* dk, void* dv, float* delta_ws, int B, int Nq, int Nk, int H, int kv_shift,

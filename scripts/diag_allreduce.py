@@ -1,6 +1,6 @@
 """Multi-GPU diagnosis (torchrun, one rank per GPU): (1) the flat-gradient all-reduce alone (47.4 MB fp32 + loss slot),
-eager and inside a CUDA graph; (2) per-rank step time of the training step with no exchange (rank skew / jitter);
-(3) the step with the exchange, with per-rank time spent waiting inside the all-reduce."""
+eager and inside a CUDA graph; (2) per-rank step time of the captured training step, which ends in that one all-reduce
+(rank skew / jitter)."""
 import os
 import sys
 
@@ -39,10 +39,6 @@ def timed(fn, n=20):
 med, mx = timed(lambda: dist.all_reduce(buf))
 if rank == 0:
     print(f"all_reduce 47.4 MB fp32, eager: median {med:.3f} ms, max {mx:.3f} ms  ({buf.numel() * 4 / med / 1e6:.0f} GB/s algbw)")
-chunks = buf[:11_849_728].chunk(9)
-med, mx = timed(lambda: [dist.all_reduce(c) for c in chunks])
-if rank == 0:
-    print(f"9 chunked all_reduces back to back: median {med:.3f} ms, max {mx:.3f} ms")
 g = torch.cuda.CUDAGraph()
 s = torch.cuda.Stream()
 s.wait_stream(torch.cuda.current_stream())
@@ -55,7 +51,7 @@ med, mx = timed(g.replay)
 if rank == 0:
     print(f"all_reduce inside a CUDA graph: median {med:.3f} ms, max {mx:.3f} ms")
 
-# (2)/(3): the training step, per-rank timing
+# (2): the training step, per-rank timing
 from gluefactory_b200 import synthetic  # noqa: E402
 from gluefactory_b200.matchers.homography_matcher import HomographyMatcher  # noqa: E402
 from gluefactory_b200.matchers.lightglue import LightGlue  # noqa: E402
@@ -85,6 +81,6 @@ stats = torch.stack([t.mean(), t.std(), t.min(), t.max()])
 allst = [torch.zeros_like(stats) for _ in range(world)]
 dist.all_gather(allst, stats)
 if rank == 0:
-    print(f"step (LGB200_EXCHANGE={os.environ.get('LGB200_EXCHANGE', 'chunked')}), per rank mean/std/min/max ms: "
+    print("captured step, per rank mean/std/min/max ms: "
           + " | ".join("/".join(f"{x:.2f}" for x in s_.tolist()) for s_ in allst))
 dist.destroy_process_group()

@@ -1,6 +1,6 @@
 """2-GPU diagnosis (torchrun): where does the synchronous step lose time against two free-running ranks?
 Eager steps with CUDA events around the gradient exchange: [forward + backward] | [exchange incl. waiting for the peer] |
-[check + Adam], per rank.  LGB200_EXCHANGE = end | chunked | none."""
+[check + Adam], per rank.  The exchange is the trainer's one all-reduce of the flat gradient buffer."""
 import os
 import sys
 
@@ -48,7 +48,7 @@ st = torch.cat([t.mean(0), t.std(0)])
 allst = [torch.zeros_like(st) for _ in range(world)]
 dist.all_gather(allst, st)
 if rank == 0:
-    print(f"LGB200_EXCHANGE={os.environ.get('LGB200_EXCHANGE', 'chunked')} (eager steps), per rank mean ms "
+    print("eager steps, per rank mean ms "
           "[fwd+bwd | exchange | check+adam | total] (std):", flush=True)
     for r, s_ in enumerate(allst):
         v = s_.tolist()

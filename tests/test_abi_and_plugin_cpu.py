@@ -33,6 +33,7 @@ def test_library_exports_every_declared_symbol(built):
     # pure host queries are callable without a GPU
     assert lib.lgb200_assign_ws_bytes(2, 64, 64) == 2 * 2 * 64 * 8
     assert lib.lgb200_ln_gelu_bwd_parts(1000) == 125
+    assert lib.lgb200_attn_bwd_ws_floats(64, 2048, 2048, 4) == 2 * 64 * 4 * 2048  # padded lse2 + delta only
 
 
 def test_plugin_surface_matches_reference_names():

@@ -59,58 +59,42 @@ def test_flat_gradient_allreduce_world2():
     assert abs(res[0] - res[1]) < 1e-6 and res[0] > 0
 
 
-def _chunk_worker(rank, world, port, out):
-    """The overlapped exchange: per-group slices all-reduced as soon as they are final + the remainder at the end must
-    equal ONE all-reduce of the whole buffer (host logic of FlatParams.chunk_ready / finish_exchange, over gloo)."""
+def _direct_worker(rank, world, port, out):
+    """Direct parameter groups (their backward writes the flat gradient buffer in place) keep their .grad views through
+    zero_grad, and MatcherTrainer.exchange_gradients is ONE sum-all-reduce of the whole buffer, loss slot included
+    (host logic over gloo)."""
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
     dist.init_process_group("gloo", rank=rank, world_size=world)
-    from gluefactory_b200.trainer import FlatParams
+    from gluefactory_b200.trainer import FlatParams, MatcherTrainer
 
     torch.manual_seed(0)
     net = torch.nn.Sequential(torch.nn.Linear(8, 16), torch.nn.Linear(16, 16), torch.nn.Linear(16, 16), torch.nn.Linear(16, 3))
-    fp = FlatParams(net)
-    fp.world = world
-    fp.exchange = "chunked"
+    tr = MatcherTrainer.__new__(MatcherTrainer)
+    tr.fp = fp = FlatParams(net)
+    tr.world, tr.group = world, None
     fp.enable_direct([list(net[1].parameters()), list(net[2].parameters())])
     assert net[1].weight.grad.data_ptr() == fp.direct_views(0)[0].data_ptr()
     fp.zero_grad()
-    assert net[1].weight.grad is not None and net[0].weight.grad is None  # direct slots stay attached
+    assert all(p.grad is not None for i in (1, 2) for p in net[i].parameters())  # direct slots stay attached
+    assert all(p.grad is None for i in (0, 3) for p in net[i].parameters())
     g = torch.Generator().manual_seed(100 + rank)
     fp.grad_ext.copy_(torch.randn(fp.grad_ext.shape, generator=g))
     want = fp.grad_ext.clone()
     dist.all_reduce(want)
-    fp.chunk_ready(1)   # backward order: the later group first
-    fp.chunk_ready(0)
-    fp.finish_exchange()
-    assert torch.equal(fp.grad_ext, want)
-    assert fp._pending == []
-    # a step in which no group fired degenerates to one all-reduce of everything
-    fp.grad_ext.copy_(torch.randn(fp.grad_ext.shape, generator=g))
-    want = fp.grad_ext.clone()
-    dist.all_reduce(want)
-    fp.finish_exchange()
-    assert torch.equal(fp.grad_ext, want)
-    # the default schedule ("end"): chunk_ready is a no-op, everything goes through the one all-reduce at the end
-    fp.exchange = "end"
-    fp.grad_ext.copy_(torch.randn(fp.grad_ext.shape, generator=g))
-    want = fp.grad_ext.clone()
-    dist.all_reduce(want)
-    fp.chunk_ready(1)
-    assert fp._pending == []
-    fp.finish_exchange()
+    tr.exchange_gradients()
     assert torch.equal(fp.grad_ext, want)
     out.put((rank, float(want.abs().sum())))
     dist.destroy_process_group()
 
 
-def test_chunked_gradient_exchange_world2():
+def test_direct_groups_and_gradient_exchange_world2():
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     os.environ["PYTHONPATH"] = root + os.pathsep + os.environ.get("PYTHONPATH", "")
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = 31500 + os.getpid() % 2000
-    procs = [ctx.Process(target=_chunk_worker, args=(r, 2, port, q)) for r in range(2)]
+    procs = [ctx.Process(target=_direct_worker, args=(r, 2, port, q)) for r in range(2)]
     for p in procs:
         p.start()
     for p in procs:
