@@ -5,12 +5,11 @@
 `HeadFn`   : one deep-supervision head (MatchAssignment + NLL terms + argmax, lightglue.py:271-290,
              losses.py:6-73) as ONE autograd node.
 
-Compared with composing the same kernels through torch autograd op by op (the `engine: autograd`
-path kept in matchers/lightglue.py as the cross-check), the explicit schedule removes the per-op
-dtype casts, the cat/slice copies and ~2/3 of the launches: weights are read from a compute-dtype
-shadow refreshed once per step, weight gradients are produced in fp32 directly by the GEMM
-(`out_dtype`), the residual update emits the next GEMM's operand in the same pass, and nothing
-N x N is ever kept besides `sim`.
+Each node schedules its kernels explicitly instead of leaving the composition to torch autograd: weights
+are read from a compute-dtype shadow refreshed once per step, weight gradients are produced in fp32
+directly by the GEMM (`out_dtype`), the residual update emits the next GEMM's operand in the same
+pass, there are no per-op dtype casts or cat/slice copies, and nothing N x N is ever kept besides
+`sim`.
 
 In `precision: bf16` every GEMM of the layer and of the head -- the nine nn.Linear projections, their input-gradient
 and weight-gradient contractions -- runs on the library's own persistent wgmma GEMM (`ops.linear`: bias and
@@ -109,6 +108,39 @@ class LinearX3Fn(torch.autograd.Function):
 
 def _bgrad(dy):
     return ops.colsum(dy)
+
+
+def similarity(md0, md1, cdt, alpha=1.0):
+    """sim [B, M, N] fp32 = alpha md0 md1^T: bf16 operands on the wgmma GEMM when cdt is bf16; in the fp32 parity mode
+    cuBLAS, or the split-operand wgmma GEMM (FP32_GEMM)."""
+    if cdt == torch.bfloat16:
+        return ops.gemm_bf16(md0.to(torch.bfloat16).contiguous(), md1.to(torch.bfloat16).contiguous(), alpha=alpha)
+    if FP32_GEMM == "x3":
+        return ops.gemm_bf16(split3(md0.float(), 2, "hhl"), split3(md1.float(), 2, "hlh"), alpha=alpha)
+    sim = torch.bmm(md0, md1.transpose(1, 2))
+    return sim.mul_(alpha) if alpha != 1 else sim
+
+
+def assign_unfused_bwd(md0, md1, sim, lse_row, lse_col, gt_u8, gcoef, rowcnt, colcnt):
+    """d(mdesc0) [B, M, D], d(mdesc1) [B, N, D] (md0's dtype) of the NLL through a stored sim: dsim = gcoef (2 gt -
+    softmax_row rowcnt - softmax_col colcnt) from lgb200_assign_bwd, then dsim md1 and dsim^T md0.  The unfused
+    counterpart of ops.assign_fused_bwd, for fp32 / bf16x3 and for operands assign_fused_ok rejects."""
+    B, M, N = sim.shape
+    cdt = md0.dtype
+    tc = cdt == torch.bfloat16 and N % 8 == 0 and M % 8 == 0
+    dsim = torch.empty(B, M, N, device=sim.device, dtype=torch.bfloat16 if tc else torch.float32)
+    ops.call("lgb200_assign_bwd", ops.ptr(sim), ops.ptr(lse_row), ops.ptr(lse_col), ops.ptr(gt_u8), ops.ptr(gcoef),
+             ops.ptr(rowcnt), ops.ptr(colcnt), ops.ptr(dsim), ops._code(dsim.dtype), B, M, N, ops.stream_ptr())
+    if tc:
+        dmd0 = ops.gemm_bf16(dsim, md1, a_mn_major=False, b_mn_major=True, out_dtype=cdt)  # dsim   md1
+        dmd1 = ops.gemm_bf16(dsim, md0, a_mn_major=True, b_mn_major=True, out_dtype=cdt)   # dsim^T md0
+    elif FP32_GEMM == "x3" and N % 8 == 0:  # (TMA needs 16-byte row strides of dsim; ragged N: cuBLAS)
+        dmd0 = ops.gemm_bf16(split3(dsim, 2, "hhl"), split3(md1, 1, "hlh"), b_mn_major=True)
+        dmd1 = ops.gemm_bf16(split3(dsim, 1, "hhl"), split3(md0, 1, "hlh"), a_mn_major=True, b_mn_major=True)
+    else:
+        dmd0 = torch.bmm(dsim, md1.float()).to(cdt)
+        dmd1 = torch.bmm(dsim.transpose(1, 2), md0.float()).to(cdt)
+    return dmd0, dmd1
 
 
 def _dgrad_acc(acc, dy, w):
@@ -345,12 +377,7 @@ class HeadFn(torch.autograd.Function):
             sim = None
             st = ops.assign_fused_stats(md0, md1, alpha, ls0, ls1, gt_u8=gt["u8"])
         else:
-            if cdt == torch.bfloat16:
-                sim = ops.gemm_bf16(md0, md1, alpha=alpha)
-            elif FP32_GEMM == "x3":
-                sim = ops.gemm_bf16(split3(md0, 2, "hhl"), split3(md1, 2, "hlh"), alpha=alpha)
-            else:
-                sim = torch.bmm(md0, md1.transpose(1, 2)).mul_(alpha)
+            sim = similarity(md0, md1, cdt, alpha)
             st = ops.assign_stats(sim, ls0, ls1, du0, du1, gt_u8=gt["u8"], dense=False)
         out = torch.empty(4, B, device=dev, dtype=torch.float32)
         f0, f1 = (fin if (fin is not None and has_tok) else (None, None))
@@ -406,19 +433,7 @@ class HeadFn(torch.autograd.Function):
             dmd = torch.empty(t0 + B * N, D, device=x.device, dtype=cdt)
             ops.assign_fused_bwd(md0, md1, alpha, lse_row, lse_col, gt_u8, sim, gc, rowcnt, colcnt, dmd[:t0], dmd[t0:])
         else:
-            tc = cdt == torch.bfloat16 and N % 8 == 0 and M % 8 == 0
-            dsim = torch.empty(B, M, N, device=x.device, dtype=torch.bfloat16 if tc else torch.float32)
-            ops.call("lgb200_assign_bwd", ops.ptr(sim), ops.ptr(lse_row), ops.ptr(lse_col), ops.ptr(gt_u8), ops.ptr(gc),
-                     ops.ptr(rowcnt), ops.ptr(colcnt), ops.ptr(dsim), ops._code(dsim.dtype), B, M, N, ops.stream_ptr())
-            if tc:
-                dmd0 = ops.gemm_bf16(dsim, md1, a_mn_major=False, b_mn_major=True, out_dtype=cdt)  # dsim   md1
-                dmd1 = ops.gemm_bf16(dsim, md0, a_mn_major=True, b_mn_major=True, out_dtype=cdt)   # dsim^T md0
-            elif FP32_GEMM == "x3" and N % 8 == 0:  # (TMA needs 16-byte row strides of dsim; ragged N: cuBLAS)
-                dmd0 = ops.gemm_bf16(split3(dsim, 2, "hhl"), split3(md1, 1, "hlh"), b_mn_major=True)
-                dmd1 = ops.gemm_bf16(split3(dsim, 1, "hhl"), split3(md0, 1, "hlh"), a_mn_major=True, b_mn_major=True)
-            else:
-                dmd0 = torch.bmm(dsim, md1.float()).to(cdt)
-                dmd1 = torch.bmm(dsim.transpose(1, 2), md0.float()).to(cdt)
+            dmd0, dmd1 = assign_unfused_bwd(md0, md1, sim, lse_row, lse_col, gt_u8, gc, rowcnt, colcnt)
             dmd = torch.cat([dmd0.reshape(t0, D), dmd1.reshape(B * N, D)], 0)
         dWfp, dbfp = _wgrad(dmd, x16), _bgrad(dmd)
         # dx = dmd W_fp + dzt[:,0] wm (the token-confidence head reads a detached x, lightglue.py:82-83), dW2, db2

@@ -12,13 +12,15 @@ the reference matcher (gluefactory/models/matchers/lightglue.py:312, 630).
 
 Same constructor (`cls(conf_dict)`), same `forward(data) -> pred`, same
 `loss(pred, data) -> (losses, metrics)`, same parameter names (state_dict /
-checkpoints are interchangeable, SURVEY.md Appendix B.2).  The arithmetic of
+checkpoints are interchangeable, SURVEY.md Appendix B.2).  Each transformer
+layer is one hand-scheduled autograd node (engine.LayerFn) and each
+deep-supervision head of the loss another (engine.HeadFn).  The arithmetic of
 the N x N path -- rotary split, self / cross attention, LayerNorm+GELU, the
 assignment head, its NLL terms, argmax and match filtering, and all of their
 backward passes -- runs in the hand-written sm_90a kernels behind the C ABI
-of include/lgb200.h.  The small dense projections (nn.Linear) go through
-cuBLAS via torch.  There is no CPU path: without the built library and an H100
-`forward` raises.
+of include/lgb200.h.  There is no CPU path: without the built library and an
+H100 `forward` raises.  `loss` takes only the pred of this module's own
+`forward`, which carries the per-layer states it needs.
 
 conf additions over the reference's default_conf:
     precision: "bf16" -> bf16 operands / fp32 accumulation on the Hopper tensor cores (default)
@@ -154,10 +156,9 @@ class LightGlue(nn.Module):
         "weights_from_version": "v0.1_arxiv",
         "loss": {"gamma": 1.0, "fn": "nll", "nll_balancing": 0.5},
         "precision": "bf16",
-        "engine": "fused",  # "fused": hand-scheduled layer/head nodes (engine.py); "autograd": op-by-op cross-check
-        # pred["ref_descriptors{0,1}"] = per-layer states stacked [B, L, N, D] (lightglue.py:540-541).  Their only
-        # reader is the matcher's own loss, which the fused engine feeds from the un-stacked layer outputs instead;
-        # "auto" therefore skips the two 0.6 GB stacks while training with engine == "fused".  True: always stack.
+        # pred["ref_descriptors{0,1}"] = per-layer states stacked [B, L, N, D] (lightglue.py:540-541).  The matcher's
+        # own loss reads the un-stacked layer outputs instead, so "auto" skips the two 0.6 GB stacks while training.
+        # True: always stack.
         "stack_ref_descriptors": "auto",
     }
     required_data_keys = ["keypoints0", "keypoints1", "descriptors0", "descriptors1"]
@@ -166,7 +167,6 @@ class LightGlue(nn.Module):
         super().__init__()
         self.conf = conf = _Conf(_merge(self.default_conf, _to_plain(conf)))
         assert conf.precision in ("bf16", "fp32", "bf16x3"), conf.precision
-        assert conf.engine in ("fused", "autograd"), conf.engine
         d, h, n = conf.descriptor_dim, conf.num_heads, conf.n_layers
         assert d % h == 0 and d // h == 64, "the lgb200 kernels are built for head_dim 64"
         self.input_proj = nn.Linear(conf.input_dim, d) if conf.input_dim != d else nn.Identity()
@@ -234,47 +234,6 @@ class LightGlue(nn.Module):
             return y.view(*shp[:-1], y.shape[-1])
         return F.linear(x, layer.weight, layer.bias)
 
-    def _ffn(self, x, msg, ffn):
-        """x + Linear(GELU(LN(Linear([x, msg]))))   (lightglue.py:163, 219-220); x is the fp32 residual."""
-        cdt = torch.bfloat16 if self._bf16 else torch.float32
-        h = self._lin(torch.cat([x.to(cdt), msg.to(cdt)], -1), ffn[0])
-        h = ops.LnGelu.apply(h.contiguous(), ffn[1].weight, ffn[1].bias, ffn[1].eps)
-        return x + self._lin(h, ffn[3]).float()
-
-    def _attend(self, q, k, v, sizes, cross):
-        """q,k,v [T, D] token-major over the concatenated tokens [image0 (B*M) ; image1 (B*N)]."""
-        B, M, N = sizes
-        H = self.conf.num_heads
-        scale = 64**-0.5
-        if M == N:
-            shp = (2 * B, M, H, 64)
-            return ops.Attention.apply(q.view(shp), k.view(shp), v.view(shp), B if cross else 0, scale).view(q.shape)
-        t0 = B * M
-        q0, q1 = q[:t0].view(B, M, H, 64), q[t0:].view(B, N, H, 64)
-        k0, k1 = k[:t0].view(B, M, H, 64), k[t0:].view(B, N, H, 64)
-        v0, v1 = v[:t0].view(B, M, H, 64), v[t0:].view(B, N, H, 64)
-        if cross:
-            o0 = ops.Attention.apply(q0, k1, v1, 0, scale)
-            o1 = ops.Attention.apply(q1, k0, v0, 0, scale)
-        else:
-            o0 = ops.Attention.apply(q0, k0, v0, 0, scale)
-            o1 = ops.Attention.apply(q1, k1, v1, 0, scale)
-        return torch.cat([o0.reshape(t0, -1), o1.reshape(B * N, -1)], 0)
-
-    def _layer(self, x, theta, layer, sizes):
-        H = self.conf.num_heads
-        sa, ca = layer.self_attn, layer.cross_attn
-        # ---- self block (lightglue.py:150-163)
-        qkv = self._lin(x, sa.Wqkv).contiguous()
-        q, k, v = ops.RopeSplit.apply(qkv, theta, H)
-        ctx = self._attend(q, k, v, sizes, cross=False)
-        x = self._ffn(x, self._lin(ctx, sa.out_proj), sa.ffn)
-        # ---- cross block (lightglue.py:195-221); both directions share to_qk / to_v
-        qk = self._lin(x, ca.to_qk).contiguous()
-        vv = self._lin(x, ca.to_v).contiguous()
-        m = self._attend(qk, qk, vv, sizes, cross=True)
-        return self._ffn(x, self._lin(m, ca.to_out), ca.ffn)
-
     def _head_inputs(self, d0, d1, i):
         """final_proj / matchability of layer i (lightglue.py:280-285)."""
         la = self.log_assignment[i]
@@ -325,23 +284,18 @@ class LightGlue(nn.Module):
         sizes = (B, M, N)
         all0, all1, layers_x = [], [], []
         L = conf.n_layers
-        fused = conf.engine == "fused"
-        if fused:
-            self._refresh_shadow()
+        self._refresh_shadow()
         if adaptive:
             return self._forward_adaptive(x, theta, sizes)
-        # head -> layer gradient hand-over of the fused training step (engine.LayerFn / HeadFn docstrings)
-        stash = {} if (fused and self.training and torch.is_grad_enabled()) else None
+        # head -> layer gradient hand-over of the training step (engine.LayerFn / HeadFn docstrings)
+        stash = {} if (self.training and torch.is_grad_enabled()) else None
         for i in range(L):
-            if fused:
-                w, params = self._layer_weights(i)
-                fp = getattr(self, "_b200_flat", None)
-                fp = fp if (fp is not None and fp.direct_groups) else None
-                sink = (fp, i, stash) if torch.is_grad_enabled() else None
-                x = engine.LayerFn.apply(x, theta, sizes, conf.num_heads, self._cdt, self.transformers[i].self_attn.ffn[1].eps,
-                                         w, sink, *params)
-            else:
-                x = self._layer(x, theta, self.transformers[i], sizes)
+            w, params = self._layer_weights(i)
+            fp = getattr(self, "_b200_flat", None)
+            fp = fp if (fp is not None and fp.direct_groups) else None
+            sink = (fp, i, stash) if torch.is_grad_enabled() else None
+            x = engine.LayerFn.apply(x, theta, sizes, conf.num_heads, self._cdt, self.transformers[i].self_attn.ffn[1].eps,
+                                     w, sink, *params)
             if self.training or i == L - 1:
                 layers_x.append(x)
                 all0.append(x[: B * M].view(B, M, D))
@@ -349,7 +303,7 @@ class LightGlue(nn.Module):
         d0, d1 = all0[-1], all1[-1]
         with torch.no_grad():
             md0, md1, z0, z1 = self._head_inputs(d0, d1, L - 1)
-            sim = ops._similarity(md0, md1, self._bf16)
+            sim = engine.similarity(md0, md1, self._cdt)
             st = ops.assign_stats(sim, F.logsigmoid(z0), F.logsigmoid(z1), F.logsigmoid(-z0), F.logsigmoid(-z1),
                                   dense=True)
             m0, m1, ms0, ms1 = ops.filter_matches(st["rowmax"], st["rowarg"], st["colarg"], conf.filter_threshold)
@@ -362,22 +316,21 @@ class LightGlue(nn.Module):
             "prune0": torch.ones_like(ms0) * L,
             "prune1": torch.ones_like(ms1) * L,
         }
-        if conf.stack_ref_descriptors is True or not (fused and self.training):
+        if conf.stack_ref_descriptors is True or not self.training:
             pred["ref_descriptors0"] = torch.stack(all0, 1)
             pred["ref_descriptors1"] = torch.stack(all1, 1)
-        if fused:
-            # private side channel for loss(): the per-layer token tensors (both images, [T, D]); avoids
-            # slicing the stacked ref_descriptors (whose backward would scatter into 9 zero-filled stacks).
-            # Also the final layer's argmax including the dustbin (labels of TokenConfidence.loss) and the
-            # row_norm monitor, both by-products of the dense pass.
-            pred["_b200_layers"] = layers_x
-            pred["_b200_sizes"] = sizes
-            pred["_b200_stash"] = stash
-            du0, du1 = F.logsigmoid(-z0), F.logsigmoid(-z1)
-            pred["_b200_final_arg"] = (
-                self._argmax_with_dustbin(st["rowmax"], st["rowarg"], du0, N).contiguous(),
-                self._argmax_with_dustbin(st["colmax"], st["colarg"], du1, M).contiguous())
-            pred["_b200_row_expsum"] = st["row_expsum"]
+        # private side channel for loss(): the per-layer token tensors (both images, [T, D]); avoids
+        # slicing the stacked ref_descriptors (whose backward would scatter into 9 zero-filled stacks).
+        # Also the final layer's argmax including the dustbin (labels of TokenConfidence.loss) and the
+        # row_norm monitor, both by-products of the dense pass.
+        pred["_b200_layers"] = layers_x
+        pred["_b200_sizes"] = sizes
+        pred["_b200_stash"] = stash
+        du0, du1 = F.logsigmoid(-z0), F.logsigmoid(-z1)
+        pred["_b200_final_arg"] = (
+            self._argmax_with_dustbin(st["rowmax"], st["rowarg"], du0, N).contiguous(),
+            self._argmax_with_dustbin(st["colmax"], st["colarg"], du1, M).contiguous())
+        pred["_b200_row_expsum"] = st["row_expsum"]
         return pred
 
     # ------------------------------------------------------------------------------------------
@@ -393,7 +346,6 @@ class LightGlue(nn.Module):
         conf = self.conf
         B, M, N = sizes
         assert B == 1, "adaptive depth / width runs one pair at a time (lightglue.py:487, 492)"
-        assert conf.engine == "fused"
         dev, D, L = x.device, conf.descriptor_dim, conf.n_layers
         do_stop, do_prune = conf.depth_confidence > 0, conf.width_confidence > 0
         ind0, ind1 = torch.arange(M, device=dev), torch.arange(N, device=dev)
@@ -431,7 +383,7 @@ class LightGlue(nn.Module):
                 prune1[:, ind1] += 1
         d0, d1 = x[:m].view(1, m, D), x[m:].view(1, n, D)
         md0, md1, z0, z1 = self._head_inputs(d0, d1, last)
-        sim = ops._similarity(md0, md1, self._bf16)
+        sim = engine.similarity(md0, md1, self._cdt)
         st = ops.assign_stats(sim, F.logsigmoid(z0), F.logsigmoid(z1), F.logsigmoid(-z0), F.logsigmoid(-z1), dense=True)
         m0, m1, ms0, ms1 = ops.filter_matches(st["rowmax"], st["rowarg"], st["colarg"], conf.filter_threshold)
         if do_prune:  # scatter back to the full keypoint sets (lightglue.py:517-526)
@@ -445,17 +397,33 @@ class LightGlue(nn.Module):
             m0, m1, ms0, ms1 = m0_, m1_, ms0_, ms1_
         else:
             prune0, prune1 = torch.ones_like(ms0) * L, torch.ones_like(ms1) * L
+        # for loss(): one state, which gets head n_layers - 1 as in eval mode; a pruned pred (m, n < M, N) is rejected there
         return {"matches0": m0, "matches1": m1, "matching_scores0": ms0, "matching_scores1": ms1,
                 "ref_descriptors0": d0[:, None], "ref_descriptors1": d1[:, None], "log_assignment": st["scores"],
-                "prune0": prune0, "prune1": prune1, "stop_layer": last}
+                "prune0": prune0, "prune1": prune1, "stop_layer": last,
+                "_b200_layers": [x], "_b200_sizes": (1, m, n), "_b200_row_expsum": st["row_expsum"]}
 
     # ------------------------------------------------------------------------------------------
-    def _loss_fused(self, pred, data, layers_x, gt_u8, rowcnt, colcnt, neg0, neg1, num_pos, num_neg0, num_neg1):
+    def _loss(self, pred, data):
         """lightglue.py:578-627 on the hand-scheduled heads (engine.HeadFn): per layer one autograd node that
         yields the NLL and the token-confidence BCE; the O(M+N) terms are two small fused kernels."""
         conf = self.conf
-        B, M, N = pred["_b200_sizes"]
-        L = len(layers_x)
+        layers_x = pred.get("_b200_layers")
+        if layers_x is None:
+            raise ValueError("LightGlue.loss needs the pred of this module's own forward: pred['_b200_layers'] is missing")
+        (B, M, N), L = pred["_b200_sizes"], len(layers_x)
+        gt = data["gt_assignment"]
+        if tuple(gt.shape) != (B, M, N):
+            raise ValueError(f"gt_assignment has shape {tuple(gt.shape)} but the forward ran on (B, M, N) = {(B, M, N)}; "
+                             "the loss cannot be taken after point pruning (width_confidence)")
+        gt_u8 = gt.contiguous().view(torch.uint8) if gt.dtype == torch.bool else gt.to(torch.uint8).contiguous()
+        # both counts in one pass over the 4.2 MB/pair mask (`gt.sum(2)` / `gt.sum(1)` each widen it first: int64 by
+        # default, fp32 with dtype=)
+        rowcnt, colcnt = ops.mask_counts(gt_u8)
+        neg0 = (data["gt_matches0"] == -1).float()
+        neg1 = (data["gt_matches1"] == -1).float()
+        num_pos = rowcnt.sum(1).clamp(min=1.0)
+        num_neg0, num_neg1 = neg0.sum(1).clamp(min=1.0), neg1.sum(1).clamp(min=1.0)
         gtd = {"u8": gt_u8, "rowcnt": rowcnt.contiguous(), "colcnt": colcnt.contiguous(), "neg0": neg0.contiguous(),
                "neg1": neg1.contiguous(), "num_pos": num_pos.contiguous(), "num_neg": (num_neg0 + num_neg1).contiguous()}
         if self._bf16 and torch.is_grad_enabled():
@@ -463,11 +431,7 @@ class LightGlue(nn.Module):
             gt_t = data.get("gt_assignment_t")  # written by the plugin's ground-truth components when asked to
             gtd["u8_t"] = (gt_t.contiguous().view(torch.uint8) if gt_t is not None and gt_t.dtype == torch.bool
                            else gt_u8.transpose(1, 2).contiguous())
-        la = pred["log_assignment"].detach()
-        fin = pred.get("_b200_final_arg")
-        if fin is None and L > 1:
-            fin = (la[:, :-1, :].max(-1).indices.to(torch.int32).contiguous(),
-                   la[:, :, :-1].max(-2).indices.to(torch.int32).contiguous())
+        fin = pred.get("_b200_final_arg")  # read only for L > 1, i.e. a training-mode forward, which always sets it
 
         def head(i):
             # the last stacked state always belongs to the LAST layer's head (lightglue.py:588 `loss_params(pred, -1)`):
@@ -497,8 +461,7 @@ class LightGlue(nn.Module):
         }
         if self.training:
             losses["confidence"] = 0.0
-        rn = pred.get("_b200_row_expsum")
-        losses["row_norm"] = rn.mean(1) if rn is not None else la.exp()[:, :-1].sum(2).mean(1)
+        losses["row_norm"] = pred["_b200_row_expsum"].mean(1)
         sum_weights = 1.0
         for i in range(L - 1):
             nll_i, conf_i, _, _ = head(i)
@@ -523,79 +486,6 @@ class LightGlue(nn.Module):
         with the ambient autocast disabled; its backward is linear in the incoming gradient (GradScaler, train.py:490)."""
         with torch.autocast(device_type="cuda", enabled=False), engine.fp32_gemm(self._gemm_mode):
             return self._loss(pred, data)
-
-    def _loss(self, pred, data):
-        conf = self.conf
-        ref0, ref1 = pred.get("ref_descriptors0"), pred.get("ref_descriptors1")
-        if ref0 is not None:
-            B, L, M, D = ref0.shape
-            N = ref1.shape[2]
-        else:  # fused training step without the stacked copies (conf.stack_ref_descriptors == "auto")
-            (B, M, N), L = pred["_b200_sizes"], len(pred["_b200_layers"])
-        gt = data["gt_assignment"]
-        gt_u8 = gt.contiguous().view(torch.uint8) if gt.dtype == torch.bool else gt.to(torch.uint8).contiguous()
-        # both counts in one pass over the 4.2 MB/pair mask (`gt.sum(2)` / `gt.sum(1)` each widen it first: int64 by
-        # default, fp32 with dtype=)
-        rowcnt, colcnt = ops.mask_counts(gt_u8)
-        neg0 = (data["gt_matches0"] == -1).float()
-        neg1 = (data["gt_matches1"] == -1).float()
-        num_pos = rowcnt.sum(1).clamp(min=1.0)
-        num_neg0, num_neg1 = neg0.sum(1).clamp(min=1.0), neg1.sum(1).clamp(min=1.0)
-        bal = conf.loss.nll_balancing
-
-        def head(i):
-            d0, d1 = ref0[:, i], ref1[:, i]
-            md0, md1, z0, z1 = self._head_inputs(d0, d1, conf.n_layers - 1 if i == L - 1 else i)  # lightglue.py:588
-            ls0, ls1, du0, du1 = F.logsigmoid(z0), F.logsigmoid(z1), F.logsigmoid(-z0), F.logsigmoid(-z1)
-            s_pos, rmax, rarg, cmax, carg = ops.AssignPositives.apply(md0, md1, ls0, ls1, du0, du1, gt_u8, rowcnt,
-                                                                      colcnt, self._bf16)
-            pos = s_pos + (rowcnt * ls0).sum(1) + (colcnt * ls1).sum(1)
-            nll_pos = -pos / num_pos
-            nll_neg = -((neg0 * du0).sum(1) + (neg1 * du1).sum(1)) / (num_neg0 + num_neg1)
-            nll = bal * nll_pos + (1 - bal) * nll_neg
-            arg0 = self._argmax_with_dustbin(rmax, rarg, du0.detach(), N)
-            arg1 = self._argmax_with_dustbin(cmax, carg, du1.detach(), M)
-            return nll, nll_pos, nll_neg, arg0, arg1
-
-        layers_x = pred.get("_b200_layers") if conf.engine == "fused" else None
-        if layers_x is not None and len(layers_x) == L:
-            return self._loss_fused(pred, data, layers_x, gt_u8, rowcnt, colcnt, neg0, neg1, num_pos, num_neg0, num_neg1)
-
-        nll, nll_pos, nll_neg, _, _ = head(L - 1)
-        losses = {
-            "total": nll,
-            "last": nll.clone().detach(),
-            "assignment_nll": nll,
-            "nll_pos": nll_pos,
-            "nll_neg": nll_neg,
-            "num_matchable": num_pos,
-            "num_unmatchable": (num_neg0 + num_neg1) / 2.0,
-        }
-        if self.training:
-            losses["confidence"] = 0.0
-        la = pred["log_assignment"].detach()
-        losses["row_norm"] = la.exp()[:, :-1].sum(2).mean(1)
-        if L > 1:
-            fin0 = la[:, :-1, :].max(-1).indices.to(torch.int32)
-            fin1 = la[:, :, :-1].max(-2).indices.to(torch.int32)
-        sum_weights = 1.0
-        for i in range(L - 1):
-            nll_i, _, _, arg0, arg1 = head(i)
-            weight = conf.loss.gamma ** (L - i - 1) if conf.loss.gamma > 0.0 else i + 1
-            sum_weights += weight
-            losses["total"] = losses["total"] + nll_i * weight
-            tok = self.token_confidence[i].token[0]
-            logit0 = F.linear(ref0[:, i].detach(), tok.weight, tok.bias).squeeze(-1)
-            logit1 = F.linear(ref1[:, i].detach(), tok.weight, tok.bias).squeeze(-1)
-            bce = F.binary_cross_entropy_with_logits
-            conf_i = (bce(logit0, (fin0 == arg0).float(), reduction="none").mean(-1)
-                      + bce(logit1, (fin1 == arg1).float(), reduction="none").mean(-1)) / 2.0
-            losses["confidence"] = losses["confidence"] + conf_i / (L - 1)
-        losses["total"] = losses["total"] / sum_weights
-        if self.training:
-            losses["total"] = losses["total"] + losses["confidence"]
-        metrics = {} if self.training else matcher_metrics(pred, data)
-        return losses, metrics
 
 
 @torch.no_grad()

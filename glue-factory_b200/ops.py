@@ -57,23 +57,6 @@ def rope_bwd(dq, dk, dv, q, k, theta, H, dtheta=None):
     return dqkv, dtheta
 
 
-class RopeSplit(torch.autograd.Function):
-    """qkv [T, H*192] (interleaved) , theta [T, 32] -> rotated q, rotated k, v  each [T, H*64]."""
-
-    @staticmethod
-    def forward(ctx, qkv, theta, H):
-        q, k, v = rope_fwd(qkv, theta, H)
-        ctx.save_for_backward(q, k, theta)
-        ctx.H = H
-        return q, k, v
-
-    @staticmethod
-    def backward(ctx, dq, dk, dv):
-        q, k, theta = ctx.saved_tensors
-        dqkv, dtheta = rope_bwd(dq, dk, dv, q, k, theta, ctx.H)
-        return dqkv, dtheta, None
-
-
 # ------------------------------------------------------------------------------------------------
 # attention (lightglue.py:118-121, 207-216)
 # ------------------------------------------------------------------------------------------------
@@ -164,20 +147,6 @@ def ln_gelu_bwd(dy, x, g, b, mean, rstd, want_dxsum=False):
     if want_dxsum:
         return dx, sums[0], sums[1], sums[2]
     return dx, sums[0], sums[1]
-
-
-class LnGelu(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, gamma, beta, eps):
-        g, b = gamma.float().contiguous(), beta.float().contiguous()
-        y, mean, rstd = ln_gelu_fwd(x, g, b, eps)
-        ctx.save_for_backward(x, g, b, mean, rstd)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        dx, dg, db = ln_gelu_bwd(dy, *ctx.saved_tensors)
-        return dx, dg, db, None
 
 
 _colsum_counters = {}
@@ -444,7 +413,8 @@ def linear(a, w, bias=None, out=None, out_dtype=torch.bfloat16, w_is_kn=False, a
 class LinearFn(torch.autograd.Function):
     """nn.Linear on the library's GEMMs with autograd: x [T, in] bf16, weight [out, in] / bias [out] fp32 parameters.
     forward y = x W^T + b (bf16 out, fp32 bias in the epilogue); backward dgrad (bf16), split-K wgrad (fp32), bias
-    gradient by the column-sum kernel.  Used by the op-by-op `engine: autograd` composition and for input_proj."""
+    gradient by the column-sum kernel.  Used for LightGlue's input_proj and dense final head in bf16, and for
+    GlueStick's 1x1 convolutions."""
 
     @staticmethod
     def forward(ctx, x, weight, bias):
@@ -463,16 +433,6 @@ class LinearFn(torch.autograd.Function):
 # ------------------------------------------------------------------------------------------------
 # assignment head (lightglue.py:256-290, losses.py)
 # ------------------------------------------------------------------------------------------------
-def _similarity(md0, md1, bf16):
-    if bf16:
-        return gemm_bf16(md0.to(torch.bfloat16).contiguous(), md1.to(torch.bfloat16).contiguous())
-    from . import engine
-
-    if engine.FP32_GEMM == "x3":  # split-operand wgmma GEMM (precision: bf16x3)
-        return gemm_bf16(engine.split3(md0.float(), 2, "hhl"), engine.split3(md1.float(), 2, "hlh"))
-    return torch.bmm(md0, md1.transpose(1, 2))
-
-
 def assign_stats(sim, ls0, ls1, dust0, dust1, gt_u8=None, dense=False):
     """Runs the two assignment passes on sim [B,M,N].  Returns a dict with lse_row/lse_col,
     rowmax/rowarg/colmax/colarg (int32, dustbin excluded), optional pos_row_sum, and when
@@ -535,44 +495,6 @@ def assign_fused_bwd(md0, md1, alpha, lse_row, lse_col, gt_u8, gt_t_u8, gcoef, r
     _chk(gt_u8), _chk(gt_t_u8), _chk(dmd0, torch.bfloat16), _chk(dmd1, torch.bfloat16)
     call("lgb200_assign_fused_bwd", ptr(md0), ptr(md1), float(alpha), ptr(lse_row), ptr(lse_col), ptr(gt_u8), ptr(gt_t_u8),
          ptr(gcoef), ptr(rowcnt), ptr(colcnt), ptr(dmd0), ptr(dmd1), B, M, N, D, stream_ptr())
-
-
-class AssignPositives(torch.autograd.Function):
-    """(mdesc0 [B,M,D], mdesc1 [B,N,D]) -> S_pos [B] = sum_ij gt_ij (2 sim_ij - lse_row_i - lse_col_j)
-    with sim = mdesc0 mdesc1^T, i.e. the similarity-dependent part of sum_P log_assignment
-    (the matchability terms are O(M+N) and are added by the caller).  Also returns the
-    (non-differentiable) row / column argmax of the full scores.  The dense log-assignment is
-    never written; backward recomputes the two softmaxes from the saved sim and LSE vectors
-    (SURVEY.md Appendix A.4)."""
-
-    @staticmethod
-    def forward(ctx, md0, md1, ls0, ls1, dust0, dust1, gt_u8, rowcnt, colcnt, bf16):
-        sim = _similarity(md0, md1, bf16)
-        st = assign_stats(sim, ls0, ls1, dust0, dust1, gt_u8=gt_u8, dense=False)
-        ctx.save_for_backward(md0, md1, sim, st["lse_row"], st["lse_col"], gt_u8, rowcnt, colcnt)
-        ctx.bf16 = bf16
-        for k in ("rowmax", "rowarg", "colmax", "colarg"):
-            ctx.mark_non_differentiable(st[k])
-        return st["pos_row_sum"].sum(1), st["rowmax"], st["rowarg"], st["colmax"], st["colarg"]
-
-    @staticmethod
-    def backward(ctx, g, *_):
-        md0, md1, sim, lse_row, lse_col, gt_u8, rowcnt, colcnt = ctx.saved_tensors
-        B, M, N = sim.shape
-        g = g.float().contiguous()
-        tc = ctx.bf16 and N % 8 == 0 and M % 8 == 0
-        dsim = torch.empty(B, M, N, device=sim.device, dtype=torch.bfloat16 if tc else torch.float32)
-        call("lgb200_assign_bwd", ptr(sim), ptr(lse_row), ptr(lse_col), ptr(gt_u8), ptr(g), ptr(rowcnt), ptr(colcnt),
-             ptr(dsim), _code(dsim.dtype), B, M, N, stream_ptr())
-        if tc:
-            b0 = md0.to(torch.bfloat16).contiguous()
-            b1 = md1.to(torch.bfloat16).contiguous()
-            dmd0 = gemm_bf16(dsim, b1, a_mn_major=False, b_mn_major=True)  # dsim @ md1
-            dmd1 = gemm_bf16(dsim, b0, a_mn_major=True, b_mn_major=True)   # dsim^T @ md0
-        else:
-            dmd0 = torch.bmm(dsim, md1.float())
-            dmd1 = torch.bmm(dsim.transpose(1, 2), md0.float())
-        return dmd0.to(md0.dtype), dmd1.to(md1.dtype), None, None, None, None, None, None, None, None
 
 
 def head_logsig(zt):

@@ -149,7 +149,7 @@ class MatcherTrainer:
         self.v = torch.zeros_like(self.fp.flat)
         self.betas, self.eps, self.wd = betas, eps, weight_decay
         layers = getattr(model, "transformers", None)
-        if layers is not None and getattr(getattr(model, "conf", None), "engine", None) == "fused":
+        if layers is not None:
             self.fp.enable_direct([list(layer.parameters()) for layer in layers])
         self._lr_dev = torch.full((1,), float(lr), device=dev, dtype=torch.float32)
         self._t_dev = torch.zeros(1, device=dev, dtype=torch.int32)

@@ -18,7 +18,7 @@ def build_pipeline(conf, weights, device="cpu", checkpointed=False, flash=False)
     """conf: LightGlue conf (synthetic.DEFAULT_CONF keys); weights: state_dict under the reference names."""
     get_model = import_reference()
     assert get_model is not None, "reference not installed under oracle/_ref (run oracle/stage_reference.py)"
-    matcher_conf = {k: v for k, v in conf.items() if k not in ("precision", "engine", "stack_ref_descriptors")}
+    matcher_conf = {k: v for k, v in conf.items() if k not in ("precision", "stack_ref_descriptors")}
     matcher_conf.update(name="matchers.lightglue", checkpointed=bool(checkpointed), flash=bool(flash))
     pipe = get_model("two_view_pipeline")({
         "extractor": {"name": None}, "matcher": matcher_conf, "ground_truth": {"name": None},

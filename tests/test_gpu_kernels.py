@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 import torch
 
-from gluefactory_b200 import ops
+from gluefactory_b200 import engine, ops
 from oracle import lightglue_oracle as O
 from tests.util import GOLDEN, rel_err
 
@@ -229,41 +229,41 @@ def test_linear_generic_kernel_agrees_with_panel_resident():
 
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("dtype,tol", [(torch.float32, 1e-6), (torch.bfloat16, 8e-3)])
-def test_rope_split(dtype, tol):
+def test_rope_fwd_bwd(dtype, tol):
     T, H = 333, 4
-    qkv = _rand(T, H * 192, seed=1, dtype=dtype).requires_grad_(True)
-    theta = _rand(T, 32, seed=2, scale=3.0).requires_grad_(True)
-    q, k, v = ops.RopeSplit.apply(qkv, theta, H)
+    qkv = _rand(T, H * 192, seed=1, dtype=dtype)
+    theta = _rand(T, 32, seed=2, scale=3.0)
+    q, k, v = ops.rope_fwd(qkv, theta, H)
     gq, gk, gv = (_rand(T, H * 64, seed=s, dtype=dtype) for s in (3, 4, 5))
-    torch.autograd.backward([q, k, v], [gq, gk, gv])
+    dqkv, dtheta = ops.rope_bwd(gq, gk, gv, q, k, theta, H)
     # oracle: lightglue.py:157-160 + 42-49
-    x = qkv.detach().double().requires_grad_(True)
-    th = theta.detach().double().requires_grad_(True)
+    x = qkv.double().requires_grad_(True)
+    th = theta.double().requires_grad_(True)
     t = x.view(1, T, H, 64, 3).permute(0, 2, 1, 3, 4)
     rq, rk, rv = O.rope(t[..., 0], th[None]), O.rope(t[..., 1], th[None]), t[..., 2]
     back = lambda z: z.permute(0, 2, 1, 3).reshape(T, H * 64)  # noqa: E731
     torch.autograd.backward([back(rq), back(rk), back(rv)], [gq.double(), gk.double(), gv.double()])
     assert rel_err(q, back(rq)) < tol and rel_err(k, back(rk)) < tol and rel_err(v, back(rv)) < tol
-    assert rel_err(qkv.grad, x.grad) < tol
-    assert rel_err(theta.grad, th.grad) < (1e-5 if dtype == torch.float32 else 2e-2)
+    assert rel_err(dqkv, x.grad) < tol
+    assert rel_err(dtheta, th.grad) < (1e-5 if dtype == torch.float32 else 2e-2)
 
 
 @pytest.mark.parametrize("dtype,tol", [(torch.float32, 2e-6), (torch.bfloat16, 8e-3)])
 @pytest.mark.parametrize("W", [256, 512])
-def test_ln_gelu(dtype, tol, W):
+def test_ln_gelu_fwd_bwd(dtype, tol, W):
     T = 1001
-    x = _rand(T, W, seed=1, dtype=dtype, scale=2.0).requires_grad_(True)
-    g = (1 + 0.1 * _rand(W, seed=2)).requires_grad_(True)
-    b = (0.1 * _rand(W, seed=3)).requires_grad_(True)
+    x = _rand(T, W, seed=1, dtype=dtype, scale=2.0)
+    g = 1 + 0.1 * _rand(W, seed=2)
+    b = 0.1 * _rand(W, seed=3)
     gy = _rand(T, W, seed=4, dtype=dtype)
-    y = ops.LnGelu.apply(x, g, b, 1e-5)
-    y.backward(gy)
-    xr, gr, br = (t.detach().double().requires_grad_(True) for t in (x, g, b))
+    y, mean, rstd = ops.ln_gelu_fwd(x, g, b, 1e-5)
+    dx, dg, db = ops.ln_gelu_bwd(gy, x, g, b, mean, rstd)
+    xr, gr, br = (t.double().requires_grad_(True) for t in (x, g, b))
     ref = torch.nn.functional.gelu(torch.nn.functional.layer_norm(xr, (W,), gr, br, 1e-5))
     ref.backward(gy.double())
     assert rel_err(y, ref) < tol
-    assert rel_err(x.grad, xr.grad) < tol
-    assert rel_err(g.grad, gr.grad) < max(tol, 1e-5) and rel_err(b.grad, br.grad) < max(tol, 1e-5)
+    assert rel_err(dx, xr.grad) < tol
+    assert rel_err(dg, gr.grad) < max(tol, 1e-5) and rel_err(db, br.grad) < max(tol, 1e-5)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -305,25 +305,31 @@ def test_assignment_head_matches_oracle(B, M, N):
 
 @pytest.mark.parametrize("bf16", [False, True])
 @pytest.mark.parametrize("B,M,N", [(2, 128, 128), (1, 200, 136), (2, 100, 250)])
-def test_assign_positives_backward(bf16, B, M, N):
+def test_assign_unfused_positives_and_dmd(bf16, B, M, N):
+    """The unfused head's positive term S_pos [B] = sum_ij gt_ij (2 sim_ij - lse_row_i - lse_col_j), sim = md0 md1^T
+    (assign_stats' pos_row_sum), and its d(mdesc) for a weight gw per pair (engine.assign_unfused_bwd)."""
     D = 256
-    md0 = _rand(B, M, D, seed=1, scale=0.3).requires_grad_(True)
-    md1 = _rand(B, N, D, seed=2, scale=0.3).requires_grad_(True)
+    cdt = torch.bfloat16 if bf16 else torch.float32
+    md0 = _rand(B, M, D, seed=1, scale=0.3)
+    md1 = _rand(B, N, D, seed=2, scale=0.3)
     z0, z1 = _rand(B, M, seed=3), _rand(B, N, seed=4)
     gt = (torch.rand(B, M, N, generator=torch.Generator().manual_seed(5)) < 0.02).to(DEV)
+    gt_u8 = gt.view(torch.uint8)
     ls = torch.nn.functional.logsigmoid
-    s_pos, *_ = ops.AssignPositives.apply(md0, md1, ls(z0), ls(z1), ls(-z0), ls(-z1), gt.view(torch.uint8),
-                                          gt.sum(2).float(), gt.sum(1).float(), bf16)
+    sim = engine.similarity(md0, md1, cdt)
+    st = ops.assign_stats(sim, ls(z0), ls(z1), ls(-z0), ls(-z1), gt_u8=gt_u8)
+    s_pos = st["pos_row_sum"].sum(1)
     gw = _rand(B, seed=6)
-    (s_pos * gw).sum().backward()
+    dmd0, dmd1 = engine.assign_unfused_bwd(md0.to(cdt), md1.to(cdt), sim, st["lse_row"], st["lse_col"], gt_u8, gw,
+                                           gt.sum(2).float(), gt.sum(1).float())
     rnd = O.bf16_round if bf16 else (lambda t: t)
-    a, b = rnd(md0.detach()).double().requires_grad_(True), rnd(md1.detach()).double().requires_grad_(True)
+    a, b = rnd(md0).double().requires_grad_(True), rnd(md1).double().requires_grad_(True)
     sim = a @ b.transpose(1, 2)
     ref = ((2 * sim - torch.logsumexp(sim, 2, keepdim=True) - torch.logsumexp(sim, 1, keepdim=True)) * gt).sum((1, 2))
     (ref * gw.double()).sum().backward()
     tol = 2e-2 if bf16 else 1e-4
     assert rel_err(s_pos, ref) < (1e-3 if bf16 else 1e-5)
-    assert rel_err(md0.grad, a.grad) < tol and rel_err(md1.grad, b.grad) < tol
+    assert rel_err(dmd0, a.grad) < tol and rel_err(dmd1, b.grad) < tol
 
 
 def test_other_heads_match_golden():

@@ -15,14 +15,14 @@ from gluefactory_b200 import synthetic
 from gluefactory_b200.matchers.lightglue import LightGlue
 from gluefactory_b200.trainer import MatcherTrainer
 from oracle import lightglue_oracle as O
-from tests.util import CASES, EXTRA_CASES, check_grad_summary, load_case, rel_err
+from tests.util import CASES, EXTRA_CASES, check_grad_summary, load_case, mirror_oracle, rel_err, report
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 
 
-def _build(conf, weights, precision, engine="fused"):
-    model = LightGlue(dict(conf, precision=precision, engine=engine))
+def _build(conf, weights, precision):
+    model = LightGlue(dict(conf, precision=precision))
     missing, unexpected = model.load_state_dict({k: v.float() for k, v in weights.items()}, strict=False)
     assert not unexpected and missing in ([], ["confidence_thresholds"])
     return model.to(DEV).train()
@@ -33,11 +33,10 @@ def _f32(data):
                                     (v.float() if v.is_floating_point() else v)) for k, v in data.items()}, DEV)
 
 
-@pytest.mark.parametrize("engine", ["fused", "autograd"])
 @pytest.mark.parametrize("name", CASES[:4] + EXTRA_CASES)
-def test_fp32_path_matches_reference_golden(name, engine):
+def test_fp32_path_matches_reference_golden(name):
     g, conf, w, data = load_case(name)
-    model = _build(conf, w, "fp32", engine)
+    model = _build(conf, w, "fp32")
     d = _f32(data)
     pred = model(d)
     losses, _ = model.loss(pred, d)
@@ -120,12 +119,21 @@ def test_bf16_path_close_to_reference_golden(name):
     assert worst < 0.1, worst
 
 
-@pytest.mark.parametrize("precision,tol", [("fp32", 1e-3), ("bf16", 3e-2)])
-def test_ragged_sizes_against_oracle(precision, tol):
-    """M != N and not multiples of the tile sizes (reference supports any keypoint count)."""
+# fp32 path against fp64 at the two shapes below, bound on the log-assignment, each loss entry and each parameter
+# gradient.  Measured on an H100 80GB HBM3 (400 W limit), worst of both shapes: log-assignment 9.8e-8, loss entries
+# 7.3e-8, gradients 2.7e-6 (the shared cross-attention to_qk bias).
+FP32_VS_FP64 = 2e-5
+
+
+@pytest.mark.parametrize("precision", ["fp32", "bf16"])
+@pytest.mark.parametrize("M,N", [(192, 192), (150, 203)])
+def test_ragged_sizes_against_oracle(M, N, precision):
+    """Forward, loss and backward against the fp64 oracle at M == N (both images in one launch) and at M != N, neither
+    a multiple of the tile sizes (the reference supports any keypoint count).  bf16 is also held to the oracle evaluated
+    with the CUDA path's bf16 rounding model (O.Bf16Mirror)."""
     conf = dict(synthetic.DEFAULT_CONF, n_layers=2)
     w = synthetic.make_weights(conf, seed=21)
-    data = synthetic.make_pairs(2, 203, seed=22, M=150)
+    data = synthetic.make_pairs(2, N, seed=22, M=M)
     model = _build(conf, w, precision)
     d = synthetic.to_device(data, DEV)
     pred = model(d)
@@ -137,12 +145,33 @@ def test_ragged_sizes_against_oracle(precision, tol):
     rp = O.lightglue_forward(w64, d64, conf)
     rl = O.lightglue_loss(w64, rp, d64, conf)
     rl["total"].mean().backward()
-    assert rel_err(losses["total"], rl["total"]) < tol
-    assert rel_err(pred["log_assignment"], rp["log_assignment"]) < tol
+    e_la = rel_err(pred["log_assignment"], rp["log_assignment"])
+    e_loss = {k: rel_err(losses[k], rl[k]) for k in rl if torch.is_tensor(rl[k])}
+    e_grad = {k: rel_err(p.grad, w64[k].grad) for k, p in model.named_parameters()}
+    report(f"ragged:{precision}:M{M}:N{N}:fp64", la=e_la, loss_max=max(e_loss.values()),
+           loss_max_key=max(e_loss, key=e_loss.get), grad_max=max(e_grad.values()), grad_max_key=max(e_grad, key=e_grad.get))
     if precision == "fp32":
         assert torch.equal(pred["matches0"].cpu(), rp["matches0"])
-    for k, p in model.named_parameters():
-        assert rel_err(p.grad, w64[k].grad) < (1e-3 if precision == "fp32" else 0.15), k
+        assert e_la < FP32_VS_FP64, e_la
+        for k, e in e_loss.items():
+            assert e < FP32_VS_FP64, (k, e)
+        for k, e in e_grad.items():
+            assert e < FP32_VS_FP64, (k, e)
+        return
+    assert e_loss["total"] < 3e-2 and e_la < 3e-2, (e_loss["total"], e_la)
+    for k, e in e_grad.items():
+        assert e < 0.15, (k, e)
+    mp, ml, mg = mirror_oracle(conf, w, data)
+    m_la = rel_err(pred["log_assignment"], mp["log_assignment"])
+    m_loss = {k: rel_err(losses[k], ml[k]) for k in ml if torch.is_tensor(ml[k])}
+    m_grad = {k: rel_err(p.grad, mg[k]) for k, p in model.named_parameters()}
+    report(f"ragged:bf16:M{M}:N{N}:mirror", la=m_la, loss_max=max(m_loss.values()),
+           loss_max_key=max(m_loss, key=m_loss.get), grad_max=max(m_grad.values()), grad_max_key=max(m_grad, key=m_grad.get))
+    assert m_la < 2e-2, m_la
+    for k, e in m_loss.items():
+        assert e < 2e-2, (k, e)
+    for k, e in m_grad.items():
+        assert e < 0.1, (k, e)
 
 
 def test_training_reduces_loss_and_eval_metrics():
@@ -164,8 +193,7 @@ def test_training_reduces_loss_and_eval_metrics():
     assert "confidence" not in losses
 
 
-@pytest.mark.parametrize("engine", ["fused", "autograd"])
-def test_eval_mode_loss_uses_last_head(engine):
+def test_eval_mode_loss_uses_last_head():
     """Validation loss (train.py:92-93): in eval mode only the last layer's state is stacked (lightglue.py:485) and
     the loss must still apply the LAST assignment head (lightglue.py:588), not head 0.  Golden = the reference in
     eval mode (tests/golden/eval_loss.npz)."""
@@ -177,7 +205,7 @@ def test_eval_mode_loss_uses_last_head(engine):
     g = dict(np.load(os.path.join(GOLDEN, "eval_loss.npz")))
     conf = ast.literal_eval(str(g["meta|conf"]))
     B, N, seed = int(g["meta|B"]), int(g["meta|N"]), int(g["meta|seed"])
-    model = _build(conf, synthetic.make_weights(conf, seed=seed), "fp32", engine).eval()
+    model = _build(conf, synthetic.make_weights(conf, seed=seed), "fp32").eval()
     d = _f32(synthetic.make_pairs(B, N, seed=seed + 1, dtype=torch.float64))
     with torch.no_grad():
         pred = model(d)
@@ -211,6 +239,11 @@ def test_adaptive_point_pruning_matches_reference():
     assert np.array_equal(pred["matches0"].cpu().numpy(), g["pred|matches0"])
     assert np.array_equal(pred["matches1"].cpu().numpy(), g["pred|matches1"])
     np.testing.assert_allclose(pred["matching_scores0"].cpu().numpy(), g["pred|matching_scores0"], rtol=1e-3, atol=1e-6)
+    # the loss needs every point: a pruned pred, or one from elsewhere, is refused
+    with pytest.raises(ValueError, match="pruning"):
+        model.loss(pred, d)
+    with pytest.raises(ValueError, match="own forward"):
+        model.loss({k: v for k, v in pred.items() if not k.startswith("_b200")}, d)
     # bf16 path: same code, pruning counts within a few points of the fp32 path
     mb = _build(conf, synthetic.make_weights(conf, seed=seed), "bf16").eval()
     with torch.no_grad():
@@ -241,7 +274,13 @@ def test_adaptive_early_stop():
     plain = _build(dict(conf, depth_confidence=-1), w, "fp32").eval()
     with torch.no_grad():
         a, b = model2(d), plain(d)
+        (la, ma), (lb, mb) = model2.loss(a, d), plain.loss(b, d)
     assert a["stop_layer"] == 3 and torch.equal(a["matches0"], b["matches0"])
+    assert la.keys() == lb.keys() and ma.keys() == mb.keys()
+    for k in lb:
+        assert torch.equal(la[k], lb[k]), k
+    for k in mb:
+        assert torch.equal(ma[k], mb[k]), k
 
 
 def test_nan_propagates_to_loss():
@@ -285,28 +324,3 @@ def test_cuda_graph_step_matches_eager_step():
     p_pre, l_pre = run(True, prefetch=True)
     np.testing.assert_allclose(l_pre, l_graph, rtol=1e-6)
     assert rel_err(p_pre, p_graph) < 1e-6
-
-
-@pytest.mark.parametrize("precision,tol", [("fp32", 2e-5), ("bf16", 2e-2)])
-@pytest.mark.parametrize("M,N", [(192, 192), (150, 203)])
-def test_fused_engine_matches_autograd_engine(precision, tol, M, N):
-    """The hand-scheduled layer/head nodes (engine.py) and the op-by-op autograd composition are two
-    independent implementations of the same backward; they must agree."""
-    conf = dict(synthetic.DEFAULT_CONF, n_layers=2)
-    w = synthetic.make_weights(conf, seed=61)
-    d = synthetic.to_device(synthetic.make_pairs(2, N, seed=62, M=M), DEV)
-    out = {}
-    for engine in ("fused", "autograd"):
-        model = _build(conf, w, precision, engine)
-        pred = model(d)
-        losses, _ = model.loss(pred, d)
-        losses["total"].mean().backward()
-        out[engine] = (pred, losses, {k: p.grad.clone() for k, p in model.named_parameters()})
-    pa, la, ga = out["autograd"]
-    pf, lf, gf = out["fused"]
-    assert rel_err(pf["log_assignment"], pa["log_assignment"]) < tol
-    for k in la:
-        if torch.is_tensor(la[k]):
-            assert rel_err(lf[k], la[k]) < tol, k
-    for k in ga:
-        assert rel_err(gf[k], ga[k]) < (tol if precision == "fp32" else 0.1), k

@@ -25,7 +25,7 @@ import torch
 from gluefactory_b200 import ops, synthetic
 from gluefactory_b200.matchers.lightglue import LightGlue
 from oracle import lightglue_oracle as O
-from tests.util import GOLDEN, load_case, probe_index, rel_err, report
+from tests.util import GOLDEN, load_case, mirror_oracle, probe_index, rel_err, report
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -123,19 +123,6 @@ def test_bf16_path_at_least_as_close_as_reference_autocast(name):
 
 
 # ------------------------------------------------------------------------------------------------ (B)
-def _mirror_oracle(conf, w, data, rnd=None):
-    """fp32 CPU evaluation with the bf16 rounding model of the CUDA path (see O.Bf16Mirror)."""
-    torch.set_num_threads(max(1, min(64, os.cpu_count() or 1)))
-    rnd = O.Bf16Mirror() if rnd is None else rnd
-    wm = {k: v.float().clone().requires_grad_(True) for k, v in w.items()}
-    dm = _cast(data, torch.float32)
-    pred = O.lightglue_forward(wm, dm, conf, rnd=rnd)
-    losses = O.lightglue_loss(wm, pred, dm, conf, training=True, rnd=rnd)
-    losses["total"].mean().backward()
-    pred = {k: (v.detach() if torch.is_tensor(v) else v) for k, v in pred.items() if not k.startswith("ref_desc")}
-    return pred, {k: (v.detach() if torch.is_tensor(v) else v) for k, v in losses.items()}, {k: p.grad for k, p in wm.items()}
-
-
 def _margin_safe(la, dim, margin):
     inner = la[:, :-1, :-1]
     top2 = inner.topk(2, dim=dim).values
@@ -154,7 +141,7 @@ def test_bf16_path_at_bench_shape_against_rounding_model(N, seed):
     w = synthetic.make_weights(conf, seed=seed)
     data = synthetic.make_pairs(1, N, seed=seed + 1)
     model, pred, losses = _run_gpu(conf, w, data)
-    rp, rl, rg = _mirror_oracle(conf, w, data)
+    rp, rl, rg = mirror_oracle(conf, w, data)
     la, rla = pred["log_assignment"].float().cpu(), rp["log_assignment"]
     d_la = (la - rla).abs()
     la_rel = (d_la.norm() / rla.norm()).item()
@@ -176,7 +163,7 @@ def test_bf16_path_at_bench_shape_against_rounding_model(N, seed):
     assert m0_agree > 0.98, m0_agree
     assert max(gerr.values()) < 5e-2 and np.median(list(gerr.values())) < 6e-3, (max(gerr, key=gerr.get), max(gerr.values()))
     if N == 1024:  # the floor, measured: a second valid rounding model (operand rounding only) against the first
-        rp2, _, rg2 = _mirror_oracle(conf, w, data, rnd=O.bf16_round)
+        rp2, _, rg2 = mirror_oracle(conf, w, data, rnd=O.bf16_round)
         floor_la = ((rp2["log_assignment"] - rla).norm() / rla.norm()).item()
         floor_g = float(np.median([rel_err(rg2[k], rg[k]) for k in rg]))
         report(f"B:N{N}:floor", la_rel_between_models=floor_la, grad_median_between_models=floor_g)

@@ -56,6 +56,23 @@ def check_grad_summary(g, name, grad, rtol, atol_scale=1.0):
         assert abs(proj - float(g[f"grad|{name}|proj"])) <= 4 * tol, (name, proj, float(g[f"grad|{name}|proj"]))
 
 
+def mirror_oracle(conf, w, data, rnd=None):
+    """fp32 CPU evaluation with the bf16 rounding model of the CUDA path (see O.Bf16Mirror), training mode:
+    (pred without the stacked states, losses, parameter gradients)."""
+    from oracle import lightglue_oracle as O
+
+    torch.set_num_threads(max(1, min(64, os.cpu_count() or 1)))
+    rnd = O.Bf16Mirror() if rnd is None else rnd
+    wm = {k: v.float().clone().requires_grad_(True) for k, v in w.items()}
+    dm = {k: ({kk: vv.float() for kk, vv in v.items()} if isinstance(v, dict) else
+              (v.float() if v.is_floating_point() else v)) for k, v in data.items()}
+    pred = O.lightglue_forward(wm, dm, conf, rnd=rnd)
+    losses = O.lightglue_loss(wm, pred, dm, conf, training=True, rnd=rnd)
+    losses["total"].mean().backward()
+    pred = {k: (v.detach() if torch.is_tensor(v) else v) for k, v in pred.items() if not k.startswith("ref_desc")}
+    return pred, {k: (v.detach() if torch.is_tensor(v) else v) for k, v in losses.items()}, {k: p.grad for k, p in wm.items()}
+
+
 def rel_err(a, b):
     a, b = a.detach().double().cpu(), b.detach().double().cpu()
     return ((a - b).norm() / b.norm().clamp(min=1e-30)).item()
