@@ -65,6 +65,8 @@ SIGNATURES = {
     "lgb200_gt_line_matches": (_i, [_vp] * 10 + [_i] * 5 + [_d] * 3 + [_vp] * 4 + [_i, _i, _i, _vp]),
     "lgb200_adam_flat": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _i, _vp, _f, _vp, _vp, _vp, _vp]),
     "lgb200_flat_grad_check": (_i, [_vp, _i64, _vp, _vp]),
+    "lgb200_flat_grad_norm_ws_bytes": (_sz, [_i64]),
+    "lgb200_flat_grad_norm": (_i, [_vp, _i64, _i64, _f, _vp, _f, _vp, _vp, _vp, _vp, _vp]),
     "lgb200_amp_update": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _vp]),
     "lgb200_cast_bf16": (_i, [_vp, _vp, _i64, _vp]),
     "lgb200_colsum_slabs": (_i, [_i64, _i]),
@@ -120,7 +122,7 @@ KERNELS_PER_CALL = {
     "lgb200_ln_gelu_fwd": 1, "lgb200_ln_gelu_bwd": 1, "lgb200_gemm_bf16": 1, "lgb200_assign_lse": 2,
     "lgb200_assign_scores": 2, "lgb200_assign_bwd": 1, "lgb200_filter_matches": 1, "lgb200_log_double_softmax": 3,
     "lgb200_adam_flat": 1, "lgb200_cast_bf16": 1, "lgb200_colsum": 1, "lgb200_residual_add_cast": 1,
-    "lgb200_gemm_bf16_splitk": 2, "lgb200_gt_from_homography": 3, "lgb200_gt_from_reprojection": 3, "lgb200_gt_epipolar_unmatched": 2, "lgb200_gt_line_matches": 5, "lgb200_flat_grad_check": 1, "lgb200_amp_update": 1,
+    "lgb200_gemm_bf16_splitk": 2, "lgb200_gt_from_homography": 3, "lgb200_gt_from_reprojection": 3, "lgb200_gt_epipolar_unmatched": 2, "lgb200_gt_line_matches": 5, "lgb200_flat_grad_check": 1, "lgb200_flat_grad_norm": 2, "lgb200_amp_update": 1,
 }
 launch_count = 0          # running total of kernels launched through `call`
 timed_entry = None        # entry-point name or a set of names: every call of them is bracketed by CUDA events

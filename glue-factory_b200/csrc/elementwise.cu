@@ -437,6 +437,76 @@ __global__ void __launch_bounds__(256) grad_check_kernel(const float* __restrict
   if (__syncthreads_or(bad) && threadIdx.x == 0) *found_inf = 1.f;
 }
 
+// Global gradient norm for clip_grad_norm_ (train.py:501-512), fused with the check above.  Pass 1: each CTA writes the
+// fp64 sum of squares of its share of g[0..n_norm) to part[blockIdx.x]; an element of g[n_norm..n_check) adds x - x
+// (0, or NaN when x is not finite), so a non-finite checked value makes the sum NaN, as an inf or NaN normed value does
+// through its square.  fp64 squares of finite floats cannot overflow.  Pass 2 (one CTA) sums the partials.  Every
+// thread's share and every tree step is fixed by n_norm and the grid, which depends on n_norm only: deterministic.
+constexpr int kNormThreads = 256;
+constexpr int kNormMaxCtas = 1024;
+
+__device__ __forceinline__ double block_sum_f64(double v) {  // fixed tree; result valid in thread 0
+  __shared__ double red[kNormThreads / 32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  v = 0.0;
+  if (threadIdx.x == 0)
+#pragma unroll
+    for (int w = 0; w < kNormThreads / 32; ++w) v += red[w];
+  return v;
+}
+
+__device__ __forceinline__ double sq4(double acc, float4 x) {
+  acc = fma((double)x.x, (double)x.x, acc);
+  acc = fma((double)x.y, (double)x.y, acc);
+  acc = fma((double)x.z, (double)x.z, acc);
+  return fma((double)x.w, (double)x.w, acc);
+}
+
+__global__ void __launch_bounds__(kNormThreads) grad_sumsq_kernel(const float* __restrict__ g, int64_t n_norm,
+                                                                 int64_t n_check, double* __restrict__ part) {
+  const float4* g4 = reinterpret_cast<const float4*>(g);
+  const int64_t nv = n_norm / 4, stride = (int64_t)gridDim.x * kNormThreads;
+  int64_t i = (int64_t)blockIdx.x * kNormThreads + threadIdx.x;
+  double acc = 0.0;
+  for (; i + stride < nv; i += 2 * stride) {  // two independent 128-bit loads in flight per thread
+    const float4 a = g4[i], b = g4[i + stride];
+    acc = sq4(sq4(acc, a), b);
+  }
+  if (i < nv) acc = sq4(acc, g4[i]);
+  if (blockIdx.x == 0 && threadIdx.x < (n_norm & 3)) {
+    const double x = g[nv * 4 + threadIdx.x];
+    acc = fma(x, x, acc);
+  }
+  for (int64_t j = n_norm + (int64_t)blockIdx.x * kNormThreads + threadIdx.x; j < n_check; j += stride)
+    acc += (double)(g[j] - g[j]);
+  acc = block_sum_f64(acc);
+  if (threadIdx.x == 0) part[blockIdx.x] = acc;
+}
+
+__global__ void __launch_bounds__(kNormThreads) grad_norm_finish_kernel(const double* __restrict__ part, int nparts,
+                                                                       float grad_scale,
+                                                                       const float* __restrict__ loss_scale,
+                                                                       float max_norm, float* __restrict__ found_inf,
+                                                                       float* __restrict__ norm_out,
+                                                                       float* __restrict__ adam_div_out) {
+  double acc = 0.0;
+  for (int j = threadIdx.x; j < nparts; j += kNormThreads) acc += part[j];
+  acc = block_sum_f64(acc);
+  if (threadIdx.x == 0) {
+    const float s = loss_scale ? *loss_scale : 1.f;
+    const float norm = (float)(sqrt(acc) * fabs((double)grad_scale / (double)s));
+    const bool bad = !isfinite(norm);
+    // torch.nn.utils.clip_grad_norm_: clip_coef = max_norm / (total_norm + 1e-6), clamped to at most 1, in fp32
+    const float coef = fminf(max_norm / (norm + 1e-6f), 1.f);
+    *found_inf = bad ? 1.f : 0.f;
+    *norm_out = norm;
+    *adam_div_out = bad ? s : s / coef;
+  }
+}
+
 // One thread: advance the step count unless the step is skipped, and update the loss scale like
 // torch.amp.GradScaler.update (backoff on overflow, growth after `growth_interval` clean steps).
 __global__ void amp_update_kernel(const float* __restrict__ found_inf, int* __restrict__ step,
@@ -1300,6 +1370,31 @@ int lgb200_flat_grad_check(const float* g, int64_t n, float* found_inf, cudaStre
   const unsigned grid = (unsigned)(blocks < 1 ? 1 : (blocks > 1184 ? 1184 : blocks));
   grad_check_kernel<<<grid, 256, 0, stream>>>(g, n, found_inf);
   return check_launch("flat_grad_check");
+}
+
+}  // extern "C"
+
+static unsigned grad_norm_ctas(int64_t n_norm) {
+  const int64_t b = (n_norm / 4 + 2 * kNormThreads - 1) / (2 * kNormThreads);
+  return (unsigned)(b < 1 ? 1 : (b > kNormMaxCtas ? kNormMaxCtas : b));
+}
+
+extern "C" {
+
+size_t lgb200_flat_grad_norm_ws_bytes(int64_t n_norm) { return grad_norm_ctas(n_norm) * sizeof(double); }
+
+int lgb200_flat_grad_norm(const float* g, int64_t n_norm, int64_t n_check, float grad_scale,
+                          const float* loss_scale_dev, float max_norm, float* found_inf, float* norm_out,
+                          float* adam_div_out, void* ws, cudaStream_t stream) {
+  LGB_REQUIRE(g && found_inf && norm_out && adam_div_out && ws, kErrInvalid, "flat_grad_norm: null pointer");
+  LGB_REQUIRE(n_norm > 0 && n_check >= n_norm, kErrInvalid, "flat_grad_norm: need 0 < n_norm <= n_check");
+  LGB_REQUIRE(grad_scale > 0.f && max_norm > 0.f, kErrInvalid, "flat_grad_norm: grad_scale and max_norm must be > 0");
+  LGB_REQUIRE(aligned16({g, ws}), kErrInvalid, "flat_grad_norm: g and ws must be 16-byte aligned");
+  const unsigned grid = grad_norm_ctas(n_norm);
+  grad_sumsq_kernel<<<grid, kNormThreads, 0, stream>>>(g, n_norm, n_check, (double*)ws);
+  grad_norm_finish_kernel<<<1, kNormThreads, 0, stream>>>((const double*)ws, (int)grid, grad_scale, loss_scale_dev,
+                                                          max_norm, found_inf, norm_out, adam_div_out);
+  return check_launch("flat_grad_norm");
 }
 
 int lgb200_amp_update(const float* found_inf, int* step_dev, float* loss_scale, int* growth_tracker,

@@ -797,6 +797,23 @@ def flat_grad_check(g, found_inf):
     call("lgb200_flat_grad_check", ptr(g), g.numel(), ptr(found_inf), stream_ptr())
 
 
+def flat_grad_norm_ws(n_norm, device):
+    """Scratch for flat_grad_norm over n_norm elements (allocate once: a captured step keeps using it)."""
+    return torch.empty(_lib.load().lgb200_flat_grad_norm_ws_bytes(int(n_norm)), device=device, dtype=torch.uint8)
+
+
+def flat_grad_norm(g, n_norm, grad_scale, loss_scale, max_norm, found_inf, norm_out, adam_div_out, ws):
+    """clip_grad_norm_ on the device (no host sync): norm_out <- ||g[:n_norm] * grad_scale / loss_scale|| (fp64 sum in
+    a fixed order), found_inf <- any non-finite element of g or a non-finite norm, adam_div_out <- the loss_scale_dev
+    that makes adam_flat_ apply the clip coefficient.  loss_scale: device scalar or None (lgb200.h)."""
+    for t in (g, found_inf, norm_out, adam_div_out):
+        _chk(t, torch.float32)
+    if loss_scale is not None:
+        _chk(loss_scale, torch.float32)
+    call("lgb200_flat_grad_norm", ptr(g), int(n_norm), g.numel(), float(grad_scale), ptr(loss_scale), float(max_norm),
+         ptr(found_inf), ptr(norm_out), ptr(adam_div_out), ptr(ws), stream_ptr())
+
+
 def amp_update(found_inf, step_dev=None, loss_scale=None, growth_tracker=None, growth_factor=2.0, backoff_factor=0.5,
                growth_interval=2000):
     """Device-side bookkeeping of one optimiser step: step count (unless skipped) + GradScaler.update rule."""

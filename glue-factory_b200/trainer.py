@@ -80,22 +80,34 @@ class FlatParams:
         ops.call("lgb200_cast_bf16", ops.ptr(self.flat), ops.ptr(self.flat16), self.numel, ops.stream_ptr())
         return self._views16
 
-    def lr_scale_per_elem(self, lr_scaling):
+    def lr_factors(self, lr_scaling):
         """The reference's LR groups (train.py:177-196 pack_lr_parameters, :353-361): `lr_scaling` is a list of
         (factor, [name substrings]); a parameter whose name contains one of the substrings trains at factor x lr
-        (first matching group wins, as the reference's filter loop).  Returns the per-element multiplier vector for
-        lgb200_adam_flat, or None when every factor is 1."""
-        scale = torch.ones(self.numel, device=self.flat.device, dtype=torch.float32)
-        hit = False
-        for p, off in zip(self.params, self.offsets):
+        (first matching group wins, as the reference's filter loop).  Returns one factor per parameter."""
+        factors = []
+        for p in self.params:
             name = self._names[id(p)]
-            for factor, filters in lr_scaling:
-                if any(f in name for f in filters):
-                    if factor != 1:
-                        scale[off:off + p.numel()] = float(factor)
-                        hit = True
-                    break
-        return scale if hit else None
+            factors.append(next((factor for factor, filters in lr_scaling or () if any(f in name for f in filters)), 1))
+        return factors
+
+    def lr_scale_per_elem(self, lr_scaling):
+        """The per-element multiplier vector of `lr_factors` for lgb200_adam_flat, or None when every factor is 1."""
+        factors = self.lr_factors(lr_scaling)
+        if all(f == 1 for f in factors):
+            return None
+        scale = torch.ones(self.numel, device=self.flat.device, dtype=torch.float32)
+        for p, off, factor in zip(self.params, self.offsets, factors):
+            if factor != 1:
+                scale[off:off + p.numel()] = float(factor)
+        return scale
+
+    def lr_groups(self, lr_scaling):
+        """[(factor, [parameter index])]: the optimiser groups pack_lr_parameters builds, one per distinct factor in
+        order of first appearance, parameters in module order."""
+        groups = {}
+        for i, factor in enumerate(self.lr_factors(lr_scaling)):
+            groups.setdefault(factor, []).append(i)
+        return list(groups.items())
 
     def zero_grad(self):
         """Detach the .grad views: autograd then hands each freshly computed gradient over by reference
@@ -129,11 +141,17 @@ class MatcherTrainer:
     `ground_truth`: device label generator (SURVEY 8f row 1), so a batch needs only keypoints, descriptors and H.
     `sync_batchnorm`: at world size > 1, convert the model's BatchNorms to nn.SyncBatchNorm over `process_group` (as
     train.py:337-339 does before the DDP wrap), so that they normalise with the statistics of the global batch;
-    `self.model` is the converted module."""
+    `self.model` is the converted module.
+    `clip_grad`: the reference's train.clip_grad (train.py:501-512), fixed at construction; falsy disables it.  The
+    check is then lgb200_flat_grad_norm: the norm of the averaged, unscaled gradient is taken on the device after the
+    all-reduce (so every rank computes the same coefficient), a non-finite norm skips the step like
+    clip_grad_norm_(error_if_nonfinite=True), and Adam receives the coefficient through its loss-scale divisor.
+    `state_dict()` / `load_state_dict()` carry the optimiser state in the formats of torch.optim.Adam and
+    torch.amp.GradScaler; the weights go through `model.state_dict()`, whose tensors are views of the flat buffer."""
 
     def __init__(self, model, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, process_group=None,
                  loss_scale=None, growth_factor=2.0, backoff_factor=0.5, growth_interval=2000, lr_scaling=None,
-                 ground_truth=None, sync_batchnorm=False):
+                 ground_truth=None, sync_batchnorm=False, clip_grad=None):
         self.group = process_group
         self.world = dist.get_world_size(process_group) if dist.is_available() and dist.is_initialized() else 1
         if sync_batchnorm and self.world > 1:  # before FlatParams: the converted modules keep the same Parameters
@@ -158,7 +176,13 @@ class MatcherTrainer:
         self._growth = None if loss_scale is None else torch.zeros(1, device=dev, dtype=torch.int32)
         self._amp = (growth_factor, backoff_factor, growth_interval)
         self._lr_scale = self.fp.lr_scale_per_elem(lr_scaling) if lr_scaling else None
+        self._groups = self.fp.lr_groups(lr_scaling)
         self._lr_host = float(lr)
+        self._max_norm = float(clip_grad) if clip_grad else None
+        if self._max_norm:
+            self._grad_norm = torch.zeros(1, device=dev, dtype=torch.float32)
+            self._adam_div = torch.ones(1, device=dev, dtype=torch.float32)
+            self._norm_ws = None  # sized by the library at the first step: construction makes no library call
         self.calls = 0  # optimiser-step attempts (skipped steps included)
 
     # ---- controls (device scalars: changing them never invalidates a captured graph)
@@ -182,6 +206,82 @@ class MatcherTrainer:
 
     def loss_scale(self):
         return None if self._scale_dev is None else float(self._scale_dev.item())
+
+    # ---- checkpoints (utils/experiments.py:113-118 saves optimizer.state_dict(); train.py:379-382 restores it)
+    def state_dict(self):
+        """{"optimizer": the state_dict of a torch.optim.Adam over pack_lr_parameters' groups (train.py:177-196),
+        "grad_scaler": torch.amp.GradScaler.state_dict() (only with loss_scale)}, holding copies of the device state."""
+        fp, t = self.fp, float(self.t)
+        layout = torch.optim.Adam([{"params": [fp.params[i] for i in ids], "lr": factor * self._lr_host}
+                                   for factor, ids in self._groups],
+                                  lr=self._lr_host, betas=self.betas, eps=self.eps, weight_decay=self.wd).state_dict()
+        state = {}
+        for k, i in enumerate(i for _, ids in self._groups for i in ids):
+            p, off = fp.params[i], fp.offsets[i]
+            state[k] = {"step": torch.tensor(t, dtype=torch.float32),
+                        "exp_avg": self.m[off:off + p.numel()].view_as(p).clone(),
+                        "exp_avg_sq": self.v[off:off + p.numel()].view_as(p).clone()}
+        out = {"optimizer": {"state": state, "param_groups": layout["param_groups"]}}
+        if self._scale_dev is not None:
+            g, b, i = self._amp
+            out["grad_scaler"] = {"scale": self.loss_scale(), "growth_factor": g, "backoff_factor": b,
+                                  "growth_interval": i, "_growth_tracker": int(self._growth.item())}
+        return out
+
+    def load_state_dict(self, state_dict):
+        """Load `state_dict()` output, or the state of a torch.optim.Adam built over the same groups, in place: a
+        captured graph stays valid.  Sets lr from the groups.  Raises ValueError, naming the first offending parameter,
+        when the groups, shapes or states do not fit this trainer (it keeps one step count for every parameter).
+        A "grad_scaler" entry is ignored without loss_scale, as by a disabled GradScaler."""
+        fp, opt = self.fp, state_dict["optimizer"]
+        groups, state = opt["param_groups"], opt["state"]
+
+        def name(i):
+            return fp._names[id(fp.params[i])]
+
+        # group of each parameter in group order, on both sides: a differing group count or size shows as a difference
+        order = [i for _, ids in self._groups for i in ids]
+        mine = [gi for gi, (_, ids) in enumerate(self._groups) for _ in ids]
+        theirs = [gi for gi, g in enumerate(groups) for _ in g["params"]]
+        if mine != theirs:
+            k = next((k for k, (a, b) in enumerate(zip(mine, theirs)) if a != b), min(len(mine), len(theirs)))
+            raise ValueError(f"optimizer state has parameter groups of sizes {[len(g['params']) for g in groups]}, the "
+                             f"trainer {[len(ids) for _, ids in self._groups]}: they first differ at parameter "
+                             f"{name(order[min(k, len(order) - 1)])!r}")
+        pairs, steps = [], []  # (trainer parameter index, source state), in group order
+        for src, (_, ids) in zip(groups, self._groups):
+            for i, key in zip(ids, src["params"]):
+                st = state.get(key)
+                if st is None or not all(k in st for k in ("step", "exp_avg", "exp_avg_sq")):
+                    raise ValueError(f"no Adam state for parameter {name(i)!r}")
+                shape = fp.params[i].shape
+                if st["exp_avg"].shape != shape or st["exp_avg_sq"].shape != shape:
+                    raise ValueError(f"parameter {name(i)!r}: state shape {tuple(st['exp_avg'].shape)}, "
+                                     f"parameter shape {tuple(shape)}")
+                steps.append(float(st["step"]))
+                if steps[-1] != steps[0]:
+                    raise ValueError(f"parameter {name(i)!r} is at step {steps[-1]:g}, the first at {steps[0]:g}: the "
+                                     "trainer keeps one step count")
+                pairs.append((i, st))
+        sc = state_dict.get("grad_scaler")
+        if self._scale_dev is not None and sc:
+            if (sc["growth_factor"], sc["backoff_factor"], sc["growth_interval"]) != self._amp:
+                raise ValueError(f"GradScaler growth_factor / backoff_factor / growth_interval "
+                                 f"{(sc['growth_factor'], sc['backoff_factor'], sc['growth_interval'])} differ from the "
+                                 f"trainer's {self._amp}, which are fixed at construction")
+        for i, st in pairs:
+            off, n = fp.offsets[i], fp.params[i].numel()
+            self.m[off:off + n].copy_(st["exp_avg"].reshape(-1))
+            self.v[off:off + n].copy_(st["exp_avg_sq"].reshape(-1))
+        self._t_dev.fill_(int(steps[0]))
+        # base lr from a group of factor 1 when there is one (exact), else from the first group with a factor != 0
+        lrs = [(f, g["lr"]) for (f, _), g in zip(self._groups, groups) if f != 0]
+        if lrs:
+            factor, lr = next((c for c in lrs if c[0] == 1), lrs[0])
+            self.lr = lr / factor
+        if self._scale_dev is not None and sc:
+            self._scale_dev.fill_(float(sc["scale"]))
+            self._growth.fill_(int(sc["_growth_tracker"]))
 
     def exchange_gradients(self):
         """The step's one exchange: ONE sum-all-reduce of the whole flat gradient buffer (+ the loss slot), behind
@@ -267,11 +367,20 @@ class MatcherTrainer:
         self.fp.loss_slot.copy_(loss.detach().reshape(1))
         self.exchange_gradients()
         # non-finite loss or gradient on ANY rank -> every rank skips this update (and backs the loss scale off)
-        ops.flat_grad_check(self.fp.grad_ext[:self.fp.numel + 4], self._found_inf)
+        checked = self.fp.grad_ext[:self.fp.numel + 4]
+        if self._max_norm:  # the same check, plus the clip coefficient folded into Adam's loss-scale divisor
+            if self._norm_ws is None:
+                self._norm_ws = ops.flat_grad_norm_ws(self.fp.numel, self.fp.flat.device)
+            ops.flat_grad_norm(checked, self.fp.numel, 1.0 / self.world, self._scale_dev, self._max_norm,
+                               self._found_inf, self._grad_norm, self._adam_div, self._norm_ws)
+            divisor = self._adam_div
+        else:
+            ops.flat_grad_check(checked, self._found_inf)
+            divisor = self._scale_dev
         ops.amp_update(self._found_inf, step_dev=self._t_dev)  # ++step unless skipped (Adam's bias correction reads it)
         ops.adam_flat_(self.fp.flat, self.fp.grad, self.m, self.v, 0, self._lr_host, self.betas, self.eps, self.wd,
                        grad_scale=1.0 / self.world, lr_scale_per_elem=self._lr_scale, step_dev=self._t_dev,
-                       lr_dev=self._lr_dev, loss_scale_dev=self._scale_dev, found_inf_dev=self._found_inf)
+                       lr_dev=self._lr_dev, loss_scale_dev=divisor, found_inf_dev=self._found_inf)
         if self._scale_dev is not None:  # GradScaler.update AFTER the step: the gradients carry the old scale
             g, b, i = self._amp
             ops.amp_update(self._found_inf, None, self._scale_dev, self._growth, g, b, i)

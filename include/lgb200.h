@@ -277,6 +277,18 @@ int lgb200_adam_flat(float* p, const float* g, float* m, float* v, int64_t n, co
                      cudaStream_t stream);
 /* found_inf[0] = 1.0f if any of g[0..n) is non-finite, else 0.0f (GradScaler.unscale_'s check, no host sync). */
 int lgb200_flat_grad_check(const float* g, int64_t n, float* found_inf, cudaStream_t stream);
+/* Gradient-norm clipping (torch.nn.utils.clip_grad_norm_ with error_if_nonfinite=True after GradScaler.unscale_,
+ * train.py:501-512) in place of lgb200_flat_grad_check, without a host sync.  norm_out = ||g[0..n_norm) * grad_scale /
+ * s||_2 with s = *loss_scale_dev (1 when NULL), summed in fp64 in a fixed order (bit-identical from call to call) and
+ * rounded to fp32.  g[n_norm..n_check) is checked but not normed (the trainer's loss slot); norm_out is NaN when one of
+ * those is non-finite.  found_inf = 1.0f when any checked value or the fp32 norm is non-finite, else 0.0f.
+ * adam_div_out = s / min(1, max_norm / (norm + 1e-6)) (s when found_inf): passed as lgb200_adam_flat's
+ * loss_scale_dev, it makes Adam apply grad_scale * coef / s.  grad_scale > 0, max_norm > 0; g 16-byte aligned.
+ * ws: lgb200_flat_grad_norm_ws_bytes(n_norm) bytes of scratch, 16-byte aligned.  Two launches.                      */
+size_t lgb200_flat_grad_norm_ws_bytes(int64_t n_norm);
+int lgb200_flat_grad_norm(const float* g, int64_t n_norm, int64_t n_check, float grad_scale,
+                          const float* loss_scale_dev, float max_norm, float* found_inf, float* norm_out,
+                          float* adam_div_out, void* ws, cudaStream_t stream);
 /* One step of bookkeeping on the device: ++*step_dev unless *found_inf, and the GradScaler.update rule on
  * *loss_scale / *growth_tracker (both may be NULL): x backoff_factor on overflow, x growth_factor after
  * growth_interval consecutive clean steps. */
