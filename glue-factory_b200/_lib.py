@@ -55,6 +55,11 @@ SIGNATURES = {
     "lgb200_sinkhorn": (_i, [_vp, _f, _i, _vp, _vp, _i, _i, _i, _vp]),
     "lgb200_sinkhorn_fwd": (_i, [_vp, _f, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "lgb200_sinkhorn_bwd": (_i, [_vp, _f, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "lgb200_sinkhorn_fwd_dev": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "lgb200_sinkhorn_bwd_dev": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "lgb200_ot_nll_fwd": (_i, [_vp] * 7 + [_i, _i, _i, _vp]),
+    "lgb200_ot_nll_bwd": (_i, [_vp] * 8 + [_i, _i, _i, _vp]),
+    "lgb200_ot_filter_stats": (_i, [_vp] * 4 + [_i, _i, _i, _vp]),
     "lgb200_gt_homography_ws_bytes": (_sz, [_i, _i, _i]),
     "lgb200_gt_from_homography": (_i, [_vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "lgb200_gt_from_reprojection": (_i, [_vp] * 8 + [_f, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
@@ -73,6 +78,7 @@ SIGNATURES = {
     "lgb200_colsum": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _i, _vp]),
     "lgb200_bn_stats": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _i, _vp]),
     "lgb200_bn_relu_fwd": (_i, [_vp] * 6 + [_f, _f] + [_vp] * 3 + [_i64, _i, _i, _vp]),
+    "lgb200_bn_running_update": (_i, [_vp, _vp, _vp, _f, _i, _vp]),
     "lgb200_bn_relu_bwd_reduce": (_i, [_vp] * 9 + [_i64, _i, _i, _vp]),
     "lgb200_bn_relu_bwd": (_i, [_vp] * 9 + [_i64, _i, _i, _vp]),
     "lgb200_posenc_wgrad_blocks": (_i, []),
@@ -123,6 +129,7 @@ KERNELS_PER_CALL = {
     "lgb200_assign_scores": 2, "lgb200_assign_bwd": 1, "lgb200_filter_matches": 1, "lgb200_log_double_softmax": 3,
     "lgb200_adam_flat": 1, "lgb200_cast_bf16": 1, "lgb200_colsum": 1, "lgb200_residual_add_cast": 1,
     "lgb200_gemm_bf16_splitk": 2, "lgb200_gt_from_homography": 3, "lgb200_gt_from_reprojection": 3, "lgb200_gt_epipolar_unmatched": 2, "lgb200_gt_line_matches": 5, "lgb200_flat_grad_check": 1, "lgb200_flat_grad_norm": 2, "lgb200_amp_update": 1,
+    "lgb200_ot_nll_fwd": 2, "lgb200_ot_nll_bwd": 1, "lgb200_ot_filter_stats": 2, "lgb200_bn_running_update": 1,
 }
 launch_count = 0          # running total of kernels launched through `call`
 timed_entry = None        # entry-point name or a set of names: every call of them is bracketed by CUDA events

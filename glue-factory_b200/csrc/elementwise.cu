@@ -790,6 +790,21 @@ constexpr int kBnMaxC = 512;
 
 __device__ __forceinline__ int64_t bn_grid_stride() { return (int64_t)gridDim.x * blockDim.x; }
 
+// One momentum step of the running statistics from the batch statistics in `sums` (unbiased variance).
+__device__ __forceinline__ void bn_running_step(const double* __restrict__ sums, float* __restrict__ rmean,
+                                                float* __restrict__ rvar, float momentum, int c, int C) {
+  const double n = sums[2 * C];
+  const double m = sums[c] / n;
+  const double var = fmax(sums[C + c] / n - m * m, 0.0);
+  rmean[c] = (1.f - momentum) * rmean[c] + momentum * (float)m;
+  rvar[c] = (1.f - momentum) * rvar[c] + momentum * (float)(var * n / (n - 1.0));
+}
+
+__global__ void bn_running_update_kernel(const double* __restrict__ sums, float* __restrict__ rmean,
+                                         float* __restrict__ rvar, float momentum, int C) {
+  for (int c = threadIdx.x; c < C; c += blockDim.x) bn_running_step(sums, rmean, rvar, momentum, c, C);
+}
+
 // sums = [sum x (C) | sum x^2 (C) | count] (fp64, possibly summed over ranks): training mode; NULL: eval mode with the
 // running statistics.  Block 0 writes the saved mean / rstd and, in training mode, updates the running statistics
 // (momentum, unbiased variance with the count in `sums`).
@@ -809,10 +824,7 @@ __global__ void __launch_bounds__(256) bn_relu_fwd_kernel(const T* __restrict__ 
       const double var = fmax(sums[C + c] / n - m * m, 0.0);
       mu = (float)m;
       rs = 1.f / sqrtf((float)var + eps);
-      if (blockIdx.x == 0 && rmean) {
-        rmean[c] = (1.f - momentum) * rmean[c] + momentum * mu;
-        rvar[c] = (1.f - momentum) * rvar[c] + momentum * (float)(var * n / (n - 1.0));
-      }
+      if (blockIdx.x == 0 && rmean) bn_running_step(sums, rmean, rvar, momentum, c, C);
     } else {
       mu = rmean[c];
       rs = 1.f / sqrtf(rvar[c] + eps);
@@ -1134,6 +1146,13 @@ int lgb200_bn_stats(const void* x, double* sums, double* ws, unsigned* counters,
   if (dtype == LGB200_BF16)
     return colsum_launch(BnStats<__nv_bfloat16>{(const __nv_bfloat16*)x}, sums, ws, counters, ntok, C, stream);
   LGB_REQUIRE(false, kErrInvalid, "bn_stats: bad dtype %d", dtype);
+}
+
+int lgb200_bn_running_update(const double* sums, float* running_mean, float* running_var, float momentum, int C,
+                             cudaStream_t stream) {
+  LGB_REQUIRE(sums && running_mean && running_var && C > 0, kErrInvalid, "bn_running_update: bad arguments");
+  bn_running_update_kernel<<<1, 256, 0, stream>>>(sums, running_mean, running_var, momentum, C);
+  return check_launch("bn_running_update");
 }
 
 int lgb200_bn_relu_fwd(const void* x, const double* sums, const float* gamma, const float* beta, float* running_mean,

@@ -107,14 +107,15 @@ __device__ __forceinline__ void sk_fill_cache(float* zs, const float* __restrict
 }
 
 __global__ void __launch_bounds__(kSkThreads, 1)
-sk_fwd_persistent_kernel(const float* __restrict__ sim, float alpha, int iters, float* __restrict__ out,
-                         float* __restrict__ u, float* __restrict__ v, float* __restrict__ uh, float* __restrict__ vh,
+sk_fwd_persistent_kernel(const float* __restrict__ sim, float alpha, const float* __restrict__ alpha_dev, int iters,
+                         float* __restrict__ out, float* __restrict__ u, float* __restrict__ v, float* __restrict__ uh, float* __restrict__ vh,
                          float* __restrict__ pm, float* __restrict__ ps, unsigned* __restrict__ bar, SkGeom g) {
   extern __shared__ float sk_smem[];
   const int M = g.M, N = g.N, S = g.S, R = g.R, B = g.B;
   float* vsm = sk_smem;                 // N + 1
   float* usm = vsm + sk_pad(N + 1);     // R + 1
   float* zs = usm + sk_pad(R + 1);      // R x N when cached
+  if (alpha_dev) alpha = __ldg(alpha_dev);  // the learnt bin score read from device memory (no host read-back)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int items = B * S;
   const float norm = -logf((float)(M + N));
@@ -254,7 +255,8 @@ sk_fwd_persistent_kernel(const float* __restrict__ sim, float alpha, int iters, 
 // sums go through per-strip partials and one merge, like the forward.  dZ lives in dsim [B,M,N] plus the dustbin
 // row dzr [B,N+1] and column dzc [B,M]; every element is only ever touched by the same thread.
 __global__ void __launch_bounds__(kSkThreads, 1)
-sk_bwd_persistent_kernel(const float* __restrict__ sim, float alpha, int iters, const float* __restrict__ grad,
+sk_bwd_persistent_kernel(const float* __restrict__ sim, float alpha, const float* __restrict__ alpha_dev, int iters,
+                         const float* __restrict__ grad,
                          const float* __restrict__ uh, const float* __restrict__ vh, float* __restrict__ dsim,
                          float* __restrict__ dzr, float* __restrict__ dzc, float* __restrict__ dv,
                          float* __restrict__ pw, unsigned* __restrict__ bar, SkGeom g) {
@@ -266,6 +268,7 @@ sk_bwd_persistent_kernel(const float* __restrict__ sim, float alpha, int iters, 
   float* uks = dvs + sk_pad(N + 1);       // u_k                   R + 1
   float* dus = uks + sk_pad(R + 1);       // du                    R + 1
   float* zs = dus + sk_pad(R + 1);        // R x N when cached
+  if (alpha_dev) alpha = __ldg(alpha_dev);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int items = B * S;
   const float norm = -logf((float)(M + N));
@@ -416,6 +419,130 @@ static size_t sk_ws_floats(int B, int M, int N) {
   return (size_t)B * (M + N + 2) + 2 * parts * (N + 1) + 64;
 }
 
+// ---- dense Sinkhorn output Z [B,M+1,N+1] (row pitch N+1): NLL head and match-filter statistics -----------------------
+// SuperGlue's loss (superglue.py:322-352) and match filter (:301-311) read only the inner block and the two dustbins of
+// Z: the reference builds dense fp32 copies of the mask and of mask * Z for it.  Here one pass reads the byte mask and
+// touches Z only where the mask is set; every reduction runs in a fixed order (bit-identical across calls).
+constexpr int kOtRows = 8;
+
+// fixed-order sum over the block (256 threads); result valid in thread 0
+__device__ __forceinline__ double ot_block_sum(double v, double* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double t = 0.0;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < 8; ++w) t += red[w];
+  __syncthreads();
+  return t;
+}
+
+// per (pair, strip of kOtRows rows): sum of Z over the positives of the strip
+__global__ void __launch_bounds__(256) ot_nll_part_kernel(const float* __restrict__ Z, const uint8_t* __restrict__ mask,
+                                                         float* __restrict__ part, int M, int N) {
+  __shared__ double red[8];
+  const int b = blockIdx.y, r0 = blockIdx.x * kOtRows, r1 = min(M, r0 + kOtRows);
+  float acc = 0.f;
+  for (int i = r0; i < r1; ++i) {
+    const uint8_t* mrow = mask + ((int64_t)b * M + i) * N;
+    const float* zrow = Z + ((int64_t)b * (M + 1) + i) * (N + 1);
+    for (int j = threadIdx.x; j < N; j += 256)
+      if (__ldg(mrow + j)) acc += __ldg(zrow + j);
+  }
+  const double t = ot_block_sum((double)acc, red);
+  if (threadIdx.x == 0) part[(int64_t)b * gridDim.x + blockIdx.x] = (float)t;
+}
+
+// per pair: pos = sum of the strip partials, neg = sum_i neg0_i Z[i,N] + sum_j neg1_j Z[M,j]
+__global__ void __launch_bounds__(256) ot_nll_final_kernel(const float* __restrict__ Z, const float* __restrict__ neg0,
+                                                          const float* __restrict__ neg1, const float* __restrict__ part,
+                                                          int nparts, float* __restrict__ pos, float* __restrict__ neg,
+                                                          int M, int N) {
+  __shared__ double red[8];
+  const int b = blockIdx.x;
+  double a = 0.0;
+  for (int p = threadIdx.x; p < nparts; p += 256) a += (double)__ldg(part + (int64_t)b * nparts + p);
+  const double tp = ot_block_sum(a, red);
+  const float* zb = Z + (int64_t)b * (M + 1) * (N + 1);
+  double c = 0.0;
+  for (int i = threadIdx.x; i < M; i += 256) c += (double)__ldg(neg0 + (int64_t)b * M + i) * __ldg(zb + (int64_t)i * (N + 1) + N);
+  for (int j = threadIdx.x; j < N; j += 256) c += (double)__ldg(neg1 + (int64_t)b * N + j) * __ldg(zb + (int64_t)M * (N + 1) + j);
+  const double tn = ot_block_sum(c, red);
+  if (threadIdx.x == 0) {
+    pos[b] = (float)tp;
+    neg[b] = (float)tn;
+  }
+}
+
+// dZ of nll_pos = -pos / num_pos and nll_neg = -neg / num_neg for incoming per-pair gradients gpos, gneg (device)
+__global__ void __launch_bounds__(256) ot_nll_bwd_kernel(const uint8_t* __restrict__ mask, const float* __restrict__ neg0,
+                                                        const float* __restrict__ neg1, const float* __restrict__ num_pos,
+                                                        const float* __restrict__ num_neg, const float* __restrict__ gpos,
+                                                        const float* __restrict__ gneg, float* __restrict__ dZ, int M, int N) {
+  const int b = blockIdx.y, r0 = blockIdx.x * kOtRows, r1 = min(M + 1, r0 + kOtRows);
+  const float cp = -(__ldg(gpos + b) / __ldg(num_pos + b)), cn = -(__ldg(gneg + b) / __ldg(num_neg + b));
+  for (int i = r0; i < r1; ++i) {
+    float* drow = dZ + ((int64_t)b * (M + 1) + i) * (N + 1);
+    if (i < M) {
+      const uint8_t* mrow = mask + ((int64_t)b * M + i) * N;
+      for (int j = threadIdx.x; j < N; j += 256) drow[j] = __ldg(mrow + j) ? cp : 0.f;
+      if (threadIdx.x == 0) drow[N] = __ldg(neg0 + (int64_t)b * M + i) * cn;
+    } else {
+      for (int j = threadIdx.x; j < N; j += 256) drow[j] = __ldg(neg1 + (int64_t)b * N + j) * cn;
+      if (threadIdx.x == 0) drow[N] = 0.f;
+    }
+  }
+}
+
+// row max / argmax of Z's inner block, first index on ties (warp per row)
+__global__ void __launch_bounds__(256) ot_rowmax_kernel(const float* __restrict__ Z, float* __restrict__ rowmax,
+                                                       int* __restrict__ rowarg, int M, int N) {
+  const int b = blockIdx.y, i = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (i >= M) return;
+  const float* zrow = Z + ((int64_t)b * (M + 1) + i) * (N + 1);
+  float best = kNInf;
+  int arg = lane < N ? lane : 0x7fffffff;
+  for (int j = lane; j < N; j += 32) {
+    const float x = __ldg(zrow + j);
+    if (x > best) best = x, arg = j;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float v2 = __shfl_xor_sync(0xffffffffu, best, o);
+    const int a2 = __shfl_xor_sync(0xffffffffu, arg, o);
+    if (v2 > best || (v2 == best && a2 < arg)) best = v2, arg = a2;
+  }
+  if (lane == 0) {
+    rowmax[(int64_t)b * M + i] = best;
+    rowarg[(int64_t)b * M + i] = arg;
+  }
+}
+
+// column argmax of Z's inner block, first index on ties (thread per column, rows in order)
+__global__ void __launch_bounds__(256) ot_colarg_kernel(const float* __restrict__ Z, int* __restrict__ colarg, int M,
+                                                       int N) {
+  const int b = blockIdx.y, j = blockIdx.x * 256 + threadIdx.x;
+  if (j >= N) return;
+  const float* zc = Z + (int64_t)b * (M + 1) * (N + 1) + j;
+  float best = __ldg(zc);
+  int arg = 0;
+  int i = 1;
+  for (; i + 3 < M; i += 4) {
+    float x[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) x[e] = __ldg(zc + (int64_t)(i + e) * (N + 1));
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      if (x[e] > best) best = x[e], arg = i + e;
+  }
+  for (; i < M; ++i) {
+    const float x = __ldg(zc + (int64_t)i * (N + 1));
+    if (x > best) best = x, arg = i;
+  }
+  colarg[(int64_t)b * N + j] = arg;
+}
+
 }  // namespace lgb
 
 using namespace lgb;
@@ -455,15 +582,27 @@ static int log_double_softmax_impl(const float* sim, float bin_score, const floa
 
 static int sk_launch(const void* fn, const SkPlan& p, size_t smem, void** args, cudaStream_t stream, const char* what) {
   if (int rc = ensure_dyn_smem(fn, (int)smem)) return rc;
-  cudaError_t e = cudaLaunchCooperativeKernel(fn, dim3(p.grid), dim3(kSkThreads), args, smem, stream);
+  // cudaLaunchKernelExC with the cooperative attribute: the same co-residency guarantee as
+  // cudaLaunchCooperativeKernel, and it is recorded into a CUDA graph when the stream is capturing
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeCooperative;
+  attr[0].val.cooperative = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(p.grid);
+  cfg.blockDim = dim3(kSkThreads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  cudaError_t e = cudaLaunchKernelExC(&cfg, fn, args);
   if (e != cudaSuccess) (void)cudaGetLastError();  // do not leave the error for the next launch check to find
   LGB_REQUIRE(e == cudaSuccess, kErrCuda, "%s: cooperative launch (%d CTAs, %zu B smem): %s", what, p.grid, smem,
               cudaGetErrorString(e));
   return check_launch(what);
 }
 
-int lgb200_sinkhorn_fwd(const float* sim, float alpha, int iters, float* out, float* uh, float* vh, void* ws, int B,
-                        int M, int N, cudaStream_t stream) {
+static int sinkhorn_fwd_impl(const float* sim, float alpha, const float* alpha_dev, int iters, float* out, float* uh,
+                             float* vh, void* ws, int B, int M, int N, cudaStream_t stream) {
   LGB_REQUIRE(sim && ws, kErrInvalid, "sinkhorn: null pointer");
   LGB_REQUIRE(B > 0 && M > 0 && N > 0 && iters >= 0, kErrInvalid, "sinkhorn: bad arguments");
   LGB_REQUIRE((uh == nullptr) == (vh == nullptr), kErrInvalid, "sinkhorn: uh and vh go together");
@@ -474,8 +613,33 @@ int lgb200_sinkhorn_fwd(const float* sim, float alpha, int iters, float* out, fl
   float* ps = pm + (size_t)(B + device_sm_count()) * (N + 1);
   unsigned* bar = reinterpret_cast<unsigned*>(ps + (size_t)(B + device_sm_count()) * (N + 1));
   LGB_REQUIRE(cudaMemsetAsync(bar, 0, sizeof(unsigned), stream) == cudaSuccess, kErrCuda, "sinkhorn: memset");
-  void* args[] = {&sim, &alpha, &iters, &out, &u, &v, &uh, &vh, &pm, &ps, &bar, &p.g};
+  void* args[] = {&sim, &alpha, &alpha_dev, &iters, &out, &u, &v, &uh, &vh, &pm, &ps, &bar, &p.g};
   return sk_launch((const void*)sk_fwd_persistent_kernel, p, p.smem_fwd, args, stream, "sinkhorn_fwd");
+}
+
+static int sinkhorn_bwd_impl(const float* sim, float alpha, const float* alpha_dev, int iters, const float* grad,
+                             const float* uh, const float* vh, float* dsim, float* dzr, float* dzc, void* ws, int B,
+                             int M, int N, cudaStream_t stream) {
+  LGB_REQUIRE(sim && grad && uh && vh && dsim && dzr && dzc && ws, kErrInvalid, "sinkhorn_bwd: null pointer");
+  LGB_REQUIRE(B > 0 && M > 0 && N > 0 && iters > 0, kErrInvalid, "sinkhorn_bwd: bad arguments");
+  SkPlan p = sk_plan(B, M, N);
+  float* dv = static_cast<float*>(ws) + (size_t)B * (M + 1);
+  float* pw = dv + (size_t)B * (N + 1);
+  unsigned* bar = reinterpret_cast<unsigned*>(pw + 2 * (size_t)(B + device_sm_count()) * (N + 1));
+  LGB_REQUIRE(cudaMemsetAsync(bar, 0, sizeof(unsigned), stream) == cudaSuccess, kErrCuda, "sinkhorn_bwd: memset");
+  void* args[] = {&sim, &alpha, &alpha_dev, &iters, &grad, &uh, &vh, &dsim, &dzr, &dzc, &dv, &pw, &bar, &p.g};
+  return sk_launch((const void*)sk_bwd_persistent_kernel, p, p.smem_bwd, args, stream, "sinkhorn_bwd");
+}
+
+int lgb200_sinkhorn_fwd(const float* sim, float alpha, int iters, float* out, float* uh, float* vh, void* ws, int B,
+                        int M, int N, cudaStream_t stream) {
+  return sinkhorn_fwd_impl(sim, alpha, nullptr, iters, out, uh, vh, ws, B, M, N, stream);
+}
+
+int lgb200_sinkhorn_fwd_dev(const float* sim, const float* alpha_dev, int iters, float* out, float* uh, float* vh,
+                            void* ws, int B, int M, int N, cudaStream_t stream) {
+  LGB_REQUIRE(alpha_dev, kErrInvalid, "sinkhorn: null bin score pointer");
+  return sinkhorn_fwd_impl(sim, 0.f, alpha_dev, iters, out, uh, vh, ws, B, M, N, stream);
 }
 
 int lgb200_sinkhorn(const float* sim, float alpha, int iters, float* out, void* ws, int B, int M, int N,
@@ -486,15 +650,46 @@ int lgb200_sinkhorn(const float* sim, float alpha, int iters, float* out, void* 
 
 int lgb200_sinkhorn_bwd(const float* sim, float alpha, int iters, const float* grad, const float* uh, const float* vh,
                         float* dsim, float* dzr, float* dzc, void* ws, int B, int M, int N, cudaStream_t stream) {
-  LGB_REQUIRE(sim && grad && uh && vh && dsim && dzr && dzc && ws, kErrInvalid, "sinkhorn_bwd: null pointer");
-  LGB_REQUIRE(B > 0 && M > 0 && N > 0 && iters > 0, kErrInvalid, "sinkhorn_bwd: bad arguments");
-  SkPlan p = sk_plan(B, M, N);
-  float* dv = static_cast<float*>(ws) + (size_t)B * (M + 1);
-  float* pw = dv + (size_t)B * (N + 1);
-  unsigned* bar = reinterpret_cast<unsigned*>(pw + 2 * (size_t)(B + device_sm_count()) * (N + 1));
-  LGB_REQUIRE(cudaMemsetAsync(bar, 0, sizeof(unsigned), stream) == cudaSuccess, kErrCuda, "sinkhorn_bwd: memset");
-  void* args[] = {&sim, &alpha, &iters, &grad, &uh, &vh, &dsim, &dzr, &dzc, &dv, &pw, &bar, &p.g};
-  return sk_launch((const void*)sk_bwd_persistent_kernel, p, p.smem_bwd, args, stream, "sinkhorn_bwd");
+  return sinkhorn_bwd_impl(sim, alpha, nullptr, iters, grad, uh, vh, dsim, dzr, dzc, ws, B, M, N, stream);
+}
+
+int lgb200_sinkhorn_bwd_dev(const float* sim, const float* alpha_dev, int iters, const float* grad, const float* uh,
+                            const float* vh, float* dsim, float* dzr, float* dzc, void* ws, int B, int M, int N,
+                            cudaStream_t stream) {
+  LGB_REQUIRE(alpha_dev, kErrInvalid, "sinkhorn_bwd: null bin score pointer");
+  return sinkhorn_bwd_impl(sim, 0.f, alpha_dev, iters, grad, uh, vh, dsim, dzr, dzc, ws, B, M, N, stream);
+}
+
+int lgb200_ot_nll_fwd(const float* Z, const uint8_t* mask, const float* neg0, const float* neg1, float* pos, float* neg,
+                      void* ws, int B, int M, int N, cudaStream_t stream) {
+  LGB_REQUIRE(Z && mask && neg0 && neg1 && pos && neg && ws, kErrInvalid, "ot_nll_fwd: null pointer");
+  LGB_REQUIRE(B > 0 && M > 0 && N > 0, kErrInvalid, "ot_nll_fwd: empty input");
+  const int nparts = (M + kOtRows - 1) / kOtRows;
+  float* part = static_cast<float*>(ws);
+  ot_nll_part_kernel<<<dim3(nparts, B), 256, 0, stream>>>(Z, mask, part, M, N);
+  if (int rc = check_launch("ot_nll_fwd")) return rc;
+  ot_nll_final_kernel<<<B, 256, 0, stream>>>(Z, neg0, neg1, part, nparts, pos, neg, M, N);
+  return check_launch("ot_nll_fwd");
+}
+
+int lgb200_ot_nll_bwd(const uint8_t* mask, const float* neg0, const float* neg1, const float* num_pos,
+                      const float* num_neg, const float* gpos, const float* gneg, float* dZ, int B, int M, int N,
+                      cudaStream_t stream) {
+  LGB_REQUIRE(mask && neg0 && neg1 && num_pos && num_neg && gpos && gneg && dZ, kErrInvalid, "ot_nll_bwd: null pointer");
+  LGB_REQUIRE(B > 0 && M > 0 && N > 0, kErrInvalid, "ot_nll_bwd: empty input");
+  ot_nll_bwd_kernel<<<dim3((M + 1 + kOtRows - 1) / kOtRows, B), 256, 0, stream>>>(mask, neg0, neg1, num_pos, num_neg,
+                                                                                 gpos, gneg, dZ, M, N);
+  return check_launch("ot_nll_bwd");
+}
+
+int lgb200_ot_filter_stats(const float* Z, float* rowmax, int* rowarg, int* colarg, int B, int M, int N,
+                           cudaStream_t stream) {
+  LGB_REQUIRE(Z && rowmax && rowarg && colarg, kErrInvalid, "ot_filter_stats: null pointer");
+  LGB_REQUIRE(B > 0 && M > 0 && N > 0, kErrInvalid, "ot_filter_stats: empty input");
+  ot_rowmax_kernel<<<dim3((M + 7) / 8, B), 256, 0, stream>>>(Z, rowmax, rowarg, M, N);
+  if (int rc = check_launch("ot_filter_stats")) return rc;
+  ot_colarg_kernel<<<dim3((N + 255) / 256, B), 256, 0, stream>>>(Z, colarg, M, N);
+  return check_launch("ot_filter_stats");
 }
 
 }  // extern "C"

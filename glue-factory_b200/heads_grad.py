@@ -106,7 +106,9 @@ class LogOptimalTransportFn(torch.autograd.Function):
         from . import ops
 
         sim = sim.contiguous()
-        out, uh, vh = ops._log_optimal_transport_fwd(sim, float(alpha), iters, keep_potentials=True)
+        # a CUDA alpha is read by the kernels on the device: no host read-back on a training step
+        a = alpha if ops._bin_dev(alpha) is not None else float(alpha)
+        out, uh, vh = ops._log_optimal_transport_fwd(sim, a, iters, keep_potentials=True)
         ctx.save_for_backward(sim, alpha, uh, vh)
         ctx.iters = iters
         return out
@@ -120,5 +122,6 @@ class LogOptimalTransportFn(torch.autograd.Function):
             M, N = sim.shape[1:]
             dsim, dalpha = grad[:, :M, :N].contiguous(), grad[:, :M, N].sum() + grad[:, M, :].sum()
         else:
-            dsim, dalpha = ops._log_optimal_transport_bwd(sim, float(alpha), ctx.iters, grad.contiguous().float(), uh, vh)
+            a = alpha if ops._bin_dev(alpha) is not None else float(alpha)
+            dsim, dalpha = ops._log_optimal_transport_bwd(sim, a, ctx.iters, grad.contiguous().float(), uh, vh)
         return dsim, dalpha.to(alpha.dtype).reshape(alpha.shape), None

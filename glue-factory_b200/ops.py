@@ -273,7 +273,7 @@ class BnRelu(torch.autograd.Function):
     dbeta come from this rank's sums (the gradient all-reduce adds the other ranks'), dx from the exchanged ones."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, running_mean, running_var, training, momentum, eps, exchange):
+    def forward(ctx, x, weight, bias, running_mean, running_var, training, momentum, eps, exchange, saved=None):
         x = x.contiguous()
         w, b = weight.detach().float().contiguous(), bias.detach().float().contiguous()
         sums = None
@@ -283,6 +283,8 @@ class BnRelu(torch.autograd.Function):
             sums = bn_stats(x)
             if exchange is not None:
                 exchange(sums)
+            if saved is not None:
+                saved.append(sums)
         y, mean, rstd = bn_relu_fwd(x, sums, w, b, running_mean, running_var, momentum, eps)
         ctx.save_for_backward(x, w, b, mean, rstd, sums)
         ctx.exchange = exchange
@@ -301,7 +303,18 @@ class BnRelu(torch.autograd.Function):
                 ctx.exchange(red)
             count = sums[2 * C:]
         dx = bn_relu_bwd(dy, x, w, b, mean, rstd, red if sums is not None else None, count)
-        return dx, dgamma, dbeta, None, None, None, None, None, None
+        return dx, dgamma, dbeta, None, None, None, None, None, None, None
+
+
+def bn_running_update(sums, bn):
+    """One more training-mode running-statistics step of BatchNorm `bn` from the batch statistics `sums` of an earlier
+    call (bn_stats layout, after any exchange), the same formula as bn_relu_fwd's; num_batches_tracked += 1."""
+    C = bn.running_mean.numel()
+    _chk(sums, torch.float64), _chk(bn.running_mean, torch.float32), _chk(bn.running_var, torch.float32)
+    assert sums.numel() == 2 * C + 1
+    call("lgb200_bn_running_update", ptr(sums), ptr(bn.running_mean), ptr(bn.running_var), float(bn.momentum), C,
+         stream_ptr())
+    bn.num_batches_tracked.add_(1)
 
 
 def bn_exchange(bn):
@@ -317,16 +330,17 @@ def bn_exchange(bn):
     return lambda t: dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
 
 
-def batchnorm_relu(x, bn, exchange=None):
+def batchnorm_relu(x, bn, exchange=None, saved=None):
     """relu(bn(x)) for an nn.BatchNorm1d / nn.SyncBatchNorm `bn` on token-major x [T, C], with the module's semantics:
     batch statistics in training mode (or without running statistics), running statistics in eval mode; a training call
-    updates running_mean / running_var and num_batches_tracked.  `exchange` as in BnRelu (see bn_exchange)."""
+    updates running_mean / running_var and num_batches_tracked.  `exchange` as in BnRelu (see bn_exchange).
+    `saved`: None or a list that receives the batch statistics a training call used (see bn_running_update)."""
     if bn.momentum is None or not bn.affine:
         raise NotImplementedError("gluefactory_b200 batchnorm_relu: momentum=None and affine=False are not built")
     rm, rv = (bn.running_mean, bn.running_var) if bn.track_running_stats else (None, None)
     if bn.training and bn.track_running_stats:
         bn.num_batches_tracked.add_(1)
-    return BnRelu.apply(x, bn.weight, bn.bias, rm, rv, bn.training or rm is None, bn.momentum, bn.eps, exchange)
+    return BnRelu.apply(x, bn.weight, bn.bias, rm, rv, bn.training or rm is None, bn.momentum, bn.eps, exchange, saved)
 
 
 def residual_add_cast(x, y, cdt, want_sum=True, out_cast=None):
@@ -738,25 +752,40 @@ def log_double_softmax(sim, bin_score):
     return _log_double_softmax_fwd(sim, bin_score)
 
 
+def _bin_dev(alpha):
+    """A CUDA tensor bin score as a 1-element fp32 device vector (read by the kernels: no host read-back), else None."""
+    if torch.is_tensor(alpha) and alpha.is_cuda:
+        return alpha.detach().reshape(-1)[:1].float().contiguous()
+    return None
+
+
 def _log_optimal_transport_fwd(sim, alpha, iters, keep_potentials=False):
     """One persistent cooperative kernel for all iterations.  keep_potentials: also return the per-iteration
-    potentials (uh [iters,B,M+1], vh [iters,B,N+1]) the backward sweep consumes."""
+    potentials (uh [iters,B,M+1], vh [iters,B,N+1]) the backward sweep consumes.  alpha: a CUDA tensor is read on the
+    device (lgb200_sinkhorn_fwd_dev), anything else is a host scalar."""
     _chk(sim, torch.float32)
     B, M, N = sim.shape
     out = torch.empty(B, M + 1, N + 1, device=sim.device, dtype=torch.float32)
     ws = torch.empty(_lib.load().lgb200_heads_ws_bytes(B, M, N), device=sim.device, dtype=torch.uint8)
-    if not keep_potentials:
+    a_dev = _bin_dev(alpha)
+    uh = vh = None
+    if keep_potentials:
+        uh = torch.empty(max(iters, 1), B, M + 1, device=sim.device, dtype=torch.float32)
+        vh = torch.empty(max(iters, 1), B, N + 1, device=sim.device, dtype=torch.float32)
+    if a_dev is not None:
+        call("lgb200_sinkhorn_fwd_dev", ptr(sim), ptr(a_dev), int(iters), ptr(out), ptr(uh), ptr(vh), ptr(ws), B, M, N,
+             stream_ptr())
+    elif keep_potentials:
+        call("lgb200_sinkhorn_fwd", ptr(sim), float(alpha), int(iters), ptr(out), ptr(uh), ptr(vh), ptr(ws), B, M, N,
+             stream_ptr())
+    else:
         call("lgb200_sinkhorn", ptr(sim), float(alpha), int(iters), ptr(out), ptr(ws), B, M, N, stream_ptr())
-        return out
-    uh = torch.empty(max(iters, 1), B, M + 1, device=sim.device, dtype=torch.float32)
-    vh = torch.empty(max(iters, 1), B, N + 1, device=sim.device, dtype=torch.float32)
-    call("lgb200_sinkhorn_fwd", ptr(sim), float(alpha), int(iters), ptr(out), ptr(uh), ptr(vh), ptr(ws), B, M, N,
-         stream_ptr())
-    return out, uh, vh
+    return (out, uh, vh) if keep_potentials else out
 
 
 def _log_optimal_transport_bwd(sim, alpha, iters, grad, uh, vh):
-    """Reverse sweep of the iterations (lgb200_sinkhorn_bwd): returns dsim [B,M,N] and d alpha (0-dim)."""
+    """Reverse sweep of the iterations (lgb200_sinkhorn_bwd, or _dev for a CUDA tensor alpha): returns dsim [B,M,N]
+    and d alpha (0-dim, on the device)."""
     _chk(sim, torch.float32)
     _chk(grad, torch.float32)
     B, M, N = sim.shape
@@ -765,8 +794,13 @@ def _log_optimal_transport_bwd(sim, alpha, iters, grad, uh, vh):
     dzr = torch.empty(B, N + 1, device=sim.device, dtype=torch.float32)
     dzc = torch.empty(B, M, device=sim.device, dtype=torch.float32)
     ws = torch.empty(_lib.load().lgb200_heads_ws_bytes(B, M, N), device=sim.device, dtype=torch.uint8)
-    call("lgb200_sinkhorn_bwd", ptr(sim), float(alpha), int(iters), ptr(grad), ptr(uh), ptr(vh), ptr(dsim), ptr(dzr),
-         ptr(dzc), ptr(ws), B, M, N, stream_ptr())
+    a_dev = _bin_dev(alpha)
+    if a_dev is not None:
+        call("lgb200_sinkhorn_bwd_dev", ptr(sim), ptr(a_dev), int(iters), ptr(grad), ptr(uh), ptr(vh), ptr(dsim),
+             ptr(dzr), ptr(dzc), ptr(ws), B, M, N, stream_ptr())
+    else:
+        call("lgb200_sinkhorn_bwd", ptr(sim), float(alpha), int(iters), ptr(grad), ptr(uh), ptr(vh), ptr(dsim),
+             ptr(dzr), ptr(dzc), ptr(ws), B, M, N, stream_ptr())
     return dsim, dzr.sum() + dzc.sum()
 
 
@@ -777,7 +811,80 @@ def log_optimal_transport(sim, alpha, iters):
         from .heads_grad import LogOptimalTransportFn
 
         return LogOptimalTransportFn.apply(sim, alpha, int(iters))
-    return _log_optimal_transport_fwd(sim, float(alpha), iters)
+    return _log_optimal_transport_fwd(sim, alpha if _bin_dev(alpha) is not None else float(alpha), iters)
+
+
+# ------------------------------------------------------------------------------------------------
+# SuperGlue's NLL head and match filter on the dense Sinkhorn output (superglue.py:301-311, 322-352)
+# ------------------------------------------------------------------------------------------------
+def ot_nll_sums(Z, mask_u8, neg0, neg1):
+    """Z [B,M+1,N+1] fp32, mask u8 [B,M,N], neg0 [B,M] / neg1 [B,N] fp32 0/1 -> (pos, neg) [B]:
+    pos = sum mask * Z[:, :M, :N], neg = sum neg0 * Z[:, :M, N] + sum neg1 * Z[:, M, :N] (lgb200_ot_nll_fwd)."""
+    _chk(Z, torch.float32), _chk(mask_u8, torch.uint8), _chk(neg0, torch.float32), _chk(neg1, torch.float32)
+    B, M1, N1 = Z.shape
+    M, N = M1 - 1, N1 - 1
+    assert mask_u8.shape == (B, M, N) and neg0.shape == (B, M) and neg1.shape == (B, N)
+    pos = torch.empty(B, device=Z.device, dtype=torch.float32)
+    neg = torch.empty_like(pos)
+    ws = torch.empty(_lib.load().lgb200_heads_ws_bytes(B, M, N), device=Z.device, dtype=torch.uint8)
+    call("lgb200_ot_nll_fwd", ptr(Z), ptr(mask_u8), ptr(neg0), ptr(neg1), ptr(pos), ptr(neg), ptr(ws), B, M, N,
+         stream_ptr())
+    return pos, neg
+
+
+def ot_nll_bwd(mask_u8, neg0, neg1, num_pos, num_neg, gpos, gneg):
+    """dZ [B,M+1,N+1] of nll_pos = -pos / num_pos and nll_neg = -neg / num_neg for incoming gradients gpos, gneg [B]
+    (lgb200_ot_nll_bwd: everything read on the device, linear in the incoming gradients)."""
+    B, M, N = mask_u8.shape
+    for t in (neg0, neg1, num_pos, num_neg, gpos, gneg):
+        _chk(t, torch.float32)
+    dZ = torch.empty(B, M + 1, N + 1, device=mask_u8.device, dtype=torch.float32)
+    call("lgb200_ot_nll_bwd", ptr(mask_u8), ptr(neg0), ptr(neg1), ptr(num_pos), ptr(num_neg), ptr(gpos), ptr(gneg),
+         ptr(dZ), B, M, N, stream_ptr())
+    return dZ
+
+
+class OtNllFn(torch.autograd.Function):
+    """(nll_pos, nll_neg) [B] of superglue.py:325-336 from the dense log assignment Z, differentiable w.r.t. Z; the
+    reference's dense fp32 copies of the mask and of mask * Z are never formed."""
+
+    @staticmethod
+    def forward(ctx, Z, mask_u8, neg0, neg1, num_pos, num_neg):
+        pos, neg = ot_nll_sums(Z, mask_u8, neg0, neg1)
+        ctx.save_for_backward(mask_u8, neg0, neg1, num_pos, num_neg)
+        return -pos / num_pos, -neg / num_neg
+
+    @staticmethod
+    def backward(ctx, gpos, gneg):
+        mask_u8, neg0, neg1, num_pos, num_neg = ctx.saved_tensors
+        z = torch.zeros_like(num_pos)
+        gpos = z if gpos is None else gpos.float().contiguous()
+        gneg = z if gneg is None else gneg.float().contiguous()
+        return ot_nll_bwd(mask_u8, neg0, neg1, num_pos, num_neg, gpos, gneg), None, None, None, None, None
+
+
+def ot_nll(Z, gt_assignment, gt_matches0, gt_matches1):
+    """superglue.py:325-336 -> (nll_pos, nll_neg, num_pos, num_neg) [B]; counts from lgb200_mask_counts."""
+    mask = gt_assignment.to(torch.uint8).contiguous()
+    neg0 = (gt_matches0 == -1).float().contiguous()
+    neg1 = (gt_matches1 == -1).float().contiguous()
+    rowcnt, _ = mask_counts(mask)
+    num_pos = rowcnt.sum(1).clamp(min=1.0)
+    num_neg = (neg0.sum(1) + neg1.sum(1)).clamp(min=1.0)
+    nll_pos, nll_neg = OtNllFn.apply(Z.contiguous(), mask, neg0, neg1, num_pos, num_neg)
+    return nll_pos, nll_neg, num_pos, num_neg
+
+
+def ot_filter_stats(Z):
+    """Row max / argmax and column argmax (int32, first index on ties) of Z[:, :-1, :-1] (lgb200_ot_filter_stats)."""
+    _chk(Z, torch.float32)
+    B, M1, N1 = Z.shape
+    M, N = M1 - 1, N1 - 1
+    rowmax = torch.empty(B, M, device=Z.device, dtype=torch.float32)
+    rowarg = torch.empty(B, M, device=Z.device, dtype=torch.int32)
+    colarg = torch.empty(B, N, device=Z.device, dtype=torch.int32)
+    call("lgb200_ot_filter_stats", ptr(Z), ptr(rowmax), ptr(rowarg), ptr(colarg), B, M, N, stream_ptr())
+    return rowmax, rowarg, colarg
 
 
 def adam_flat_(p, g, m, v, step, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, grad_scale=1.0, lr_scale_per_elem=None,

@@ -251,6 +251,16 @@ def make_gluestick_weights(state_dict_like, seed=0, dtype=torch.float32):
     return out
 
 
+def make_superglue_batch(B, M, N, seed, D=256, dtype=torch.float32):
+    """Synthetic SuperGlue batch: make_pairs (keypoints, descriptors, homography labels; M view-0 and N view-1 points)
+    plus per-keypoint detection scores in [0, 1)."""
+    d = make_pairs(B, N, seed=seed, D=D, M=M, dtype=dtype)
+    rs = np.random.RandomState(seed + 7)
+    for i, n in (("0", M), ("1", N)):
+        d[f"keypoint_scores{i}"] = torch.from_numpy(rs.uniform(0, 1, size=(B, n))).to(dtype)
+    return d
+
+
 # ----------------------------------------------------------------------------
 # pose + depth ground truth (MegaDepth-style supervision, matchers/depth_matcher.py)
 # ----------------------------------------------------------------------------

@@ -221,6 +221,28 @@ int lgb200_sinkhorn_fwd(const float* sim, float alpha, int iters, float* out, fl
                         int M, int N, cudaStream_t stream);
 int lgb200_sinkhorn_bwd(const float* sim, float alpha, int iters, const float* grad, const float* uh, const float* vh,
                         float* dsim, float* dzr, float* dzc, void* ws, int B, int M, int N, cudaStream_t stream);
+/* The same two with the (learnt) bin score alpha read from device memory at kernel start: no host read-back, so a
+ * training step that runs them can be captured into a CUDA graph.  Results equal the host-scalar entry points'.  */
+int lgb200_sinkhorn_fwd_dev(const float* sim, const float* alpha_dev, int iters, float* out, float* uh, float* vh,
+                            void* ws, int B, int M, int N, cudaStream_t stream);
+int lgb200_sinkhorn_bwd_dev(const float* sim, const float* alpha_dev, int iters, const float* grad, const float* uh,
+                            const float* vh, float* dsim, float* dzr, float* dzc, void* ws, int B, int M, int N,
+                            cudaStream_t stream);
+/* NLL head on the dense Sinkhorn output Z [B,M+1,N+1] (row pitch N+1; superglue.py:322-352), gt mask u8 [B,M,N],
+ * neg0 [B,M] / neg1 [B,N] the 0/1 unmatched indicators (fp32).  Forward, per pair: pos = sum mask * Z[:M,:N],
+ * neg = sum neg0 * Z[:M,N] + sum neg1 * Z[M,:N], in a fixed order (two calls are bit-identical); ws: at least
+ * 4 * B * ceil(M / 8) bytes (lgb200_heads_ws_bytes suffices).  Backward of nll_pos = -pos / num_pos and
+ * nll_neg = -neg / num_neg (num_pos, num_neg [B] the clamped counts) for the incoming gradients gpos, gneg [B], all
+ * read on the device: writes every element of dZ [B,M+1,N+1] (0 off the positives and the bins, corner included). */
+int lgb200_ot_nll_fwd(const float* Z, const uint8_t* mask, const float* neg0, const float* neg1, float* pos, float* neg,
+                      void* ws, int B, int M, int N, cudaStream_t stream);
+int lgb200_ot_nll_bwd(const uint8_t* mask, const float* neg0, const float* neg1, const float* num_pos,
+                      const float* num_neg, const float* gpos, const float* gneg, float* dZ, int B, int M, int N,
+                      cudaStream_t stream);
+/* Row max / argmax and column argmax of the inner block Z[:, :M, :N] (row pitch N+1), first index on ties like
+ * torch's CPU max: the inputs of lgb200_filter_matches for SuperGlue's filter (superglue.py:301-311).             */
+int lgb200_ot_filter_stats(const float* Z, float* rowmax, int* rowarg, int* colarg, int B, int M, int N,
+                           cudaStream_t stream);
 
 /* column sums of a tall [rows, cols] matrix = bias gradient of an nn.Linear (autograd of lightglue.py:156 etc.).
  * ws: lgb200_colsum_slabs(rows, cols) * cols floats of scratch; counters: (cols+63)/64 uint32, zero before the
@@ -262,6 +284,11 @@ int lgb200_bn_relu_bwd_reduce(const void* dy, const void* x, const float* gamma,
 int lgb200_bn_relu_bwd(const void* dy, const void* x, const float* gamma, const float* beta, const float* mean,
                        const float* rstd, const double* sums, const double* count, void* dx, int64_t ntok, int C,
                        int dtype, cudaStream_t stream);
+/* The running-statistics update of bn_relu_fwd alone (same formula), from the batch statistics `sums` of an earlier
+ * bn_stats call: a second training-mode call of the same BatchNorm on the same batch without redoing the pass over x
+ * (SuperGlue's checkpointed GNN recomputes each layer in the backward, updating its BatchNorms again).  One launch. */
+int lgb200_bn_running_update(const double* sums, float* running_mean, float* running_var, float momentum, int C,
+                             cudaStream_t stream);
 
 /* ---- flat-buffer optimiser (train.py:358-361, 513) and casts --------------------------------------- */
 /* Adam over the flat buffers, one launch.  g is multiplied by grad_scale (1/world for the summed all-reduce).
