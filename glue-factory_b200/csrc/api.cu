@@ -71,7 +71,9 @@ int make_tmap(CUtensorMap* out, const void* base, bool fp32, int rank, const uin
   auto encode = [&]() {
     return fn(out, fp32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank,
               const_cast<void*>(base), gdim, gstr, bx, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-              swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+              swizzle_bytes == 32   ? CU_TENSOR_MAP_SWIZZLE_32B
+              : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                    : CU_TENSOR_MAP_SWIZZLE_128B,
               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   };
   CUresult r = encode();
@@ -143,32 +145,51 @@ int lgb200_check_device(void) {
   return 0;
 }
 
-int lgb200_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk, int H,
-                    int kv_shift, float scale, int dtype, cudaStream_t stream) {
+int lgb200_attn_fwd_hd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk,
+                       int H, int kv_shift, float scale, int dtype, int head_dim, cudaStream_t stream) {
   LGB_REQUIRE(q && k && v && out && lse, kErrInvalid, "attn_fwd: null pointer");
   LGB_REQUIRE(B > 0 && Nq > 0 && Nk > 0 && H > 0, kErrInvalid, "attn_fwd: empty input B=%d Nq=%d Nk=%d H=%d", B, Nq,
               Nk, H);
   LGB_REQUIRE(kv_shift >= 0 && kv_shift < B, kErrInvalid, "attn_fwd: kv_shift %d out of range", kv_shift);
-  if (dtype == LGB200_F32) return attn_fwd_simt(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream);
+  LGB_REQUIRE(head_dim == 32 || head_dim == 64, kErrUnsupported, "attn_fwd: head_dim %d (built for 32 and 64)",
+              head_dim);
+  if (dtype == LGB200_F32) return attn_fwd_simt(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, head_dim, stream);
   LGB_REQUIRE(dtype == LGB200_BF16, kErrInvalid, "attn_fwd: bad dtype %d", dtype);
-  return attn_fwd_tc(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream);
+  return attn_fwd_tc(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, head_dim, stream);
+}
+
+int lgb200_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk, int H,
+                    int kv_shift, float scale, int dtype, cudaStream_t stream) {
+  return lgb200_attn_fwd_hd(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, dtype, 64, stream);
 }
 
 int64_t lgb200_attn_bwd_ws_floats(int B, int Nq, int Nk, int H) { return attn_bwd_ws_floats(B, Nq, Nk, H); }
 
-int lgb200_attn_bwd(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
-                    void* dq, void* dk, void* dv, float* delta_ws, int B, int Nq, int Nk, int H, int kv_shift,
-                    float scale, int dtype, cudaStream_t stream) {
+int lgb200_attn_bwd_hd(const void* q, const void* k, const void* v, const void* out, const float* lse,
+                       const void* dout, void* dq, void* dk, void* dv, float* delta_ws, int B, int Nq, int Nk, int H,
+                       int kv_shift, float scale, int dtype, int head_dim, cudaStream_t stream) {
   LGB_REQUIRE(q && k && v && out && lse && dout && dq && dk && dv && delta_ws, kErrInvalid, "attn_bwd: null pointer");
   LGB_REQUIRE(B > 0 && Nq > 0 && Nk > 0 && H > 0, kErrInvalid, "attn_bwd: empty input");
   LGB_REQUIRE(kv_shift >= 0 && kv_shift < B, kErrInvalid, "attn_bwd: kv_shift %d out of range", kv_shift);
+  LGB_REQUIRE(head_dim == 32 || head_dim == 64, kErrUnsupported, "attn_bwd: head_dim %d (built for 32 and 64)",
+              head_dim);
   const bool shared_qk = attn_bwd_is_shared_qk(q, k, dq, dk, B, Nq, Nk, kv_shift);
   LGB_REQUIRE(!shared_qk || dtype == LGB200_BF16, kErrUnsupported,
               "attn_bwd: dq == dk (shared-qk cross-attention) runs on the bf16 tensor-core path only");
+  LGB_REQUIRE(!shared_qk || head_dim == 64, kErrUnsupported,
+              "attn_bwd: dq == dk (shared-qk cross-attention) is built for head_dim 64 only");
   if (dtype == LGB200_F32)
-    return attn_bwd_simt(q, k, v, out, lse, dout, dq, dk, dv, delta_ws, B, Nq, Nk, H, kv_shift, scale, stream);
+    return attn_bwd_simt(q, k, v, out, lse, dout, dq, dk, dv, delta_ws, B, Nq, Nk, H, kv_shift, scale, head_dim,
+                         stream);
   LGB_REQUIRE(dtype == LGB200_BF16, kErrInvalid, "attn_bwd: bad dtype %d", dtype);
-  return attn_bwd_tc(q, k, v, out, lse, dout, dq, dk, dv, delta_ws, B, Nq, Nk, H, kv_shift, scale, stream);
+  return attn_bwd_tc(q, k, v, out, lse, dout, dq, dk, dv, delta_ws, B, Nq, Nk, H, kv_shift, scale, head_dim, stream);
+}
+
+int lgb200_attn_bwd(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
+                    void* dq, void* dk, void* dv, float* delta_ws, int B, int Nq, int Nk, int H, int kv_shift,
+                    float scale, int dtype, cudaStream_t stream) {
+  return lgb200_attn_bwd_hd(q, k, v, out, lse, dout, dq, dk, dv, delta_ws, B, Nq, Nk, H, kv_shift, scale, dtype, 64,
+                            stream);
 }
 
 }  // extern "C"

@@ -1,15 +1,15 @@
 // fp32 CUDA-core attention (forward + backward) -- the full-precision parity path (`precision="fp32"`).  The bf16
 // wgmma kernels (attn_tc.cu) are tested against fp64 torch, not against this file.
 //
-//   out = softmax(scale * q k^T) v       per (batch, head), head_dim = 64
+//   out = softmax(scale * q k^T) v       per (batch, head), head_dim kD = 64 or 32
 // (reference: gluefactory/models/matchers/lightglue.py:118-121 self-attention,
 //  :207-216 cross-attention evaluated as two one-directional passes).
 //
-// Tensors are token-major [B, N, H, 64].  The key/value batch of query batch b is
+// Tensors are token-major [B, N, H, kD].  The key/value batch of query batch b is
 // (b + kv_shift) % B, which expresses the two directions of cross-attention on the
 // concatenated [image0; image1] batch as ONE launch.
 //
-// Work split: two threads per row ("row" = query in fwd/dq, key in dkv), each owning 32 of the 64
+// Work split: two threads per row ("row" = query in fwd/dq, key in dkv), each owning half of the kD
 // channels; dot products are completed with one shuffle.  The opposite operand is staged through
 // shared memory in 64-row tiles and read as warp-wide broadcasts.
 #include <math.h>
@@ -19,22 +19,23 @@
 
 namespace lgb {
 
-constexpr int kD = 64;
-constexpr int kHalf = 32;
 constexpr int kTile = 64;  // rows per smem tile == rows per CTA
 
-// cooperative load of `rows` x 64 (row stride ld elements) into smem [kTile][kD], zero-filled past nvalid
+// cooperative load of `rows` x kD (row stride ld elements) into smem [kTile][kD], zero-filled past nvalid
+template <int kD>
 __device__ __forceinline__ void load_tile(float (*dst)[kD], const float* src, int64_t ld, int nvalid) {
   for (int idx = threadIdx.x; idx < kTile * kD; idx += blockDim.x) {
-    const int r = idx >> 6, c = idx & 63;
+    const int r = idx >> (kD == 64 ? 6 : 5), c = idx & (kD - 1);
     dst[r][c] = r < nvalid ? src[(int64_t)r * ld + c] : 0.f;
   }
 }
 
+template <int kD>
 __global__ void __launch_bounds__(128) attn_fwd_simt_kernel(const float* __restrict__ q, const float* __restrict__ k,
                                                             const float* __restrict__ v, float* __restrict__ out,
                                                             float* __restrict__ lse, int B, int Nq, int Nk, int H,
                                                             int kv_shift, float scale) {
+  constexpr int kHalf = kD / 2;
   __shared__ float sk[kTile][kD];
   __shared__ float sv[kTile][kD];
   const int b = blockIdx.z, h = blockIdx.y;
@@ -83,7 +84,8 @@ __global__ void __launch_bounds__(128) attn_fwd_simt_kernel(const float* __restr
   }
 }
 
-// delta[b,h,i] = sum_d dout[b,i,h,d] * out[b,i,h,d]   (8 lanes per row)
+// delta[b,h,i] = sum_d dout[b,i,h,d] * out[b,i,h,d]   (8 lanes per row, kD / 8 channels each)
+template <int kD>
 __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict__ out, const float* __restrict__ dout,
                                                          float* __restrict__ delta, int64_t nrows /*B*N*H*/, int N,
                                                          int H) {
@@ -93,7 +95,7 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict
   float acc = 0.f;
   if (r < nrows) {
 #pragma unroll
-    for (int e = 0; e < 8; ++e) acc += out[r * kD + sub * 8 + e] * dout[r * kD + sub * 8 + e];
+    for (int e = 0; e < kD / 8; ++e) acc += out[r * kD + sub * (kD / 8) + e] * dout[r * kD + sub * (kD / 8) + e];
   }
   acc += __shfl_xor_sync(0xffffffffu, acc, 1);
   acc += __shfl_xor_sync(0xffffffffu, acc, 2);
@@ -108,11 +110,13 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict
 }
 
 // dq_i = scale * sum_j p_ij (dp_ij - delta_i) k_j
+template <int kD>
 __global__ void __launch_bounds__(128)
     attn_bwd_dq_simt_kernel(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
                             const float* __restrict__ dout, const float* __restrict__ lse,
                             const float* __restrict__ delta, float* __restrict__ dq, int B, int Nq, int Nk, int H,
                             int kv_shift, float scale) {
+  constexpr int kHalf = kD / 2;
   __shared__ float sk[kTile][kD];
   __shared__ float sv[kTile][kD];
   const int b = blockIdx.z, h = blockIdx.y;
@@ -160,11 +164,13 @@ __global__ void __launch_bounds__(128)
 
 // dv_j = sum_i p_ij do_i ;  dk_j = scale * sum_i p_ij (dp_ij - delta_i) q_i
 // launched over KEY batches kb; the query batch is qb = (kb - kv_shift) mod B.
+template <int kD>
 __global__ void __launch_bounds__(128)
     attn_bwd_dkv_simt_kernel(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
                              const float* __restrict__ dout, const float* __restrict__ lse,
                              const float* __restrict__ delta, float* __restrict__ dk, float* __restrict__ dv, int B,
                              int Nq, int Nk, int H, int kv_shift, float scale) {
+  constexpr int kHalf = kD / 2;
   __shared__ float sq[kTile][kD];
   __shared__ float sdo[kTile][kD];
   __shared__ float sl[kTile], sd[kTile];
@@ -221,35 +227,55 @@ __global__ void __launch_bounds__(128)
   }
 }
 
-int attn_fwd_simt(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk, int H,
-                  int kv_shift, float scale, cudaStream_t stream) {
+template <int kD>
+static int attn_fwd_simt_hd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk,
+                            int H, int kv_shift, float scale, cudaStream_t stream) {
   dim3 grid((Nq + kTile - 1) / kTile, H, B);
-  attn_fwd_simt_kernel<<<grid, 128, 0, stream>>>((const float*)q, (const float*)k, (const float*)v, (float*)out, lse, B,
-                                                 Nq, Nk, H, kv_shift, scale);
+  attn_fwd_simt_kernel<kD><<<grid, 128, 0, stream>>>((const float*)q, (const float*)k, (const float*)v, (float*)out,
+                                                     lse, B, Nq, Nk, H, kv_shift, scale);
   return check_launch("attn_fwd_simt");
 }
 
-int attn_delta(const void* out, const void* dout, float* delta, int B, int N, int H, cudaStream_t stream) {
+int attn_fwd_simt(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk, int H,
+                  int kv_shift, float scale, int head_dim, cudaStream_t stream) {
+  return head_dim == 32 ? attn_fwd_simt_hd<32>(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream)
+                        : attn_fwd_simt_hd<64>(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream);
+}
+
+int attn_delta(const void* out, const void* dout, float* delta, int B, int N, int H, int head_dim,
+               cudaStream_t stream) {
   const int64_t nrows = (int64_t)B * N * H;
   const unsigned grid = (unsigned)((nrows * 8 + 255) / 256);
-  attn_delta_kernel<<<grid, 256, 0, stream>>>((const float*)out, (const float*)dout, delta, nrows, N, H);
+  if (head_dim == 32)
+    attn_delta_kernel<32><<<grid, 256, 0, stream>>>((const float*)out, (const float*)dout, delta, nrows, N, H);
+  else
+    attn_delta_kernel<64><<<grid, 256, 0, stream>>>((const float*)out, (const float*)dout, delta, nrows, N, H);
   return check_launch("attn_delta");
+}
+
+template <int kD>
+static int attn_bwd_simt_hd(const void* q, const void* k, const void* v, const void* out, const float* lse,
+                            const void* dout, void* dq, void* dk, void* dv, float* delta, int B, int Nq, int Nk, int H,
+                            int kv_shift, float scale, cudaStream_t stream) {
+  int rc = attn_delta(out, dout, delta, B, Nq, H, kD, stream);
+  if (rc) return rc;
+  dim3 gq((Nq + kTile - 1) / kTile, H, B);
+  attn_bwd_dq_simt_kernel<kD><<<gq, 128, 0, stream>>>((const float*)q, (const float*)k, (const float*)v,
+                                                      (const float*)dout, lse, delta, (float*)dq, B, Nq, Nk, H,
+                                                      kv_shift, scale);
+  dim3 gk((Nk + kTile - 1) / kTile, H, B);
+  attn_bwd_dkv_simt_kernel<kD><<<gk, 128, 0, stream>>>((const float*)q, (const float*)k, (const float*)v,
+                                                       (const float*)dout, lse, delta, (float*)dk, (float*)dv, B, Nq,
+                                                       Nk, H, kv_shift, scale);
+  return check_launch("attn_bwd_simt");
 }
 
 int attn_bwd_simt(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
                   void* dq, void* dk, void* dv, float* delta, int B, int Nq, int Nk, int H, int kv_shift, float scale,
-                  cudaStream_t stream) {
-  int rc = attn_delta(out, dout, delta, B, Nq, H, stream);
-  if (rc) return rc;
-  dim3 gq((Nq + kTile - 1) / kTile, H, B);
-  attn_bwd_dq_simt_kernel<<<gq, 128, 0, stream>>>((const float*)q, (const float*)k, (const float*)v,
-                                                  (const float*)dout, lse, delta, (float*)dq, B, Nq, Nk, H, kv_shift,
-                                                  scale);
-  dim3 gk((Nk + kTile - 1) / kTile, H, B);
-  attn_bwd_dkv_simt_kernel<<<gk, 128, 0, stream>>>((const float*)q, (const float*)k, (const float*)v,
-                                                   (const float*)dout, lse, delta, (float*)dk, (float*)dv, B, Nq, Nk, H,
-                                                   kv_shift, scale);
-  return check_launch("attn_bwd_simt");
+                  int head_dim, cudaStream_t stream) {
+  return head_dim == 32
+             ? attn_bwd_simt_hd<32>(q, k, v, out, lse, dout, dq, dk, dv, delta, B, Nq, Nk, H, kv_shift, scale, stream)
+             : attn_bwd_simt_hd<64>(q, k, v, out, lse, dout, dq, dk, dv, delta, B, Nq, Nk, H, kv_shift, scale, stream);
 }
 
 }  // namespace lgb

@@ -1,6 +1,12 @@
 // Flash attention on the Hopper tensor cores (sm_90a): out = softmax(scale * q k^T) v
-// for head_dim 64, bf16 operands, fp32 accumulation, never materialising the N x N similarity.
-// (reference: lightglue.py:118-121 self-attention; :207-216 cross-attention.)
+// for head_dim 64 or 32, bf16 operands, fp32 accumulation, never materialising the N x N similarity.
+// (reference: lightglue.py:118-121 self-attention; :207-216 cross-attention; gluestick.py:524-529.)
+//
+// The description below is for head_dim D = 64.  The forward, dQ and dK / dV kernels are templates on D; at D = 32
+// (GlueStick with 128-channel descriptors, 4 heads) a q / k / v row is 64 bytes, so the tiles use the 64-byte swizzle,
+// Q K^T takes two k-steps instead of four, and the products with a D-wide output (P V, dQ, dK, dV) are m64n32k16.  At
+// D = 32 a 64 x 64 tile costs half the tensor-core time of D = 64 but the same 4096 exponentials, so the forward is
+// bound by the exponentials there.  The shared-qk backward is built for D = 64 only.
 //
 // FORWARD.  One CTA = one (batch, head, 128-query tile): two consumer warpgroups of 64 query rows each and one TMA
 // producer warp.  Q/K/V tiles are brought in by TMA (4-D tensor map over the token-major [B,N,H,64] layout, 128-byte
@@ -21,6 +27,8 @@
 // similarity, so one sweep per image yields dV and dq + dk (attn_bwd_shared_qk_kernel, below).
 #include <math.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "host_util.h"
 #include "lgb200.h"
@@ -29,12 +37,32 @@ namespace lgb {
 
 constexpr int FA_BM = 128;     // queries per CTA
 constexpr int FA_BN = 64;      // keys per iteration
-constexpr int FA_D = 64;
 constexpr int FA_STAGES = 4;
-constexpr int FA_QBYTES = FA_BM * FA_D * 2;   // 16 KiB
-constexpr int FA_KBYTES = FA_BN * FA_D * 2;   // 8 KiB
-constexpr int FA_SMEM = FA_QBYTES + FA_STAGES * 2 * FA_KBYTES + 256;
 constexpr int FA_THREADS = 2 * 128 + 32;      // two consumer warpgroups + the producer warp
+
+// Tile geometry at head dim D: a q / k / v row is one head of D bf16, 2D bytes, which is also the swizzle span of the
+// TMA tiles and of the wgmma descriptors (128 B at D = 64, 64 B at D = 32).
+template <int D>
+struct Hd {
+  static_assert(D == 32 || D == 64, "head_dim 32 or 64");
+  static constexpr int ROW = 2 * D;                    // bytes per row = swizzle span
+  static constexpr int SBO = 8 * ROW;                  // 8-row swizzle atom
+  static constexpr int WG = 64 * ROW;                  // a warpgroup's 64 rows of a resident tile
+  static constexpr int MN_KSTEP = (16 * ROW) >> 4;     // descriptor step of one K=16 slice of an MN-major operand
+  static constexpr int NACC = D / 2;                   // fp32 accumulators per thread of a 64 x D tile
+  static constexpr int QBYTES = FA_BM * ROW;           // forward: Q tile (16 KiB at D = 64)
+  static constexpr int KBYTES = FA_BN * ROW;           // forward: one K or V stage (8 KiB at D = 64)
+  static constexpr int SMEM = QBYTES + FA_STAGES * 2 * KBYTES + 256;
+};
+
+// wgmma with a D-wide output (P V, dS K, P^T dO, dS^T Q)
+template <int D, int TB>
+__device__ __forceinline__ void wgmma_m64nD_rs(float (&d)[D / 2], const uint32_t (&a)[4], uint64_t db, int acc) {
+  if constexpr (D == 64)
+    wgmma_m64n64_rs<TB>(d, a, db, acc);
+  else
+    wgmma_m64n32_rs<TB>(d, a, db, acc);
+}
 constexpr int FA_PRODUCER = 8;
 constexpr float kLn2 = 0.6931471805599453f, kLog2e = 1.4426950408889634f;
 
@@ -48,26 +76,30 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-// bf16 store of a 64 x 64 accumulator (the warpgroup's rows row_base.., valid while < nrows) into the token-major
-// [.., N, H, 64] layout at (batch, head)
-__device__ __forceinline__ void store_acc_rows(const float (&d)[32], __nv_bfloat16* __restrict__ dst, int bat, int N,
-                                               int H, int h, int row_base, float mul) {
+// bf16 store of a 64 x D accumulator (the warpgroup's rows row_base.., valid while < nrows) into the token-major
+// [.., N, H, D] layout at (batch, head)
+template <int D>
+__device__ __forceinline__ void store_acc_rows(const float (&d)[D / 2], __nv_bfloat16* __restrict__ dst, int bat,
+                                               int N, int H, int h, int row_base, float mul) {
   const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     const int row = row_base + wq * 16 + (lane >> 2) + 8 * i;
     if (row >= N) continue;
-    __nv_bfloat16* o = dst + (((int64_t)bat * N + row) * H + h) * FA_D + 2 * (lane & 3);
+    __nv_bfloat16* o = dst + (((int64_t)bat * N + row) * H + h) * D + 2 * (lane & 3);
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
+    for (int j = 0; j < D / 8; ++j)
       *reinterpret_cast<__nv_bfloat162*>(o + 8 * j) = __floats2bfloat162_rn(d[4 * j + 2 * i] * mul, d[4 * j + 2 * i + 1] * mul);
   }
 }
 
+template <int D>
 __global__ void __launch_bounds__(FA_THREADS, 1)
     attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                        const __grid_constant__ CUtensorMap tmV, __nv_bfloat16* __restrict__ out,
                        float* __restrict__ lse, int B, int Nq, int Nk, int H, int kv_shift, float scale_log2) {
+  using G = Hd<D>;
+  constexpr int FA_QBYTES = G::QBYTES, FA_KBYTES = G::KBYTES;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + FA_QBYTES;
@@ -114,16 +146,17 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
   }
   const int wg = threadIdx.x >> 7, t4 = lane & 3;
   const bool signal = (threadIdx.x & 127) == 0;
-  const uint64_t dQ0 = make_smem_desc(smem_u32(sQ) + wg * 8192, 8192, 1024);
-  const uint64_t dK0 = make_smem_desc(smem_u32(sK), 8192, 1024), dV0 = make_smem_desc(smem_u32(sV), 8192, 1024);
-  float o[32], sv[32], m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, alpha[2];
+  const uint64_t dQ0 = make_smem_desc(smem_u32(sQ) + wg * G::WG, 8192, G::SBO, G::ROW);
+  const uint64_t dK0 = make_smem_desc(smem_u32(sK), 8192, G::SBO, G::ROW);
+  const uint64_t dV0 = make_smem_desc(smem_u32(sV), 8192, G::SBO, G::ROW);
+  float o[G::NACC], sv[32], m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, alpha[2];
   uint32_t pa[4][4];
 #pragma unroll
-  for (int e = 0; e < 32; ++e) o[e] = 0.f;
+  for (int e = 0; e < G::NACC; ++e) o[e] = 0.f;
   auto issue_s = [&](int s) {  // S = Q K^T of stage s into sv (the caller waits for the stage, fences and commits)
     const uint64_t so = (uint64_t)((s * FA_KBYTES) >> 4);
 #pragma unroll
-    for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(sv, dQ0 + kk * 2, dK0 + so + kk * 2, kk != 0);
+    for (int kk = 0; kk < D / 16; ++kk) wgmma_m64n64_ss<0, 0>(sv, dQ0 + kk * 2, dK0 + so + kk * 2, kk != 0);
   };
   // online softmax of S_j in place (sv becomes P_j); O is not touched: its rescale by alpha waits until the P V
   // product that is in flight meanwhile has retired
@@ -158,7 +191,7 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
   };
   auto rescale_pack = [&]() {  // O *= alpha, P_j -> bf16 A fragments
 #pragma unroll
-    for (int x = 0; x < 32; ++x) o[x] *= alpha[(x >> 1) & 1];
+    for (int x = 0; x < G::NACC; ++x) o[x] *= alpha[(x >> 1) & 1];
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) acc_to_afrag(sv, kk, pa[kk]);
   };
@@ -182,7 +215,7 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
     issue_s(s1);
     wgmma_commit();
 #pragma unroll
-    for (int kk = 0; kk < FA_BN / 16; ++kk) wgmma_m64n64_rs<1>(o, pa[kk], dV0 + so + kk * 128, 1);
+    for (int kk = 0; kk < FA_BN / 16; ++kk) wgmma_m64nD_rs<D, 1>(o, pa[kk], dV0 + so + kk * G::MN_KSTEP, 1);
     wgmma_commit();
     wgmma_wait<1>();
     wgmma_hold(sv);
@@ -197,7 +230,7 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < FA_BN / 16; ++kk)
-      wgmma_m64n64_rs<1>(o, pa[kk], dV0 + (uint64_t)((s * FA_KBYTES) >> 4) + kk * 128, 1);
+      wgmma_m64nD_rs<D, 1>(o, pa[kk], dV0 + (uint64_t)((s * FA_KBYTES) >> 4) + kk * G::MN_KSTEP, 1);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_hold(o);
@@ -208,35 +241,45 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
     l[i] = quad_sum(l[i]);
     const float inv = 1.f / l[i];
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
+    for (int jj = 0; jj < D / 8; ++jj) {
       o[4 * jj + 2 * i] *= inv;
       o[4 * jj + 2 * i + 1] *= inv;
     }
     const int row = rbase + 8 * i;
     if (t4 == 0 && row < Nq) lse[((int64_t)b * H + h) * Nq + row] = (m[i] + log2f(l[i])) * kLn2;
   }
-  store_acc_rows(o, out, b, Nq, H, h, q0 + wg * 64, 1.f);
+  store_acc_rows<D>(o, out, b, Nq, H, h, q0 + wg * 64, 1.f);
 }
 
+// 4-D tensor map over the token-major [B, N, H, D] layout: boxes of box_rows tokens of one head, swizzled by the row
+template <int D>
 static int make_qkv_tmap(CUtensorMap* tm, const void* base, int B, int N, int H, int box_rows) {
-  const uint64_t dims[4] = {64, (uint64_t)H, (uint64_t)N, (uint64_t)B};
-  const uint64_t str[3] = {64 * 2, (uint64_t)H * 64 * 2, (uint64_t)N * H * 64 * 2};
-  const uint32_t box[4] = {64, 1, (uint32_t)box_rows, 1};
-  return make_tmap_bf16(tm, base, 4, dims, str, box);
+  const uint64_t dims[4] = {D, (uint64_t)H, (uint64_t)N, (uint64_t)B};
+  const uint64_t str[3] = {D * 2, (uint64_t)H * D * 2, (uint64_t)N * H * D * 2};
+  const uint32_t box[4] = {D, 1, (uint32_t)box_rows, 1};
+  return make_tmap_bf16(tm, base, 4, dims, str, box, Hd<D>::ROW);
+}
+
+template <int D>
+static int attn_fwd_tc_hd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk,
+                          int H, int kv_shift, float scale, cudaStream_t stream) {
+  constexpr int FA_SMEM = Hd<D>::SMEM;
+  CUtensorMap tq, tk, tv;
+  int rc;
+  if ((rc = make_qkv_tmap<D>(&tq, q, B, Nq, H, FA_BM))) return rc;  // K/V boxes: FA_BN rows
+  if ((rc = make_qkv_tmap<D>(&tk, k, B, Nk, H, FA_BN))) return rc;
+  if ((rc = make_qkv_tmap<D>(&tv, v, B, Nk, H, FA_BN))) return rc;
+  if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_fwd_tc_kernel<D>), FA_SMEM))) return rc;
+  dim3 grid((Nq + FA_BM - 1) / FA_BM, H, B);
+  attn_fwd_tc_kernel<D><<<grid, FA_THREADS, FA_SMEM, stream>>>(tq, tk, tv, static_cast<__nv_bfloat16*>(out), lse, B, Nq,
+                                                               Nk, H, kv_shift, scale * kLog2e);
+  return check_launch("attn_fwd_tc");
 }
 
 int attn_fwd_tc(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk, int H,
-                int kv_shift, float scale, cudaStream_t stream) {
-  CUtensorMap tq, tk, tv;
-  int rc;
-  if ((rc = make_qkv_tmap(&tq, q, B, Nq, H, FA_BM))) return rc;  // K/V boxes: FA_BN rows
-  if ((rc = make_qkv_tmap(&tk, k, B, Nk, H, FA_BN))) return rc;
-  if ((rc = make_qkv_tmap(&tv, v, B, Nk, H, FA_BN))) return rc;
-  if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_fwd_tc_kernel), FA_SMEM))) return rc;
-  dim3 grid((Nq + FA_BM - 1) / FA_BM, H, B);
-  attn_fwd_tc_kernel<<<grid, FA_THREADS, FA_SMEM, stream>>>(tq, tk, tv, static_cast<__nv_bfloat16*>(out), lse, B, Nq, Nk,
-                                                            H, kv_shift, scale * kLog2e);
-  return check_launch("attn_fwd_tc");
+                int kv_shift, float scale, int head_dim, cudaStream_t stream) {
+  return head_dim == 32 ? attn_fwd_tc_hd<32>(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream)
+                        : attn_fwd_tc_hd<64>(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -253,13 +296,17 @@ int attn_fwd_tc(const void* q, const void* k, const void* v, void* out, float* l
 // ---------------------------------------------------------------------------------------------
 constexpr int FB_R = 128;            // rows owned by the CTA
 constexpr int FB_C = 64;             // inner tile
-constexpr int FB_CBYTES = FB_C * FA_D * 2;  // 8 KiB
 constexpr int FF_STAGES = 3;
-constexpr int FF_STAGE_BYTES = 17 * 1024;                 // Q 8 KiB | dO 8 KiB | lse2 256 B | delta 256 B (| pad)
-constexpr int FF_OFF_STAGE = 2 * FB_R * FA_D * 2;         // after the resident K and V tiles (16 KiB each)
-constexpr int FF_SMEM = FF_OFF_STAGE + FF_STAGES * FF_STAGE_BYTES + 256;
 constexpr int FQ_STAGES = 4;
-constexpr int FQ_SMEM = 2 * FB_R * FA_D * 2 + FQ_STAGES * 2 * FB_CBYTES + 256;
+template <int D>
+struct HdB {
+  static constexpr int RBYTES = FB_R * Hd<D>::ROW;        // a resident tile (16 KiB at D = 64)
+  static constexpr int CBYTES = FB_C * Hd<D>::ROW;        // a streamed tile (8 KiB at D = 64)
+  static constexpr int FF_STAGE_BYTES = 2 * CBYTES + 1024;  // Q | dO | lse2 256 B | delta 256 B (| pad to 1 KiB)
+  static constexpr int FF_OFF_STAGE = 2 * RBYTES;         // after the resident K and V tiles
+  static constexpr int FF_SMEM = FF_OFF_STAGE + FF_STAGES * FF_STAGE_BYTES + 256;
+  static constexpr int FQ_SMEM = 2 * RBYTES + FQ_STAGES * 2 * CBYTES + 256;
+};
 
 __device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
@@ -268,10 +315,13 @@ __device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_
                : "memory");
 }
 // delta = rowsum(dout * out) * scale; lse2 = lse * log2(e); both written token-tile padded: [B*H][nq_pad] with +inf / 0 in the pad
+// (8 lanes per row, D / 8 channels each)
+template <int D>
 __global__ void __launch_bounds__(256)
     attn_bwd_prep_fused_kernel(const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __restrict__ dout,
                                const float* __restrict__ lse, float* __restrict__ lse2p, float* __restrict__ deltap,
                                int64_t nrows_pad /* B * nq_pad * H */, int N, int nq_pad, int H, float scale) {
+  using Vec = std::conditional_t<D == 64, uint4, uint2>;  // D / 8 bf16
   const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t r = gid >> 3;  // (b, n_pad, h)
   const int sub = (int)(gid & 7);
@@ -283,13 +333,13 @@ __global__ void __launch_bounds__(256)
   const int64_t b = bn / nq_pad;
   float acc = 0.f;
   if (live && n < N) {
-    const int64_t src = ((b * N + n) * H + h) * FA_D + sub * 8;
-    const uint4 a = *reinterpret_cast<const uint4*>(out + src);
-    const uint4 g = *reinterpret_cast<const uint4*>(dout + src);
+    const int64_t src = ((b * N + n) * H + h) * D + sub * (D / 8);
+    const Vec a = *reinterpret_cast<const Vec*>(out + src);
+    const Vec g = *reinterpret_cast<const Vec*>(dout + src);
     const __nv_bfloat162* pa = reinterpret_cast<const __nv_bfloat162*>(&a);
     const __nv_bfloat162* pg = reinterpret_cast<const __nv_bfloat162*>(&g);
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
+    for (int e = 0; e < D / 16; ++e) {
       const float2 fa = __bfloat1622float2(pa[e]), fg = __bfloat1622float2(pg[e]);
       acc = fmaf(fa.x, fg.x, acc);
       acc = fmaf(fa.y, fg.y, acc);
@@ -305,16 +355,19 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+template <int D>
 __global__ void __launch_bounds__(FA_THREADS, 1)
     attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
                         const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                         const float* __restrict__ lse2p, const float* __restrict__ deltap,
                         __nv_bfloat16* __restrict__ dk, __nv_bfloat16* __restrict__ dv, int B, int Nq, int nq_pad,
                         int Nk, int H, int kv_shift, float scale, float scale_log2) {
+  using G = Hd<D>;
+  constexpr int FB_CBYTES = HdB<D>::CBYTES, FF_STAGE_BYTES = HdB<D>::FF_STAGE_BYTES, FF_SMEM = HdB<D>::FF_SMEM;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sK = smem;
-  uint8_t* sV = smem + FB_R * FA_D * 2;
-  uint8_t* sStage = smem + FF_OFF_STAGE;
+  uint8_t* sV = smem + HdB<D>::RBYTES;
+  uint8_t* sStage = smem + HdB<D>::FF_OFF_STAGE;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + FF_SMEM - 256);
   uint64_t* kv_full = bars;
   uint64_t* in_full = bars + 1;               // [FF_STAGES]
@@ -344,7 +397,7 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
 
   if (warp == FA_PRODUCER) {
     if (lane == 0) {
-      mbar_expect_tx(kv_full, 2 * FB_R * FA_D * 2);
+      mbar_expect_tx(kv_full, 2 * HdB<D>::RBYTES);
       tma_load_4d(sK, &tmK, kv_full, 0, h, k0, kb);
       tma_load_4d(sV, &tmV, kv_full, 0, h, k0, kb);
       const float* l2 = lse2p + ((int64_t)qb * H + h) * nq_pad;
@@ -364,12 +417,12 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
   }
   const int wg = threadIdx.x >> 7, t4 = lane & 3;
   const bool signal = (threadIdx.x & 127) == 0;
-  const uint64_t dK0 = make_smem_desc(smem_u32(sK) + wg * 8192, 8192, 1024);
-  const uint64_t dV0 = make_smem_desc(smem_u32(sV) + wg * 8192, 8192, 1024);
-  const uint64_t dSt0 = make_smem_desc(smem_u32(sStage), 8192, 1024);
-  float acc_v[32], acc_k[32];
+  const uint64_t dK0 = make_smem_desc(smem_u32(sK) + wg * G::WG, 8192, G::SBO, G::ROW);
+  const uint64_t dV0 = make_smem_desc(smem_u32(sV) + wg * G::WG, 8192, G::SBO, G::ROW);
+  const uint64_t dSt0 = make_smem_desc(smem_u32(sStage), 8192, G::SBO, G::ROW);
+  float acc_v[G::NACC], acc_k[G::NACC];
 #pragma unroll
-  for (int e = 0; e < 32; ++e) acc_v[e] = acc_k[e] = 0.f;
+  for (int e = 0; e < G::NACC; ++e) acc_v[e] = acc_k[e] = 0.f;
   mbar_wait(kv_full, 0);
   for (int i = 0; i < ntiles; ++i) {
     const int s = i % FF_STAGES;
@@ -379,9 +432,9 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
     float st[32], dp[32];
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(st, dK0 + kk * 2, dSt0 + so + kk * 2, kk != 0);
+    for (int kk = 0; kk < D / 16; ++kk) wgmma_m64n64_ss<0, 0>(st, dK0 + kk * 2, dSt0 + so + kk * 2, kk != 0);
 #pragma unroll
-    for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(dp, dV0 + kk * 2, dSt0 + so_do + kk * 2, kk != 0);
+    for (int kk = 0; kk < D / 16; ++kk) wgmma_m64n64_ss<0, 0>(dp, dV0 + kk * 2, dSt0 + so_do + kk * 2, kk != 0);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_hold(st);
@@ -407,28 +460,31 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
     }
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < FB_C / 16; ++kk) wgmma_m64n64_rs<1>(acc_v, pa[kk], dSt0 + so_do + kk * 128, 1);
+    for (int kk = 0; kk < FB_C / 16; ++kk) wgmma_m64nD_rs<D, 1>(acc_v, pa[kk], dSt0 + so_do + kk * G::MN_KSTEP, 1);
 #pragma unroll
-    for (int kk = 0; kk < FB_C / 16; ++kk) wgmma_m64n64_rs<1>(acc_k, da[kk], dSt0 + so + kk * 128, 1);
+    for (int kk = 0; kk < FB_C / 16; ++kk) wgmma_m64nD_rs<D, 1>(acc_k, da[kk], dSt0 + so + kk * G::MN_KSTEP, 1);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_hold(acc_v);
     wgmma_hold(acc_k);
     if (signal) mbar_arrive(&in_empty[s]);
   }
-  store_acc_rows(acc_v, dv, kb, Nk, H, h, k0 + wg * 64, 1.f);
-  store_acc_rows(acc_k, dk, kb, Nk, H, h, k0 + wg * 64, 1.f);
+  store_acc_rows<D>(acc_v, dv, kb, Nk, H, h, k0 + wg * 64, 1.f);
+  store_acc_rows<D>(acc_k, dk, kb, Nk, H, h, k0 + wg * 64, 1.f);
 }
 
+template <int D>
 __global__ void __launch_bounds__(FA_THREADS, 1)
     attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
                        const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                        const float* __restrict__ lse2p, const float* __restrict__ deltap, __nv_bfloat16* __restrict__ dq,
                        int B, int Nq, int nq_pad, int Nk, int H, int kv_shift, float scale, float scale_log2) {
+  using G = Hd<D>;
+  constexpr int FB_CBYTES = HdB<D>::CBYTES;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
-  uint8_t* sDO = smem + FB_R * FA_D * 2;
-  uint8_t* sK = smem + 2 * FB_R * FA_D * 2;       // [FQ_STAGES]
+  uint8_t* sDO = smem + HdB<D>::RBYTES;
+  uint8_t* sK = smem + 2 * HdB<D>::RBYTES;       // [FQ_STAGES]
   uint8_t* sV = sK + FQ_STAGES * FB_CBYTES;       // [FQ_STAGES]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sV + FQ_STAGES * FB_CBYTES);
   uint64_t* qd_full = bars;
@@ -459,7 +515,7 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
 
   if (warp == FA_PRODUCER) {
     if (lane == 0) {
-      mbar_expect_tx(qd_full, 2 * FB_R * FA_D * 2);
+      mbar_expect_tx(qd_full, 2 * HdB<D>::RBYTES);
       tma_load_4d(sQ, &tmQ, qd_full, 0, h, q0, b);
       tma_load_4d(sDO, &tmDO, qd_full, 0, h, q0, b);
       for (int j = 0; j < ntiles; ++j) {
@@ -474,9 +530,10 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
   }
   const int wg = threadIdx.x >> 7;
   const bool signal = (threadIdx.x & 127) == 0;
-  const uint64_t dQ0 = make_smem_desc(smem_u32(sQ) + wg * 8192, 8192, 1024);
-  const uint64_t dDO0 = make_smem_desc(smem_u32(sDO) + wg * 8192, 8192, 1024);
-  const uint64_t dK0 = make_smem_desc(smem_u32(sK), 8192, 1024), dV0 = make_smem_desc(smem_u32(sV), 8192, 1024);
+  const uint64_t dQ0 = make_smem_desc(smem_u32(sQ) + wg * G::WG, 8192, G::SBO, G::ROW);
+  const uint64_t dDO0 = make_smem_desc(smem_u32(sDO) + wg * G::WG, 8192, G::SBO, G::ROW);
+  const uint64_t dK0 = make_smem_desc(smem_u32(sK), 8192, G::SBO, G::ROW);
+  const uint64_t dV0 = make_smem_desc(smem_u32(sV), 8192, G::SBO, G::ROW);
   float l2[2], dl[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
@@ -485,9 +542,9 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
     l2[r] = row < Nq ? lse2p[o] : INFINITY;
     dl[r] = row < Nq ? deltap[o] : 0.f;
   }
-  float acc[32];
+  float acc[G::NACC];
 #pragma unroll
-  for (int e = 0; e < 32; ++e) acc[e] = 0.f;
+  for (int e = 0; e < G::NACC; ++e) acc[e] = 0.f;
   mbar_wait(qd_full, 0);
   for (int j = 0; j < ntiles; ++j) {
     const int s = j % FQ_STAGES;
@@ -496,9 +553,9 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
     float sv[32], dp[32];
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(sv, dQ0 + kk * 2, dK0 + so + kk * 2, kk != 0);
+    for (int kk = 0; kk < D / 16; ++kk) wgmma_m64n64_ss<0, 0>(sv, dQ0 + kk * 2, dK0 + so + kk * 2, kk != 0);
 #pragma unroll
-    for (int kk = 0; kk < FA_D / 16; ++kk) wgmma_m64n64_ss<0, 0>(dp, dDO0 + kk * 2, dV0 + so + kk * 2, kk != 0);
+    for (int kk = 0; kk < D / 16; ++kk) wgmma_m64n64_ss<0, 0>(dp, dDO0 + kk * 2, dV0 + so + kk * 2, kk != 0);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_hold(sv);
@@ -513,13 +570,13 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
     for (int kk = 0; kk < 4; ++kk) acc_to_afrag(dp, kk, da[kk]);
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < FB_C / 16; ++kk) wgmma_m64n64_rs<1>(acc, da[kk], dK0 + so + kk * 128, 1);
+    for (int kk = 0; kk < FB_C / 16; ++kk) wgmma_m64nD_rs<D, 1>(acc, da[kk], dK0 + so + kk * G::MN_KSTEP, 1);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_hold(acc);
     if (signal) mbar_arrive(&in_empty[s]);
   }
-  store_acc_rows(acc, dq, b, Nq, H, h, q0 + wg * 64, 1.f);
+  store_acc_rows<D>(acc, dq, b, Nq, H, h, q0 + wg * 64, 1.f);
 }
 
 // Shared-qk cross-attention (reference: lightglue.py:207-216): sequence b attends to its partner p = (b + B/2) mod B
@@ -535,8 +592,10 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
 // dK / dV kernel per direction.  The summation order is fixed (no atomics).  Padding follows the generic kernels: rows
 // of p past N load as zeros with lse2 = +inf, so they meet a zero qk_p / dO_p row and P' = 0; rows of b past N are not
 // stored.
+constexpr int FA_D = 64;                                  // the shared-qk kernel's head dim
+constexpr int FB_CBYTES = HdB<FA_D>::CBYTES;              // 8 KiB
 constexpr int FX_STAGES = 4;
-constexpr int FX_STAGE_BYTES = 25 * 1024;                 // qk_p 8 KiB | v_p 8 KiB | dO_p 8 KiB | lse2 256 B | delta 256 B
+constexpr int FX_STAGE_BYTES = 25 * 1024;                // qk_p 8 KiB | v_p 8 KiB | dO_p 8 KiB | lse2 256 B | delta 256 B
 constexpr int FX_OFF_STAGE = 3 * FB_R * FA_D * 2;         // after the resident qk_b, v_b, dO_b tiles (16 KiB each)
 constexpr int FX_SMEM = FX_OFF_STAGE + FX_STAGES * FX_STAGE_BYTES + 256;
 // a whole producer warpgroup, so that setmaxnreg can move registers from it to the two consumer warpgroups: S, dP,
@@ -679,8 +738,8 @@ __global__ void __launch_bounds__(FX_THREADS, 1)
     wgmma_hold(acc_q);
     if (signal) mbar_arrive(&in_empty[s]);
   }
-  store_acc_rows(acc_v, dv, b, N, H, h, r0 + wg * 64, 1.f);
-  store_acc_rows(acc_q, dqk, b, N, H, h, r0 + wg * 64, 1.f);
+  store_acc_rows<FA_D>(acc_v, dv, b, N, H, h, r0 + wg * 64, 1.f);
+  store_acc_rows<FA_D>(acc_q, dqk, b, N, H, h, r0 + wg * 64, 1.f);
 }
 
 int64_t attn_bwd_ws_floats(int B, int Nq, int Nk, int H) {
@@ -689,29 +748,31 @@ int64_t attn_bwd_ws_floats(int B, int Nq, int Nk, int H) {
   return 2 * (int64_t)B * H * nq_pad;
 }
 
-int attn_bwd_tc(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
-                void* dq, void* dk, void* dv, float* ws, int B, int Nq, int Nk, int H, int kv_shift, float scale,
-                cudaStream_t stream) {
+template <int D>
+static int attn_bwd_tc_hd(const void* q, const void* k, const void* v, const void* out, const float* lse,
+                          const void* dout, void* dq, void* dk, void* dv, float* ws, int B, int Nq, int Nk, int H,
+                          int kv_shift, float scale, cudaStream_t stream) {
+  constexpr int FQ_SMEM = HdB<D>::FQ_SMEM, FF_SMEM = HdB<D>::FF_SMEM;
   const int nq_pad = (Nq + FB_C - 1) / FB_C * FB_C;
   float* lse2p = ws;
   float* deltap = lse2p + (int64_t)B * H * nq_pad;
   int rc;
   {
     const int64_t nrows = (int64_t)B * nq_pad * H;
-    attn_bwd_prep_fused_kernel<<<(unsigned)((nrows * 8 + 255) / 256), 256, 0, stream>>>(
+    attn_bwd_prep_fused_kernel<D><<<(unsigned)((nrows * 8 + 255) / 256), 256, 0, stream>>>(
         static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), lse, lse2p, deltap, nrows, Nq,
         nq_pad, H, scale);
   }
   const float sl2 = scale * kLog2e;
-  if (attn_bwd_is_shared_qk(q, k, dq, dk, B, Nq, Nk, kv_shift)) {  // dq (= dk) receives dq + dk
+  if (D == FA_D && attn_bwd_is_shared_qk(q, k, dq, dk, B, Nq, Nk, kv_shift)) {  // dq (= dk) receives dq + dk
     CUtensorMap tqr, tvr, tdor, tqs, tvs, tdos;
     if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_shared_qk_kernel), FX_SMEM))) return rc;
-    if ((rc = make_qkv_tmap(&tqr, q, B, Nq, H, FB_R))) return rc;
-    if ((rc = make_qkv_tmap(&tvr, v, B, Nq, H, FB_R))) return rc;
-    if ((rc = make_qkv_tmap(&tdor, dout, B, Nq, H, FB_R))) return rc;
-    if ((rc = make_qkv_tmap(&tqs, q, B, Nq, H, FB_C))) return rc;
-    if ((rc = make_qkv_tmap(&tvs, v, B, Nq, H, FB_C))) return rc;
-    if ((rc = make_qkv_tmap(&tdos, dout, B, Nq, H, FB_C))) return rc;
+    if ((rc = make_qkv_tmap<FA_D>(&tqr, q, B, Nq, H, FB_R))) return rc;
+    if ((rc = make_qkv_tmap<FA_D>(&tvr, v, B, Nq, H, FB_R))) return rc;
+    if ((rc = make_qkv_tmap<FA_D>(&tdor, dout, B, Nq, H, FB_R))) return rc;
+    if ((rc = make_qkv_tmap<FA_D>(&tqs, q, B, Nq, H, FB_C))) return rc;
+    if ((rc = make_qkv_tmap<FA_D>(&tvs, v, B, Nq, H, FB_C))) return rc;
+    if ((rc = make_qkv_tmap<FA_D>(&tdos, dout, B, Nq, H, FB_C))) return rc;
     attn_bwd_shared_qk_kernel<<<dim3((Nq + FB_R - 1) / FB_R, H, B), FX_THREADS, FX_SMEM, stream>>>(
         tqr, tvr, tdor, tqs, tvs, tdos, lse2p, deltap, static_cast<__nv_bfloat16*>(dq), static_cast<__nv_bfloat16*>(dv),
         B, Nq, nq_pad, H, kv_shift, scale, sl2);
@@ -719,24 +780,32 @@ int attn_bwd_tc(const void* q, const void* k, const void* v, const void* out, co
   }
   CUtensorMap tq, tdo, tk, tv;
   // dQ kernel: 128-query resident tiles, 64-key streamed tiles
-  if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_dq_kernel), FQ_SMEM))) return rc;
-  if ((rc = make_qkv_tmap(&tq, q, B, Nq, H, FB_R))) return rc;
-  if ((rc = make_qkv_tmap(&tdo, dout, B, Nq, H, FB_R))) return rc;
-  if ((rc = make_qkv_tmap(&tk, k, B, Nk, H, FB_C))) return rc;
-  if ((rc = make_qkv_tmap(&tv, v, B, Nk, H, FB_C))) return rc;
-  attn_bwd_dq_kernel<<<dim3((Nq + FB_R - 1) / FB_R, H, B), FA_THREADS, FQ_SMEM, stream>>>(
+  if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_dq_kernel<D>), FQ_SMEM))) return rc;
+  if ((rc = make_qkv_tmap<D>(&tq, q, B, Nq, H, FB_R))) return rc;
+  if ((rc = make_qkv_tmap<D>(&tdo, dout, B, Nq, H, FB_R))) return rc;
+  if ((rc = make_qkv_tmap<D>(&tk, k, B, Nk, H, FB_C))) return rc;
+  if ((rc = make_qkv_tmap<D>(&tv, v, B, Nk, H, FB_C))) return rc;
+  attn_bwd_dq_kernel<D><<<dim3((Nq + FB_R - 1) / FB_R, H, B), FA_THREADS, FQ_SMEM, stream>>>(
       tq, tdo, tk, tv, lse2p, deltap, static_cast<__nv_bfloat16*>(dq), B, Nq, nq_pad, Nk, H, kv_shift, scale, sl2);
   if ((rc = check_launch("attn_bwd_dq"))) return rc;
   // dK / dV kernel: 128-key resident tiles, 64-query streamed tiles
-  if ((rc = make_qkv_tmap(&tq, q, B, Nq, H, FB_C))) return rc;
-  if ((rc = make_qkv_tmap(&tdo, dout, B, Nq, H, FB_C))) return rc;
-  if ((rc = make_qkv_tmap(&tk, k, B, Nk, H, FB_R))) return rc;
-  if ((rc = make_qkv_tmap(&tv, v, B, Nk, H, FB_R))) return rc;
-  if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_dkv_kernel), FF_SMEM))) return rc;
-  attn_bwd_dkv_kernel<<<dim3((Nk + FB_R - 1) / FB_R, H, B), FA_THREADS, FF_SMEM, stream>>>(
+  if ((rc = make_qkv_tmap<D>(&tq, q, B, Nq, H, FB_C))) return rc;
+  if ((rc = make_qkv_tmap<D>(&tdo, dout, B, Nq, H, FB_C))) return rc;
+  if ((rc = make_qkv_tmap<D>(&tk, k, B, Nk, H, FB_R))) return rc;
+  if ((rc = make_qkv_tmap<D>(&tv, v, B, Nk, H, FB_R))) return rc;
+  if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_dkv_kernel<D>), FF_SMEM))) return rc;
+  attn_bwd_dkv_kernel<D><<<dim3((Nk + FB_R - 1) / FB_R, H, B), FA_THREADS, FF_SMEM, stream>>>(
       tq, tdo, tk, tv, lse2p, deltap, static_cast<__nv_bfloat16*>(dk), static_cast<__nv_bfloat16*>(dv), B, Nq, nq_pad,
       Nk, H, kv_shift, scale, sl2);
   return check_launch("attn_bwd_dkv");
+}
+
+int attn_bwd_tc(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
+                void* dq, void* dk, void* dv, float* ws, int B, int Nq, int Nk, int H, int kv_shift, float scale,
+                int head_dim, cudaStream_t stream) {
+  return head_dim == 32
+             ? attn_bwd_tc_hd<32>(q, k, v, out, lse, dout, dq, dk, dv, ws, B, Nq, Nk, H, kv_shift, scale, stream)
+             : attn_bwd_tc_hd<64>(q, k, v, out, lse, dout, dq, dk, dv, ws, B, Nq, Nk, H, kv_shift, scale, stream);
 }
 
 }  // namespace lgb

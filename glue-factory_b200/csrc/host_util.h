@@ -17,20 +17,21 @@ int ensure_dyn_smem(const void* func, int bytes);
 // SM count of the CURRENT device (cached per device ordinal)
 int device_sm_count();
 
-// fp32 CUDA-core attention (attn_simt.cu)
+// fp32 CUDA-core attention (attn_simt.cu); head_dim 32 or 64, checked by the api.cu entry points
 int attn_fwd_simt(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk, int H,
-                  int kv_shift, float scale, cudaStream_t stream);
+                  int kv_shift, float scale, int head_dim, cudaStream_t stream);
 int attn_bwd_simt(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
                   void* dq, void* dk, void* dv, float* delta, int B, int Nq, int Nk, int H, int kv_shift, float scale,
-                  cudaStream_t stream);
-int attn_delta(const void* out, const void* dout, float* delta, int B, int N, int H, cudaStream_t stream);
+                  int head_dim, cudaStream_t stream);
+int attn_delta(const void* out, const void* dout, float* delta, int B, int N, int H, int head_dim,
+               cudaStream_t stream);
 
-// wgmma attention (attn_tc.cu)
+// wgmma attention (attn_tc.cu); head_dim as above, the shared-qk backward at 64 only
 int attn_fwd_tc(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk, int H,
-                int kv_shift, float scale, cudaStream_t stream);
+                int kv_shift, float scale, int head_dim, cudaStream_t stream);
 int attn_bwd_tc(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
                 void* dq, void* dk, void* dv, float* delta, int B, int Nq, int Nk, int H, int kv_shift, float scale,
-                cudaStream_t stream);
+                int head_dim, cudaStream_t stream);
 
 // lgb200_attn_bwd's shared-qk cross-attention case (q == k, dq == dk, both directions in one batch)
 inline bool attn_bwd_is_shared_qk(const void* q, const void* k, const void* dq, const void* dk, int B, int Nq, int Nk,

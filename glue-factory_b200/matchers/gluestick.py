@@ -10,9 +10,10 @@ Layout and kernels.  The reference keeps channels first ([B, D, N], Conv1d with 
 node features are token-major [B*N, D] like in the LightGlue plugin, so
   * every Conv1d(k=1) with a tensor-core-sized input is the library's wgmma GEMM (`ops.LinearFn`: bias in the
     epilogue, split-K weight gradient); the tiny encoder layers (3 / 5 / 32 input channels) are plain fp32 linears;
-  * the attention core (gluestick.py:524-529) is the same wgmma flash-attention pair as LightGlue's.  GlueStick splits
-    heads as channel = d * H + h; instead of permuting activations, the rows of the q / k / v projection weights and the
-    columns of the merge weight are permuted once per call so the projections emit head-major [B, N, H, 64] directly;
+  * the attention core (gluestick.py:524-529) is the same wgmma flash-attention pair as LightGlue's, at head dim 64
+    (descriptor_dim 256) or 32 (descriptor_dim 128, the configs' DISK variant).  GlueStick splits heads as
+    channel = d * H + h; instead of permuting activations, the rows of the q / k / v projection weights and the
+    columns of the merge weight are permuted once per call so the projections emit head-major [B, N, H, D / 4] directly;
   * the assignment is `log_double_softmax` with a learnt bin (gluestick.py:772-783) on the similarity produced by the
     batched wgmma GEMM: forward kernels + closed-form backward (`ops.log_double_softmax`, heads_grad.py);
   * match filtering (`_get_matches`, gluestick.py:318-331) is `filter_matches_kernel`;
@@ -129,7 +130,8 @@ class GlueStick(PointGNN):
         if conf.line_attention or conf.inter_supervision or conf.skip_init:
             raise NotImplementedError("gluefactory_b200 gluestick: line_attention / inter_supervision / skip_init are not built")
         D = conf.descriptor_dim
-        assert D == 256, "the lgb200 attention kernels are built for 4 heads of 64 channels"
+        if D not in (128, 256):  # 4 heads of 32 or 64 channels: the head dims the attention kernels are built for
+            raise NotImplementedError(f"gluefactory_b200 gluestick: descriptor_dim {D} is not supported (128 or 256)")
         if conf.input_dim != D:
             self.input_proj = nn.Conv1d(conf.input_dim, D, kernel_size=1)
             nn.init.constant_(self.input_proj.bias, 0.0)

@@ -60,26 +60,40 @@ def rope_bwd(dq, dk, dv, q, k, theta, H, dtheta=None):
 # ------------------------------------------------------------------------------------------------
 # attention (lightglue.py:118-121, 207-216)
 # ------------------------------------------------------------------------------------------------
+def _head_dim(q):
+    D = q.shape[3]
+    assert D in (32, 64), "head_dim must be 32 or 64"
+    return D
+
+
 def attn_fwd(q, k, v, kv_shift, scale):
     _chk(q), _chk(k), _chk(v)
-    B, Nq, H, D = q.shape
+    B, Nq, H, _ = q.shape
+    D = _head_dim(q)
     Nk = k.shape[1]
-    assert D == 64, "head_dim must be 64"
     out = torch.empty_like(q)
     lse = torch.empty(B, H, Nq, device=q.device, dtype=torch.float32)
-    call("lgb200_attn_fwd", ptr(q), ptr(k), ptr(v), ptr(out), ptr(lse), B, Nq, Nk, H, kv_shift, float(scale),
-         _code(q.dtype), stream_ptr())
+    args = (ptr(q), ptr(k), ptr(v), ptr(out), ptr(lse), B, Nq, Nk, H, kv_shift, float(scale), _code(q.dtype))
+    if D == 64:
+        call("lgb200_attn_fwd", *args, stream_ptr())
+    else:
+        call("lgb200_attn_fwd_hd", *args, D, stream_ptr())
     return out, lse
 
 
 def attn_bwd(q, k, v, out, lse, dout, kv_shift, scale):
     B, Nq, H, _ = q.shape
+    D = _head_dim(q)
     Nk = k.shape[1]
     dout = dout.contiguous()
     dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
     delta = torch.empty(_lib.load().lgb200_attn_bwd_ws_floats(B, Nq, Nk, H), device=q.device, dtype=torch.float32)
-    call("lgb200_attn_bwd", ptr(q), ptr(k), ptr(v), ptr(out), ptr(lse), ptr(dout), ptr(dq), ptr(dk), ptr(dv),
-         ptr(delta), B, Nq, Nk, H, kv_shift, float(scale), _code(q.dtype), stream_ptr())
+    args = (ptr(q), ptr(k), ptr(v), ptr(out), ptr(lse), ptr(dout), ptr(dq), ptr(dk), ptr(dv), ptr(delta), B, Nq, Nk,
+            H, kv_shift, float(scale), _code(q.dtype))
+    if D == 64:
+        call("lgb200_attn_bwd", *args, stream_ptr())
+    else:
+        call("lgb200_attn_bwd_hd", *args, D, stream_ptr())
     return dq, dk, dv
 
 
@@ -101,8 +115,8 @@ def attn_bwd_shared_qk(qk, v, out, lse, dout, scale):
 
 
 class Attention(torch.autograd.Function):
-    """q [B,Nq,H,64], k,v [B,Nk,H,64] -> softmax(q k^T / 8) v, keys of batch b taken from batch
-    (b + kv_shift) % B."""
+    """q [B,Nq,H,D], k,v [B,Nk,H,D] -> softmax(scale q k^T) v, keys of batch b taken from batch
+    (b + kv_shift) % B.  Head dim D = 64 or 32, read from the shape."""
 
     @staticmethod
     def forward(ctx, q, k, v, kv_shift, scale):
@@ -372,12 +386,14 @@ def add_f32_cast_(x, y, cdt):
 
 
 def gluestick_attention(query, key, value):
-    """GlueStick's attention core (models/matchers/gluestick.py:524-529) on the same kernels: query [B, 64, H, N],
-    key/value [B, 64, H, M] (channels first, channel = d * H + h) -> [B, 64, H, N].  The reference forces fp32 here
-    (AMP_CUSTOM_FWD_F32): fp32 inputs run the full-precision kernels, bf16 inputs the wgmma ones."""
-    assert query.shape[1] == 64, "head dimension 64 only"
-    tm = lambda t: t.permute(0, 3, 2, 1).contiguous()  # noqa: E731  -> token-major [B, N, H, 64]
-    out = Attention.apply(tm(query), tm(key), tm(value), 0, 0.125)
+    """GlueStick's attention core (models/matchers/gluestick.py:524-529) on the same kernels: query [B, dh, H, N],
+    key/value [B, dh, H, M] (channels first, channel = d * H + h) -> [B, dh, H, N], head dim dh = 64 or 32.  The
+    reference forces fp32 here (AMP_CUSTOM_FWD_F32): fp32 inputs run the full-precision kernels, bf16 inputs the
+    wgmma ones."""
+    dh = query.shape[1]
+    assert dh in (32, 64), "head dimension 32 or 64 only"
+    tm = lambda t: t.permute(0, 3, 2, 1).contiguous()  # noqa: E731  -> token-major [B, N, H, dh]
+    out = Attention.apply(tm(query), tm(key), tm(value), 0, dh ** -0.5)
     return out.permute(0, 3, 2, 1)
 
 

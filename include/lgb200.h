@@ -17,8 +17,9 @@
  *    [batch, rows, cols] row-major for similarity/score matrices.
  *  - `dtype` is LGB200_F32 (full-precision parity path, CUDA cores) or
  *    LGB200_BF16 (bf16 operands, fp32 accumulation, Hopper tensor cores).
- *  - head dimension is fixed to 64 (descriptor_dim / num_heads in every
- *    LightGlue configuration, lightglue.py:349).
+ *  - head dimension is 64 (descriptor_dim / num_heads in every
+ *    LightGlue configuration, lightglue.py:349); the attention entry points
+ *    with an `_hd` suffix also take 32.
  */
 #ifndef LGB200_H_
 #define LGB200_H_
@@ -80,6 +81,15 @@ int64_t lgb200_attn_bwd_ws_floats(int B, int Nq, int Nk, int H);
 int lgb200_attn_bwd(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
                     void* dq, void* dk, void* dv, float* delta_ws, int B, int Nq, int Nk, int H, int kv_shift,
                     float scale, int dtype, cudaStream_t stream);
+/* The same two at head dimension head_dim = 32 or 64 (every tensor above [.., H, head_dim]); any other value returns
+ * LGB200_ERR_UNSUPPORTED.  lgb200_attn_fwd / lgb200_attn_bwd are these with head_dim = 64.  Head dimension 32 is
+ * GlueStick with 128-channel descriptors and 4 heads (gluestick.py:524-551).  The workspace does not depend on
+ * head_dim; the shared-qk backward is built for head_dim 64 only.                                              */
+int lgb200_attn_fwd_hd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk,
+                       int H, int kv_shift, float scale, int dtype, int head_dim, cudaStream_t stream);
+int lgb200_attn_bwd_hd(const void* q, const void* k, const void* v, const void* out, const float* lse,
+                       const void* dout, void* dq, void* dk, void* dv, float* delta_ws, int B, int Nq, int Nk, int H,
+                       int kv_shift, float scale, int dtype, int head_dim, cudaStream_t stream);
 
 /* ---- FFN LayerNorm + GELU -------------------------------------------------------------------------
  * replaces nn.LayerNorm(2D) + nn.GELU() of the ffn Sequential (lightglue.py:143-148, 178-183).
