@@ -27,7 +27,11 @@ node features are token-major [B*N, D] like in the LightGlue plugin, so
 gluestick.py:17-22; the fp32 mode reproduces that); `precision: "fp32"` is the parity path (fp32 cuBLAS linears,
 CUDA-core attention).  No CPU fallback.
 
-Not built (raise NotImplementedError): `line_attention`, `inter_supervision`, inputs without lines.
+Intermediate line supervision (`inter_supervision`, gluestick.py:96-107, 272-292, 378-460): for each listed GNN block
+the node features after its cross layer go through the same line head as the final ones (`_line_head`) with that
+block's `inter_line_proj`, and their NLL is added to the total with the block's `loss.inter_supervision` weight.
+
+Not built (raise NotImplementedError): `line_attention`, `skip_init`, inputs without lines.
 """
 import torch
 from torch import nn
@@ -127,8 +131,10 @@ class GlueStick(PointGNN):
         super().__init__()
         self.conf = conf = _Conf(_merge(self.default_conf, _to_plain(conf)))
         assert conf.precision in ("bf16", "fp32"), conf.precision
-        if conf.line_attention or conf.inter_supervision or conf.skip_init:
-            raise NotImplementedError("gluefactory_b200 gluestick: line_attention / inter_supervision / skip_init are not built")
+        if conf.line_attention or conf.skip_init:
+            raise NotImplementedError("gluefactory_b200 gluestick: line_attention / skip_init are not built")
+        if conf.inter_supervision is not None:
+            self._check_inter_supervision(conf)
         D = conf.descriptor_dim
         if D not in (128, 256):  # 4 heads of 32 or 64 channels: the head dims the attention kernels are built for
             raise NotImplementedError(f"gluefactory_b200 gluestick: descriptor_dim {D} is not supported (128 or 256)")
@@ -147,6 +153,13 @@ class GlueStick(PointGNN):
         self.final_line_proj = nn.Conv1d(D, D, kernel_size=1)
         nn.init.constant_(self.final_line_proj.bias, 0.0)
         nn.init.orthogonal_(self.final_line_proj.weight, gain=1)
+        if conf.inter_supervision is not None:
+            self.inter_line_proj = nn.ModuleList([nn.Conv1d(D, D, kernel_size=1) for _ in conf.inter_supervision])
+            self.layer2idx = {}
+            for i, block in enumerate(conf.inter_supervision):
+                nn.init.constant_(self.inter_line_proj[i].bias, 0.0)
+                nn.init.orthogonal_(self.inter_line_proj[i].weight, gain=1)
+                self.layer2idx[block] = i
         self.register_parameter("bin_score", bin_score)
         self.register_parameter("line_bin_score", line_bin_score)
         if conf.weights:
@@ -155,6 +168,20 @@ class GlueStick(PointGNN):
                 sd = {k.replace("matcher.", "").replace("module.", ""): v for k, v in sd["model"].items() if "matcher." in k}
             self.load_state_dict(sd, strict=False)
         self._register_head_perm(D)
+
+    @staticmethod
+    def _check_inter_supervision(conf):
+        """The reference takes the features of block l after the cross layer i with i // 2 == l, and weighs that head
+        with loss.inter_supervision[position of l]; anything else would fail mid-forward there (KeyError / IndexError)."""
+        blocks = {i // 2 for i, t in enumerate(conf.GNN_layers) if t == "cross"}
+        for block in conf.inter_supervision:
+            if isinstance(block, bool) or block not in blocks:
+                raise ValueError(f"gluefactory_b200 gluestick: inter_supervision entry {block!r} is not the block index "
+                                 f"(i // 2) of a cross layer i in GNN_layers; valid: {sorted(blocks)}")
+        weights = conf.loss.get("inter_supervision") or []
+        if len(weights) < len(conf.inter_supervision):
+            raise ValueError(f"gluefactory_b200 gluestick: loss.inter_supervision {list(weights)} has fewer weights than "
+                             f"inter_supervision {list(conf.inter_supervision)} has entries")
 
     def _line_layer(self, d0, d1, enc0, enc1, idx0, idx1, layer, B):
         """LineLayer (gluestick.py:589-691, line_attention = False)."""
@@ -215,49 +242,70 @@ class GlueStick(PointGNN):
 
         enc0, enc1 = line_enc(data["lines0"], data["line_scores0"], size0), line_enc(data["lines1"], data["line_scores1"], size1)
         idx0, idx1 = data["lines_junc_idx0"].reshape(B, -1), data["lines_junc_idx1"].reshape(B, -1)
+        inter = {}  # block -> both images' features after its cross layer (gluestick.py:762-768)
         for i, layer in enumerate(self.gnn.layers):
             d0, d1 = self._gnn_layer(d0, d1, layer.update, layer.type == "cross", B)
             if layer.type == "self":
                 for _ in range(self.conf.num_line_iterations):
                     d0, d1 = self._line_layer(d0, d1, enc0, enc1, idx0, idx1, self.gnn.line_layers[i // 2], B)
+            if self.conf.inter_supervision and layer.type == "cross" and i // 2 in self.conf.inter_supervision:
+                inter[i // 2] = (d0, d1)
         # points (keypoints and line junctions together)
         scores = ops.log_double_softmax(self._similarity(self._conv(d0, self.final_proj), self._conv(d1, self.final_proj), B),
                                         self.bin_score)
         m0, m1, ms0, ms1 = self._matches(scores.detach())
         pred = {"log_assignment": scores, "matches0": m0, "matches1": m1, "matching_scores0": ms0, "matching_scores1": ms1}
-        # lines: junction similarity gathered per endpoint pair, best of the two endpoint orderings (gluestick.py:333-377)
-        ld0 = d0.view(B, n0, D)[:, :2 * L0].reshape(-1, D)
-        ld1 = d1.view(B, n1, D)[:, :2 * L1].reshape(-1, D)
-        s = self._similarity(self._conv(ld0, self.final_line_proj), self._conv(ld1, self.final_line_proj), B)
+        lscores, lm0, lm1, lms0, lms1, raw = self._line_head(d0, d1, idx0, idx1, L0, L1, self.final_line_proj, B)
+        pred.update({"line_log_assignment": lscores, "line_matches0": lm0, "line_matches1": lm1,
+                     "line_matching_scores0": lms0, "line_matching_scores1": lms1, "raw_line_scores": raw})
+        for block in self.conf.inter_supervision or []:
+            proj = self.inter_line_proj[self.layer2idx[block]]
+            la, lm0, lm1, lms0, lms1, _ = self._line_head(*inter[block], idx0, idx1, L0, L1, proj, B)
+            pred.update({f"line_{block}_log_assignment": la, f"line_{block}_matches0": lm0,
+                         f"line_{block}_matches1": lm1, f"line_{block}_matching_scores0": lms0,
+                         f"line_{block}_matching_scores1": lms1})
+        return pred
+
+    def _line_head(self, d0, d1, idx0, idx1, L0, L1, proj, B):
+        """_get_line_matches (gluestick.py:336-376) with the projection `proj`: junction similarity gathered per endpoint
+        pair, best of the two endpoint orderings, log_double_softmax with the line bin score, match filtering.
+        Returns (log-assignment, matches0, matches1, matching_scores0, matching_scores1, raw line scores)."""
+        D = d0.shape[1]
+        ld0 = d0.view(B, -1, D)[:, :2 * L0].reshape(-1, D)
+        ld1 = d1.view(B, -1, D)[:, :2 * L1].reshape(-1, D)
+        s = self._similarity(self._conv(ld0, proj), self._conv(ld1, proj), B)
         n20, n21 = idx0.shape[1], idx1.shape[1]
         s = torch.gather(s, 2, idx1[:, None, :].expand(B, s.shape[1], n21))
         s = torch.gather(s, 1, idx0[:, :, None].expand(B, n20, n21)).reshape(B, n20 // 2, 2, n21 // 2, 2)
         raw = 0.5 * torch.maximum(s[:, :, 0, :, 0] + s[:, :, 1, :, 1], s[:, :, 0, :, 1] + s[:, :, 1, :, 0])
         lscores = ops.log_double_softmax(raw.contiguous(), self.line_bin_score)
-        lm0, lm1, lms0, lms1 = self._matches(lscores.detach())
-        pred.update({"line_log_assignment": lscores, "line_matches0": lm0, "line_matches1": lm1,
-                     "line_matching_scores0": lms0, "line_matching_scores1": lms1, "raw_line_scores": raw})
-        return pred
+        return (lscores, *self._matches(lscores.detach()), raw)
 
-    def _sub_loss(self, pred, data, losses, bin_score, prefix):
-        """gluestick.py:379-415."""
+    def _sub_loss(self, pred, data, losses, bin_score, prefix, block=None):
+        """gluestick.py:379-415; `block`: an intermediate line head (pred keys line_{block}_*, ground truth gt_line_*),
+        weighted by its loss.inter_supervision entry and without the statistics entries."""
+        suffix = "" if block is None else f"{block}_"
         positive = data["gt_" + prefix + "assignment"].float()
         num_pos = positive.sum((1, 2)).clamp(min=1.0)
         neg0 = (data["gt_" + prefix + "matches0"] == -1).float()
         neg1 = (data["gt_" + prefix + "matches1"] == -1).float()
         num_neg = (neg0.sum(1) + neg1.sum(1)).clamp(min=1.0)
-        la = pred[prefix + "log_assignment"]
+        la = pred[prefix + suffix + "log_assignment"]
         nll_pos = -(la[:, :-1, :-1] * positive).sum((1, 2)) / num_pos
         nll_neg = (-(la[:, :-1, -1] * neg0).sum(1) - (la[:, -1, :-1] * neg1).sum(1)) / num_neg
         bal = self.conf.loss.nll_balancing
         nll = bal * nll_pos + (1 - bal) * nll_neg
-        losses[prefix + "assignment_nll"] = nll
+        losses[prefix + suffix + "assignment_nll"] = nll
         if self.conf.loss.nll_weight > 0:
-            losses["total"] = losses["total"] + nll * self.conf.loss.nll_weight
-        losses[prefix + "num_matchable"] = num_pos
-        losses[prefix + "num_unmatchable"] = num_neg
-        losses[prefix + "sinkhorn_norm"] = la.exp()[:, :-1].sum(2).mean(1)
-        losses[prefix + "bin_score"] = bin_score[None]
+            term = nll * self.conf.loss.nll_weight
+            if block is not None:
+                term = term * self.conf.loss.inter_supervision[self.layer2idx[block]]
+            losses["total"] = losses["total"] + term
+        if block is None:
+            losses[prefix + "num_matchable"] = num_pos
+            losses[prefix + "num_unmatchable"] = num_neg
+            losses[prefix + "sinkhorn_norm"] = la.exp()[:, :-1].sum(2).mean(1)
+            losses[prefix + "bin_score"] = bin_score[None]
         return losses
 
     def loss(self, pred, data):
@@ -266,13 +314,21 @@ class GlueStick(PointGNN):
             losses = {"total": 0}
             losses = self._sub_loss(pred, data, losses, self.bin_score, "")
             losses = self._sub_loss(pred, data, losses, self.line_bin_score, "line_")
+            for block in self.conf.inter_supervision or []:
+                losses = self._sub_loss(pred, data, losses, self.line_bin_score, "line_", block)
             metrics = {}
             if not self.training:
-                metrics = {**matcher_metrics(pred, data),
-                           **{"line_" + k: v for k, v in matcher_metrics(
-                               {"matches0": pred["line_matches0"], "matching_scores0": pred["line_matching_scores0"]},
-                               {"gt_matches0": data["gt_line_matches0"]}).items()}}
+                metrics = {**matcher_metrics(pred, data), **_line_metrics(pred, data, "line_")}
+                for block in self.conf.inter_supervision or []:
+                    metrics.update(_line_metrics(pred, data, f"line_{block}_"))
             return losses, metrics
+
+
+def _line_metrics(pred, data, prefix):
+    """matcher_metrics(pred, data, prefix, prefix_gt="line_") (models/utils/metrics.py:4-50) of a line head."""
+    m = matcher_metrics({"matches0": pred[prefix + "matches0"], "matching_scores0": pred[prefix + "matching_scores0"]},
+                        {"gt_matches0": data["gt_line_matches0"]})
+    return {prefix + k: v for k, v in m.items()}
 
 
 __main_model__ = GlueStick
