@@ -301,34 +301,56 @@ def run_gluestick(name="gluestick_l4_n160", n_gnn=4, B=2, N=160, L=24, seed=31):
           f"{path} ({os.path.getsize(path) / 1e6:.2f} MB)")
 
 
-def run_gt_pose_depth():
-    """Golden labels from the reference's own gt_matches_from_pose_depth (geometry/gt_generation.py:13-106) with its
-    Camera / Pose wrappers, for th_epi None / 5 and th_consistency None / 3: stores the inputs of the O(M N) pass
-    (reprojections and masks, as the reference computed them) and its outputs."""
+def _pose_depth_labels(out, tag, sc, B, M, N, seed, epi, cc):
+    """Runs the reference's gt_matches_from_pose_depth on a scene and stores the inputs of the O(M N) pass
+    (reprojections and masks, as the reference computed them) and its outputs under `tag|...`."""
+    from gluefactory.geometry.depth import sample_depth
     from gluefactory.geometry.gt_generation import gt_matches_from_pose_depth
     from gluefactory.geometry.wrappers import Camera, Pose
 
+    data = {"view0": {"camera": Camera.from_calibration_matrix(sc["K0"]), "depth": sc["depth0"]},
+            "view1": {"camera": Camera.from_calibration_matrix(sc["K1"]), "depth": sc["depth1"]},
+            "T_0to1": Pose.from_Rt(sc["R"], sc["t"])}
+    r = gt_matches_from_pose_depth(sc["kp0"], sc["kp1"], data, pos_th=3.0, neg_th=5.0, epi_th=epi, cc_th=cc)
+    out[f"{tag}|meta"] = np.array([B, M, N, seed, -1 if epi is None else epi, -1 if cc is None else cc], dtype=np.float64)
+    for k in ("matches0", "matches1", "proj_0to1", "proj_1to0", "visible0", "visible1", "depth_keypoints0",
+              "depth_keypoints1"):
+        out[f"{tag}|{k}"] = r[k].numpy()
+    out[f"{tag}|positives"] = r["assignment"].nonzero().numpy()
+    out[f"{tag}|valid0"] = sample_depth(sc["kp0"], sc["depth0"])[1].numpy()
+    out[f"{tag}|valid1"] = sample_depth(sc["kp1"], sc["depth1"])[1].numpy()
+    print(f"gt_pose_depth {tag}: positives={int(r['assignment'].sum())} unmatched0={int((r['matches0'] == -1).sum())} "
+          f"ignored0={int((r['matches0'] == -2).sum())}")
+
+
+def run_gt_pose_depth():
+    """Golden labels from the reference's own gt_matches_from_pose_depth (geometry/gt_generation.py:13-106) with its
+    Camera / Pose wrappers, for th_epi None / 5 and th_consistency None / 3."""
     out = {}
     for tag, (B, M, N, seed, epi, cc) in {"a": (2, 300, 260, 61, None, None), "b": (1, 513, 640, 62, 5.0, None),
                                           "c": (2, 200, 333, 63, 5.0, 3.0)}.items():
-        sc = synthetic.pose_depth_scene(B, M, N, seed)
-        data = {"view0": {"camera": Camera.from_calibration_matrix(sc["K0"]), "depth": sc["depth0"]},
-                "view1": {"camera": Camera.from_calibration_matrix(sc["K1"]), "depth": sc["depth1"]},
-                "T_0to1": Pose.from_Rt(sc["R"], sc["t"])}
-        r = gt_matches_from_pose_depth(sc["kp0"], sc["kp1"], data, pos_th=3.0, neg_th=5.0, epi_th=epi, cc_th=cc)
-        out[f"{tag}|meta"] = np.array([B, M, N, seed, -1 if epi is None else epi, -1 if cc is None else cc], dtype=np.float64)
-        for k in ("matches0", "matches1", "proj_0to1", "proj_1to0", "visible0", "visible1", "depth_keypoints0",
-                  "depth_keypoints1"):
-            out[f"{tag}|{k}"] = r[k].numpy()
-        out[f"{tag}|positives"] = r["assignment"].nonzero().numpy()
-        from gluefactory.geometry.depth import sample_depth
-        out[f"{tag}|valid0"] = sample_depth(sc["kp0"], sc["depth0"])[1].numpy()
-        out[f"{tag}|valid1"] = sample_depth(sc["kp1"], sc["depth1"])[1].numpy()
-        print(f"gt_pose_depth {tag}: positives={int(r['assignment'].sum())} unmatched0={int((r['matches0'] == -1).sum())} "
-              f"ignored0={int((r['matches0'] == -2).sum())}")
+        _pose_depth_labels(out, tag, synthetic.pose_depth_scene(B, M, N, seed), B, M, N, seed, epi, cc)
     path = os.path.join(OUT, "gt_pose_depth.npz")
     np.savez_compressed(path, **out)
     print("gt_pose_depth ->", path, f"({os.path.getsize(path) / 1e6:.2f} MB)")
+
+
+def run_gt_pose_depth_masks():
+    """The same on a scene whose depth maps have large invalid regions (`tag|zero0/1`: rows of [y0, y1, x0, x1] blocks
+    set to 0 in depth0 / depth1), so that about half of the points have no depth, many epipolar candidates arise and
+    some of them have no still-ignored partner.  A file of its own: gt_pose_depth.npz is not regenerated."""
+    out = {}
+    zero = {"zero0": np.array([[0, 480, 320, 640]]), "zero1": np.array([[240, 480, 0, 640], [0, 480, 0, 160]])}
+    for tag, (B, M, N, seed, epi, cc) in {"d": (2, 300, 333, 64, 5.0, None), "e": (2, 40, 2, 65, 5.0, 3.0)}.items():
+        sc = synthetic.pose_depth_scene(B, M, N, seed)
+        for i in "01":
+            for y0, y1, x0, x1 in zero[f"zero{i}"]:
+                sc[f"depth{i}"][:, y0:y1, x0:x1] = 0.0
+            out[f"{tag}|zero{i}"] = zero[f"zero{i}"]
+        _pose_depth_labels(out, tag, sc, B, M, N, seed, epi, cc)
+    path = os.path.join(OUT, "gt_pose_depth_masks.npz")
+    np.savez_compressed(path, **out)
+    print("gt_pose_depth_masks ->", path, f"({os.path.getsize(path) / 1e6:.2f} MB)")
 
 
 def run_adaptive():
@@ -408,7 +430,7 @@ if __name__ == "__main__":
     if only:
         for name in only:
             {"gluestick_attn": run_gluestick_attention, "gt_homography": run_gt_homography,
-             "heads_grad": run_heads_grad, "autocast": run_autocast_cases, "eval_loss": run_eval_loss, "gluestick": run_gluestick, "gt_pose_depth": run_gt_pose_depth, "adaptive": run_adaptive,
+             "heads_grad": run_heads_grad, "autocast": run_autocast_cases, "eval_loss": run_eval_loss, "gluestick": run_gluestick, "gt_pose_depth": run_gt_pose_depth, "gt_pose_depth_masks": run_gt_pose_depth_masks, "adaptive": run_adaptive,
              "sift": lambda: run_case("lg_sift_d256_l2_n96", dict(synthetic.DEFAULT_CONF, n_layers=2, input_dim=128,
                                                                   add_scale_ori=True), B=1, N=96, M=80, seed=16)}[name]()
         sys.exit(0)
@@ -432,4 +454,5 @@ if __name__ == "__main__":
     run_eval_loss()
     run_gluestick()
     run_gt_pose_depth()
+    run_gt_pose_depth_masks()
     run_adaptive()
