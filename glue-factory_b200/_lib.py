@@ -25,6 +25,8 @@ SIGNATURES = {
     "lgb200_check_device": (_i, []),
     "lgb200_rope_split_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp]),
     "lgb200_rope_split_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp]),
+    "lgb200_rope_split_fwd_hd": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp]),
+    "lgb200_rope_split_bwd_hd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp]),
     "lgb200_attn_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp]),
     "lgb200_attn_bwd_ws_floats": (_i64, [_i, _i, _i, _i]),
     "lgb200_attn_bwd": (_i, [_vp] * 10 + [_i, _i, _i, _i, _i, _f, _i, _vp]),
@@ -133,6 +135,7 @@ KERNELS_PER_CALL = {
     "lgb200_gemm_bf16_splitk": 2, "lgb200_gt_from_homography": 3, "lgb200_gt_from_reprojection": 3, "lgb200_gt_epipolar_unmatched": 2, "lgb200_gt_line_matches": 5, "lgb200_flat_grad_check": 1, "lgb200_flat_grad_norm": 2, "lgb200_amp_update": 1,
     "lgb200_ot_nll_fwd": 2, "lgb200_ot_nll_bwd": 1, "lgb200_ot_filter_stats": 2, "lgb200_bn_running_update": 1,
     "lgb200_attn_fwd_hd": 1, "lgb200_attn_bwd_hd": 3,  # prep + dQ + dKV (fp32: delta + dQ + dKV)
+    "lgb200_rope_split_fwd_hd": 1, "lgb200_rope_split_bwd_hd": 1,
 }
 launch_count = 0          # running total of kernels launched through `call`
 timed_entry = None        # entry-point name or a set of names: every call of them is bracketed by CUDA events

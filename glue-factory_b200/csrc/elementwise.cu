@@ -1,6 +1,6 @@
 // Memory-bound helpers of the matcher layer:
-//   * rope_split  : de-interleave the Wqkv output (feature = h*192 + d*3 + {q,k,v}) and apply the
-//                   cached rotary encoding to q and k   (lightglue.py:42-49, 156-160)
+//   * rope_split  : de-interleave the Wqkv output (feature = h*3*hd + d*3 + {q,k,v}, head dim hd = 64 or 32) and
+//                   apply the cached rotary encoding to q and k   (lightglue.py:42-49, 156-160)
 //   * ln_gelu     : LayerNorm(2D) + exact-erf GELU of the FFN (lightglue.py:143-148)
 //   * adam_flat   : Adam on the flat parameter buffer (train.py:358-361, 513)
 // All use 128-bit loads/stores; row reductions are warp shuffles.
@@ -48,25 +48,27 @@ template <> struct Vec8<__nv_bfloat16> {
 };
 
 // ---------------------------------------------------------------------------------------------
-// rope_split: thread <-> (token, group of 4 rotary pairs = 8 channels), loops over heads.
-// qkv row layout per head: [q0 k0 v0 q1 k1 v1 ... q63 k63 v63]; the 8 channels of a group are 24
-// consecutive elements.  Outputs are token-major [T, H*64].
+// rope_split: thread <-> (token, group of 4 rotary pairs = 8 channels), loops over heads.  HD = head dim (64 or 32).
+// qkv row layout per head: [q0 k0 v0 q1 k1 v1 ... q(HD-1) k(HD-1) v(HD-1)]; the 8 channels of a group are 24
+// consecutive elements.  Outputs are token-major [T, H*HD]; theta is [T, HD/2].
 // ---------------------------------------------------------------------------------------------
-template <typename T>
+template <typename T, int HD>
 __global__ void __launch_bounds__(256) rope_split_fwd_kernel(const T* __restrict__ qkv, const float* __restrict__ theta,
                                                             T* __restrict__ q, T* __restrict__ k, T* __restrict__ v,
                                                             int64_t ntok, int H) {
+  static_assert(HD == 32 || HD == 64, "head_dim 32 or 64");
+  constexpr int kGroups = HD / 8, kShift = HD == 64 ? 3 : 2;
   const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t tok = gid >> 3;
-  const int grp = (int)(gid & 7);
+  const int64_t tok = gid >> kShift;
+  const int grp = (int)(gid & (kGroups - 1));
   if (tok >= ntok) return;
   float c[4], s[4];
   {
-    const float4 th = *reinterpret_cast<const float4*>(theta + tok * 32 + grp * 4);
+    const float4 th = *reinterpret_cast<const float4*>(theta + tok * (HD / 2) + grp * 4);
     sincosf(th.x, &s[0], &c[0]); sincosf(th.y, &s[1], &c[1]); sincosf(th.z, &s[2], &c[2]); sincosf(th.w, &s[3], &c[3]);
   }
   for (int h = 0; h < H; ++h) {
-    const T* src = qkv + tok * (int64_t)(H * 192) + h * 192 + grp * 24;
+    const T* src = qkv + tok * (int64_t)(H * 3 * HD) + h * 3 * HD + grp * 24;
     Vec8<T> a = Vec8<T>::load(src), b = Vec8<T>::load(src + 8), d = Vec8<T>::load(src + 16);
     float f[24];
 #pragma unroll
@@ -83,7 +85,7 @@ __global__ void __launch_bounds__(256) rope_split_fwd_kernel(const T* __restrict
       ov.v[2 * p] = v0;
       ov.v[2 * p + 1] = v1;
     }
-    const int64_t o = tok * (int64_t)(H * 64) + h * 64 + grp * 8;
+    const int64_t o = tok * (int64_t)(H * HD) + h * HD + grp * 8;
     oq.store(q + o);
     ok.store(k + o);
     ov.store(v + o);
@@ -92,23 +94,25 @@ __global__ void __launch_bounds__(256) rope_split_fwd_kernel(const T* __restrict
 
 // backward: dq,dk are gradients w.r.t. the ROTATED q,k; q,k are the rotated values saved by forward.
 //   d(unrotated) = R(-theta) d(rotated);  dtheta_p += sum_heads ( dq'[2p+1] q'[2p] - dq'[2p] q'[2p+1] ) + same for k
-template <typename T>
+template <typename T, int HD>
 __global__ void __launch_bounds__(256) rope_split_bwd_kernel(const T* __restrict__ dq, const T* __restrict__ dk,
                                                             const T* __restrict__ dv, const T* __restrict__ q,
                                                             const T* __restrict__ k, const float* __restrict__ theta,
                                                             T* __restrict__ dqkv, float* __restrict__ dtheta,
                                                             int64_t ntok, int H) {
+  static_assert(HD == 32 || HD == 64, "head_dim 32 or 64");
+  constexpr int kGroups = HD / 8, kShift = HD == 64 ? 3 : 2;
   const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t tok = gid >> 3;
-  const int grp = (int)(gid & 7);
+  const int64_t tok = gid >> kShift;
+  const int grp = (int)(gid & (kGroups - 1));
   if (tok >= ntok) return;
   float c[4], s[4], dth[4] = {0.f, 0.f, 0.f, 0.f};
   {
-    const float4 th = *reinterpret_cast<const float4*>(theta + tok * 32 + grp * 4);
+    const float4 th = *reinterpret_cast<const float4*>(theta + tok * (HD / 2) + grp * 4);
     sincosf(th.x, &s[0], &c[0]); sincosf(th.y, &s[1], &c[1]); sincosf(th.z, &s[2], &c[2]); sincosf(th.w, &s[3], &c[3]);
   }
   for (int h = 0; h < H; ++h) {
-    const int64_t o = tok * (int64_t)(H * 64) + h * 64 + grp * 8;
+    const int64_t o = tok * (int64_t)(H * HD) + h * HD + grp * 8;
     Vec8<T> gq = Vec8<T>::load(dq + o), gk = Vec8<T>::load(dk + o), gv = Vec8<T>::load(dv + o);
     Vec8<T> rq = Vec8<T>::load(q + o), rk = Vec8<T>::load(k + o);
     float f[24];
@@ -126,12 +130,12 @@ __global__ void __launch_bounds__(256) rope_split_bwd_kernel(const T* __restrict
     Vec8<T> a, b, d;
 #pragma unroll
     for (int i = 0; i < 8; ++i) { a.v[i] = f[i]; b.v[i] = f[8 + i]; d.v[i] = f[16 + i]; }
-    T* dst = dqkv + tok * (int64_t)(H * 192) + h * 192 + grp * 24;
+    T* dst = dqkv + tok * (int64_t)(H * 3 * HD) + h * 3 * HD + grp * 24;
     a.store(dst);
     b.store(dst + 8);
     d.store(dst + 16);
   }
-  float4* pt = reinterpret_cast<float4*>(dtheta + tok * 32 + grp * 4);
+  float4* pt = reinterpret_cast<float4*>(dtheta + tok * (HD / 2) + grp * 4);
   float4 acc = *pt;  // accumulated across layers; this thread is the only writer of these 4 floats
   acc.x += dth[0]; acc.y += dth[1]; acc.z += dth[2]; acc.w += dth[3];
   *pt = acc;
@@ -548,14 +552,17 @@ __global__ void __launch_bounds__(256) cast_bf16_kernel(const float* __restrict_
 
 // dW[c][d] = sum_t g[t][c] * kp[t][d]: the weight gradient of the Fourier position encoder's projection
 // (lightglue.py:37-44; theta = kp Wr^T with kp [T, 2 or 4]), a tall-skinny contraction cuBLAS runs as split-K sgemm +
-// memset (0.2 ms per step).  C == 32: a warp reads one 128-byte row of g, 8 rows in flight per CTA; per-CTA partials.
+// memset (0.2 ms per step).  C = head_dim / 2 = 32 or 16 angles: a warp reads 32 / C consecutive 4C-byte rows of g
+// (128 bytes), 256 / C rows in flight per CTA; per-CTA partials, summed over the CTA's rows in a fixed order.
+template <int C>
 __global__ void __launch_bounds__(256) posenc_wgrad_kernel(const float* __restrict__ g, const float* __restrict__ kp,
                                                           float* __restrict__ part, int64_t T, int KD) {
-  __shared__ float red[8][32][4];
-  const int c = threadIdx.x & 31, slot = threadIdx.x >> 5;
+  constexpr int kRows = 256 / C;
+  __shared__ float red[kRows][C][4];
+  const int c = threadIdx.x % C, slot = threadIdx.x / C;
   float acc[4] = {0.f, 0.f, 0.f, 0.f};
-  for (int64_t t = (int64_t)blockIdx.x * 8 + slot; t < T; t += (int64_t)gridDim.x * 8) {
-    const float gv = __ldg(g + t * 32 + c);
+  for (int64_t t = (int64_t)blockIdx.x * kRows + slot; t < T; t += (int64_t)gridDim.x * kRows) {
+    const float gv = __ldg(g + t * C + c);
 #pragma unroll
     for (int d = 0; d < 4; ++d)
       if (d < KD) acc[d] = fmaf(gv, __ldg(kp + t * KD + d), acc[d]);
@@ -568,8 +575,8 @@ __global__ void __launch_bounds__(256) posenc_wgrad_kernel(const float* __restri
     for (int d = 0; d < 4; ++d) {
       float v = 0.f;
 #pragma unroll
-      for (int s8 = 0; s8 < 8; ++s8) v += red[s8][c][d];
-      if (d < KD) part[((int64_t)blockIdx.x * 32 + c) * KD + d] = v;
+      for (int s8 = 0; s8 < kRows; ++s8) v += red[s8][c][d];
+      if (d < KD) part[((int64_t)blockIdx.x * C + c) * KD + d] = v;
     }
   }
 }
@@ -1104,8 +1111,12 @@ int lgb200_colsum_slabs(int64_t rows, int cols) {
 int lgb200_posenc_wgrad_blocks(void) { return 2 * device_sm_count(); }
 int lgb200_posenc_wgrad(const float* g, const float* kp, float* part, int64_t T, int C, int KD, cudaStream_t stream) {
   LGB_REQUIRE(g && kp && part && T > 0, kErrInvalid, "posenc_wgrad: bad arguments");
-  LGB_REQUIRE(C == 32 && KD >= 1 && KD <= 4, kErrInvalid, "posenc_wgrad: C must be 32 and 1 <= KD <= 4 (got %d, %d)", C, KD);
-  posenc_wgrad_kernel<<<lgb200_posenc_wgrad_blocks(), 256, 0, stream>>>(g, kp, part, T, KD);
+  LGB_REQUIRE((C == 32 || C == 16) && KD >= 1 && KD <= 4, kErrInvalid,
+              "posenc_wgrad: C must be 32 or 16 and 1 <= KD <= 4 (got %d, %d)", C, KD);
+  if (C == 32)
+    posenc_wgrad_kernel<32><<<lgb200_posenc_wgrad_blocks(), 256, 0, stream>>>(g, kp, part, T, KD);
+  else
+    posenc_wgrad_kernel<16><<<lgb200_posenc_wgrad_blocks(), 256, 0, stream>>>(g, kp, part, T, KD);
   return check_launch("posenc_wgrad");
 }
 
@@ -1256,44 +1267,61 @@ int lgb200_residual_add_cast(const float* x, const void* y, float* x_out, void* 
   return lgb200_residual_add_cast_pitched(x, y, x_out, x_cast, 1, n, n, dtype, stream);
 }
 
-int lgb200_rope_split_fwd(const void* qkv, const float* theta, void* q, void* k, void* v, int64_t ntok, int H,
-                          int dtype, cudaStream_t stream) {
+int lgb200_rope_split_fwd_hd(const void* qkv, const float* theta, void* q, void* k, void* v, int64_t ntok, int H,
+                             int dtype, int head_dim, cudaStream_t stream) {
+  LGB_REQUIRE(head_dim == 32 || head_dim == 64, kErrUnsupported, "rope_split_fwd: head_dim %d (built for 32 and 64)",
+              head_dim);
   LGB_REQUIRE(qkv && theta && q && k && v, kErrInvalid, "rope_split_fwd: null pointer");
   LGB_REQUIRE(ntok > 0 && H > 0, kErrInvalid, "rope_split_fwd: empty input");
   LGB_REQUIRE(aligned16({qkv, theta, q, k, v}), kErrInvalid, "rope_split_fwd: misaligned pointer (16 bytes needed)");
-  const int64_t nthr = ntok * 8;
+  LGB_REQUIRE(dtype == LGB200_F32 || dtype == LGB200_BF16, kErrInvalid, "rope_split_fwd: bad dtype %d", dtype);
+  const int64_t nthr = ntok * (head_dim / 8);
   const unsigned grid = (unsigned)((nthr + 255) / 256);
-  if (dtype == LGB200_F32)
-    rope_split_fwd_kernel<float><<<grid, 256, 0, stream>>>((const float*)qkv, theta, (float*)q, (float*)k, (float*)v,
-                                                           ntok, H);
-  else if (dtype == LGB200_BF16)
-    rope_split_fwd_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16*)qkv, theta, (__nv_bfloat16*)q,
-                                                                   (__nv_bfloat16*)k, (__nv_bfloat16*)v, ntok, H);
-  else
-    LGB_REQUIRE(false, kErrInvalid, "rope_split_fwd: bad dtype %d", dtype);
+  if (dtype == LGB200_F32) {
+    auto kern = head_dim == 64 ? rope_split_fwd_kernel<float, 64> : rope_split_fwd_kernel<float, 32>;
+    kern<<<grid, 256, 0, stream>>>((const float*)qkv, theta, (float*)q, (float*)k, (float*)v, ntok, H);
+  } else {
+    auto kern = head_dim == 64 ? rope_split_fwd_kernel<__nv_bfloat16, 64> : rope_split_fwd_kernel<__nv_bfloat16, 32>;
+    kern<<<grid, 256, 0, stream>>>((const __nv_bfloat16*)qkv, theta, (__nv_bfloat16*)q, (__nv_bfloat16*)k,
+                                   (__nv_bfloat16*)v, ntok, H);
+  }
   return check_launch("rope_split_fwd");
+}
+
+int lgb200_rope_split_fwd(const void* qkv, const float* theta, void* q, void* k, void* v, int64_t ntok, int H,
+                          int dtype, cudaStream_t stream) {
+  return lgb200_rope_split_fwd_hd(qkv, theta, q, k, v, ntok, H, dtype, 64, stream);
+}
+
+int lgb200_rope_split_bwd_hd(const void* dq, const void* dk, const void* dv, const void* q, const void* k,
+                             const float* theta, void* dqkv, float* dtheta, int64_t ntok, int H, int dtype,
+                             int head_dim, cudaStream_t stream) {
+  LGB_REQUIRE(head_dim == 32 || head_dim == 64, kErrUnsupported, "rope_split_bwd: head_dim %d (built for 32 and 64)",
+              head_dim);
+  LGB_REQUIRE(dq && dk && dv && q && k && theta && dqkv && dtheta, kErrInvalid, "rope_split_bwd: null pointer");
+  LGB_REQUIRE(ntok > 0 && H > 0, kErrInvalid, "rope_split_bwd: empty input");
+  LGB_REQUIRE(aligned16({dq, dk, dv, q, k, theta, dqkv, dtheta}), kErrInvalid,
+              "rope_split_bwd: misaligned pointer (16 bytes needed)");
+  LGB_REQUIRE(dtype == LGB200_F32 || dtype == LGB200_BF16, kErrInvalid, "rope_split_bwd: bad dtype %d", dtype);
+  const int64_t nthr = ntok * (head_dim / 8);
+  const unsigned grid = (unsigned)((nthr + 255) / 256);
+  if (dtype == LGB200_F32) {
+    auto kern = head_dim == 64 ? rope_split_bwd_kernel<float, 64> : rope_split_bwd_kernel<float, 32>;
+    kern<<<grid, 256, 0, stream>>>((const float*)dq, (const float*)dk, (const float*)dv, (const float*)q,
+                                   (const float*)k, theta, (float*)dqkv, dtheta, ntok, H);
+  } else {
+    auto kern = head_dim == 64 ? rope_split_bwd_kernel<__nv_bfloat16, 64> : rope_split_bwd_kernel<__nv_bfloat16, 32>;
+    kern<<<grid, 256, 0, stream>>>((const __nv_bfloat16*)dq, (const __nv_bfloat16*)dk, (const __nv_bfloat16*)dv,
+                                   (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, theta, (__nv_bfloat16*)dqkv,
+                                   dtheta, ntok, H);
+  }
+  return check_launch("rope_split_bwd");
 }
 
 int lgb200_rope_split_bwd(const void* dq, const void* dk, const void* dv, const void* q, const void* k,
                           const float* theta, void* dqkv, float* dtheta, int64_t ntok, int H, int dtype,
                           cudaStream_t stream) {
-  LGB_REQUIRE(dq && dk && dv && q && k && theta && dqkv && dtheta, kErrInvalid, "rope_split_bwd: null pointer");
-  LGB_REQUIRE(ntok > 0 && H > 0, kErrInvalid, "rope_split_bwd: empty input");
-  LGB_REQUIRE(aligned16({dq, dk, dv, q, k, theta, dqkv, dtheta}), kErrInvalid,
-              "rope_split_bwd: misaligned pointer (16 bytes needed)");
-  const int64_t nthr = ntok * 8;
-  const unsigned grid = (unsigned)((nthr + 255) / 256);
-  if (dtype == LGB200_F32)
-    rope_split_bwd_kernel<float><<<grid, 256, 0, stream>>>((const float*)dq, (const float*)dk, (const float*)dv,
-                                                           (const float*)q, (const float*)k, theta, (float*)dqkv,
-                                                           dtheta, ntok, H);
-  else if (dtype == LGB200_BF16)
-    rope_split_bwd_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(
-        (const __nv_bfloat16*)dq, (const __nv_bfloat16*)dk, (const __nv_bfloat16*)dv, (const __nv_bfloat16*)q,
-        (const __nv_bfloat16*)k, theta, (__nv_bfloat16*)dqkv, dtheta, ntok, H);
-  else
-    LGB_REQUIRE(false, kErrInvalid, "rope_split_bwd: bad dtype %d", dtype);
-  return check_launch("rope_split_bwd");
+  return lgb200_rope_split_bwd_hd(dq, dk, dv, q, k, theta, dqkv, dtheta, ntok, H, dtype, 64, stream);
 }
 
 }  // extern "C"

@@ -156,17 +156,19 @@ def _dgrad_acc(acc, dy, w):
 
 
 def _attend_fwd(q, k, v, sizes, H, cross):
-    """q,k,v [T, H*64] over tokens [image0 (B*M); image1 (B*N)] -> (out [T, H*64], lse tuple)."""
+    """q,k,v [T, H*hd] over tokens [image0 (B*M); image1 (B*N)] -> (out [T, H*hd], lse tuple).  The head dim hd = 64 or
+    32 is read from the shapes; the scale is hd^-1/2 (lightglue.py:139, 173)."""
     B, M, N = sizes
-    scale = 0.125
+    hd = q.shape[1] // H
+    scale = hd ** -0.5
     if M == N:
-        shp = (2 * B, M, H, 64)
+        shp = (2 * B, M, H, hd)
         out, lse = ops.attn_fwd(q.view(shp), k.view(shp), v.view(shp), B if cross else 0, scale)
         return out.view(q.shape), (lse,)
     t0 = B * M
-    q0, q1 = q[:t0].view(B, M, H, 64), q[t0:].view(B, N, H, 64)
-    k0, k1 = k[:t0].view(B, M, H, 64), k[t0:].view(B, N, H, 64)
-    v0, v1 = v[:t0].view(B, M, H, 64), v[t0:].view(B, N, H, 64)
+    q0, q1 = q[:t0].view(B, M, H, hd), q[t0:].view(B, N, H, hd)
+    k0, k1 = k[:t0].view(B, M, H, hd), k[t0:].view(B, N, H, hd)
+    v0, v1 = v[:t0].view(B, M, H, hd), v[t0:].view(B, N, H, hd)
     if cross:
         o0, l0 = ops.attn_fwd(q0, k1, v1, 0, scale)
         o1, l1 = ops.attn_fwd(q1, k0, v0, 0, scale)
@@ -178,14 +180,15 @@ def _attend_fwd(q, k, v, sizes, H, cross):
 
 def _attend_bwd(q, k, v, out, lses, dout, sizes, H, cross):
     B, M, N = sizes
-    scale = 0.125
+    hd = q.shape[1] // H
+    scale = hd ** -0.5
     if M == N:
-        shp = (2 * B, M, H, 64)
+        shp = (2 * B, M, H, hd)
         dq, dk, dv = ops.attn_bwd(q.view(shp), k.view(shp), v.view(shp), out.view(shp), lses[0], dout.view(shp),
                                   B if cross else 0, scale)
         return dq.view(q.shape), dk.view(q.shape), dv.view(q.shape)
     t0 = B * M
-    sp = lambda t: (t[:t0].view(B, M, H, 64), t[t0:].view(B, N, H, 64))  # noqa: E731
+    sp = lambda t: (t[:t0].view(B, M, H, hd), t[t0:].view(B, N, H, hd))  # noqa: E731
     (q0, q1), (k0, k1), (v0, v1), (o0, o1), (g0, g1) = sp(q), sp(k), sp(v), sp(out), sp(dout.contiguous())
     if cross:
         dq0, dk1, dv1 = ops.attn_bwd(q0, k1, v1, o0, lses[0], g0, 0, scale)
@@ -199,12 +202,14 @@ def _attend_bwd(q, k, v, out, lses, dout, sizes, H, cross):
 
 def _attend_bwd_shared_qk(qk, v, out, lses, dout, sizes, H):
     """Cross-attention backward with one to_qk projection as query in one direction and key in the other
-    (lightglue.py:207-216) -> (dqk = dq + dk, dv)."""
+    (lightglue.py:207-216) -> (dqk = dq + dk, dv).  The one-sweep shared-qk kernel is built for head dim 64; at
+    head dim 32, and whenever M != N, both directions write separate dq / dk buffers that are then added."""
     B, M, N = sizes
-    if M != N:
+    hd = qk.shape[1] // H
+    if M != N or hd != 64:
         dq, dk, dv = _attend_bwd(qk, qk, v, out, lses, dout, sizes, H, cross=True)
         return dq.add_(dk), dv
-    shp = (2 * B, M, H, 64)
+    shp = (2 * B, M, H, hd)
     dqk, dv = ops.attn_bwd_shared_qk(qk.view(shp), v.view(shp), out.view(shp), lses[0], dout.view(shp), 0.125)
     return dqk.view(qk.shape), dv.view(qk.shape)
 

@@ -168,11 +168,15 @@ class LightGlue(nn.Module):
         self.conf = conf = _Conf(_merge(self.default_conf, _to_plain(conf)))
         assert conf.precision in ("bf16", "fp32", "bf16x3"), conf.precision
         d, h, n = conf.descriptor_dim, conf.num_heads, conf.n_layers
-        assert d % h == 0 and d // h == 64, "the lgb200 kernels are built for head_dim 64"
+        # head_dim = descriptor_dim // num_heads (lightglue.py:347): 64 (256 / 4, the default) or 32 (128 / 4, 256 / 8)
+        if d % h or d // h not in (32, 64):
+            raise NotImplementedError(f"gluefactory_b200 lightglue: head_dim = descriptor_dim // num_heads must be 32 or "
+                                      f"64, the head dims the kernels are built for (descriptor_dim {d}, num_heads {h})")
+        hd = d // h
         self.input_proj = nn.Linear(conf.input_dim, d) if conf.input_dim != d else nn.Identity()
         # add_scale_ori (SIFT-style features, lightglue.py:347-349, 426-443): scale and orientation join (x, y) as inputs
-        # of the learnt Fourier encoding, Wr becomes [32, 4]; only the rotary ANGLES change, not the kernels
-        self.posenc = LearnableFourierPositionalEncoding(2 + 2 * bool(conf.add_scale_ori), 64, 64)
+        # of the learnt Fourier encoding, Wr becomes [hd/2, 4]; only the rotary ANGLES change, not the kernels
+        self.posenc = LearnableFourierPositionalEncoding(2 + 2 * bool(conf.add_scale_ori), hd, hd)
         self.transformers = nn.ModuleList([TransformerLayer(d, h) for _ in range(n)])
         self.log_assignment = nn.ModuleList([MatchAssignment(d) for _ in range(n)])
         self.token_confidence = nn.ModuleList([TokenConfidence(d) for _ in range(n - 1)])

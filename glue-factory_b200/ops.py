@@ -36,24 +36,37 @@ def _chk(t, dtype=None, strided_rows=False):
 # rotary split (lightglue.py:157-160)
 # ------------------------------------------------------------------------------------------------
 def rope_fwd(qkv, theta, H):
+    """qkv [T, H*3*hd] (feature = h*3*hd + d*3 + {q,k,v}), theta [T, hd/2] -> rotated q, k and v [T, H*hd]; the head
+    dim hd = 64 or 32 is read from the shapes."""
     _chk(qkv)
     _chk(theta, torch.float32)
     T = qkv.shape[0]
-    q = torch.empty(T, H * 64, device=qkv.device, dtype=qkv.dtype)
+    hd = qkv.shape[1] // (3 * H)
+    assert qkv.shape[1] == 3 * H * hd and theta.shape == (T, hd // 2), (tuple(qkv.shape), tuple(theta.shape), H)
+    q = torch.empty(T, H * hd, device=qkv.device, dtype=qkv.dtype)
     k, v = torch.empty_like(q), torch.empty_like(q)
-    call("lgb200_rope_split_fwd", ptr(qkv), ptr(theta), ptr(q), ptr(k), ptr(v), T, H, _code(qkv.dtype), stream_ptr())
+    args = (ptr(qkv), ptr(theta), ptr(q), ptr(k), ptr(v), T, H, _code(qkv.dtype))
+    if hd == 64:
+        call("lgb200_rope_split_fwd", *args, stream_ptr())
+    else:
+        call("lgb200_rope_split_fwd_hd", *args, hd, stream_ptr())
     return q, k, v
 
 
 def rope_bwd(dq, dk, dv, q, k, theta, H, dtheta=None):
     """Returns dqkv; ACCUMULATES into dtheta (allocated zeroed when None)."""
     T = q.shape[0]
+    hd = q.shape[1] // H
+    assert q.shape[1] == H * hd and theta.shape == (T, hd // 2), (tuple(q.shape), tuple(theta.shape), H)
     dq, dk, dv = (g.contiguous() for g in (dq, dk, dv))
-    dqkv = torch.empty(T, H * 192, device=q.device, dtype=q.dtype)
+    dqkv = torch.empty(T, H * 3 * hd, device=q.device, dtype=q.dtype)
     if dtheta is None:
         dtheta = torch.zeros_like(theta)
-    call("lgb200_rope_split_bwd", ptr(dq), ptr(dk), ptr(dv), ptr(q), ptr(k), ptr(theta), ptr(dqkv), ptr(dtheta),
-         T, H, _code(q.dtype), stream_ptr())
+    args = (ptr(dq), ptr(dk), ptr(dv), ptr(q), ptr(k), ptr(theta), ptr(dqkv), ptr(dtheta), T, H, _code(q.dtype))
+    if hd == 64:
+        call("lgb200_rope_split_bwd", *args, stream_ptr())
+    else:
+        call("lgb200_rope_split_bwd_hd", *args, hd, stream_ptr())
     return dqkv, dtheta
 
 
@@ -167,8 +180,9 @@ _colsum_counters = {}
 
 
 class PosencTheta(torch.autograd.Function):
-    """theta = kp Wr^T (lightglue.py:37-44; kp [T, 2|4] fp32, Wr [C, kd]); the weight gradient -- a [C,T] x [T,kd]
-    contraction over all tokens -- runs as one streaming kernel + a 296-row sum instead of a split-K sgemm."""
+    """theta = kp Wr^T (lightglue.py:37-44; kp [T, 2|4] fp32, Wr [C, kd], C = head_dim / 2 = 32 or 16); the weight
+    gradient -- a [C,T] x [T,kd] contraction over all tokens -- runs as one streaming kernel + a 296-row sum instead of
+    a split-K sgemm."""
 
     @staticmethod
     def forward(ctx, kp, weight):
@@ -180,7 +194,7 @@ class PosencTheta(torch.autograd.Function):
         (kp,) = ctx.saved_tensors
         T, C = g.shape
         kd = kp.shape[1]
-        if C != 32 or kd > 4 or not g.is_cuda:
+        if C not in (16, 32) or kd > 4 or not g.is_cuda:
             return None, g.t() @ kp
         g = g.contiguous()
         nb = _lib.load().lgb200_posenc_wgrad_blocks()

@@ -17,9 +17,9 @@
  *    [batch, rows, cols] row-major for similarity/score matrices.
  *  - `dtype` is LGB200_F32 (full-precision parity path, CUDA cores) or
  *    LGB200_BF16 (bf16 operands, fp32 accumulation, Hopper tensor cores).
- *  - head dimension is 64 (descriptor_dim / num_heads in every
- *    LightGlue configuration, lightglue.py:349); the attention entry points
- *    with an `_hd` suffix also take 32.
+ *  - head dimension is 64 (descriptor_dim / num_heads of the default
+ *    LightGlue configuration, lightglue.py:347); the attention and rotary
+ *    entry points with an `_hd` suffix also take 32.
  */
 #ifndef LGB200_H_
 #define LGB200_H_
@@ -62,6 +62,15 @@ int lgb200_rope_split_fwd(const void* qkv, const float* theta, void* q, void* k,
 int lgb200_rope_split_bwd(const void* dq, const void* dk, const void* dv, const void* q, const void* k,
                           const float* theta, void* dqkv, float* dtheta, int64_t ntok, int H, int dtype,
                           cudaStream_t stream);
+/* The same two at head dimension head_dim = 32 or 64: qkv / dqkv [ntok, H*3*head_dim] with feature
+ * = h*3*head_dim + d*3 + {q,k,v}, theta / dtheta [ntok, head_dim/2], q,k,v [ntok, H*head_dim]; any other value
+ * returns LGB200_ERR_UNSUPPORTED before any CUDA call.  lgb200_rope_split_fwd / _bwd are these with head_dim = 64.
+ * Head dimension 32 is LightGlue with descriptor_dim 128 and 4 heads, or 256 and 8 heads.                       */
+int lgb200_rope_split_fwd_hd(const void* qkv, const float* theta, void* q, void* k, void* v, int64_t ntok, int H,
+                             int dtype, int head_dim, cudaStream_t stream);
+int lgb200_rope_split_bwd_hd(const void* dq, const void* dk, const void* dv, const void* q, const void* k,
+                             const float* theta, void* dqkv, float* dtheta, int64_t ntok, int H, int dtype,
+                             int head_dim, cudaStream_t stream);
 
 /* ---- attention ----------------------------------------------------------------------------------
  * replaces F.scaled_dot_product_attention (lightglue.py:118-121) and the cross-attention einsum/
@@ -261,8 +270,8 @@ int lgb200_colsum_slabs(int64_t rows, int cols);
 /* rowcnt [B,M] = sum_j mask, colcnt [B,N] = sum_i mask of a 0/1 byte mask [B,M,N] (the `gt.sum(2)` / `gt.sum(1)` of
  * lightglue.py:595-600) in one pass; N % 16 == 0, N <= 4096, mask 16-byte aligned; counts are exact.            */
 /* Weight gradient of the position encoder's projection (autograd of lightglue.py:37-44, theta = kp Wr^T):
- * part [lgb200_posenc_wgrad_blocks()][C][KD] per-CTA partials of sum_t g[t][c] kp[t][d]; g [T,C] fp32 with C == 32,
- * kp [T,KD] fp32, KD <= 4.  The caller sums the partials over their first dimension.                          */
+ * part [lgb200_posenc_wgrad_blocks()][C][KD] per-CTA partials of sum_t g[t][c] kp[t][d]; g [T,C] fp32 with C == 32
+ * or 16 (head_dim / 2), kp [T,KD] fp32, KD <= 4.  The caller sums the partials over their first dimension.       */
 int lgb200_posenc_wgrad_blocks(void);
 int lgb200_posenc_wgrad(const float* g, const float* kp, float* part, int64_t T, int C, int KD, cudaStream_t stream);
 int lgb200_mask_counts(const uint8_t* mask, float* rowcnt, float* colcnt, int B, int M, int N, cudaStream_t stream);
