@@ -73,6 +73,9 @@ SIGNATURES = {
     "lgb200_gt_lines_ws_bytes": (_sz, [_i, _i, _i]),
     "lgb200_gt_line_matches": (_i, [_vp] * 10 + [_i] * 5 + [_d] * 3 + [_vp] * 4 + [_i, _i, _i, _vp]),
     "lgb200_adam_flat": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _i, _vp, _f, _vp, _vp, _vp, _vp]),
+    "lgb200_adamw_flat": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _i, _vp, _f, _vp, _vp, _vp, _vp]),
+    "lgb200_sgd_flat": (_i, [_vp, _vp, _vp, _i64, _vp, _f, _f, _f, _i, _f, _i, _vp, _f, _vp, _vp, _vp, _vp]),
+    "lgb200_rmsprop_flat": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _f, _vp, _vp, _vp, _vp]),
     "lgb200_flat_grad_check": (_i, [_vp, _i64, _vp, _vp]),
     "lgb200_flat_grad_norm_ws_bytes": (_sz, [_i64]),
     "lgb200_flat_grad_norm": (_i, [_vp, _i64, _i64, _f, _vp, _f, _vp, _vp, _vp, _vp, _vp]),
@@ -136,6 +139,7 @@ KERNELS_PER_CALL = {
     "lgb200_ot_nll_fwd": 2, "lgb200_ot_nll_bwd": 1, "lgb200_ot_filter_stats": 2, "lgb200_bn_running_update": 1,
     "lgb200_attn_fwd_hd": 1, "lgb200_attn_bwd_hd": 3,  # prep + dQ + dKV (fp32: delta + dQ + dKV)
     "lgb200_rope_split_fwd_hd": 1, "lgb200_rope_split_bwd_hd": 1,
+    "lgb200_adamw_flat": 1, "lgb200_sgd_flat": 1, "lgb200_rmsprop_flat": 1,
 }
 launch_count = 0          # running total of kernels launched through `call`
 timed_entry = None        # entry-point name or a set of names: every call of them is bracketed by CUDA events

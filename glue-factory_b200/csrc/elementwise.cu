@@ -135,6 +135,7 @@ __global__ void __launch_bounds__(256) rope_split_bwd_kernel(const T* __restrict
     b.store(dst + 8);
     d.store(dst + 16);
   }
+  if (!dtheta) return;  // the angles need no gradient (frozen position encoder)
   float4* pt = reinterpret_cast<float4*>(dtheta + tok * (HD / 2) + grp * 4);
   float4 acc = *pt;  // accumulated across layers; this thread is the only writer of these 4 floats
   acc.x += dth[0]; acc.y += dth[1]; acc.z += dth[2]; acc.w += dth[3];
@@ -368,8 +369,13 @@ __global__ void __launch_bounds__(256, 2)
 }
 
 // ---------------------------------------------------------------------------------------------
-// Adam on the flat buffer.  g is multiplied by grad_scale (1/world for the summed all-reduce, or the
-// inverse AMP loss scale).  Matches torch.optim.Adam (no amsgrad, L2 weight decay added to the grad).
+// Optimiser updates on the flat buffers: one kernel body (flat_update_kernel) handles the controls every rule shares
+// -- the skip flag, the device lr / step / loss-scale divisor, grad_scale (1/world for the summed all-reduce) and the
+// per-element lr_scaling factor -- and hands each element to an update rule (AdamRule, AdamWRule, SgdRule,
+// RmspropRule), which restates torch.optim.<X>'s single-tensor arithmetic in its order of operations (no amsgrad, no
+// maximize).  Each thread owns 4 consecutive elements (128-bit loads); the grid depends on n only.
+// fp32 words read + written per element (one more read with lr_scale): Adam / AdamW 7 (p, g, exp_avg, exp_avg_sq in;
+// p, exp_avg, exp_avg_sq out); SGD 3, with momentum 5; RMSprop 5, + 2 with momentum, + 2 centered (9 for both).
 // ---------------------------------------------------------------------------------------------
 struct AdamDev {  // optional device-resident controls (all may be null); see lgb200_adam_flat in lgb200.h
   const int* step;          // 1-based step count (CUDA-graph replay)
@@ -378,49 +384,126 @@ struct AdamDev {  // optional device-resident controls (all may be null); see lg
   const float* found_inf;   // != 0: skip the update entirely (GradScaler.step / the NaN guard of train.py:477-480)
 };
 
-__global__ void __launch_bounds__(256) adam_flat_kernel(float* __restrict__ p, const float* __restrict__ g,
-                                                       float* __restrict__ m, float* __restrict__ v, int64_t n,
-                                                       const float* __restrict__ lr_scale_or_null, float lr,
-                                                       float beta1, float beta2, float eps, float wd, float bc1,
-                                                       float bc2_sqrt, float grad_scale, AdamDev dev) {
+// torch.optim.Adam, L2 weight decay added to the gradient.  bc1 / bc2_sqrt: host bias corrections, recomputed here
+// when the step count lives on the device.
+struct AdamRule {
+  float beta1, beta2, eps, wd, bc1, bc2_sqrt;
+  __device__ void prepare(const int* step) {
+    if (step) {
+      const float t = (float)(*step);
+      bc1 = 1.f - powf(beta1, t);
+      bc2_sqrt = sqrtf(1.f - powf(beta2, t));
+    }
+  }
+  __device__ void operator()(float& p, float g, float grad_scale, float l, float& m, float& v, float&) const {
+    float gr = g * grad_scale + wd * p;
+    m = beta1 * m + (1.f - beta1) * gr;
+    v = beta2 * v + (1.f - beta2) * gr * gr;
+    const float denom = sqrtf(v) / bc2_sqrt + eps;
+    p -= (l / bc1) * (m / denom);
+  }
+};
+
+// torch.optim.AdamW: decoupled decay p *= 1 - lr_group * wd before the Adam step (lr_group includes lr_scaling).
+struct AdamWRule : AdamRule {
+  __device__ void operator()(float& p, float g, float grad_scale, float l, float& m, float& v, float&) const {
+    p *= 1.f - l * wd;
+    const float gr = g * grad_scale;
+    m = beta1 * m + (1.f - beta1) * gr;
+    v = beta2 * v + (1.f - beta2) * gr * gr;
+    const float denom = sqrtf(v) / bc2_sqrt + eps;
+    p -= (l / bc1) * (m / denom);
+  }
+};
+
+// torch.optim.SGD.  On the first step (step count 1) the momentum buffer becomes the gradient itself, undampened.
+struct SgdRule {
+  float momentum, dampening, wd;
+  int nesterov, step;
+  __device__ void prepare(const int* step_dev) {
+    if (step_dev) step = *step_dev;
+  }
+  __device__ void operator()(float& p, float g, float grad_scale, float l, float& buf, float&, float&) const {
+    float gr = g * grad_scale;
+    if (wd != 0.f) gr = gr + wd * p;
+    if (momentum != 0.f) {
+      buf = step <= 1 ? gr : momentum * buf + (1.f - dampening) * gr;
+      gr = nesterov ? gr + momentum * buf : buf;
+    }
+    p = p + -l * gr;
+  }
+};
+
+// torch.optim.RMSprop (step count unused by the arithmetic).
+struct RmspropRule {
+  float alpha, eps, wd, momentum;
+  int centered;
+  __device__ void prepare(const int*) {}
+  __device__ void operator()(float& p, float g, float grad_scale, float l, float& sq, float& buf, float& gavg) const {
+    float gr = g * grad_scale;
+    if (wd != 0.f) gr = gr + wd * p;
+    sq = sq * alpha + (1.f - alpha) * gr * gr;
+    float avg;
+    if (centered) {
+      gavg = gavg + (1.f - alpha) * (gr - gavg);  // lerp with weight 1 - alpha < 0.5
+      avg = sqrtf(sq - gavg * gavg);
+    } else {
+      avg = sqrtf(sq);
+    }
+    avg = avg + eps;
+    if (momentum > 0.f) {
+      buf = buf * momentum + gr / avg;
+      p = p + -l * buf;
+    } else {
+      p = p + -l * (gr / avg);
+    }
+  }
+};
+
+// s0..s2: the rule's state buffers in its argument order; a null one is neither read nor written.
+template <class Rule>
+__global__ void __launch_bounds__(256) flat_update_kernel(float* __restrict__ p, const float* __restrict__ g,
+                                                         float* __restrict__ s0, float* __restrict__ s1,
+                                                         float* __restrict__ s2, int64_t n,
+                                                         const float* __restrict__ lr_scale_or_null, float lr,
+                                                         float grad_scale, Rule rule, AdamDev dev) {
   const int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
   if (i0 >= n) return;
   if (dev.found_inf && *dev.found_inf != 0.f) return;  // whole grid takes the same branch
-  if (dev.step) {  // step count lives in device memory (CUDA-graph replay): bias corrections computed here
-    const float t = (float)(*dev.step);
-    bc1 = 1.f - powf(beta1, t);
-    bc2_sqrt = sqrtf(1.f - powf(beta2, t));
-  }
+  rule.prepare(dev.step);
   if (dev.lr) lr = *dev.lr;
   if (dev.loss_scale) grad_scale *= 1.f / *dev.loss_scale;
+  float* s[3] = {s0, s1, s2};
   if (i0 + 4 <= n) {
     float4 pp = *reinterpret_cast<float4*>(p + i0), gg = *reinterpret_cast<const float4*>(g + i0);
-    float4 mm = *reinterpret_cast<float4*>(m + i0), vv = *reinterpret_cast<float4*>(v + i0);
-    float P[4] = {pp.x, pp.y, pp.z, pp.w}, G[4] = {gg.x, gg.y, gg.z, gg.w};
-    float Mm[4] = {mm.x, mm.y, mm.z, mm.w}, V[4] = {vv.x, vv.y, vv.z, vv.w};
+    float P[4] = {pp.x, pp.y, pp.z, pp.w}, G[4] = {gg.x, gg.y, gg.z, gg.w}, S[3][4] = {};
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+      if (s[k]) {
+        const float4 x = *reinterpret_cast<float4*>(s[k] + i0);
+        S[k][0] = x.x, S[k][1] = x.y, S[k][2] = x.z, S[k][3] = x.w;
+      }
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       const float l = lr_scale_or_null ? lr * lr_scale_or_null[i0 + e] : lr;
-      float gr = G[e] * grad_scale + wd * P[e];
-      Mm[e] = beta1 * Mm[e] + (1.f - beta1) * gr;
-      V[e] = beta2 * V[e] + (1.f - beta2) * gr * gr;
-      const float denom = sqrtf(V[e]) / bc2_sqrt + eps;
-      P[e] -= (l / bc1) * (Mm[e] / denom);
+      rule(P[e], G[e], grad_scale, l, S[0][e], S[1][e], S[2][e]);
     }
     *reinterpret_cast<float4*>(p + i0) = make_float4(P[0], P[1], P[2], P[3]);
-    *reinterpret_cast<float4*>(m + i0) = make_float4(Mm[0], Mm[1], Mm[2], Mm[3]);
-    *reinterpret_cast<float4*>(v + i0) = make_float4(V[0], V[1], V[2], V[3]);
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+      if (s[k]) *reinterpret_cast<float4*>(s[k] + i0) = make_float4(S[k][0], S[k][1], S[k][2], S[k][3]);
   } else {
     for (int64_t i = i0; i < n; ++i) {
       const float l = lr_scale_or_null ? lr * lr_scale_or_null[i] : lr;
-      float gr = g[i] * grad_scale + wd * p[i];
-      m[i] = beta1 * m[i] + (1.f - beta1) * gr;
-      v[i] = beta2 * v[i] + (1.f - beta2) * gr * gr;
-      const float denom = sqrtf(v[i]) / bc2_sqrt + eps;
-      p[i] -= (l / bc1) * (m[i] / denom);
+      float x[3] = {s0 ? s0[i] : 0.f, s1 ? s1[i] : 0.f, s2 ? s2[i] : 0.f};
+      rule(p[i], g[i], grad_scale, l, x[0], x[1], x[2]);
+      for (int k = 0; k < 3; ++k)
+        if (s[k]) s[k][i] = x[k];
     }
   }
 }
+
+static unsigned flat_update_grid(int64_t n) { return (unsigned)(((n + 3) / 4 + 255) / 256); }
 
 // found_inf = 1 when any of g[0..n) is non-finite (the flat gradient after the all-reduce; the trainer appends the
 // loss as one more element), else 0 -- GradScaler.unscale_'s inf check (train.py:490-512) without the host sync.
@@ -1032,15 +1115,18 @@ __global__ void __launch_bounds__(256) head_token_bwd_kernel(const float* __rest
       const int col = ch * 256 + lane * 8;
       if (col < D) {
         const Vec8<float> v = Vec8<float>::load(x + tok * D + col);
-        const Vec8<T> g = Vec8<T>::load(dmdw + tok * D + col);
-        Vec8<float> o;
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
-          o.v[e] = fmaf(dz.x, m[ch].v[e], g.v[e]);
           a0[ch][e] = fmaf(dz.x, v.v[e], a0[ch][e]);
           a1[ch][e] = fmaf(dz.y, v.v[e], a1[ch][e]);
         }
-        o.store(dx + tok * D + col);
+        if (dx) {  // null: x needs no gradient (every layer up to this head is frozen)
+          const Vec8<T> g = Vec8<T>::load(dmdw + tok * D + col);
+          Vec8<float> o;
+#pragma unroll
+          for (int e = 0; e < 8; ++e) o.v[e] = fmaf(dz.x, m[ch].v[e], g.v[e]);
+          o.store(dx + tok * D + col);
+        }
       }
     }
   }
@@ -1298,7 +1384,7 @@ int lgb200_rope_split_bwd_hd(const void* dq, const void* dk, const void* dv, con
                              int head_dim, cudaStream_t stream) {
   LGB_REQUIRE(head_dim == 32 || head_dim == 64, kErrUnsupported, "rope_split_bwd: head_dim %d (built for 32 and 64)",
               head_dim);
-  LGB_REQUIRE(dq && dk && dv && q && k && theta && dqkv && dtheta, kErrInvalid, "rope_split_bwd: null pointer");
+  LGB_REQUIRE(dq && dk && dv && q && k && theta && dqkv, kErrInvalid, "rope_split_bwd: null pointer");
   LGB_REQUIRE(ntok > 0 && H > 0, kErrInvalid, "rope_split_bwd: empty input");
   LGB_REQUIRE(aligned16({dq, dk, dv, q, k, theta, dqkv, dtheta}), kErrInvalid,
               "rope_split_bwd: misaligned pointer (16 bytes needed)");
@@ -1401,11 +1487,63 @@ int lgb200_adam_flat(float* p, const float* g, float* m, float* v, int64_t n, co
               kErrInvalid, "adam_flat: buffers must be 16-byte aligned");
   const float bc1 = step >= 1 ? 1.f - powf(beta1, (float)step) : 1.f;
   const float bc2s = step >= 1 ? sqrtf(1.f - powf(beta2, (float)step)) : 1.f;
-  const unsigned grid = (unsigned)(((n + 3) / 4 + 255) / 256);
-  AdamDev dev{step_dev, lr_dev, loss_scale_dev, found_inf_dev};
-  adam_flat_kernel<<<grid, 256, 0, stream>>>(p, g, m, v, n, lr_scale_per_elem, lr, beta1, beta2, eps, weight_decay, bc1,
-                                             bc2s, grad_scale, dev);
+  const AdamRule rule{beta1, beta2, eps, weight_decay, bc1, bc2s};
+  flat_update_kernel<<<flat_update_grid(n), 256, 0, stream>>>(p, g, m, v, nullptr, n, lr_scale_per_elem, lr, grad_scale,
+                                                              rule, AdamDev{step_dev, lr_dev, loss_scale_dev,
+                                                                            found_inf_dev});
   return check_launch("adam_flat");
+}
+
+int lgb200_adamw_flat(float* p, const float* g, float* m, float* v, int64_t n, const float* lr_scale_per_elem,
+                      float lr, float beta1, float beta2, float eps, float weight_decay, int step, const int* step_dev,
+                      float grad_scale, const float* lr_dev, const float* loss_scale_dev, const float* found_inf_dev,
+                      cudaStream_t stream) {
+  LGB_REQUIRE(p && g && m && v, kErrInvalid, "adamw_flat: null pointer");
+  LGB_REQUIRE(n > 0 && (step >= 1 || step_dev), kErrInvalid, "adamw_flat: bad n/step");
+  LGB_REQUIRE(aligned16({p, g, m, v}), kErrInvalid, "adamw_flat: buffers must be 16-byte aligned");
+  AdamWRule rule;
+  rule.beta1 = beta1, rule.beta2 = beta2, rule.eps = eps, rule.wd = weight_decay;
+  rule.bc1 = step >= 1 ? 1.f - powf(beta1, (float)step) : 1.f;
+  rule.bc2_sqrt = step >= 1 ? sqrtf(1.f - powf(beta2, (float)step)) : 1.f;
+  flat_update_kernel<<<flat_update_grid(n), 256, 0, stream>>>(p, g, m, v, nullptr, n, lr_scale_per_elem, lr, grad_scale,
+                                                              rule, AdamDev{step_dev, lr_dev, loss_scale_dev,
+                                                                            found_inf_dev});
+  return check_launch("adamw_flat");
+}
+
+int lgb200_sgd_flat(float* p, const float* g, float* momentum_buffer, int64_t n, const float* lr_scale_per_elem,
+                    float lr, float momentum, float dampening, int nesterov, float weight_decay, int step,
+                    const int* step_dev, float grad_scale, const float* lr_dev, const float* loss_scale_dev,
+                    const float* found_inf_dev, cudaStream_t stream) {
+  LGB_REQUIRE(p && g, kErrInvalid, "sgd_flat: null pointer");
+  LGB_REQUIRE((momentum != 0.f) == (momentum_buffer != nullptr), kErrInvalid,
+              "sgd_flat: momentum_buffer must be given exactly when momentum != 0");
+  LGB_REQUIRE(!nesterov || (momentum > 0.f && dampening == 0.f), kErrInvalid,
+              "sgd_flat: nesterov needs momentum > 0 and zero dampening");
+  LGB_REQUIRE(n > 0 && (step >= 1 || step_dev), kErrInvalid, "sgd_flat: bad n/step");
+  LGB_REQUIRE(aligned16({p, g, momentum_buffer}), kErrInvalid, "sgd_flat: buffers must be 16-byte aligned");
+  const SgdRule rule{momentum, dampening, weight_decay, nesterov, step};
+  flat_update_kernel<<<flat_update_grid(n), 256, 0, stream>>>(p, g, momentum_buffer, nullptr, nullptr, n,
+                                                              lr_scale_per_elem, lr, grad_scale, rule,
+                                                              AdamDev{step_dev, lr_dev, loss_scale_dev, found_inf_dev});
+  return check_launch("sgd_flat");
+}
+
+int lgb200_rmsprop_flat(float* p, const float* g, float* square_avg, float* momentum_buffer, float* grad_avg,
+                        int64_t n, const float* lr_scale_per_elem, float lr, float alpha, float eps,
+                        float weight_decay, float momentum, float grad_scale, const float* lr_dev,
+                        const float* loss_scale_dev, const float* found_inf_dev, cudaStream_t stream) {
+  LGB_REQUIRE(p && g && square_avg, kErrInvalid, "rmsprop_flat: null pointer");
+  LGB_REQUIRE((momentum > 0.f) == (momentum_buffer != nullptr), kErrInvalid,
+              "rmsprop_flat: momentum_buffer must be given exactly when momentum > 0");
+  LGB_REQUIRE(n > 0, kErrInvalid, "rmsprop_flat: bad n");
+  LGB_REQUIRE(aligned16({p, g, square_avg, momentum_buffer, grad_avg}), kErrInvalid,
+              "rmsprop_flat: buffers must be 16-byte aligned");
+  const RmspropRule rule{alpha, eps, weight_decay, momentum, grad_avg != nullptr};
+  flat_update_kernel<<<flat_update_grid(n), 256, 0, stream>>>(p, g, square_avg, momentum_buffer, grad_avg, n,
+                                                              lr_scale_per_elem, lr, grad_scale, rule,
+                                                              AdamDev{nullptr, lr_dev, loss_scale_dev, found_inf_dev});
+  return check_launch("rmsprop_flat");
 }
 
 int lgb200_flat_grad_check(const float* g, int64_t n, float* found_inf, cudaStream_t stream) {
@@ -1482,8 +1620,8 @@ int lgb200_head_token_fwd(const float* x, const float* wm, const float* bm, cons
 int lgb200_head_token_bwd(const float* x, const void* dmdw, const float* dzt, const float* wm, float* dx, float* dW2,
                           float* db2, float* ws, unsigned* counter, int64_t ntok, int D, int dtype,
                           cudaStream_t stream) {
-  LGB_REQUIRE(x && dmdw && dzt && wm && dx && dW2 && db2 && ws && counter && ntok > 0, kErrInvalid,
-              "head_token_bwd: bad arguments");
+  LGB_REQUIRE(x && dzt && wm && dW2 && db2 && ws && counter && ntok > 0 && (dmdw == nullptr) == (dx == nullptr),
+              kErrInvalid, "head_token_bwd: bad arguments");
   LGB_REQUIRE(D % 8 == 0 && D > 0 && D <= 512, kErrUnsupported, "head_token_bwd: D=%d not a multiple of 8 in (0,512]", D);
 #define LGB_HT_BWD(T, NCH)                                                                                     \
   head_token_bwd_kernel<T, NCH><<<kHeadBwdParts, 256, 0, stream>>>(x, (const T*)dmdw, dzt, wm, dx, dW2, db2, ws, \

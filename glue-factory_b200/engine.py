@@ -311,44 +311,49 @@ class LayerFn(torch.autograd.Function):
             else:
                 dx = dx + extra
                 dy2 = dx.to(cdt)
-        gv = fp.direct_views(slot) if fp is not None else [None] * 22  # LAYER_PARAMS order
+        gv = fp.direct_views(slot) if fp is not None else [None] * 22  # LAYER_PARAMS order; None for a frozen slot
+        need = ctx.needs_input_grad[8:]  # per LAYER_PARAMS slot: a frozen parameter's GEMM / column sum is skipped
+        wg = lambda i, d, a: _wgrad(d, a, gv[i]) if need[i] else None  # noqa: E731
+        bg = lambda i, d: _bgrad(d) if need[i] else None  # noqa: E731
         # ---- cross block
-        dW3c, db3c = _wgrad(dy2, gg, gv[20]), _bgrad(dy2)
+        dW3c, db3c = wg(20, dy2, gg), bg(21, dy2)
         dgg = _dgrad(dy2, W3c)
         dh2, dg2, dbe2, db0c = ops.ln_gelu_bwd(dgg, h2, g2, be2, mean2, rstd2, want_dxsum=True)
         del dgg
-        dW0c = _wgrad(dh2, cat2, gv[16])
+        dW0c = wg(16, dh2, cat2)
         dmsg2 = _dgrad(dh2, W0c[:, D:])
         dx1 = _dgrad_acc(dx, dh2, W0c[:, :D])  # fp32 accumulation of the residual-stream gradient
         del dh2
-        dWout, dbout = _wgrad(dmsg2, m, gv[14]), _bgrad(dmsg2)
+        dWout, dbout = wg(14, dmsg2, m), bg(15, dmsg2)
         dm = _dgrad(dmsg2, Wout)
         dqk, dvv = _attend_bwd_shared_qk(qk, vv, m, lse2, dm, sizes, H)
-        dWqk, dbqk = _wgrad(dqk, x1_16, gv[10]), _bgrad(dqk)
-        dWv, dbv = _wgrad(dvv, x1_16, gv[12]), _bgrad(dvv)
+        dWqk, dbqk = wg(10, dqk, x1_16), bg(11, dqk)
+        dWv, dbv = wg(12, dvv, x1_16), bg(13, dvv)
         dx1 = _dgrad_acc(dx1, dqk, Wqk)
         dx1 = _dgrad_acc(dx1, dvv, Wv)
         # ---- self block
         dy = dx1.to(cdt)
-        dW3, db3 = _wgrad(dy, g, gv[8]), _bgrad(dy)
+        dW3, db3 = wg(8, dy, g), bg(9, dy)
         dg = _dgrad(dy, W3)
         dh, dg1, dbe1, db0 = ops.ln_gelu_bwd(dg, h, g1, be1, mean1, rstd1, want_dxsum=True)
         del dg
-        dW0 = _wgrad(dh, cat1, gv[4])
+        dW0 = wg(4, dh, cat1)
         dmsg = _dgrad(dh, W0[:, D:])
-        dx0 = _dgrad_acc(dx1, dh, W0[:, :D])
+        dx0 = _dgrad_acc(dx1, dh, W0[:, :D]) if ctx.needs_input_grad[0] else None
         del dh
-        dWo, dbo = _wgrad(dmsg, att, gv[2]), _bgrad(dmsg)
+        dWo, dbo = wg(2, dmsg, att), bg(3, dmsg)
         datt = _dgrad(dmsg, Wo)
         dq, dk, dv = _attend_bwd(q, k, v, att, lse1, datt, sizes, H, cross=False)
-        dqkv, dtheta = ops.rope_bwd(dq, dk, dv, q, k, theta, H)
-        dWqkv, dbqkv = _wgrad(dqkv, x16, gv[0]), _bgrad(dqkv)
-        dx0 = _dgrad_acc(dx0, dqkv, Wqkv)
+        dqkv, dtheta = ops.rope_bwd(dq, dk, dv, q, k, theta, H, need_dtheta=ctx.needs_input_grad[1])
+        dWqkv, dbqkv = wg(0, dqkv, x16), bg(1, dqkv)
+        if dx0 is not None:
+            dx0 = _dgrad_acc(dx0, dqkv, Wqkv)
         grads = (dWqkv, dbqkv, dWo, dbo, dW0, db0, dg1, dbe1, dW3, db3,
                  dWqk, dbqk, dWv, dbv, dWout, dbout, dW0c, db0c, dg2, dbe2, dW3c, db3c)
+        grads = tuple(gr if need[i] else None for i, gr in enumerate(grads))  # the LayerNorm kernel's by-products
         if fp is not None:
-            # the nine weight gradients are already in place; the 13 vectors go in with one multi-tensor copy
-            small = [i for i in range(22) if grads[i].data_ptr() != gv[i].data_ptr()]
+            # the trainable weight gradients are already in place; the vectors go in with one multi-tensor copy
+            small = [i for i in range(22) if grads[i] is not None and grads[i].data_ptr() != gv[i].data_ptr()]
             torch._foreach_copy_([gv[i] for i in small], [grads[i].view_as(gv[i]) for i in small])
             grads = (None,) * 22
         return (dx0, dtheta, None, None, None, None, None, None) + grads
@@ -431,21 +436,32 @@ class HeadFn(torch.autograd.Function):
                  ops.ptr(num_pos), ops.ptr(num_neg), float(bal), ops.ptr(g_nll), ops.ptr(g_conf), ops.ptr(dzt), B, M, N,
                  ops.stream_ptr())
         # similarity: dsim = gc (2 gt - softmax_row * rowcnt - softmax_col * colcnt), gc includes d^-1/2
-        gc = (g_nll * (-bal * alpha) / num_pos).contiguous()
-        md0, md1 = md[:t0].view(B, M, D), md[t0:].view(B, N, D)
-        if fused:
-            # dsim is recomputed tile by tile and contracted with the other image's descriptors in the same kernel
-            dmd = torch.empty(t0 + B * N, D, device=x.device, dtype=cdt)
-            ops.assign_fused_bwd(md0, md1, alpha, lse_row, lse_col, gt_u8, sim, gc, rowcnt, colcnt, dmd[:t0], dmd[t0:])
-        else:
-            dmd0, dmd1 = assign_unfused_bwd(md0, md1, sim, lse_row, lse_col, gt_u8, gc, rowcnt, colcnt)
-            dmd = torch.cat([dmd0.reshape(t0, D), dmd1.reshape(B * N, D)], 0)
-        dWfp, dbfp = _wgrad(dmd, x16), _bgrad(dmd)
-        # dx = dmd W_fp + dzt[:,0] wm (the token-confidence head reads a detached x, lightglue.py:82-83), dW2, db2
-        dx, dW2, db2 = ops.head_token_bwd(x, _dgrad(dmd, wfp), dzt, wm.view(-1))
-        dwt, dbt = (dW2[1:2], db2[1:2]) if has_tok else (None, None)
-        if ctx.stash is not None:
+        # frozen parameters (and an x that needs no gradient, when every layer up to this head is frozen) are skipped
+        need_x, need_wfp, need_bfp, need_wm, need_bm, need_wt, need_bt = (ctx.needs_input_grad[i]
+                                                                           for i in (0, 9, 10, 11, 12, 13, 14))
+        dmd = None
+        if need_x or need_wfp or need_bfp:
+            gc = (g_nll * (-bal * alpha) / num_pos).contiguous()
+            md0, md1 = md[:t0].view(B, M, D), md[t0:].view(B, N, D)
+            if fused:
+                # dsim is recomputed tile by tile and contracted with the other image's descriptors in the same kernel
+                dmd = torch.empty(t0 + B * N, D, device=x.device, dtype=cdt)
+                ops.assign_fused_bwd(md0, md1, alpha, lse_row, lse_col, gt_u8, sim, gc, rowcnt, colcnt, dmd[:t0],
+                                     dmd[t0:])
+            else:
+                dmd0, dmd1 = assign_unfused_bwd(md0, md1, sim, lse_row, lse_col, gt_u8, gc, rowcnt, colcnt)
+                dmd = torch.cat([dmd0.reshape(t0, D), dmd1.reshape(B * N, D)], 0)
+        dWfp = _wgrad(dmd, x16) if need_wfp else None
+        dbfp = _bgrad(dmd) if need_bfp else None
+        dx = dW2 = db2 = None
+        if need_x or need_wm or need_bm or need_wt or need_bt:
+            # dx = dmd W_fp + dzt[:,0] wm (the token-confidence head reads a detached x, lightglue.py:82-83), dW2, db2
+            dx, dW2, db2 = ops.head_token_bwd(x, _dgrad(dmd, wfp) if need_x else None, dzt, wm.view(-1))
+        pick = lambda t, row, want: t[row:row + 1] if want else None  # noqa: E731
+        dwm, dbm = pick(dW2, 0, need_wm), pick(db2, 0, need_bm)
+        dwt, dbt = (pick(dW2, 1, need_wt), pick(db2, 1, need_bt)) if has_tok else (None, None)
+        if ctx.stash is not None and dx is not None:
             d, key = ctx.stash
             d[key] = dx if key not in d else d[key] + dx
             dx = None
-        return dx, None, None, None, None, None, None, None, None, dWfp, dbfp, dW2[0:1], db2[0:1], dwt, dbt
+        return dx, None, None, None, None, None, None, None, None, dWfp, dbfp, dwm, dbm, dwt, dbt

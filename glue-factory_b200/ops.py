@@ -53,14 +53,15 @@ def rope_fwd(qkv, theta, H):
     return q, k, v
 
 
-def rope_bwd(dq, dk, dv, q, k, theta, H, dtheta=None):
-    """Returns dqkv; ACCUMULATES into dtheta (allocated zeroed when None)."""
+def rope_bwd(dq, dk, dv, q, k, theta, H, dtheta=None, need_dtheta=True):
+    """Returns (dqkv, dtheta); ACCUMULATES into dtheta (allocated zeroed when None).  need_dtheta=False: the angles
+    need no gradient (frozen position encoder), none is computed and dtheta is returned as None."""
     T = q.shape[0]
     hd = q.shape[1] // H
     assert q.shape[1] == H * hd and theta.shape == (T, hd // 2), (tuple(q.shape), tuple(theta.shape), H)
     dq, dk, dv = (g.contiguous() for g in (dq, dk, dv))
     dqkv = torch.empty(T, H * 3 * hd, device=q.device, dtype=q.dtype)
-    if dtheta is None:
+    if dtheta is None and need_dtheta:
         dtheta = torch.zeros_like(theta)
     args = (ptr(dq), ptr(dk), ptr(dv), ptr(q), ptr(k), ptr(theta), ptr(dqkv), ptr(dtheta), T, H, _code(q.dtype))
     if hd == 64:
@@ -457,8 +458,9 @@ def linear(a, w, bias=None, out=None, out_dtype=torch.bfloat16, w_is_kn=False, a
 class LinearFn(torch.autograd.Function):
     """nn.Linear on the library's GEMMs with autograd: x [T, in] bf16, weight [out, in] / bias [out] fp32 parameters.
     forward y = x W^T + b (bf16 out, fp32 bias in the epilogue); backward dgrad (bf16), split-K wgrad (fp32), bias
-    gradient by the column-sum kernel.  Used for LightGlue's input_proj and dense final head in bf16, and for
-    GlueStick's 1x1 convolutions."""
+    gradient by the column-sum kernel; the weight and bias gradients of a frozen (requires_grad=False) weight or bias
+    are not computed.  Used for LightGlue's input_proj and dense final head in bf16, and for GlueStick's and
+    SuperGlue's 1x1 convolutions."""
 
     @staticmethod
     def forward(ctx, x, weight, bias):
@@ -470,8 +472,9 @@ class LinearFn(torch.autograd.Function):
     def backward(ctx, dy):
         x, w16 = ctx.saved_tensors
         dy = dy.contiguous()
-        dx = linear(dy, w16, w_is_kn=True) if ctx.needs_input_grad[0] else None
-        return dx, wgrad_bf16(dy, x), colsum(dy)
+        need = ctx.needs_input_grad
+        dx = linear(dy, w16, w_is_kn=True) if need[0] else None
+        return dx, wgrad_bf16(dy, x) if need[1] else None, colsum(dy) if need[2] else None
 
 
 # ------------------------------------------------------------------------------------------------
@@ -729,20 +732,22 @@ def head_token_fwd(x, wm, bm, wt, bt, cdt):
 
 
 def head_token_bwd(x, dmdw, dzt, wm):
-    """-> (dx [T,D] fp32 = float(dmdw) + dzt[:,0] wm, dW2 [2,D] = dzt^T x, db2 [2])."""
-    _chk(x, torch.float32), _chk(dmdw), _chk(dzt, torch.float32)
+    """-> (dx [T,D] fp32 = float(dmdw) + dzt[:,0] wm, dW2 [2,D] = dzt^T x, db2 [2]); dmdw None: dx is None."""
+    _chk(x, torch.float32), _chk(dzt, torch.float32)
+    if dmdw is not None:
+        _chk(dmdw)
     T, D = x.shape
     dev = x.device
     cnt = _head_token_counters.get(dev)
     if cnt is None:
         cnt = _head_token_counters[dev] = torch.zeros(1, device=dev, dtype=torch.int32)
-    dx = torch.empty_like(x)
+    dx = torch.empty_like(x) if dmdw is not None else None
     dW2 = torch.empty(2, D, device=dev, dtype=torch.float32)
     db2 = torch.empty(2, device=dev, dtype=torch.float32)
     ws = torch.empty(_lib.load().lgb200_head_token_bwd_ws_floats(D), device=dev, dtype=torch.float32)
     wmf = wm.detach().float().contiguous()
     call("lgb200_head_token_bwd", ptr(x), ptr(dmdw), ptr(dzt), ptr(wmf), ptr(dx), ptr(dW2), ptr(db2), ptr(ws), ptr(cnt),
-         T, D, _code(dmdw.dtype), stream_ptr())
+         T, D, _code(dmdw.dtype if dmdw is not None else x.dtype), stream_ptr())
     return dx, dW2, db2
 
 
@@ -926,6 +931,40 @@ def adam_flat_(p, g, m, v, step, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=
     call("lgb200_adam_flat", ptr(p), ptr(g), ptr(m), ptr(v), p.numel(), ptr(lr_scale_per_elem), float(lr),
          float(betas[0]), float(betas[1]), float(eps), float(weight_decay), int(step), ptr(step_dev), float(grad_scale),
          ptr(lr_dev), ptr(loss_scale_dev), ptr(found_inf_dev), stream_ptr())
+
+
+def adamw_flat_(p, g, m, v, step, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01, grad_scale=1.0,
+                lr_scale_per_elem=None, step_dev=None, lr_dev=None, loss_scale_dev=None, found_inf_dev=None):
+    """In-place torch.optim.AdamW on flat fp32 buffers; arguments as adam_flat_ (lgb200_adamw_flat)."""
+    for t in (p, g, m, v):
+        _chk(t, torch.float32)
+    call("lgb200_adamw_flat", ptr(p), ptr(g), ptr(m), ptr(v), p.numel(), ptr(lr_scale_per_elem), float(lr),
+         float(betas[0]), float(betas[1]), float(eps), float(weight_decay), int(step), ptr(step_dev), float(grad_scale),
+         ptr(lr_dev), ptr(loss_scale_dev), ptr(found_inf_dev), stream_ptr())
+
+
+def sgd_flat_(p, g, momentum_buffer, step, lr, momentum=0.0, dampening=0.0, nesterov=False, weight_decay=0.0,
+              grad_scale=1.0, lr_scale_per_elem=None, step_dev=None, lr_dev=None, loss_scale_dev=None,
+              found_inf_dev=None):
+    """In-place torch.optim.SGD on flat fp32 buffers (lgb200_sgd_flat): momentum_buffer is None exactly when
+    momentum == 0; at step count 1 the buffer is set to the gradient."""
+    for t in (p, g) + ((momentum_buffer,) if momentum_buffer is not None else ()):
+        _chk(t, torch.float32)
+    call("lgb200_sgd_flat", ptr(p), ptr(g), ptr(momentum_buffer), p.numel(), ptr(lr_scale_per_elem), float(lr),
+         float(momentum), float(dampening), int(bool(nesterov)), float(weight_decay), int(step), ptr(step_dev),
+         float(grad_scale), ptr(lr_dev), ptr(loss_scale_dev), ptr(found_inf_dev), stream_ptr())
+
+
+def rmsprop_flat_(p, g, square_avg, momentum_buffer, grad_avg, lr, alpha=0.99, eps=1e-8, weight_decay=0.0,
+                  momentum=0.0, grad_scale=1.0, lr_scale_per_elem=None, lr_dev=None, loss_scale_dev=None,
+                  found_inf_dev=None):
+    """In-place torch.optim.RMSprop on flat fp32 buffers (lgb200_rmsprop_flat): momentum_buffer is None exactly when
+    momentum == 0, grad_avg is given for `centered`."""
+    for t in (p, g, square_avg) + tuple(t for t in (momentum_buffer, grad_avg) if t is not None):
+        _chk(t, torch.float32)
+    call("lgb200_rmsprop_flat", ptr(p), ptr(g), ptr(square_avg), ptr(momentum_buffer), ptr(grad_avg), p.numel(),
+         ptr(lr_scale_per_elem), float(lr), float(alpha), float(eps), float(weight_decay), float(momentum),
+         float(grad_scale), ptr(lr_dev), ptr(loss_scale_dev), ptr(found_inf_dev), stream_ptr())
 
 
 def flat_grad_check(g, found_inf):

@@ -9,12 +9,19 @@ changes SURVEY.md section 2.2 (C1) calls for:
     gradient buffer (the nn.Parameters are views), so the gradient exchange is a
     single `all_reduce` over NVLink per optimiser step instead of DDP's bucketed
     hooks plus the extra scalar all-reduce of train.py:483-488;
-  * Adam runs as one kernel over the flat buffers (`lgb200_adam_flat`), with the
-    1/world averaging folded into it.
+  * the optimiser (Adam, AdamW, SGD or RMSprop: train.optimizer) runs as one kernel
+    over the flat buffers (`lgb200_<rule>_flat`), with the 1/world averaging folded
+    into it.
+
+Frozen parameters (train.opt_regexp, or requires_grad=False) stay in the flat
+parameter buffer, behind the trainable ones, but are outside the gradient buffer,
+the all-reduce and the optimiser; the backward skips their gradients.
 
 The matcher is per-pair, so image pairs shard across ranks with no other
 collective (SURVEY.md section 8e).
 """
+import re
+
 import torch
 import torch.distributed as dist
 
@@ -25,27 +32,38 @@ _ALIGN = 64  # elements; keeps every parameter view 256-byte aligned
 
 
 class FlatParams:
-    """Re-homes the trainable parameters of `module` into one flat buffer (+ flat grad buffer)."""
+    """Re-homes the parameters of `module` into one flat buffer (+ flat grad buffer).
+
+    The trainable parameters (`params`) come first and occupy flat[:numel]; the frozen ones (requires_grad=False,
+    `frozen`) follow, so that the one cast kernel of shadow_bf16 keeps refreshing their bf16 views too, while the
+    gradient buffer, the all-reduce and the optimiser cover the trainable range only."""
 
     def __init__(self, module):
         self.params = [p for p in module.parameters() if p.requires_grad]
+        self.frozen = [p for p in module.parameters() if not p.requires_grad]
         assert self.params, "no trainable parameters"
         dev, dt = self.params[0].device, torch.float32
         self.offsets, n = [], 0
-        for p in self.params:
+        for p in self.params + self.frozen:
             assert p.dtype == dt and p.device == dev
             self.offsets.append(n)
             n += (p.numel() + _ALIGN - 1) // _ALIGN * _ALIGN
-        self.numel = n
+            if len(self.offsets) == len(self.params):
+                self.numel = n  # the trainable range
+        self.frozen_offsets = self.offsets[len(self.params):]
+        del self.offsets[len(self.params):]
+        self.numel_all = n
         self.flat = torch.zeros(n, device=dev, dtype=dt)
         # one extra aligned slot behind the gradients carries the step's loss through the SAME all-reduce, so that
         # every rank sees a non-finite loss of any rank and skips the update together (train.py:477-488)
+        n = self.numel
         self.grad_ext = torch.zeros(n + _ALIGN, device=dev, dtype=dt)
         self.grad = self.grad_ext[:n]
         self.loss_slot = self.grad_ext[n:n + 1]
-        for p, off in zip(self.params, self.offsets):
+        for p, off in zip(self.params + self.frozen, self.offsets + self.frozen_offsets):
             self.flat[off:off + p.numel()].copy_(p.data.reshape(-1))
             p.data = self.flat[off:off + p.numel()].view_as(p)
+        for p, off in zip(self.params, self.offsets):
             p.grad = self.grad[off:off + p.numel()].view_as(p)
         # bf16 shadow of the whole buffer (one cast kernel per step) for the tensor-core GEMMs
         self._names = {id(p): n for n, p in module.named_parameters()}
@@ -59,11 +77,12 @@ class FlatParams:
         module._b200_flat = self
 
     def enable_direct(self, groups):
-        """groups: lists of parameters (e.g. one transformer layer) whose backward writes the flat gradient buffer."""
+        """groups: lists of parameters (e.g. one transformer layer) whose backward writes the flat gradient buffer.
+        A frozen parameter has no gradient slot: its entry in the group's view list is None."""
         index = {id(p): i for i, p in enumerate(self.params)}
         for params in groups:
-            self.direct_groups.append([self.grad_views[index[id(p)]] for p in params])
-            self._direct_ids.update(id(p) for p in params)
+            self.direct_groups.append([self.grad_views[index[id(p)]] if id(p) in index else None for p in params])
+            self._direct_ids.update(id(p) for p in params if id(p) in index)
         for p, v in zip(self.params, self.grad_views):
             if id(p) in self._direct_ids:
                 p.grad = v
@@ -74,10 +93,10 @@ class FlatParams:
     def shadow_bf16(self):
         """name -> bf16 view of the parameter, refreshed from the fp32 master copy by ONE cast kernel."""
         if self.flat16 is None:
-            self.flat16 = torch.empty(self.numel, device=self.flat.device, dtype=torch.bfloat16)
+            self.flat16 = torch.empty(self.numel_all, device=self.flat.device, dtype=torch.bfloat16)
             self._views16 = {self._names[id(p)]: self.flat16[off:off + p.numel()].view_as(p)
-                             for p, off in zip(self.params, self.offsets)}
-        ops.call("lgb200_cast_bf16", ops.ptr(self.flat), ops.ptr(self.flat16), self.numel, ops.stream_ptr())
+                             for p, off in zip(self.params + self.frozen, self.offsets + self.frozen_offsets)}
+        ops.call("lgb200_cast_bf16", ops.ptr(self.flat), ops.ptr(self.flat16), self.numel_all, ops.stream_ptr())
         return self._views16
 
     def lr_factors(self, lr_scaling):
@@ -127,6 +146,48 @@ class FlatParams:
             p.grad = v
 
 
+# train.optimizer (train.py:347-352) -> the torch.optim class whose options, state layout and arithmetic the flat
+# kernel restates
+OPTIMIZERS = {"sgd": torch.optim.SGD, "adam": torch.optim.Adam, "adamw": torch.optim.AdamW, "rmsprop": torch.optim.RMSprop}
+# options that only choose among torch's own implementations of the same arithmetic: accepted and ignored
+_IMPLEMENTATION_OPTIONS = ("foreach", "fused", "capturable", "differentiable")
+
+
+def _resolve_optimizer(optimizer, lr, options):
+    """-> (rule, torch's full option dict for one group without params / lr, per-parameter state keys in torch's order,
+    whether that state holds a step count).  rule: the flat kernel ("adam", "adamw", "sgd", "rmsprop")."""
+    if optimizer not in OPTIMIZERS:
+        raise ValueError(f"optimizer {optimizer!r} is not one of {sorted(OPTIMIZERS)}")
+    for key in ("maximize", "amsgrad"):
+        if options.get(key):
+            raise ValueError(f"optimizer option {key}=True is not supported by the flat-buffer trainer")
+    # torch validates the values and fills in its defaults
+    probe = {k: v for k, v in options.items() if k not in _IMPLEMENTATION_OPTIONS}
+    group = OPTIMIZERS[optimizer]([torch.zeros(1, requires_grad=True)], lr=lr, **probe).param_groups[0]
+    opts = {k: v for k, v in group.items() if k not in ("params", "lr")}
+    if optimizer in ("adam", "adamw"):
+        rule = "adamw" if optimizer == "adamw" or opts.get("decoupled_weight_decay") else "adam"
+        return rule, opts, ["exp_avg", "exp_avg_sq"], True
+    if optimizer == "sgd":
+        return "sgd", opts, ["momentum_buffer"] if opts["momentum"] != 0 else [], False
+    keys = ["square_avg"] + (["momentum_buffer"] if opts["momentum"] > 0 else []) + (["grad_avg"] if opts["centered"] else [])
+    return "rmsprop", opts, keys, True
+
+
+def select_parameters(model, opt_regexp):
+    """train.py:125-141 filter_parameters over the model's own parameter names: every trainable parameter whose name
+    `re.search(opt_regexp, name)` does not match is frozen (requires_grad_(False)).  Returns the selected names;
+    raises ValueError, changing nothing, when no trainable parameter matches."""
+    named = [(n, p) for n, p in model.named_parameters() if p.requires_grad]
+    keep = [n for n, _ in named if re.search(opt_regexp, n)]
+    if not keep:
+        raise ValueError(f"opt_regexp {opt_regexp!r} matches no trainable parameter")
+    for n, p in named:
+        if not re.search(opt_regexp, n):
+            p.requires_grad_(False)
+    return keep
+
+
 class MatcherTrainer:
     """model: a matcher with forward(data)->pred and loss(pred, data)->(losses, metrics).
 
@@ -134,7 +195,7 @@ class MatcherTrainer:
     sequence with no host synchronisation:
         loss -> backward -> flat gradients (+ the loss in the extra slot) -> ONE all-reduce
              -> lgb200_flat_grad_check (any non-finite value on any rank?) -> lgb200_amp_update (step count)
-             -> lgb200_adam_flat (skipped on the device when the check fired: train.py:477-480, 503-512).
+             -> lgb200_<optimizer>_flat (skipped on the device when the check fired: train.py:477-480, 503-512).
     `loss_scale`: None (default; bf16 needs no loss scaling) or an initial GradScaler scale (train.py:456, 490):
     the loss is multiplied by the device-resident scale, the gradients are un-scaled inside the Adam kernel and the
     scale follows torch.amp.GradScaler.update.  `lr_scaling`: the reference's LR groups (train.py:353-361).
@@ -146,12 +207,37 @@ class MatcherTrainer:
     check is then lgb200_flat_grad_norm: the norm of the averaged, unscaled gradient is taken on the device after the
     all-reduce (so every rank computes the same coefficient), a non-finite norm skips the step like
     clip_grad_norm_(error_if_nonfinite=True), and Adam receives the coefficient through its loss-scale divisor.
-    `state_dict()` / `load_state_dict()` carry the optimiser state in the formats of torch.optim.Adam and
+    `optimizer`: the reference's train.optimizer (train.py:347-361): "adam" (default), "adamw", "sgd" or "rmsprop", and
+    `optimizer_options` its train.optimizer_options: torch's option names and defaults for that class (weight_decay 0.01
+    for adamw; Adam with decoupled_weight_decay=True runs as AdamW).  `betas` / `eps` / `weight_decay` are Adam's and
+    are overridden by optimizer_options.  maximize=True and amsgrad=True raise ValueError; foreach, fused, capturable
+    and differentiable only choose among torch's implementations and are ignored.  Each rule is one kernel over the
+    flat buffers (lgb200_{adam,adamw,sgd,rmsprop}_flat) with the same device-side controls; state buffers exist only
+    where torch keeps that state (none for SGD without momentum).
+    `opt_regexp`: the reference's train.opt_regexp (train.py:125-141, 353-356): trainable parameters whose name
+    re.search does not match are frozen (requires_grad_(False)); ValueError when none matches.  Names are the model's
+    own (the name space of `lr_scaling`), so a glue-factory pattern that includes the pipeline's `matcher.` prefix needs
+    that prefix dropped.  Frozen parameters, whether frozen here or by the caller, stay in the flat parameter buffer
+    but have no gradient, optimiser state or place in the all-reduce, and their weight gradients are never computed.
+    `state_dict()` / `load_state_dict()` carry the optimiser state in the formats of torch.optim.<X> and
     torch.amp.GradScaler; the weights go through `model.state_dict()`, whose tensors are views of the flat buffer."""
 
     def __init__(self, model, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, process_group=None,
                  loss_scale=None, growth_factor=2.0, backoff_factor=0.5, growth_interval=2000, lr_scaling=None,
-                 ground_truth=None, sync_batchnorm=False, clip_grad=None):
+                 ground_truth=None, sync_batchnorm=False, clip_grad=None, optimizer="adam", optimizer_options=None,
+                 opt_regexp=None):
+        if optimizer == "adam":
+            options = {"betas": betas, "eps": eps, "weight_decay": weight_decay, **(optimizer_options or {})}
+        elif (tuple(betas), eps, weight_decay) != ((0.9, 0.999), 1e-8, 0.0):
+            raise ValueError(f"the betas / eps / weight_decay keywords are Adam's: give {optimizer!r} its options "
+                             "through optimizer_options")
+        else:
+            options = dict(optimizer_options or {})
+        self.optimizer = optimizer
+        self._rule, self._opt, self._state_keys, self._state_has_step = _resolve_optimizer(optimizer, float(lr), options)
+        self._opt_given = options  # what a torch.optim.<X> over the same groups is built with (state_dict layout)
+        if opt_regexp:
+            select_parameters(model, opt_regexp)
         self.group = process_group
         self.world = dist.get_world_size(process_group) if dist.is_available() and dist.is_initialized() else 1
         if sync_batchnorm and self.world > 1:  # before FlatParams: the converted modules keep the same Parameters
@@ -163,9 +249,9 @@ class MatcherTrainer:
         self.ground_truth = ground_truth
         self.fp = FlatParams(model)
         dev = self.fp.flat.device
-        self.m = torch.zeros_like(self.fp.flat)
-        self.v = torch.zeros_like(self.fp.flat)
-        self.betas, self.eps, self.wd = betas, eps, weight_decay
+        # optimiser state: one flat buffer per torch state key, over the trainable range
+        self.state_buffers = {k: torch.zeros(self.fp.numel, device=dev) for k in self._state_keys}
+        self.m, self.v = self.state_buffers.get("exp_avg"), self.state_buffers.get("exp_avg_sq")  # Adam / AdamW only
         layers = getattr(model, "transformers", None)
         if layers is not None:
             self.fp.enable_direct([list(layer.parameters()) for layer in layers])
@@ -209,18 +295,21 @@ class MatcherTrainer:
 
     # ---- checkpoints (utils/experiments.py:113-118 saves optimizer.state_dict(); train.py:379-382 restores it)
     def state_dict(self):
-        """{"optimizer": the state_dict of a torch.optim.Adam over pack_lr_parameters' groups (train.py:177-196),
-        "grad_scaler": torch.amp.GradScaler.state_dict() (only with loss_scale)}, holding copies of the device state."""
+        """{"optimizer": the state_dict of a torch.optim.<optimizer> over pack_lr_parameters' groups (train.py:177-196),
+        "grad_scaler": torch.amp.GradScaler.state_dict() (only with loss_scale)}, holding copies of the device state.
+        SGD keeps no step count: as torch, it has no state before its first step and none at all without momentum."""
         fp, t = self.fp, float(self.t)
-        layout = torch.optim.Adam([{"params": [fp.params[i] for i in ids], "lr": factor * self._lr_host}
-                                   for factor, ids in self._groups],
-                                  lr=self._lr_host, betas=self.betas, eps=self.eps, weight_decay=self.wd).state_dict()
+        layout = OPTIMIZERS[self.optimizer]([{"params": [fp.params[i] for i in ids], "lr": factor * self._lr_host}
+                                             for factor, ids in self._groups],
+                                            lr=self._lr_host, **self._opt_given).state_dict()
         state = {}
-        for k, i in enumerate(i for _, ids in self._groups for i in ids):
-            p, off = fp.params[i], fp.offsets[i]
-            state[k] = {"step": torch.tensor(t, dtype=torch.float32),
-                        "exp_avg": self.m[off:off + p.numel()].view_as(p).clone(),
-                        "exp_avg_sq": self.v[off:off + p.numel()].view_as(p).clone()}
+        if self._state_has_step or (self._state_keys and t >= 1):
+            for k, i in enumerate(i for _, ids in self._groups for i in ids):
+                p, off = fp.params[i], fp.offsets[i]
+                st = {"step": torch.tensor(t, dtype=torch.float32)} if self._state_has_step else {}
+                for key, buf in self.state_buffers.items():
+                    st[key] = buf[off:off + p.numel()].view_as(p).clone()
+                state[k] = st
         out = {"optimizer": {"state": state, "param_groups": layout["param_groups"]}}
         if self._scale_dev is not None:
             g, b, i = self._amp
@@ -229,9 +318,11 @@ class MatcherTrainer:
         return out
 
     def load_state_dict(self, state_dict):
-        """Load `state_dict()` output, or the state of a torch.optim.Adam built over the same groups, in place: a
+        """Load `state_dict()` output, or the state of a torch.optim.<optimizer> built over the same groups, in place: a
         captured graph stays valid.  Sets lr from the groups.  Raises ValueError, naming the first offending parameter,
-        when the groups, shapes or states do not fit this trainer (it keeps one step count for every parameter).
+        when the groups, shapes or states do not fit this trainer (it keeps one step count for every parameter), e.g.
+        the state of another optimiser.  An SGD state carries no step count: the count becomes 1 when momentum buffers
+        are loaded (the next step is not the first) and 0 when the state is empty.
         A "grad_scaler" entry is ignored without loss_scale, as by a disabled GradScaler."""
         fp, opt = self.fp, state_dict["optimizer"]
         groups, state = opt["param_groups"], opt["state"]
@@ -248,17 +339,27 @@ class MatcherTrainer:
             raise ValueError(f"optimizer state has parameter groups of sizes {[len(g['params']) for g in groups]}, the "
                              f"trainer {[len(ids) for _, ids in self._groups]}: they first differ at parameter "
                              f"{name(order[min(k, len(order) - 1)])!r}")
+        want = (["step"] if self._state_has_step else []) + self._state_keys
+        label = OPTIMIZERS[self.optimizer].__name__
+        # SGD before its first step, or without momentum, has no state at all
+        fresh = not self._state_has_step and not any(state.get(key) for g in groups for key in g["params"])
         pairs, steps = [], []  # (trainer parameter index, source state), in group order
         for src, (_, ids) in zip(groups, self._groups):
             for i, key in zip(ids, src["params"]):
-                st = state.get(key)
-                if st is None or not all(k in st for k in ("step", "exp_avg", "exp_avg_sq")):
-                    raise ValueError(f"no Adam state for parameter {name(i)!r}")
+                if fresh:
+                    continue
+                st = state.get(key) or {}
+                if any(k not in st for k in want):
+                    raise ValueError(f"no {label} state for parameter {name(i)!r}: it holds {sorted(st)}, the trainer "
+                                     f"needs {want}")
+                if set(st) != set(want):
+                    raise ValueError(f"parameter {name(i)!r}: state {sorted(st)} is not the {label} state {want}")
                 shape = fp.params[i].shape
-                if st["exp_avg"].shape != shape or st["exp_avg_sq"].shape != shape:
-                    raise ValueError(f"parameter {name(i)!r}: state shape {tuple(st['exp_avg'].shape)}, "
-                                     f"parameter shape {tuple(shape)}")
-                steps.append(float(st["step"]))
+                for k in self._state_keys:
+                    if st[k].shape != shape:
+                        raise ValueError(f"parameter {name(i)!r}: state shape {tuple(st[k].shape)}, "
+                                         f"parameter shape {tuple(shape)}")
+                steps.append(float(st["step"]) if self._state_has_step else 1.0)
                 if steps[-1] != steps[0]:
                     raise ValueError(f"parameter {name(i)!r} is at step {steps[-1]:g}, the first at {steps[0]:g}: the "
                                      "trainer keeps one step count")
@@ -271,9 +372,12 @@ class MatcherTrainer:
                                  f"trainer's {self._amp}, which are fixed at construction")
         for i, st in pairs:
             off, n = fp.offsets[i], fp.params[i].numel()
-            self.m[off:off + n].copy_(st["exp_avg"].reshape(-1))
-            self.v[off:off + n].copy_(st["exp_avg_sq"].reshape(-1))
-        self._t_dev.fill_(int(steps[0]))
+            for k, buf in self.state_buffers.items():
+                buf[off:off + n].copy_(st[k].reshape(-1))
+        if fresh:
+            for buf in self.state_buffers.values():
+                buf.zero_()
+        self._t_dev.fill_(int(steps[0]) if steps else 0)
         # base lr from a group of factor 1 when there is one (exact), else from the first group with a factor != 0
         lrs = [(f, g["lr"]) for (f, _), g in zip(self._groups, groups) if f != 0]
         if lrs:
@@ -292,9 +396,9 @@ class MatcherTrainer:
 
     # ---- CUDA-graph replay of the whole step (removes the ~2500 per-step launch calls from the host)
     def capture(self, example, device, warmup=3):
-        """Capture forward + loss + backward + all-reduce + Adam into one CUDA graph.  `example` fixes the
+        """Capture forward + loss + backward + all-reduce + optimiser step into one CUDA graph.  `example` fixes the
         shapes; later batches are copied into the captured static input buffers.  The warm-up steps run on the
-        example batch but leave no trace: parameters, Adam moments, step count and loss scale are restored."""
+        example batch but leave no trace: parameters, optimiser state, step count and loss scale are restored."""
         # private static inputs: to_device() returns device tensors as they are, and step_graphed() overwrites these
         self._static = _clone(to_device(example, device))
         keep = [t.clone() for t in self._state_tensors()]
@@ -314,7 +418,7 @@ class MatcherTrainer:
         return self
 
     def _state_tensors(self):
-        ts = [self.fp.flat, self.m, self.v, self._t_dev]
+        ts = [self.fp.flat, *self.state_buffers.values(), self._t_dev]
         if self._scale_dev is not None:
             ts += [self._scale_dev, self._growth]
         return ts
@@ -378,14 +482,31 @@ class MatcherTrainer:
             ops.flat_grad_check(checked, self._found_inf)
             divisor = self._scale_dev
         ops.amp_update(self._found_inf, step_dev=self._t_dev)  # ++step unless skipped (Adam's bias correction reads it)
-        ops.adam_flat_(self.fp.flat, self.fp.grad, self.m, self.v, 0, self._lr_host, self.betas, self.eps, self.wd,
-                       grad_scale=1.0 / self.world, lr_scale_per_elem=self._lr_scale, step_dev=self._t_dev,
-                       lr_dev=self._lr_dev, loss_scale_dev=divisor, found_inf_dev=self._found_inf)
+        self._optimizer_step(divisor)
         if self._scale_dev is not None:  # GradScaler.update AFTER the step: the gradients carry the old scale
             g, b, i = self._amp
             ops.amp_update(self._found_inf, None, self._scale_dev, self._growth, g, b, i)
         self.calls += 1
         return loss.detach(), losses
+
+
+    def _optimizer_step(self, divisor):
+        """The update rule's one kernel over the trainable range of the flat buffers, skipped on the device when the
+        check fired; `divisor`: the loss scale, or the clip coefficient's divisor."""
+        fp, o, b = self.fp, self._opt, self.state_buffers
+        p = fp.flat[:fp.numel]
+        common = dict(grad_scale=1.0 / self.world, lr_scale_per_elem=self._lr_scale, lr_dev=self._lr_dev,
+                      loss_scale_dev=divisor, found_inf_dev=self._found_inf)
+        if self._rule in ("adam", "adamw"):
+            update = ops.adam_flat_ if self._rule == "adam" else ops.adamw_flat_
+            update(p, fp.grad, b["exp_avg"], b["exp_avg_sq"], 0, self._lr_host, o["betas"], o["eps"],
+                   o["weight_decay"], step_dev=self._t_dev, **common)
+        elif self._rule == "sgd":
+            ops.sgd_flat_(p, fp.grad, b.get("momentum_buffer"), 0, self._lr_host, o["momentum"], o["dampening"],
+                          o["nesterov"], o["weight_decay"], step_dev=self._t_dev, **common)
+        else:
+            ops.rmsprop_flat_(p, fp.grad, b["square_avg"], b.get("momentum_buffer"), b.get("grad_avg"), self._lr_host,
+                              o["alpha"], o["eps"], o["weight_decay"], o["momentum"], **common)
 
 
 def _clone(tree):

@@ -58,7 +58,8 @@ int lgb200_check_device(void);
 int lgb200_rope_split_fwd(const void* qkv, const float* theta, void* q, void* k, void* v, int64_t ntok, int H,
                           int dtype, cudaStream_t stream);
 /* dq,dk are gradients w.r.t. the rotated q,k (saved by forward as q,k); writes dqkv [ntok, H*192]
- * and ACCUMULATES dtheta [ntok, 32] (the gradient that reaches posenc.Wr from every layer).   */
+ * and ACCUMULATES dtheta [ntok, 32] (the gradient that reaches posenc.Wr from every layer); dtheta NULL:
+ * not computed (a frozen position encoder).                                                  */
 int lgb200_rope_split_bwd(const void* dq, const void* dk, const void* dv, const void* q, const void* k,
                           const float* theta, void* dqkv, float* dtheta, int64_t ntok, int H, int dtype,
                           cudaStream_t stream);
@@ -199,6 +200,7 @@ int lgb200_head_logsig(const float* zt, float* ls, float* du, int64_t T, cudaStr
  *                   ls/du as head_logsig, x_cast (nullable) = x in `dtype` for final_proj.
  *   head_token_bwd: dx = float(dmdw) + dzt[:,0] wm   (dmdw [T,D] in `dtype` = d md . W_final_proj; the confidence
  *                   head reads a detached x, lightglue.py:82-83), dW2 [2,D] = dzt^T x, db2 [2] = column sums of dzt.
+ *                   dmdw and dx both NULL: dx is not computed (x needs no gradient).
  *                   ws: head_token_bwd_ws_floats(D) floats; counter: one uint32, zero before the first call. */
 int lgb200_head_token_bwd_ws_floats(int D);
 int lgb200_head_token_fwd(const float* x, const float* wm, const float* bm, const float* wt, const float* bt,
@@ -321,6 +323,27 @@ int lgb200_adam_flat(float* p, const float* g, float* m, float* v, int64_t n, co
                      float beta1, float beta2, float eps, float weight_decay, int step, const int* step_dev,
                      float grad_scale, const float* lr_dev, const float* loss_scale_dev, const float* found_inf_dev,
                      cudaStream_t stream);
+/* The other rules of train.py:347-361 (train.optimizer) over the same flat buffers, with the same controls as
+ * lgb200_adam_flat (grad_scale, lr_scale_per_elem, the *_dev pointers; found_inf_dev set: parameters and state are left
+ * untouched), each in the arithmetic and order of operations of torch.optim.<X>'s single-tensor step (no maximize).
+ * All buffers 16-byte aligned; one launch each.
+ * AdamW: Adam with decoupled decay, p *= 1 - lr * lr_scale * weight_decay, before the update.
+ * SGD: momentum_buffer non-NULL exactly when momentum != 0.  The first step (step count 1, read from step_dev when
+ * given) sets the buffer to the gradient itself, undampened.  nesterov needs momentum > 0 and dampening 0.
+ * RMSprop: momentum_buffer non-NULL exactly when momentum > 0; grad_avg non-NULL selects `centered`.  It keeps no
+ * step-dependent term, so it takes no step count.                                                                  */
+int lgb200_adamw_flat(float* p, const float* g, float* m, float* v, int64_t n, const float* lr_scale_per_elem,
+                      float lr, float beta1, float beta2, float eps, float weight_decay, int step, const int* step_dev,
+                      float grad_scale, const float* lr_dev, const float* loss_scale_dev, const float* found_inf_dev,
+                      cudaStream_t stream);
+int lgb200_sgd_flat(float* p, const float* g, float* momentum_buffer, int64_t n, const float* lr_scale_per_elem,
+                    float lr, float momentum, float dampening, int nesterov, float weight_decay, int step,
+                    const int* step_dev, float grad_scale, const float* lr_dev, const float* loss_scale_dev,
+                    const float* found_inf_dev, cudaStream_t stream);
+int lgb200_rmsprop_flat(float* p, const float* g, float* square_avg, float* momentum_buffer, float* grad_avg,
+                        int64_t n, const float* lr_scale_per_elem, float lr, float alpha, float eps,
+                        float weight_decay, float momentum, float grad_scale, const float* lr_dev,
+                        const float* loss_scale_dev, const float* found_inf_dev, cudaStream_t stream);
 /* found_inf[0] = 1.0f if any of g[0..n) is non-finite, else 0.0f (GradScaler.unscale_'s check, no host sync). */
 int lgb200_flat_grad_check(const float* g, int64_t n, float* found_inf, cudaStream_t stream);
 /* Gradient-norm clipping (torch.nn.utils.clip_grad_norm_ with error_if_nonfinite=True after GradScaler.unscale_,
