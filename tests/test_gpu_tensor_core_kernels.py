@@ -667,7 +667,7 @@ def _assign_inputs(B, M, N, D, seed):
     return md0, md1, D ** -0.5, ls0, ls1, gt, gc
 
 
-ASSIGN_SHAPES = [(32, 2048, 2048, 256), (4, 384, 320, 64), (4, 300, 257, 128), (4, 191, 321, 192), (4, 1000, 777, 256)]
+ASSIGN_SHAPES = [(32, 2048, 2048, 256), (32, 2048, 2048, 128), (4, 384, 320, 64), (4, 300, 257, 128), (4, 191, 321, 192), (4, 1000, 777, 256)]
 
 
 @GPU
