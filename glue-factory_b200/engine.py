@@ -14,8 +14,7 @@ pass, there are no per-op dtype casts or cat/slice copies, and nothing N x N is 
 In `precision: bf16` every GEMM of the layer and of the head -- the nine nn.Linear projections, their input-gradient
 and weight-gradient contractions -- runs on the library's own persistent wgmma GEMM (`ops.linear`: bias and
 fp32 accumulate-into-dx epilogues; `ops.wgrad_bf16`: split-K, fp32 out); no cuBLAS kernel is launched.  The fp32
-parity mode keeps fp32 cuBLAS (`torch.addmm/mm`) for the projections; `precision: bf16x3` runs the same fp32 data flow with
-every GEMM on the wgmma kernel through split bf16 operands (see FP32_GEMM).
+parity mode (`precision: fp32`) keeps fp32 cuBLAS (`torch.addmm/mm`) for the projections.
 """
 import torch
 import torch.nn.functional as F
@@ -25,46 +24,11 @@ from . import ops
 _head_counters = {}
 
 
-# How the fp32 parity mode multiplies matrices: "cublas" (torch.addmm / mm) or "x3" -- every fp32 operand split into
-# bf16 hi + lo, and  A B ~= Ah Bh + Ah Bl + Al Bh  evaluated as ONE wgmma GEMM over the 3x longer contraction
-# [Ah | Ah | Al] x [Bh | Bl | Bh] (fp32 accumulation in tensor memory; the dropped Al Bl term is 2^-16 relative).  This is
-# `precision: bf16x3`: the fp32 goldens (1e-3, bit-exact match indices) are then met with every GEMM of the path on the
-# same persistent wgmma kernel, TMA pipeline and epilogues the bf16 mode uses.
-FP32_GEMM = "cublas"
-
-
-class fp32_gemm:
-    """with engine.fp32_gemm("x3"): ...  (LayerFn / HeadFn remember the mode of their forward for their backward)"""
-
-    def __init__(self, mode):
-        assert mode in ("cublas", "x3"), mode
-        self.mode = mode
-
-    def __enter__(self):
-        global FP32_GEMM
-        self.prev, FP32_GEMM = FP32_GEMM, self.mode
-
-    def __exit__(self, *exc):
-        global FP32_GEMM
-        FP32_GEMM = self.prev
-
-
-def split3(x, dim, pattern):
-    """fp32 -> bf16 hi / lo parts concatenated along `dim` in the order of `pattern` ("hhl" for the left operand of a
-    contraction over `dim`, "hlh" for the right one)."""
-    hi = x.to(torch.bfloat16)
-    lo = (x - hi.float()).to(torch.bfloat16)
-    return torch.cat([hi if c == "h" else lo for c in pattern], dim)
-
-
 def _lin(x, W, b, out=None):
     """y = x W^T + b.  bf16: own wgmma GEMM with the fp32 bias added in the epilogue (W = bf16 shadow, b = the fp32
-    parameter); fp32 parity mode: cuBLAS, or the split-operand wgmma GEMM (FP32_GEMM)."""
+    parameter); fp32 parity mode: cuBLAS."""
     if x.dtype == torch.bfloat16:
         return ops.linear(x, W, b, out=out)
-    if FP32_GEMM == "x3":
-        return ops.linear(split3(x, 1, "hhl"), split3(W, 1, "hlh"), b.float().contiguous(), out=out,
-                          out_dtype=torch.float32)
     return torch.addmm(b, x, W.t()) if out is None else torch.addmm(b, x, W.t(), out=out)
 
 
@@ -72,8 +36,6 @@ def _dgrad(dy, W):
     """dx = dy W (compute dtype)."""
     if dy.dtype == torch.bfloat16:
         return ops.linear(dy, W, w_is_kn=True)
-    if FP32_GEMM == "x3":
-        return ops.linear(split3(dy, 1, "hhl"), split3(W, 0, "hlh"), w_is_kn=True, out_dtype=torch.float32)
     return torch.mm(dy, W)
 
 
@@ -81,29 +43,8 @@ def _wgrad(dy, a, out=None):
     """dW [out, in] fp32 = dy^T a for compute-dtype dy [T, out], a [T, in] (row-strided views allowed); `out`: write
     straight into this fp32 view (a parameter's slot of the trainer's flat gradient buffer)."""
     if dy.dtype == torch.float32:
-        if FP32_GEMM == "x3":
-            return ops.wgrad_bf16(split3(dy, 0, "hhl"), split3(a, 0, "hlh"), out=out)
         return torch.mm(dy.t(), a) if out is None else torch.mm(dy.t(), a, out=out)
     return ops.wgrad_bf16(dy, a, out=out)
-
-
-class LinearX3Fn(torch.autograd.Function):
-    """nn.Linear in the `bf16x3` mode for the callers outside LayerFn / HeadFn (input_proj, the dense evaluation
-    head): fp32 in / out, forward, dgrad and wgrad on the split-operand wgmma GEMM."""
-
-    @staticmethod
-    def forward(ctx, x, weight, bias):
-        ctx.save_for_backward(x, weight)
-        with fp32_gemm("x3"):
-            return _lin(x, weight.detach().float(), bias.detach())
-
-    @staticmethod
-    def backward(ctx, dy):
-        x, weight = ctx.saved_tensors
-        dy = dy.contiguous()
-        with fp32_gemm("x3"):
-            dx = _dgrad(dy, weight.detach().float()) if ctx.needs_input_grad[0] else None
-            return dx, _wgrad(dy, x), dy.sum(0)
 
 
 def _bgrad(dy):
@@ -112,11 +53,9 @@ def _bgrad(dy):
 
 def similarity(md0, md1, cdt, alpha=1.0):
     """sim [B, M, N] fp32 = alpha md0 md1^T: bf16 operands on the wgmma GEMM when cdt is bf16; in the fp32 parity mode
-    cuBLAS, or the split-operand wgmma GEMM (FP32_GEMM)."""
+    cuBLAS."""
     if cdt == torch.bfloat16:
         return ops.gemm_bf16(md0.to(torch.bfloat16).contiguous(), md1.to(torch.bfloat16).contiguous(), alpha=alpha)
-    if FP32_GEMM == "x3":
-        return ops.gemm_bf16(split3(md0.float(), 2, "hhl"), split3(md1.float(), 2, "hlh"), alpha=alpha)
     sim = torch.bmm(md0, md1.transpose(1, 2))
     return sim.mul_(alpha) if alpha != 1 else sim
 
@@ -124,7 +63,7 @@ def similarity(md0, md1, cdt, alpha=1.0):
 def assign_unfused_bwd(md0, md1, sim, lse_row, lse_col, gt_u8, gcoef, rowcnt, colcnt):
     """d(mdesc0) [B, M, D], d(mdesc1) [B, N, D] (md0's dtype) of the NLL through a stored sim: dsim = gcoef (2 gt -
     softmax_row rowcnt - softmax_col colcnt) from lgb200_assign_bwd, then dsim md1 and dsim^T md0.  The unfused
-    counterpart of ops.assign_fused_bwd, for fp32 / bf16x3 and for operands assign_fused_ok rejects."""
+    counterpart of ops.assign_fused_bwd, for fp32 and for operands assign_fused_ok rejects."""
     B, M, N = sim.shape
     cdt = md0.dtype
     tc = cdt == torch.bfloat16 and N % 8 == 0 and M % 8 == 0
@@ -134,9 +73,6 @@ def assign_unfused_bwd(md0, md1, sim, lse_row, lse_col, gt_u8, gcoef, rowcnt, co
     if tc:
         dmd0 = ops.gemm_bf16(dsim, md1, a_mn_major=False, b_mn_major=True, out_dtype=cdt)  # dsim   md1
         dmd1 = ops.gemm_bf16(dsim, md0, a_mn_major=True, b_mn_major=True, out_dtype=cdt)   # dsim^T md0
-    elif FP32_GEMM == "x3" and N % 8 == 0:  # (TMA needs 16-byte row strides of dsim; ragged N: cuBLAS)
-        dmd0 = ops.gemm_bf16(split3(dsim, 2, "hhl"), split3(md1, 1, "hlh"), b_mn_major=True)
-        dmd1 = ops.gemm_bf16(split3(dsim, 1, "hhl"), split3(md0, 1, "hlh"), a_mn_major=True, b_mn_major=True)
     else:
         dmd0 = torch.bmm(dsim, md1.float()).to(cdt)
         dmd1 = torch.bmm(dsim.transpose(1, 2), md0.float()).to(cdt)
@@ -149,8 +85,6 @@ def _dgrad_acc(acc, dy, w):
     is accumulated in fp32 and never re-read by an SM (an acc that is not 16-byte aligned is read-modify-written from
     registers instead).  Every `acc` handed in is a gradient buffer this engine owns."""
     if dy.dtype == torch.float32:
-        if FP32_GEMM == "x3":
-            return ops.linear(split3(dy, 1, "hhl"), split3(w, 0, "hlh"), out=acc, w_is_kn=True, accumulate=True)
         return acc.addmm_(dy, w)
     return ops.linear(dy, w, out=acc, w_is_kn=True, accumulate=True)
 
@@ -277,17 +211,11 @@ class LayerFn(torch.autograd.Function):
                               rstd2, gg, *lse1, *lse2, *w)
         ctx.meta = (sizes, H, cdt, len(lse1), len(lse2), D)
         ctx.sink = sink
-        ctx.gemm_mode = FP32_GEMM
         ctx.set_materialize_grads(False)  # the output's gradient may arrive through the stash only
         return x2
 
     @staticmethod
     def backward(ctx, dx):
-        with fp32_gemm(ctx.gemm_mode):
-            return LayerFn._backward(ctx, dx)
-
-    @staticmethod
-    def _backward(ctx, dx):
         sizes, H, cdt, n1, n2, D = ctx.meta
         sv = ctx.saved_tensors
         (theta, cat1, q, k, v, att, h, mean1, rstd1, g, cat2, qk, vv, m, h2, mean2, rstd2, gg) = sv[:18]
@@ -409,18 +337,12 @@ class HeadFn(torch.autograd.Function):
             saved += [f0, f1]
         ctx.save_for_backward(*saved)
         ctx.meta = (sizes, cdt, bal, alpha, has_tok, f0 is not None, fused)
-        ctx.gemm_mode = FP32_GEMM
         ctx.stash = stash
         ctx.mark_non_differentiable(nll_pos, nll_neg)
         return nll, conf, nll_pos, nll_neg
 
     @staticmethod
     def backward(ctx, g_nll, g_conf, *_):
-        with fp32_gemm(ctx.gemm_mode):
-            return HeadFn._backward(ctx, g_nll, g_conf)
-
-    @staticmethod
-    def _backward(ctx, g_nll, g_conf):
         sv = ctx.saved_tensors
         (x, x16, md, sim, lse_row, lse_col, zt, rowmax, rowarg, colmax, colarg, wfp, wm, gt_u8, rowcnt, colcnt, neg0,
          neg1, num_pos, num_neg) = sv[:20]

@@ -25,9 +25,6 @@ H100 `forward` raises.  `loss` takes only the pred of this module's own
 conf additions over the reference's default_conf:
     precision: "bf16" -> bf16 operands / fp32 accumulation on the Hopper tensor cores (default)
                "fp32" -> full-precision parity path (CUDA cores + fp32 cuBLAS)
-               "bf16x3" -> the fp32 data flow with every GEMM on the wgmma kernel: fp32 operands split into bf16
-                         hi + lo parts, three partial products accumulated in fp32 tensor memory (engine.FP32_GEMM);
-                         attention on the fp32 CUDA-core kernel.  Meets the fp32 goldens like "fp32" does.
 """
 import copy
 import math
@@ -166,7 +163,7 @@ class LightGlue(nn.Module):
     def __init__(self, conf=None):
         super().__init__()
         self.conf = conf = _Conf(_merge(self.default_conf, _to_plain(conf)))
-        assert conf.precision in ("bf16", "fp32", "bf16x3"), conf.precision
+        assert conf.precision in ("bf16", "fp32"), conf.precision
         d, h, n = conf.descriptor_dim, conf.num_heads, conf.n_layers
         # head_dim = descriptor_dim // num_heads (lightglue.py:347): 64 (256 / 4, the default) or 32 (128 / 4, 256 / 8)
         if d % h or d // h not in (32, 64):
@@ -194,10 +191,6 @@ class LightGlue(nn.Module):
     @property
     def _bf16(self):
         return self.conf.precision == "bf16"
-
-    @property
-    def _gemm_mode(self):
-        return "x3" if self.conf.precision == "bf16x3" else "cublas"
 
     @property
     def _cdt(self):
@@ -232,10 +225,6 @@ class LightGlue(nn.Module):
             shp = x.shape
             y = ops.LinearFn.apply(x.reshape(-1, shp[-1]).to(torch.bfloat16).contiguous(), layer.weight, layer.bias)
             return y.view(*shp[:-1], y.shape[-1])
-        if self.conf.precision == "bf16x3":
-            shp = x.shape
-            y = engine.LinearX3Fn.apply(x.reshape(-1, shp[-1]).float().contiguous(), layer.weight, layer.bias)
-            return y.view(*shp[:-1], y.shape[-1])
         return F.linear(x, layer.weight, layer.bias)
 
     def _head_inputs(self, d0, d1, i):
@@ -255,7 +244,7 @@ class LightGlue(nn.Module):
         autocast disabled (fp32 keypoint normalisation / rotary angles / residual stream as in the reference's
         custom_fwd(cast_inputs=float32) regions, bf16 tensor-core operands inside the kernels) and every input is
         converted explicitly -- descriptors may arrive in fp16, cf. the `.half()` quirk of lightglue.py:451-453."""
-        with torch.autocast(device_type="cuda", enabled=False), engine.fp32_gemm(self._gemm_mode):
+        with torch.autocast(device_type="cuda", enabled=False):
             return self._forward(data)
 
     def _forward(self, data):
@@ -488,7 +477,7 @@ class LightGlue(nn.Module):
     def loss(self, pred, data):
         """lightglue.py:578-627 without materialising any of the per-layer log-assignment matrices.  Like forward, runs
         with the ambient autocast disabled; its backward is linear in the incoming gradient (GradScaler, train.py:490)."""
-        with torch.autocast(device_type="cuda", enabled=False), engine.fp32_gemm(self._gemm_mode):
+        with torch.autocast(device_type="cuda", enabled=False):
             return self._loss(pred, data)
 
 

@@ -129,30 +129,13 @@ def _dropin_checks():
             gt_cls({})({"H_0to1": torch.eye(3)[None], "keypoints0": torch.zeros(1, 4, 2), "keypoints1": torch.zeros(1, 4, 2)})
 
 
-def test_split_operand_host_logic():
-    """Host side of the tensor-core parity mode (`precision: bf16x3`): the bf16 hi / lo split of an fp32 operand loses
-    2^-16 at most, the K-concatenated products [Ah|Ah|Al] x [Bh|Bl|Bh] reproduce A B to ~1e-5, and the mode switch is
-    scoped (a node's backward runs under the mode of its forward)."""
-    from gluefactory_b200 import engine
+def test_lightglue_rejects_removed_precision_mode():
+    """`precision` takes `bf16` or `fp32`; a config naming the former `bf16x3` mode fails at construction rather than
+    running some other numeric path.  `fp32` meets the goldens that mode was held to."""
+    from gluefactory_b200.matchers.lightglue import LightGlue
 
-    g = torch.Generator().manual_seed(0)
-    a, b = torch.randn(37, 64, generator=g), torch.randn(53, 64, generator=g)
-    a3, b3 = engine.split3(a, 1, "hhl"), engine.split3(b, 1, "hlh")
-    assert a3.dtype == torch.bfloat16 and a3.shape == (37, 192)
-    hi, lo = a3[:, :64].float(), a3[:, 128:].float()
-    assert ((hi + lo) - a).abs().max() <= a.abs().max() * 2.0 ** -15
-    ref = a.double() @ b.double().t()
-    got = a3.double() @ b3.double().t()
-    plain = a.bfloat16().double() @ b.bfloat16().double().t()
-    err = lambda x: ((x - ref).norm() / ref.norm()).item()  # noqa: E731
-    assert err(got) < 2e-5 and err(got) < err(plain) / 50
-    assert engine.FP32_GEMM == "cublas"
-    with engine.fp32_gemm("x3"):
-        assert engine.FP32_GEMM == "x3"
-        with engine.fp32_gemm("cublas"):
-            assert engine.FP32_GEMM == "cublas"
-        assert engine.FP32_GEMM == "x3"
-    assert engine.FP32_GEMM == "cublas"
+    with pytest.raises(AssertionError, match="bf16x3"):
+        LightGlue({"precision": "bf16x3", "n_layers": 1})
 
 
 def test_mask_counts_host_fallback():

@@ -2,9 +2,9 @@
 against the fixtures produced by the unmodified reference (scripts/make_lightglue_hd32_golden.py): forward, loss and
 backward in fp64 for M == N, M != N, 8 heads and `add_scale_ori`, and eval-mode point pruning in fp32.
 
-The bars are those of the head-dim-64 fixtures (tests/test_gpu_matcher.py): `fp32` and `bf16x3` with match indices
-bit-exact and log-assignment, matching scores, every loss entry and the gradient summaries within 1e-3; `bf16` with
-the log-assignment within 0.15, the total loss within 2e-2, indices equal wherever the reference's top-2 margin exceeds
+The bars are those of the head-dim-64 fixtures (tests/test_gpu_matcher.py): `fp32` with match indices bit-exact and
+log-assignment, matching scores, every loss entry and the gradient summaries within 1e-3; `bf16` with the
+log-assignment within 0.15, the total loss within 2e-2, indices equal wherever the reference's top-2 margin exceeds
 0.3, and every gradient norm within 10 %."""
 import ast
 import os
@@ -49,13 +49,12 @@ def _run(name, precision):
     return g, model, pred, losses
 
 
-@pytest.mark.parametrize("precision", ["fp32", "bf16x3"])
 @pytest.mark.parametrize("name", HD32_CASES)
-def test_fp32_and_bf16x3_match_reference_golden(name, precision):
-    g, model, pred, losses = _run(name, precision)
+def test_fp32_matches_reference_golden(name):
+    g, model, pred, losses = _run(name, "fp32")
     assert np.array_equal(pred["matches0"].cpu().numpy(), g["pred|matches0"])
     assert np.array_equal(pred["matches1"].cpu().numpy(), g["pred|matches1"])
-    report(f"hd32 {name} {precision}", la=rel_err(pred["log_assignment"], torch.from_numpy(g["pred|log_assignment"])))
+    report(f"hd32 {name} fp32", la=rel_err(pred["log_assignment"], torch.from_numpy(g["pred|log_assignment"])))
     np.testing.assert_allclose(pred["log_assignment"].cpu().numpy(), g["pred|log_assignment"], rtol=1e-3, atol=1e-3)
     np.testing.assert_allclose(pred["matching_scores0"].cpu().numpy(), g["pred|matching_scores0"], rtol=1e-3, atol=1e-6)
     np.testing.assert_allclose(pred["matching_scores1"].cpu().numpy(), g["pred|matching_scores1"], rtol=1e-3, atol=1e-6)

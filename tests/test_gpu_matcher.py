@@ -52,37 +52,6 @@ def test_fp32_path_matches_reference_golden(name):
         check_grad_summary(g, k, p.grad, rtol=1e-3)
 
 
-@pytest.mark.parametrize("name", CASES[:4] + EXTRA_CASES)
-def test_bf16x3_tensor_core_parity_mode_matches_reference_golden(name):
-    """`precision: bf16x3`: the fp32 goldens -- bit-exact match indices, 1e-3 on log-scores, losses and every
-    gradient -- with EVERY GEMM of the path (projections, their dgrad / wgrad, the similarity and its two backward
-    contractions) on the persistent wgmma kernel through split bf16 operands (engine.FP32_GEMM == "x3")."""
-    g, conf, w, data = load_case(name)
-    model = _build(conf, w, "bf16x3")
-    d = _f32(data)
-    pred = model(d)
-    losses, _ = model.loss(pred, d)
-    losses["total"].mean().backward()
-    assert np.array_equal(pred["matches0"].cpu().numpy(), g["pred|matches0"])
-    assert np.array_equal(pred["matches1"].cpu().numpy(), g["pred|matches1"])
-    np.testing.assert_allclose(pred["log_assignment"].cpu().numpy(), g["pred|log_assignment"], rtol=1e-3, atol=1e-3)
-    for k in ["total", "last", "assignment_nll", "nll_pos", "nll_neg", "confidence", "row_norm"]:
-        np.testing.assert_allclose(losses[k].detach().cpu().numpy(), g["loss|" + k], rtol=1e-3, err_msg=k)
-    for k, p in model.named_parameters():
-        check_grad_summary(g, k, p.grad, rtol=1e-3)
-
-
-def test_bf16x3_full_size_forward():
-    g, conf, w, data = load_case(CASES[4])
-    model = _build(conf, w, "bf16x3").eval()
-    with torch.no_grad():
-        pred = model(_f32(data))
-    assert np.array_equal(pred["matches0"].cpu().numpy(), g["pred|matches0"])
-    assert np.array_equal(pred["matches1"].cpu().numpy(), g["pred|matches1"])
-    np.testing.assert_allclose(pred["log_assignment"][:, ::8, ::8].cpu().numpy(), g["pred|log_assignment"],
-                               rtol=1e-3, atol=1e-3)
-
-
 def test_fp32_path_full_size_forward():
     g, conf, w, data = load_case(CASES[4])
     model = _build(conf, w, "fp32").eval()
