@@ -31,12 +31,20 @@ Intermediate line supervision (`inter_supervision`, gluestick.py:96-107, 272-292
 the node features after its cross layer go through the same line head as the final ones (`_line_head`) with that
 block's `inter_line_proj`, and their NLL is added to the total with the block's `loss.inter_supervision` weight.
 
-Not built (raise NotImplementedError): `line_attention`, `skip_init`, inputs without lines.
+Views without keypoints or lines follow the reference: no keypoints in a view returns its early-exit pred
+(`_empty_pred`); no lines in a view skips every LineLayer and line head and returns zero / -1 line outputs, and `loss`
+then raises ValueError (no loss is defined here for such views: the reference drops the line term without
+inter_supervision and fails with it).  A view without `image_size` is normalised with
+`view["image"].shape[-2:]`.  `weights` is a path or a name resolved to DATA_PATH/weights/{weights}_{version}.tar from
+the local disk only (matchers/_weights.py).
+
+Not built (raise NotImplementedError): `line_attention`, `skip_init`.
 """
 import torch
 from torch import nn
 
 from .. import _lib, ops
+from . import _weights
 from ._point_gnn import PointGNN
 from .lightglue import _Conf, _merge, _to_plain, matcher_metrics
 
@@ -163,7 +171,10 @@ class GlueStick(PointGNN):
         self.register_parameter("bin_score", bin_score)
         self.register_parameter("line_bin_score", line_bin_score)
         if conf.weights:
-            sd = torch.load(conf.weights, map_location="cpu")
+            # a path, else the file the reference's download writes to (gluestick.py:114-130); never downloaded here
+            root = _weights.data_path()
+            cand = [root / "weights" / f"{conf.weights}_{conf.version}.tar"] if root is not None else []
+            sd = _weights.load_weights(conf.weights, cand, "gluestick")
             if "model" in sd:  # full glue-factory checkpoint (gluestick.py:131-139)
                 sd = {k.replace("matcher.", "").replace("module.", ""): v for k, v in sd["model"].items() if "matcher." in k}
             self.load_state_dict(sd, strict=False)
@@ -214,14 +225,15 @@ class GlueStick(PointGNN):
     def _forward(self, data):
         for key in self.required_data_keys:
             assert key in data, f"Missing key {key} in data"
-        _lib.load()  # raises unless the CUDA library is built and the device is an H100 (no CPU fallback)
-        kp0, kp1 = data["keypoints0"].float(), data["keypoints1"].float()
+        kp0, kp1 = data["keypoints0"], data["keypoints1"]
         B, n0 = kp0.shape[:2]
         n1 = kp1.shape[1]
         L0, L1 = data["lines0"].shape[1], data["lines1"].shape[1]
-        if n0 == 0 or n1 == 0 or L0 == 0 or L1 == 0:
-            raise NotImplementedError("gluefactory_b200 gluestick: empty keypoint / line sets are not supported")
-        size0, size1 = data["view0"]["image_size"], data["view1"]["image_size"]
+        if n0 == 0 or n1 == 0:  # nothing to match: no computation
+            return _empty_pred(B, n0, n1, L0, L1, kp0.device)
+        _lib.load()  # raises unless the CUDA library is built and the device is an H100 (no CPU fallback)
+        kp0, kp1 = kp0.float(), kp1.float()
+        size0, size1 = _image_size(data["view0"], kp0), _image_size(data["view1"], kp1)
         D = self.conf.descriptor_dim
         d0 = data["descriptors0"].float().reshape(B * n0, -1)
         d1 = data["descriptors1"].float().reshape(B * n1, -1)
@@ -240,21 +252,30 @@ class GlueStick(PointGNN):
             inp = torch.cat([ln.reshape(B, 2 * Ln, 2), off, scores.float().repeat(1, 2)[..., None]], -1)
             return self._mlp(inp.reshape(-1, 5), self.lenc.encoder)
 
-        enc0, enc1 = line_enc(data["lines0"], data["line_scores0"], size0), line_enc(data["lines1"], data["line_scores1"], size1)
-        idx0, idx1 = data["lines_junc_idx0"].reshape(B, -1), data["lines_junc_idx1"].reshape(B, -1)
+        # a view without lines: no line encoding, LineLayer or line head runs, intermediate ones included
+        # (gluestick.py:213-240, 257-312, 734-740)
+        lines = L0 > 0 and L1 > 0
+        if lines:
+            enc0 = line_enc(data["lines0"], data["line_scores0"], size0)
+            enc1 = line_enc(data["lines1"], data["line_scores1"], size1)
+            idx0, idx1 = data["lines_junc_idx0"].reshape(B, -1), data["lines_junc_idx1"].reshape(B, -1)
         inter = {}  # block -> both images' features after its cross layer (gluestick.py:762-768)
         for i, layer in enumerate(self.gnn.layers):
             d0, d1 = self._gnn_layer(d0, d1, layer.update, layer.type == "cross", B)
-            if layer.type == "self":
+            if layer.type == "self" and lines:
                 for _ in range(self.conf.num_line_iterations):
                     d0, d1 = self._line_layer(d0, d1, enc0, enc1, idx0, idx1, self.gnn.line_layers[i // 2], B)
-            if self.conf.inter_supervision and layer.type == "cross" and i // 2 in self.conf.inter_supervision:
+            if (lines and self.conf.inter_supervision and layer.type == "cross"
+                    and i // 2 in self.conf.inter_supervision):
                 inter[i // 2] = (d0, d1)
         # points (keypoints and line junctions together)
         scores = ops.log_double_softmax(self._similarity(self._conv(d0, self.final_proj), self._conv(d1, self.final_proj), B),
                                         self.bin_score)
         m0, m1, ms0, ms1 = self._matches(scores.detach())
         pred = {"log_assignment": scores, "matches0": m0, "matches1": m1, "matching_scores0": ms0, "matching_scores1": ms1}
+        if not lines:
+            pred.update(_no_line_outputs(B, L0, L1, kp0.device), raw_line_scores=kp0.new_zeros(B, L0, L1))
+            return pred
         lscores, lm0, lm1, lms0, lms1, raw = self._line_head(d0, d1, idx0, idx1, L0, L1, self.final_line_proj, B)
         pred.update({"line_log_assignment": lscores, "line_matches0": lm0, "line_matches1": lm1,
                      "line_matching_scores0": lms0, "line_matching_scores1": lms1, "raw_line_scores": raw})
@@ -310,6 +331,9 @@ class GlueStick(PointGNN):
 
     def loss(self, pred, data):
         """gluestick.py:417-462."""
+        if data["lines0"].shape[1] == 0 or data["lines1"].shape[1] == 0:
+            raise ValueError("gluefactory_b200 gluestick: the line loss needs lines in both views (lines0 has "
+                             f"{data['lines0'].shape[1]}, lines1 {data['lines1'].shape[1]})")
         with torch.autocast(device_type="cuda", enabled=False):
             losses = {"total": 0}
             losses = self._sub_loss(pred, data, losses, self.bin_score, "")
@@ -322,6 +346,37 @@ class GlueStick(PointGNN):
                 for block in self.conf.inter_supervision or []:
                     metrics.update(_line_metrics(pred, data, f"line_{block}_"))
             return losses, metrics
+
+
+def _image_size(view, kpts):
+    """view["image_size"] as given, or (w, h) from view["image"].shape[-2:] when a view has none
+    (gluestick.py:146-156, normalize_keypoints :477-482)."""
+    if "image_size" in view:
+        return view["image_size"]
+    h, w = view["image"].shape[-2:]
+    return kpts.new_tensor([[w, h]])
+
+
+def _no_line_outputs(B, L0, L1, device):
+    """The line head's outputs for a view without lines (gluestick.py:293-308)."""
+    return {"line_log_assignment": torch.zeros(B, L0, L1, dtype=torch.float, device=device),
+            "line_matches0": torch.full((B, L0), -1, device=device, dtype=torch.int64),
+            "line_matches1": torch.full((B, L1), -1, device=device, dtype=torch.int64),
+            "line_matching_scores0": torch.zeros((B, L0), device=device, dtype=torch.float32),
+            "line_matching_scores1": torch.zeros((B, L1), device=device, dtype=torch.float32)}
+
+
+def _empty_pred(B, n0, n1, L0, L1, device):
+    """The reference's pred for a view without keypoints (gluestick.py:163-195), key for key.  As there,
+    log_assignment is [B, M, N] (no bin row / column) and line_matching_scores1 is [B, N]."""
+    pred = {"log_assignment": torch.zeros(B, n0, n1, dtype=torch.float, device=device),
+            "matches0": torch.full((B, n0), -1, device=device, dtype=torch.int64),
+            "matches1": torch.full((B, n1), -1, device=device, dtype=torch.int64),
+            "matching_scores0": torch.zeros((B, n0), device=device, dtype=torch.float32),
+            "matching_scores1": torch.zeros((B, n1), device=device, dtype=torch.float32)}
+    pred.update(_no_line_outputs(B, L0, L1, device))
+    pred["line_matching_scores1"] = torch.zeros((B, n1), device=device, dtype=torch.float32)
+    return pred
 
 
 def _line_metrics(pred, data, prefix):

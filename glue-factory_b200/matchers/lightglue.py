@@ -20,7 +20,10 @@ assignment head, its NLL terms, argmax and match filtering, and all of their
 backward passes -- runs in the hand-written sm_90a kernels behind the C ABI
 of include/lgb200.h.  There is no CPU path: without the built library and an
 H100 `forward` raises.  `loss` takes only the pred of this module's own
-`forward`, which carries the per-layer states it needs.
+`forward`, which carries the per-layer states it needs.  `weights` is a path
+or a pretrained name (superpoint, disk, ...) looked up where the reference
+looks, DATA_PATH then torch-hub's cache, and never downloaded
+(matchers/_weights.py).
 
 conf additions over the reference's default_conf:
     precision: "bf16" -> bf16 operands / fp32 accumulation on the Hopper tensor cores (default)
@@ -34,6 +37,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from .. import _lib, engine, ops
+from . import _weights
 
 
 class _Conf(dict):
@@ -181,11 +185,19 @@ class LightGlue(nn.Module):
             "confidence_thresholds",
             torch.tensor([min(max(0.8 + 0.1 * math.exp(-4.0 * i / n), 0.0), 1.0) for i in range(n)]))
         if conf.weights is not None:
-            state_dict = torch.load(conf.weights, map_location="cpu")
+            state_dict = _weights.load_weights(conf.weights, self._weights_candidates(conf), "lightglue")
             for i in range(n):  # legacy names, lightglue.py:384-391
                 state_dict = {k.replace(f"self_attn.{i}", f"transformers.{i}.self_attn"): v for k, v in state_dict.items()}
                 state_dict = {k.replace(f"cross_attn.{i}", f"transformers.{i}.cross_attn"): v for k, v in state_dict.items()}
             self.load_state_dict(state_dict, strict=False)
+
+    @staticmethod
+    def _weights_candidates(conf):
+        """Where the reference looks for `weights` when it is not a path (lightglue.py:365-382): DATA_PATH / weights
+        (skipped without glue-factory), then torch-hub's cache file of the pretrained download."""
+        root = _weights.data_path()
+        hub = _weights.hub_checkpoint(f"{conf.weights}_{conf.weights_from_version}".replace(".", "-") + ".pth")
+        return ([root / str(conf.weights)] if root is not None else []) + [hub]
 
     # ------------------------------------------------------------------------------------------
     @property
