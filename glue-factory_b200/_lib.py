@@ -32,6 +32,9 @@ SIGNATURES = {
     "lgb200_attn_bwd": (_i, [_vp] * 10 + [_i, _i, _i, _i, _i, _f, _i, _vp]),
     "lgb200_attn_fwd_hd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _i, _vp]),
     "lgb200_attn_bwd_hd": (_i, [_vp] * 10 + [_i, _i, _i, _i, _i, _f, _i, _i, _vp]),
+    "lgb200_attn_fwd_varlen": (_i, [_vp] * 9 + [_i, _i, _i, _i, _i, _f, _i, _i, _vp]),
+    "lgb200_adaptive_compact_ws_ints": (_i64, [_i, _i]),
+    "lgb200_adaptive_compact": (_i, [_vp] * 18 + [_f, _f] + [_i] * 10 + [_vp]),
     "lgb200_ln_gelu_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _f, _i, _vp]),
     "lgb200_ln_gelu_bwd_parts": (_i, [_i64]),
     "lgb200_ln_gelu_bwd": (_i, [_vp] * 10 + [_i64, _i, _i, _vp]),
@@ -140,6 +143,7 @@ KERNELS_PER_CALL = {
     "lgb200_attn_fwd_hd": 1, "lgb200_attn_bwd_hd": 3,  # prep + dQ + dKV (fp32: delta + dQ + dKV)
     "lgb200_rope_split_fwd_hd": 1, "lgb200_rope_split_bwd_hd": 1,
     "lgb200_adamw_flat": 1, "lgb200_sgd_flat": 1, "lgb200_rmsprop_flat": 1,
+    "lgb200_attn_fwd_varlen": 1, "lgb200_adaptive_compact": 2,  # decide + gather
 }
 launch_count = 0          # running total of kernels launched through `call`
 timed_entry = None        # entry-point name or a set of names: every call of them is bracketed by CUDA events

@@ -163,6 +163,24 @@ int lgb200_attn_fwd(const void* q, const void* k, const void* v, void* out, floa
   return lgb200_attn_fwd_hd(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, dtype, 64, stream);
 }
 
+int lgb200_attn_fwd_varlen(const void* q, const void* k, const void* v, void* out, float* lse, const int* q_off,
+                           const int* q_len, const int* k_off, const int* k_len, int S, int max_q_len, int Tq, int Tk,
+                           int H, float scale, int dtype, int head_dim, cudaStream_t stream) {
+  LGB_REQUIRE(q && k && v && out && lse && q_off && q_len && k_off && k_len, kErrInvalid,
+              "attn_fwd_varlen: null pointer");
+  LGB_REQUIRE(S >= 0 && max_q_len >= 0 && Tq >= 0 && Tk >= 0 && H > 0, kErrInvalid,
+              "attn_fwd_varlen: bad extents S=%d max_q_len=%d Tq=%d Tk=%d H=%d", S, max_q_len, Tq, Tk, H);
+  LGB_REQUIRE(head_dim == 32 || head_dim == 64, kErrUnsupported, "attn_fwd_varlen: head_dim %d (built for 32 and 64)",
+              head_dim);
+  LGB_REQUIRE(dtype == LGB200_F32 || dtype == LGB200_BF16, kErrInvalid, "attn_fwd_varlen: bad dtype %d", dtype);
+  if (S == 0 || max_q_len == 0 || Tq == 0 || Tk == 0) return 0;  // no sequence has both queries and keys
+  if (dtype == LGB200_F32)
+    return attn_fwd_varlen_simt(q, k, v, out, lse, q_off, q_len, k_off, k_len, S, max_q_len, Tq, H, scale, head_dim,
+                                stream);
+  return attn_fwd_varlen_tc(q, k, v, out, lse, q_off, q_len, k_off, k_len, S, max_q_len, Tq, Tk, H, scale, head_dim,
+                            stream);
+}
+
 int64_t lgb200_attn_bwd_ws_floats(int B, int Nq, int Nk, int H) { return attn_bwd_ws_floats(B, Nq, Nk, H); }
 
 int lgb200_attn_bwd_hd(const void* q, const void* k, const void* v, const void* out, const float* lse,

@@ -7,7 +7,8 @@
 //
 // Tensors are token-major [B, N, H, kD].  The key/value batch of query batch b is
 // (b + kv_shift) % B, which expresses the two directions of cross-attention on the
-// concatenated [image0; image1] batch as ONE launch.
+// concatenated [image0; image1] batch as ONE launch.  The forward also takes packed sequences of
+// different lengths in one token-major [T, H, kD] buffer (attn_fwd_varlen_simt_kernel).
 //
 // Work split: two threads per row ("row" = query in fwd/dq, key in dkv), each owning half of the kD
 // channels; dot products are completed with one shuffle.  The opposite operand is staged through
@@ -30,32 +31,35 @@ __device__ __forceinline__ void load_tile(float (*dst)[kD], const float* src, in
   }
 }
 
-template <int kD>
-__global__ void __launch_bounds__(128) attn_fwd_simt_kernel(const float* __restrict__ q, const float* __restrict__ k,
-                                                            const float* __restrict__ v, float* __restrict__ out,
-                                                            float* __restrict__ lse, int B, int Nq, int Nk, int H,
-                                                            int kv_shift, float scale) {
+// One CTA of the forward: 64 query rows r0.. of head h.  Uniform batches (VARLEN false): query batch b, key batch kb,
+// lse [B, H, Nq].  Packed sequences (VARLEN true): b / kb are the token rows of the sequence's first query / key,
+// Nq / Nk its lengths, lse [H, Tq].
+template <int kD, bool VARLEN>
+__device__ __forceinline__ void attn_fwd_simt_cta(const float* __restrict__ q, const float* __restrict__ k,
+                                                  const float* __restrict__ v, float* __restrict__ out,
+                                                  float* __restrict__ lse, int b, int kb, int r0, int Nq, int Nk,
+                                                  int H, int h, int Tq, float scale) {
   constexpr int kHalf = kD / 2;
   __shared__ float sk[kTile][kD];
   __shared__ float sv[kTile][kD];
-  const int b = blockIdx.z, h = blockIdx.y;
-  const int kb = (b + kv_shift) % B;
-  const int row = blockIdx.x * kTile + (threadIdx.x >> 1);
+  const int row = r0 + (threadIdx.x >> 1);
   const int half = threadIdx.x & 1;
   const int64_t ld = (int64_t)H * kD;
   const bool rvalid = row < Nq;
+  const int64_t qrow = VARLEN ? (int64_t)b + row : (int64_t)b * Nq + row;
+  const int64_t krow = VARLEN ? (int64_t)kb : (int64_t)kb * Nk;
   float qr[kHalf], o[kHalf];
 #pragma unroll
   for (int d = 0; d < kHalf; ++d) {
-    qr[d] = rvalid ? q[((int64_t)b * Nq + row) * ld + h * kD + half * kHalf + d] * scale : 0.f;
+    qr[d] = rvalid ? q[qrow * ld + h * kD + half * kHalf + d] * scale : 0.f;
     o[d] = 0.f;
   }
   float m = -INFINITY, l = 0.f;
   for (int j0 = 0; j0 < Nk; j0 += kTile) {
     const int nv = min(kTile, Nk - j0);
     __syncthreads();
-    load_tile(sk, k + ((int64_t)kb * Nk + j0) * ld + h * kD, ld, nv);
-    load_tile(sv, v + ((int64_t)kb * Nk + j0) * ld + h * kD, ld, nv);
+    load_tile(sk, k + (krow + j0) * ld + h * kD, ld, nv);
+    load_tile(sv, v + (krow + j0) * ld + h * kD, ld, nv);
     __syncthreads();
     for (int j = 0; j < nv; ++j) {
       float s = 0.f;
@@ -78,10 +82,37 @@ __global__ void __launch_bounds__(128) attn_fwd_simt_kernel(const float* __restr
   if (rvalid) {
     const float inv = 1.f / l;
 #pragma unroll
-    for (int d = 0; d < kHalf; ++d)
-      out[((int64_t)b * Nq + row) * ld + h * kD + half * kHalf + d] = o[d] * inv;
-    if (half == 0) lse[((int64_t)b * H + h) * Nq + row] = m + logf(l);
+    for (int d = 0; d < kHalf; ++d) out[qrow * ld + h * kD + half * kHalf + d] = o[d] * inv;
+    if (half == 0) {
+      if constexpr (VARLEN)
+        lse[(int64_t)h * Tq + b + row] = m + logf(l);
+      else
+        lse[((int64_t)b * H + h) * Nq + row] = m + logf(l);
+    }
   }
+}
+
+template <int kD>
+__global__ void __launch_bounds__(128) attn_fwd_simt_kernel(const float* __restrict__ q, const float* __restrict__ k,
+                                                            const float* __restrict__ v, float* __restrict__ out,
+                                                            float* __restrict__ lse, int B, int Nq, int Nk, int H,
+                                                            int kv_shift, float scale) {
+  const int b = blockIdx.z;
+  attn_fwd_simt_cta<kD, false>(q, k, v, out, lse, b, (b + kv_shift) % B, blockIdx.x * kTile, Nq, Nk, H, blockIdx.y, 0,
+                               scale);
+}
+
+// Packed sequences (see attn_fwd_varlen_tc_kernel): sequence s = blockIdx.z
+template <int kD>
+__global__ void __launch_bounds__(128)
+    attn_fwd_varlen_simt_kernel(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
+                                float* __restrict__ out, float* __restrict__ lse, const int* __restrict__ q_off,
+                                const int* __restrict__ q_len, const int* __restrict__ k_off,
+                                const int* __restrict__ k_len, int Tq, int H, float scale) {
+  const int s = blockIdx.z, r0 = blockIdx.x * kTile;
+  const int nq = q_len[s], nk = k_len[s];
+  if (r0 >= nq || nk <= 0) return;
+  attn_fwd_simt_cta<kD, true>(q, k, v, out, lse, q_off[s], k_off[s], r0, nq, nk, H, blockIdx.y, Tq, scale);
 }
 
 // delta[b,h,i] = sum_d dout[b,i,h,d] * out[b,i,h,d]   (8 lanes per row, kD / 8 channels each)
@@ -240,6 +271,19 @@ int attn_fwd_simt(const void* q, const void* k, const void* v, void* out, float*
                   int kv_shift, float scale, int head_dim, cudaStream_t stream) {
   return head_dim == 32 ? attn_fwd_simt_hd<32>(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream)
                         : attn_fwd_simt_hd<64>(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream);
+}
+
+int attn_fwd_varlen_simt(const void* q, const void* k, const void* v, void* out, float* lse, const int* q_off,
+                         const int* q_len, const int* k_off, const int* k_len, int S, int max_q_len, int Tq, int H,
+                         float scale, int head_dim, cudaStream_t stream) {
+  dim3 grid((max_q_len + kTile - 1) / kTile, H, S);
+  if (head_dim == 32)
+    attn_fwd_varlen_simt_kernel<32><<<grid, 128, 0, stream>>>((const float*)q, (const float*)k, (const float*)v,
+                                                              (float*)out, lse, q_off, q_len, k_off, k_len, Tq, H, scale);
+  else
+    attn_fwd_varlen_simt_kernel<64><<<grid, 128, 0, stream>>>((const float*)q, (const float*)k, (const float*)v,
+                                                              (float*)out, lse, q_off, q_len, k_off, k_len, Tq, H, scale);
+  return check_launch("attn_fwd_varlen_simt");
 }
 
 int attn_delta(const void* out, const void* dout, float* delta, int B, int N, int H, int head_dim,

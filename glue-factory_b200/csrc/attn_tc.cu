@@ -93,11 +93,17 @@ __device__ __forceinline__ void store_acc_rows(const float (&d)[D / 2], __nv_bfl
   }
 }
 
-template <int D>
-__global__ void __launch_bounds__(FA_THREADS, 1)
-    attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                       const __grid_constant__ CUtensorMap tmV, __nv_bfloat16* __restrict__ out,
-                       float* __restrict__ lse, int B, int Nq, int Nk, int H, int kv_shift, float scale_log2) {
+// One CTA of the forward: query tile q0 of head h.  Uniform batches (VARLEN false): TMA coordinates (.., q0, b) and
+// (.., key row, kb) of the 4-D maps, rows past Nq / keys past Nk are the map's zero fill.  Packed sequences (VARLEN
+// true): 3-D maps over [T, H, D], the sequence's queries start at token row b and its keys at row kb; Nq / Nk are
+// the sequence's lengths and Tq the query map's token count (row pitch of lse [H, Tq]).  Rows of the tiles past a
+// sequence's end hold the next sequence's tokens: their keys are masked out like the padding, their queries are not
+// stored.
+template <int D, bool VARLEN>
+__device__ __forceinline__ void attn_fwd_tc_cta(const CUtensorMap* tmQ, const CUtensorMap* tmK, const CUtensorMap* tmV,
+                                                __nv_bfloat16* __restrict__ out, float* __restrict__ lse, int q0,
+                                                int h, int b, int kb, int Nq, int Nk, int H, int Tq,
+                                                float scale_log2) {
   using G = Hd<D>;
   constexpr int FA_QBYTES = G::QBYTES, FA_KBYTES = G::KBYTES;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -110,8 +116,6 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
   uint64_t* kv_empty = kv_full + FA_STAGES;   // [FA_STAGES]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * FA_BM, h = blockIdx.y, b = blockIdx.z;
-  const int kb = (b + kv_shift) % B;
   const int ntiles = (Nk + FA_BN - 1) / FA_BN;
 
   if (threadIdx.x == 0) {
@@ -124,22 +128,30 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
     mbar_fence_init();
   }
   if (warp == FA_PRODUCER && lane == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
+    tma_prefetch_desc(tmQ);
+    tma_prefetch_desc(tmK);
+    tma_prefetch_desc(tmV);
   }
   __syncthreads();
 
   if (warp == FA_PRODUCER) {
     if (lane == 0) {
       mbar_expect_tx(q_full, FA_QBYTES);
-      tma_load_4d(sQ, &tmQ, q_full, 0, h, q0, b);
+      if constexpr (VARLEN)
+        tma_load_3d(sQ, tmQ, q_full, 0, h, b + q0);
+      else
+        tma_load_4d(sQ, tmQ, q_full, 0, h, q0, b);
       for (int j = 0; j < ntiles; ++j) {
         const int s = j % FA_STAGES;
         mbar_wait(&kv_empty[s], ((j / FA_STAGES) & 1) ^ 1);
         mbar_expect_tx(&kv_full[s], 2 * FA_KBYTES);
-        tma_load_4d(sK + s * FA_KBYTES, &tmK, &kv_full[s], 0, h, j * FA_BN, kb);
-        tma_load_4d(sV + s * FA_KBYTES, &tmV, &kv_full[s], 0, h, j * FA_BN, kb);
+        if constexpr (VARLEN) {
+          tma_load_3d(sK + s * FA_KBYTES, tmK, &kv_full[s], 0, h, kb + j * FA_BN);
+          tma_load_3d(sV + s * FA_KBYTES, tmV, &kv_full[s], 0, h, kb + j * FA_BN);
+        } else {
+          tma_load_4d(sK + s * FA_KBYTES, tmK, &kv_full[s], 0, h, j * FA_BN, kb);
+          tma_load_4d(sV + s * FA_KBYTES, tmV, &kv_full[s], 0, h, j * FA_BN, kb);
+        }
       }
     }
     return;
@@ -246,9 +258,42 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
       o[4 * jj + 2 * i + 1] *= inv;
     }
     const int row = rbase + 8 * i;
-    if (t4 == 0 && row < Nq) lse[((int64_t)b * H + h) * Nq + row] = (m[i] + log2f(l[i])) * kLn2;
+    if constexpr (VARLEN) {
+      if (t4 == 0 && row < Nq) lse[(int64_t)h * Tq + b + row] = (m[i] + log2f(l[i])) * kLn2;
+    } else {
+      if (t4 == 0 && row < Nq) lse[((int64_t)b * H + h) * Nq + row] = (m[i] + log2f(l[i])) * kLn2;
+    }
   }
-  store_acc_rows<D>(o, out, b, Nq, H, h, q0 + wg * 64, 1.f);
+  if constexpr (VARLEN)
+    store_acc_rows<D>(o, out + (int64_t)b * H * D, 0, Nq, H, h, q0 + wg * 64, 1.f);
+  else
+    store_acc_rows<D>(o, out, b, Nq, H, h, q0 + wg * 64, 1.f);
+}
+
+template <int D>
+__global__ void __launch_bounds__(FA_THREADS, 1)
+    attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                       const __grid_constant__ CUtensorMap tmV, __nv_bfloat16* __restrict__ out,
+                       float* __restrict__ lse, int B, int Nq, int Nk, int H, int kv_shift, float scale_log2) {
+  const int b = blockIdx.z;
+  attn_fwd_tc_cta<D, false>(&tmQ, &tmK, &tmV, out, lse, blockIdx.x * FA_BM, blockIdx.y, b, (b + kv_shift) % B, Nq, Nk,
+                            H, 0, scale_log2);
+}
+
+// Packed sequences: sequence s = blockIdx.z has queries [q_off[s], q_off[s] + q_len[s]) and keys / values
+// [k_off[s], k_off[s] + k_len[s]) of the token-major [T, H, D] buffers.  The grid covers the longest sequence; the
+// CTAs of query tiles past a sequence's length, and every CTA of a sequence without queries or keys, exit at once.
+template <int D>
+__global__ void __launch_bounds__(FA_THREADS, 1)
+    attn_fwd_varlen_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                              const __grid_constant__ CUtensorMap tmV, __nv_bfloat16* __restrict__ out,
+                              float* __restrict__ lse, const int* __restrict__ q_off, const int* __restrict__ q_len,
+                              const int* __restrict__ k_off, const int* __restrict__ k_len, int Tq, int H,
+                              float scale_log2) {
+  const int s = blockIdx.z, q0 = blockIdx.x * FA_BM;
+  const int nq = q_len[s], nk = k_len[s];
+  if (q0 >= nq || nk <= 0) return;
+  attn_fwd_tc_cta<D, true>(&tmQ, &tmK, &tmV, out, lse, q0, blockIdx.y, q_off[s], k_off[s], nq, nk, H, Tq, scale_log2);
 }
 
 // 4-D tensor map over the token-major [B, N, H, D] layout: boxes of box_rows tokens of one head, swizzled by the row
@@ -280,6 +325,42 @@ int attn_fwd_tc(const void* q, const void* k, const void* v, void* out, float* l
                 int kv_shift, float scale, int head_dim, cudaStream_t stream) {
   return head_dim == 32 ? attn_fwd_tc_hd<32>(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream)
                         : attn_fwd_tc_hd<64>(q, k, v, out, lse, B, Nq, Nk, H, kv_shift, scale, stream);
+}
+
+// 3-D tensor map over a packed token-major [T, H, D] buffer: boxes of box_rows tokens of one head
+template <int D>
+static int make_packed_tmap(CUtensorMap* tm, const void* base, int T, int H, int box_rows) {
+  const uint64_t dims[3] = {D, (uint64_t)H, (uint64_t)T};
+  const uint64_t str[2] = {D * 2, (uint64_t)H * D * 2};
+  const uint32_t box[3] = {D, 1, (uint32_t)box_rows};
+  return make_tmap_bf16(tm, base, 3, dims, str, box, Hd<D>::ROW);
+}
+
+template <int D>
+static int attn_fwd_varlen_tc_hd(const void* q, const void* k, const void* v, void* out, float* lse, const int* q_off,
+                                 const int* q_len, const int* k_off, const int* k_len, int S, int max_q_len, int Tq,
+                                 int Tk, int H, float scale, cudaStream_t stream) {
+  constexpr int FA_SMEM = Hd<D>::SMEM;
+  CUtensorMap tq, tk, tv;
+  int rc;
+  if ((rc = make_packed_tmap<D>(&tq, q, Tq, H, FA_BM))) return rc;
+  if ((rc = make_packed_tmap<D>(&tk, k, Tk, H, FA_BN))) return rc;
+  if ((rc = make_packed_tmap<D>(&tv, v, Tk, H, FA_BN))) return rc;
+  if ((rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_fwd_varlen_tc_kernel<D>), FA_SMEM))) return rc;
+  dim3 grid((max_q_len + FA_BM - 1) / FA_BM, H, S);
+  attn_fwd_varlen_tc_kernel<D><<<grid, FA_THREADS, FA_SMEM, stream>>>(tq, tk, tv, static_cast<__nv_bfloat16*>(out), lse,
+                                                                      q_off, q_len, k_off, k_len, Tq, H,
+                                                                      scale * kLog2e);
+  return check_launch("attn_fwd_varlen_tc");
+}
+
+int attn_fwd_varlen_tc(const void* q, const void* k, const void* v, void* out, float* lse, const int* q_off,
+                       const int* q_len, const int* k_off, const int* k_len, int S, int max_q_len, int Tq, int Tk,
+                       int H, float scale, int head_dim, cudaStream_t stream) {
+  return head_dim == 32 ? attn_fwd_varlen_tc_hd<32>(q, k, v, out, lse, q_off, q_len, k_off, k_len, S, max_q_len, Tq,
+                                                    Tk, H, scale, stream)
+                        : attn_fwd_varlen_tc_hd<64>(q, k, v, out, lse, q_off, q_len, k_off, k_len, S, max_q_len, Tq,
+                                                    Tk, H, scale, stream);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -1634,3 +1634,219 @@ int lgb200_head_token_bwd(const float* x, const void* dmdw, const float* dzt, co
 }
 
 }  // extern "C"
+
+namespace lgb {
+
+// ---------------------------------------------------------------------------------------------
+// LightGlue's adaptive depth / width on a batch of pairs (lightglue.py:461-526, 545-576), one layer's step.
+// The tokens of pair b are two segments of the packed [T, D] state: image 0 is segment 2b, image 1 segment 2b + 1,
+// described by seg [4][2B] = (offset, length, partner's offset, partner's length).
+//   decide (one CTA per pair): a pair with tokens left stops when 1 - #(token confidence < thr) / (M + N) exceeds
+//     depth_conf (or always, on the last layer); a stopped pair's tokens move, unpruned, to the pair's block of the
+//     final buffer (b (M + N), image 1 at + M).  Otherwise a token stays when its matchability > width_thr or, with
+//     early stopping on, its confidence is still <= thr; a block scan per segment gives each kept token its place,
+//     and its prune counter (original keypoint index ind[t]) goes up by one.  The sigmoids are 1 / (1 + exp(-z)) in
+//     fp32, as torch.sigmoid computes them, so every decision is the one the one-pair loop made.
+//   gather (grid-stride, one warp per token row): every CTA scans the kept counts into the new segment offsets
+//     (pair-major: pair 0 image 0, pair 0 image 1, pair 1 image 0, ...) and copies x, theta and ind of its rows; CTA 0
+//     writes the new seg and status = (kept tokens, 1 if a continuing pair kept no token of a view).
+// ---------------------------------------------------------------------------------------------
+constexpr int kAcThreads = 1024;
+
+__device__ __forceinline__ float sigmoid_f32(float z) { return 1.f / (1.f + expf(-z)); }
+
+// exclusive prefix sum over the CTA (every thread calls it); *total = the sum over the CTA
+__device__ __forceinline__ int block_exclusive_scan(int v, int* sh, int* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  int x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) sh[warp] = x;
+  __syncthreads();
+  if (warp == 0) {
+    int w = lane < nw ? sh[lane] : 0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, w, o);
+      if (lane >= o) w += y;
+    }
+    sh[lane] = w;
+  }
+  __syncthreads();
+  const int r = (warp ? sh[warp - 1] : 0) + x - v;
+  *total = sh[nw - 1];
+  __syncthreads();
+  return r;
+}
+
+__global__ void __launch_bounds__(kAcThreads)
+    adaptive_decide_kernel(const int* __restrict__ ind, const float* __restrict__ zt, const int* __restrict__ seg,
+                           int* __restrict__ fin_len, int* __restrict__ stop_layer, int64_t* __restrict__ prune0,
+                           int64_t* __restrict__ prune1, int* __restrict__ dst_seg, int* __restrict__ dst_pos,
+                           int* __restrict__ cnt, int* __restrict__ state, const float* __restrict__ conf_thr,
+                           float depth_conf, float width_thr, int do_stop, int do_prune, int layer, int finish, int B,
+                           int M, int N) {
+  __shared__ int sh[32];
+  __shared__ int s_low;
+  const int b = blockIdx.x, S = 2 * B;
+  const int off0 = seg[2 * b], off1 = seg[2 * b + 1], n0 = seg[S + 2 * b], n1 = seg[S + 2 * b + 1];
+  if (n0 == 0 && n1 == 0) {  // stopped at an earlier layer
+    if (threadIdx.x == 0) {
+      cnt[2 * b] = cnt[2 * b + 1] = 0;
+      state[b] = 0;
+    }
+    return;
+  }
+  const bool conf = do_stop && !finish;
+  const float thr = conf ? *conf_thr : 0.f;
+  bool stop = finish;
+  if (conf) {
+    if (threadIdx.x == 0) s_low = 0;
+    __syncthreads();
+    int c = 0;
+    for (int i = threadIdx.x; i < n0 + n1; i += blockDim.x) {
+      const int t = i < n0 ? off0 + i : off1 + i - n0;
+      c += sigmoid_f32(zt[2 * t + 1]) < thr;
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+    if ((threadIdx.x & 31) == 0) atomicAdd(&s_low, c);
+    __syncthreads();
+    // relative to the pair's ORIGINAL point count (lightglue.py:489), in fp32 as the one-pair loop computes it
+    stop = 1.f - (float)s_low / (float)(M + N) > depth_conf;
+  }
+  if (stop) {
+    for (int i = threadIdx.x; i < n0 + n1; i += blockDim.x) {
+      const int t = i < n0 ? off0 + i : off1 + i - n0;
+      dst_seg[t] = -2;
+      dst_pos[t] = b * (M + N) + (i < n0 ? i : M + i - n0);
+    }
+    if (threadIdx.x == 0) {
+      fin_len[2 * b] = n0;
+      fin_len[2 * b + 1] = n1;
+      stop_layer[b] = layer;
+      cnt[2 * b] = cnt[2 * b + 1] = 0;
+      state[b] = 0;
+    }
+    return;
+  }
+  for (int img = 0; img < 2; ++img) {
+    const int off = img ? off1 : off0, n = img ? n1 : n0;
+    int64_t* prune = img ? prune1 + (int64_t)b * N : prune0 + (int64_t)b * M;
+    int base = 0;
+    for (int c0 = 0; c0 < n; c0 += blockDim.x) {  // uniform trip count: every thread reaches the scan's barriers
+      const int i = c0 + threadIdx.x;
+      bool keep = i < n;
+      if (keep && do_prune) {
+        const int t = off + i;
+        // low-confidence points are never pruned (lightglue.py:556-557)
+        keep = sigmoid_f32(zt[2 * t]) > width_thr || (do_stop && sigmoid_f32(zt[2 * t + 1]) <= thr);
+      }
+      int tot;
+      const int p = block_exclusive_scan(keep ? 1 : 0, sh, &tot);
+      if (i < n) {
+        const int t = off + i;
+        dst_seg[t] = keep ? 2 * b + img : -1;
+        dst_pos[t] = base + p;
+        if (keep && do_prune) prune[ind[t]] += 1;
+      }
+      base += tot;
+    }
+    if (threadIdx.x == 0) cnt[2 * b + img] = base;
+  }
+  if (threadIdx.x == 0) state[b] = 1;
+}
+
+__global__ void __launch_bounds__(256)
+    adaptive_gather_kernel(const float* __restrict__ x, const float* __restrict__ theta, const int* __restrict__ ind,
+                           const int* __restrict__ dst_seg, const int* __restrict__ dst_pos,
+                           const int* __restrict__ cnt, const int* __restrict__ state, float* __restrict__ x_out,
+                           float* __restrict__ theta_out, int* __restrict__ ind_out, float* __restrict__ x_fin,
+                           int* __restrict__ ind_fin, int* __restrict__ seg_out, int* __restrict__ status, int B, int T,
+                           int D, int R) {
+  extern __shared__ int s_off[];  // [2B] offsets of the new segments
+  __shared__ int sh[32];
+  const int S = 2 * B;
+  {
+    const int per = (S + blockDim.x - 1) / blockDim.x, s0 = threadIdx.x * per;
+    int loc = 0;
+    for (int s = s0; s < s0 + per && s < S; ++s) loc += cnt[s];
+    int tot;
+    int run = block_exclusive_scan(loc, sh, &tot);
+    for (int s = s0; s < s0 + per && s < S; ++s) {
+      s_off[s] = run;
+      run += cnt[s];
+    }
+    __syncthreads();
+    if (blockIdx.x == 0) {
+      for (int s = threadIdx.x; s < S; s += blockDim.x) {
+        seg_out[s] = s_off[s];
+        seg_out[S + s] = cnt[s];
+        seg_out[2 * S + s] = s_off[s ^ 1];
+        seg_out[3 * S + s] = cnt[s ^ 1];
+      }
+      bool emptied = false;
+      for (int b = threadIdx.x; b < B; b += blockDim.x) emptied |= state[b] && (cnt[2 * b] == 0 || cnt[2 * b + 1] == 0);
+      emptied = __syncthreads_or(emptied);
+      if (threadIdx.x == 0) {
+        status[0] = tot;
+        status[1] = emptied ? 1 : 0;
+      }
+    }
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int64_t t = (int64_t)blockIdx.x * 8 + warp; t < T; t += (int64_t)gridDim.x * 8) {
+    const int sg = dst_seg[t];
+    if (sg == -1) continue;  // pruned
+    const bool fin = sg == -2;
+    const int64_t dst = fin ? (int64_t)dst_pos[t] : (int64_t)s_off[sg] + dst_pos[t];
+    const float4* src = reinterpret_cast<const float4*>(x + t * D);
+    float4* dx = reinterpret_cast<float4*>((fin ? x_fin : x_out) + dst * D);
+    for (int c = lane; c < D / 4; c += 32) dx[c] = src[c];
+    if (!fin)
+      for (int c = lane; c < R; c += 32) theta_out[dst * R + c] = theta[t * R + c];
+    if (lane == 0) (fin ? ind_fin : ind_out)[dst] = ind[t];
+  }
+}
+
+}  // namespace lgb
+
+extern "C" {
+
+int64_t lgb200_adaptive_compact_ws_ints(int T, int B) { return 2 * (int64_t)T + 3 * (int64_t)B; }
+
+int lgb200_adaptive_compact(const float* x, const float* theta, const int* ind, const float* zt, const int* seg,
+                            float* x_out, float* theta_out, int* ind_out, int* seg_out, float* x_fin, int* ind_fin,
+                            int* fin_len, int* stop_layer, int64_t* prune0, int64_t* prune1, int* status, int* ws,
+                            const float* conf_thr, float depth_conf, float width_thr, int do_stop, int do_prune,
+                            int layer, int finish, int B, int M, int N, int T, int D, int R, cudaStream_t stream) {
+  LGB_REQUIRE(x && theta && ind && seg && x_out && theta_out && ind_out && seg_out && x_fin && ind_fin && fin_len &&
+                  stop_layer && prune0 && prune1 && status && ws,
+              kErrInvalid, "adaptive_compact: null pointer");
+  LGB_REQUIRE(finish || ((zt != nullptr) && (!do_stop || conf_thr != nullptr)), kErrInvalid,
+              "adaptive_compact: the stop / prune decisions need zt (and conf_thr with early stopping)");
+  LGB_REQUIRE(B > 0 && B <= 4096 && M > 0 && N > 0 && T > 0 && (int64_t)T <= (int64_t)B * (M + N), kErrInvalid,
+              "adaptive_compact: bad extents B=%d M=%d N=%d T=%d", B, M, N, T);
+  LGB_REQUIRE(D > 0 && D % 4 == 0 && R > 0 && aligned16({x, x_out, x_fin}), kErrInvalid,
+              "adaptive_compact: D=%d must be a multiple of 4 and x / x_out / x_fin 16-byte aligned", D);
+  int* dst_seg = ws;
+  int* dst_pos = ws + T;
+  int* cnt = ws + 2 * (int64_t)T;
+  int* state = cnt + 2 * B;
+  adaptive_decide_kernel<<<B, kAcThreads, 0, stream>>>(ind, zt, seg, fin_len, stop_layer, prune0, prune1, dst_seg,
+                                                       dst_pos, cnt, state, conf_thr, depth_conf, width_thr, do_stop,
+                                                       do_prune, layer, finish, B, M, N);
+  int rc = check_launch("adaptive_decide");
+  if (rc) return rc;
+  const int64_t rows = ((int64_t)T + 7) / 8, cap = 4 * (int64_t)device_sm_count();
+  adaptive_gather_kernel<<<(unsigned)(rows < cap ? rows : cap), 256, 2 * B * sizeof(int), stream>>>(
+      x, theta, ind, dst_seg, dst_pos, cnt, state, x_out, theta_out, ind_out, x_fin, ind_fin, seg_out, status, B, T, D,
+      R);
+  return check_launch("adaptive_gather");
+}
+
+}  // extern "C"
+

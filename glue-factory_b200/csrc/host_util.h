@@ -25,6 +25,9 @@ int attn_bwd_simt(const void* q, const void* k, const void* v, const void* out, 
                   int head_dim, cudaStream_t stream);
 int attn_delta(const void* out, const void* dout, float* delta, int B, int N, int H, int head_dim,
                cudaStream_t stream);
+int attn_fwd_varlen_simt(const void* q, const void* k, const void* v, void* out, float* lse, const int* q_off,
+                         const int* q_len, const int* k_off, const int* k_len, int S, int max_q_len, int Tq, int H,
+                         float scale, int head_dim, cudaStream_t stream);
 
 // wgmma attention (attn_tc.cu); head_dim as above, the shared-qk backward at 64 only
 int attn_fwd_tc(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Nq, int Nk, int H,
@@ -32,6 +35,9 @@ int attn_fwd_tc(const void* q, const void* k, const void* v, void* out, float* l
 int attn_bwd_tc(const void* q, const void* k, const void* v, const void* out, const float* lse, const void* dout,
                 void* dq, void* dk, void* dv, float* delta, int B, int Nq, int Nk, int H, int kv_shift, float scale,
                 int head_dim, cudaStream_t stream);
+int attn_fwd_varlen_tc(const void* q, const void* k, const void* v, void* out, float* lse, const int* q_off,
+                       const int* q_len, const int* k_off, const int* k_len, int S, int max_q_len, int Tq, int Tk,
+                       int H, float scale, int head_dim, cudaStream_t stream);
 
 // lgb200_attn_bwd's shared-qk cross-attention case (q == k, dq == dk, both directions in one batch)
 inline bool attn_bwd_is_shared_qk(const void* q, const void* k, const void* dq, const void* dk, int B, int Nq, int Nk,

@@ -16,6 +16,8 @@ and weight-gradient contractions -- runs on the library's own persistent wgmma G
 fp32 accumulate-into-dx epilogues; `ops.wgrad_bf16`: split-K, fp32 out); no cuBLAS kernel is launched.  The fp32
 parity mode (`precision: fp32`) keeps fp32 cuBLAS (`torch.addmm/mm`) for the projections.
 """
+from typing import NamedTuple
+
 import torch
 import torch.nn.functional as F
 
@@ -89,12 +91,27 @@ def _dgrad_acc(acc, dy, w):
     return ops.linear(dy, w, out=acc, w_is_kn=True, accumulate=True)
 
 
+class Ragged(NamedTuple):
+    """`sizes` of a forward-only layer over pairs of different lengths (adaptive depth / width): seg [4, 2B] int32 on
+    the device = (offset, length, partner's offset, partner's length) of segment 2b (image 0 of pair b) and 2b + 1
+    (image 1); max_len bounds every length."""
+    seg: torch.Tensor
+    max_len: int
+
+
 def _attend_fwd(q, k, v, sizes, H, cross):
     """q,k,v [T, H*hd] over tokens [image0 (B*M); image1 (B*N)] -> (out [T, H*hd], lse tuple).  The head dim hd = 64 or
-    32 is read from the shapes; the scale is hd^-1/2 (lightglue.py:139, 173)."""
-    B, M, N = sizes
+    32 is read from the shapes; the scale is hd^-1/2 (lightglue.py:139, 173).  Ragged sizes: one launch over the
+    packed segments, each attending to itself (self) or to its partner (cross)."""
     hd = q.shape[1] // H
     scale = hd ** -0.5
+    if isinstance(sizes, Ragged):
+        off, ln, poff, pln = sizes.seg
+        shp = (q.shape[0], H, hd)
+        out, lse = ops.attn_fwd_varlen(q.view(shp), k.view(shp), v.view(shp), off, ln, poff if cross else off,
+                                       pln if cross else ln, sizes.max_len, scale)
+        return out.view(q.shape), (lse,)
+    B, M, N = sizes
     if M == N:
         shp = (2 * B, M, H, hd)
         out, lse = ops.attn_fwd(q.view(shp), k.view(shp), v.view(shp), B if cross else 0, scale)

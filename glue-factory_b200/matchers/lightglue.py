@@ -25,6 +25,17 @@ or a pretrained name (superpoint, disk, ...) looked up where the reference
 looks, DATA_PATH then torch-hub's cache, and never downloaded
 (matchers/_weights.py).
 
+Adaptive depth / width (`depth_confidence` / `width_confidence` > 0, eval mode) takes any batch size; every pair
+stops and is pruned on its own, with the result it would have alone.  For one pair the outputs keep the reference's
+shapes: `log_assignment` [1, m+1, n+1] over the m / n points left at the end, `stop_layer` an int.  For B > 1 pairs:
+    log_assignment        [B, M+1, N+1] in the original keypoint indexing; the rows / columns of pruned points are
+                          -inf, the dustbin row and column are kept
+    stop_layer            [B] int64 tensor, the layer whose assignment head each pair used
+    ref_descriptors{0,1}  [B, 1, M|N, D], each pair's final state in the original indexing, zero at pruned points
+    matches*, matching_scores*, prune*: the shapes of the plain forward and the dtypes of the one-pair call (prune*
+                          int64 layer counts with width_confidence, else fp32 n_layers as in the plain forward)
+`loss` refuses such a pred (ValueError).
+
 conf additions over the reference's default_conf:
     precision: "bf16" -> bf16 operands / fp32 accumulation on the Hopper tensor cores (default)
                "fp32" -> full-precision parity path (CUDA cores + fp32 cuBLAS)
@@ -149,7 +160,7 @@ class LightGlue(nn.Module):
         "num_heads": 4,
         "flash": False,  # accepted for config compatibility; attention is always the fused kernel
         "mp": False,
-        "depth_confidence": -1,  # > 0: early stopping at inference (eval mode, one pair; _forward_adaptive)
+        "depth_confidence": -1,  # > 0: early stopping at inference (eval mode, each pair on its own; _forward_adaptive)
         "width_confidence": -1,  # > 0: point pruning at inference
         "filter_threshold": 0.0,
         "checkpointed": False,  # accepted; the fused attention keeps no N x N activations to checkpoint
@@ -341,78 +352,119 @@ class LightGlue(nn.Module):
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
     def _forward_adaptive(self, x, theta, sizes):
-        """Inference-time adaptive depth / width (lightglue.py:461-526, 545-576; eval only, one pair): after every
-        layer but the last, (a) stop when the fraction of confident points exceeds depth_confidence, (b) drop the points
-        predicted unmatchable (matchability <= 1 - width_confidence) unless their confidence is still low, compacting the
-        token matrix and the rotary angles with index_select.  The layers run on the same kernels (M != N after the
-        first pruning); the two per-token logits come from one head_token pass.  On an early stop the assignment head of
-        the stopping layer is used (upstream LightGlue's behaviour; the in-tree reference cannot take that branch: it
-        stacks an empty list after the break, lightglue.py:485-492, 533)."""
+        """Inference-time adaptive depth / width (lightglue.py:461-526, 545-576; eval only), every pair on its own: after
+        every layer but the last, (a) a pair stops when the fraction of its confident points exceeds depth_confidence,
+        (b) a pair that goes on drops the points predicted unmatchable (matchability <= 1 - width_confidence) unless their
+        confidence is still low.  The pairs' tokens stay packed in one [T, D] state whose segments shrink layer by layer
+        (ops.adaptive_compact, one stop / prune / gather step per layer on the device); the layers run on the same GEMM
+        kernels and on the length-aware attention (engine.Ragged), and a stopped pair has no tokens in later layers.  The
+        only host read per layer is the kept-token count, which sizes the next layer.  A pair's assignment comes from
+        the head of the layer it stopped at (upstream LightGlue's behaviour; the in-tree reference cannot take that
+        branch: it stacks an empty list after the break, lightglue.py:485-492, 533).  Pairs with the same stop layer and
+        the same point counts (no pruning) run their head as one batch; a pair whose counts no other pair shares runs
+        it alone.  The results are scattered back to the original keypoint indices (lightglue.py:517-526).  See the
+        module docstring for the output shapes at B > 1."""
         conf = self.conf
         B, M, N = sizes
-        assert B == 1, "adaptive depth / width runs one pair at a time (lightglue.py:487, 492)"
         dev, D, L = x.device, conf.descriptor_dim, conf.n_layers
         do_stop, do_prune = conf.depth_confidence > 0, conf.width_confidence > 0
-        ind0, ind1 = torch.arange(M, device=dev), torch.arange(N, device=dev)
-        prune0 = torch.ones(1, M, device=dev, dtype=torch.int64)
-        prune1 = torch.ones(1, N, device=dev, dtype=torch.int64)
-        m, n = M, N
-        last = L - 1
+        i32 = dict(device=dev, dtype=torch.int32)
+        # tokens [image 0 of every pair; image 1 of every pair] as _forward packed them; segment 2b / 2b + 1 = pair b
+        off = torch.stack([torch.arange(B) * M, B * M + torch.arange(B) * N], 1).reshape(-1)
+        ln = torch.tensor([M, N]).repeat(B)
+        seg = torch.stack([off, ln, off.view(B, 2).flip(1).reshape(-1), ln.view(B, 2).flip(1).reshape(-1)]).to(**i32)
+        ind = torch.cat([torch.arange(M, **i32).repeat(B), torch.arange(N, **i32).repeat(B)])
+        fin = {"x": torch.empty(B * (M + N), D, device=dev), "ind": torch.empty(B * (M + N), **i32),
+               "len": torch.zeros(2 * B, **i32), "stop": torch.full((B,), L - 1, **i32),
+               "prune0": torch.ones(B, M, device=dev, dtype=torch.int64),
+               "prune1": torch.ones(B, N, device=dev, dtype=torch.int64)}
+        ragged = engine.Ragged(seg, max(M, N))
         for i in range(L):
             w, params = self._layer_weights(i)
-            x = engine.LayerFn.apply(x, theta, (1, m, n), conf.num_heads, self._cdt, self.transformers[i].self_attn.ffn[1].eps,
+            x = engine.LayerFn.apply(x, theta, ragged, conf.num_heads, self._cdt, self.transformers[i].self_attn.ffn[1].eps,
                                      w, None, *params)
-            if i == L - 1:
+            zt = None
+            if i < L - 1:
+                la, tk = self.log_assignment[i], self.token_confidence[i].token[0]
+                _, zt, _, _ = ops.head_token_fwd(x, la.matchability.weight.view(-1), la.matchability.bias,
+                                                 tk.weight.view(-1), tk.bias, self._cdt)
+            x, theta, ind, seg, status = ops.adaptive_compact(
+                x, theta, ind, zt, ragged.seg, fin, i, sizes, conf_thr=self.confidence_thresholds[i:i + 1].float(),
+                depth_conf=conf.depth_confidence, width_conf=conf.width_confidence, finish=i == L - 1)
+            kept, emptied = status.tolist()  # the layer loop's one host read: it sizes the next layer
+            assert not emptied, "point pruning removed every keypoint of a view"
+            if kept == 0:
                 break
-            la, tk = self.log_assignment[i], self.token_confidence[i].token[0]
-            _, zt, _, _ = ops.head_token_fwd(x, la.matchability.weight.view(-1), la.matchability.bias, tk.weight.view(-1),
-                                             tk.bias, self._cdt)
-            token = torch.sigmoid(zt[:, 1]) if do_stop else None  # token confidences only exist with early stopping on
-            if do_stop:
-                thr = self.confidence_thresholds[i]
-                ratio = 1.0 - (token < thr).float().sum() / (M + N)  # relative to the ORIGINAL point count (lightglue.py:489)
-                if bool(ratio > conf.depth_confidence):
-                    last = i
-                    break
-            if do_prune:
-                keep = torch.sigmoid(zt[:, 0]) > (1 - conf.width_confidence)
-                if token is not None:  # low-confidence points are never pruned (lightglue.py:556-557)
-                    keep = keep | (token <= self.confidence_thresholds[i])
-                k0, k1 = torch.where(keep[:m])[0], torch.where(keep[m:])[0]
-                ind0, ind1 = ind0.index_select(0, k0), ind1.index_select(0, k1)
-                sel = torch.cat([k0, k1 + m])
-                x, theta = x.index_select(0, sel).contiguous(), theta.index_select(0, sel).contiguous()
-                m, n = int(k0.numel()), int(k1.numel())
-                assert m > 0 and n > 0, "point pruning removed every keypoint of a view"
-                prune0[:, ind0] += 1
-                prune1[:, ind1] += 1
-        d0, d1 = x[:m].view(1, m, D), x[m:].view(1, n, D)
-        md0, md1, z0, z1 = self._head_inputs(d0, d1, last)
-        sim = engine.similarity(md0, md1, self._cdt)
-        st = ops.assign_stats(sim, F.logsigmoid(z0), F.logsigmoid(z1), F.logsigmoid(-z0), F.logsigmoid(-z1), dense=True)
-        m0, m1, ms0, ms1 = ops.filter_matches(st["rowmax"], st["rowarg"], st["colarg"], conf.filter_threshold)
-        if do_prune:  # scatter back to the full keypoint sets (lightglue.py:517-526)
-            m0_ = torch.full((1, M), -1, device=dev, dtype=m0.dtype)
-            m1_ = torch.full((1, N), -1, device=dev, dtype=m1.dtype)
-            m0_[:, ind0] = torch.where(m0 == -1, -1, ind1[None].gather(1, m0.clamp(min=0)))
-            m1_[:, ind1] = torch.where(m1 == -1, -1, ind0[None].gather(1, m1.clamp(min=0)))
-            ms0_, ms1_ = torch.zeros(1, M, device=dev), torch.zeros(1, N, device=dev)
-            ms0_[:, ind0] = ms0
-            ms1_[:, ind1] = ms1
-            m0, m1, ms0, ms1 = m0_, m1_, ms0_, ms1_
-        else:
+            x, theta, ind = x[:kept], theta[:kept], ind[:kept]
+            ragged = engine.Ragged(seg, max(M, N))
+        lens_stop = torch.cat([fin["len"], fin["stop"]]).tolist()
+        lens, stops = lens_stop[:2 * B], lens_stop[2 * B:]
+        xf, indf = fin["x"], fin["ind"].long()
+        m0 = torch.full((B, M), -1, device=dev, dtype=torch.int64)
+        m1 = torch.full((B, N), -1, device=dev, dtype=torch.int64)
+        ms0, ms1 = torch.zeros(B, M, device=dev), torch.zeros(B, N, device=dev)
+        # pairs with the same stop layer and the same point counts share one batched head; after pruning the counts
+        # differ from pair to pair, and such pairs run their head alone
+        groups = {}
+        for b in range(B):
+            groups.setdefault((stops[b], lens[2 * b], lens[2 * b + 1]), []).append(b)
+        heads = []
+        for (layer, m, n), bs in sorted(groups.items()):
+            if len(bs) == 1:
+                base = bs[0] * (M + N)
+                r0, r1 = slice(base, base + m), slice(base + M, base + M + n)
+                d0, d1 = xf[r0].view(1, m, D), xf[r1].view(1, n, D)
+                i0, i1 = indf[r0].view(1, m), indf[r1].view(1, n)
+            else:
+                base = torch.tensor(bs, device=dev)[:, None] * (M + N)
+                r0 = (base + torch.arange(m, device=dev)).view(-1)
+                r1 = (base + M + torch.arange(n, device=dev)).view(-1)
+                d0, d1 = xf.index_select(0, r0).view(-1, m, D), xf.index_select(0, r1).view(-1, n, D)
+                i0, i1 = indf.index_select(0, r0).view(-1, m), indf.index_select(0, r1).view(-1, n)
+            md0, md1, z0, z1 = self._head_inputs(d0, d1, layer)
+            sim = engine.similarity(md0, md1, self._cdt)
+            st = ops.assign_stats(sim, F.logsigmoid(z0), F.logsigmoid(z1), F.logsigmoid(-z0), F.logsigmoid(-z1),
+                                  dense=True)
+            a0, a1, s0, s1 = ops.filter_matches(st["rowmax"], st["rowarg"], st["colarg"], conf.filter_threshold)
+            pb = torch.tensor(bs, device=dev)[:, None]
+            m0[pb, i0] = torch.where(a0 == -1, -1, i1.gather(1, a0.clamp(min=0)))
+            m1[pb, i1] = torch.where(a1 == -1, -1, i0.gather(1, a1.clamp(min=0)))
+            ms0[pb, i0], ms1[pb, i1] = s0, s1
+            heads.append((pb, d0, d1, i0, i1, st))
+        if do_prune:
+            prune0, prune1 = fin["prune0"], fin["prune1"]
+        else:  # without pruning every point sees every layer: fp32 like the plain forward's (lightglue.py:528-529)
             prune0, prune1 = torch.ones_like(ms0) * L, torch.ones_like(ms1) * L
-        # for loss(): one state, which gets head n_layers - 1 as in eval mode; a pruned pred (m, n < M, N) is rejected there
-        return {"matches0": m0, "matches1": m1, "matching_scores0": ms0, "matching_scores1": ms1,
-                "ref_descriptors0": d0[:, None], "ref_descriptors1": d1[:, None], "log_assignment": st["scores"],
-                "prune0": prune0, "prune1": prune1, "stop_layer": last,
-                "_b200_layers": [x], "_b200_sizes": (1, m, n), "_b200_row_expsum": st["row_expsum"]}
+        pred = {"matches0": m0, "matches1": m1, "matching_scores0": ms0, "matching_scores1": ms1,
+                "prune0": prune0, "prune1": prune1}
+        if B == 1:  # one pair: the pruned shapes of the reference's one-pair loop
+            _, d0, d1, _, _, st = heads[0]
+            # for loss(): one state, which gets head n_layers - 1 as in eval mode; a pruned pred is rejected there
+            pred.update({"ref_descriptors0": d0[:, None], "ref_descriptors1": d1[:, None],
+                         "log_assignment": st["scores"], "stop_layer": stops[0],
+                         "_b200_layers": [torch.cat([d0[0], d1[0]])], "_b200_sizes": (1, d0.shape[1], d1.shape[1]),
+                         "_b200_row_expsum": st["row_expsum"]})
+            return pred
+        # B > 1: the original indexing, -inf / zero at pruned points (see the module docstring)
+        la = torch.full((B, M + 1, N + 1), -math.inf, device=dev)
+        ref0, ref1 = torch.zeros(B, 1, M, D, device=dev), torch.zeros(B, 1, N, D, device=dev)
+        for pb, d0, d1, i0, i1, st in heads:
+            rows = torch.cat([i0, i0.new_full((i0.shape[0], 1), M)], 1)
+            cols = torch.cat([i1, i1.new_full((i1.shape[0], 1), N)], 1)
+            la[pb[:, :, None], rows[:, :, None], cols[:, None, :]] = st["scores"]
+            ref0[pb, 0, i0], ref1[pb, 0, i1] = d0, d1
+        pred.update({"log_assignment": la, "ref_descriptors0": ref0, "ref_descriptors1": ref1,
+                     "stop_layer": torch.tensor(stops, device=dev, dtype=torch.int64), "_b200_ragged": True})
+        return pred
 
     # ------------------------------------------------------------------------------------------
     def _loss(self, pred, data):
         """lightglue.py:578-627 on the hand-scheduled heads (engine.HeadFn): per layer one autograd node that
         yields the NLL and the token-confidence BCE; the O(M+N) terms are two small fused kernels."""
         conf = self.conf
+        if pred.get("_b200_ragged"):
+            raise ValueError("LightGlue.loss cannot be taken on the pred of an adaptive forward over several pairs: each "
+                             "pair stopped and was pruned on its own (depth_confidence / width_confidence)")
         layers_x = pred.get("_b200_layers")
         if layers_x is None:
             raise ValueError("LightGlue.loss needs the pred of this module's own forward: pred['_b200_layers'] is missing")

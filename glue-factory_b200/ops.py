@@ -95,6 +95,26 @@ def attn_fwd(q, k, v, kv_shift, scale):
     return out, lse
 
 
+def attn_fwd_varlen(q, k, v, q_off, q_len, k_off, k_len, max_q_len, scale, out=None):
+    """Forward over packed sequences: q [Tq, H, D], k / v [Tk, H, D] token-major; sequence s has the queries
+    q_off[s] .. q_off[s] + q_len[s] - 1 and the keys k_off[s] .. k_off[s] + k_len[s] - 1 (int32 CUDA tensors of S
+    entries, never read on the host); max_q_len bounds every q_len.  Returns (out [Tq, H, D], lse [H, Tq]); only the
+    query rows of the sequences are written, so `out` (allocated when None) keeps its other rows."""
+    _chk(q), _chk(k), _chk(v)
+    Tq, H, D = q.shape
+    assert D in (32, 64), "head_dim must be 32 or 64"
+    assert k.shape[1:] == q.shape[1:] and v.shape == k.shape and k.dtype == q.dtype == v.dtype
+    seqs = [_chk(t, torch.int32) for t in (q_off, q_len, k_off, k_len)]
+    S = q_off.numel()
+    assert all(t.numel() == S for t in seqs)
+    out = torch.empty_like(q) if out is None else _chk(out, q.dtype)
+    assert out.shape == q.shape
+    lse = torch.empty(H, Tq, device=q.device, dtype=torch.float32)
+    call("lgb200_attn_fwd_varlen", ptr(q), ptr(k), ptr(v), ptr(out), ptr(lse), *(ptr(t) for t in seqs), S,
+         int(max_q_len), Tq, k.shape[0], H, float(scale), _code(q.dtype), D, stream_ptr())
+    return out, lse
+
+
 def attn_bwd(q, k, v, out, lse, dout, kv_shift, scale):
     B, Nq, H, _ = q.shape
     D = _head_dim(q)
@@ -729,6 +749,35 @@ def head_token_fwd(x, wm, bm, wt, bt, cdt):
     call("lgb200_head_token_fwd", ptr(x), ptr(wm), ptr(bm), ptr(wt), ptr(bt), ptr(xc), ptr(zt), ptr(ls), ptr(du), T, D,
          _code(cdt), stream_ptr())
     return xc, zt, ls, du
+
+
+def adaptive_compact(x, theta, ind, zt, seg, fin, layer, sizes, conf_thr=None, depth_conf=-1.0, width_conf=-1.0,
+                     finish=False):
+    """One layer's stop / prune step of adaptive depth / width on a batch of pairs (lgb200_adaptive_compact,
+    include/lgb200.h).  x [T, D], theta [T, R] fp32, ind [T] int32, zt [T, 2] (None when finish), seg [4, 2B] int32.
+    fin: dict of the per-batch outputs updated in place -- x [B (M + N), D], ind [B (M + N)], len [2B], stop [B]
+    (int32) and prune0 [B, M] / prune1 [B, N] (int64).  Returns (x, theta, ind, seg, status): the packed state of the
+    next layer with T rows of capacity, and status [2] int32 = (kept tokens, emptied-view flag), still on the device."""
+    B, M, N = sizes
+    T, D = x.shape
+    R = theta.shape[1]
+    _chk(x, torch.float32), _chk(theta, torch.float32), _chk(ind, torch.int32), _chk(seg, torch.int32)
+    if zt is not None:
+        _chk(zt, torch.float32)
+    if conf_thr is not None:  # read as one fp32 on the device
+        _chk(conf_thr, torch.float32)
+        assert conf_thr.numel() >= 1 and conf_thr.device == x.device
+    dev = x.device
+    x_out, theta_out, ind_out = torch.empty_like(x), torch.empty_like(theta), torch.empty_like(ind)
+    seg_out = torch.empty_like(seg)
+    status = torch.empty(2, device=dev, dtype=torch.int32)
+    ws = torch.empty(_lib.load().lgb200_adaptive_compact_ws_ints(T, B), device=dev, dtype=torch.int32)
+    do_stop, do_prune = depth_conf > 0, width_conf > 0
+    call("lgb200_adaptive_compact", ptr(x), ptr(theta), ptr(ind), ptr(zt), ptr(seg), ptr(x_out), ptr(theta_out),
+         ptr(ind_out), ptr(seg_out), ptr(fin["x"]), ptr(fin["ind"]), ptr(fin["len"]), ptr(fin["stop"]),
+         ptr(fin["prune0"]), ptr(fin["prune1"]), ptr(status), ptr(ws), ptr(conf_thr), float(depth_conf),
+         float(1 - width_conf), int(do_stop), int(do_prune), int(layer), int(finish), B, M, N, T, D, R, stream_ptr())
+    return x_out, theta_out, ind_out, seg_out, status
 
 
 def head_token_bwd(x, dmdw, dzt, wm):

@@ -100,6 +100,18 @@ int lgb200_attn_fwd_hd(const void* q, const void* k, const void* v, void* out, f
 int lgb200_attn_bwd_hd(const void* q, const void* k, const void* v, const void* out, const float* lse,
                        const void* dout, void* dq, void* dk, void* dv, float* delta_ws, int B, int Nq, int Nk, int H,
                        int kv_shift, float scale, int dtype, int head_dim, cudaStream_t stream);
+/* Forward only, over packed sequences of different lengths (LightGlue's adaptive depth / width on a batch of pairs):
+ * q, out [Tq, H, head_dim]; k, v [Tk, H, head_dim] (token-major, dtype / head_dim as in lgb200_attn_fwd_hd); lse
+ * [H, Tq] fp32.  Sequence s < S has the queries q_off[s] .. q_off[s] + q_len[s] - 1 and attends to the keys / values
+ * k_off[s] .. k_off[s] + k_len[s] - 1; the four int32 arrays of S entries are device memory and are read by the
+ * kernel only (no host copy).  max_q_len bounds every q_len[s] and sizes the grid.  Only the query rows of the
+ * sequences are written (rows in no sequence keep their contents); a sequence with q_len or k_len 0 does no work.
+ * Key rows past a sequence's end but inside [0, Tk) are read by whole tiles and masked out of the softmax, so they
+ * must hold finite values (the tokens of other sequences).  Self-attention: k_off / k_len = q_off / q_len;
+ * cross-attention: each sequence's keys are its partner's tokens.                                                  */
+int lgb200_attn_fwd_varlen(const void* q, const void* k, const void* v, void* out, float* lse, const int* q_off,
+                           const int* q_len, const int* k_off, const int* k_len, int S, int max_q_len, int Tq, int Tk,
+                           int H, float scale, int dtype, int head_dim, cudaStream_t stream);
 
 /* ---- FFN LayerNorm + GELU -------------------------------------------------------------------------
  * replaces nn.LayerNorm(2D) + nn.GELU() of the ffn Sequential (lightglue.py:143-148, 178-183).
@@ -221,6 +233,27 @@ int lgb200_head_terms_bwd(const float* zt, const float* rowcnt, const float* col
                           const int* colarg, const int* fin0, const int* fin1, const float* num_pos,
                           const float* num_neg, float bal, const float* g_nll, const float* g_conf, float* dzt, int B,
                           int M, int N, cudaStream_t stream);
+
+/* ---- adaptive depth / width on a batch of pairs (LightGlue eval, lightglue.py:461-526, 545-576) ------------------
+ * One layer's stop / prune step on the packed token state x [T, D] fp32 (D % 4 == 0), theta [T, R] fp32 (rotary
+ * angles), ind [T] int32 (each token's keypoint index in its image).  Pair b < B owns segment 2b (image 0) and
+ * 2b + 1 (image 1); seg [4][2B] int32 = (offset, length, partner's offset, partner's length), a stopped pair has
+ * length 0.  zt [T, 2] = head_token_fwd's (matchability, token-confidence) logits of x; conf_thr: one fp32 threshold
+ * of this layer (device).  Per pair with tokens left:
+ *   stop   when finish != 0, or when do_stop and 1 - #(sigmoid(zt[:,1]) < thr) / (M + N) > depth_conf: its tokens go
+ *          unpruned to rows b (M + N) + i (image 0) / b (M + N) + M + i (image 1) of x_fin [B (M + N), D] and
+ *          ind_fin, fin_len[2b], fin_len[2b + 1] = its lengths, stop_layer[b] = layer;
+ *   else   a token stays when !do_prune, or sigmoid(zt[t,0]) > width_thr, or do_stop and sigmoid(zt[t,1]) <= thr;
+ *          kept tokens are packed pair-major into x_out / theta_out / ind_out (capacity T rows), seg_out gets the new
+ *          segments and, with do_prune, prune0 [B, M] / prune1 [B, N] int64 rise by one at the kept keypoints.
+ * status [2] int32 = (tokens kept, 1 if a pair that goes on kept no token of one of its views).  zt / conf_thr may be
+ * NULL when finish != 0.  ws: lgb200_adaptive_compact_ws_ints(T, B) int32.  Two kernels, no host synchronisation.  */
+int64_t lgb200_adaptive_compact_ws_ints(int T, int B);
+int lgb200_adaptive_compact(const float* x, const float* theta, const int* ind, const float* zt, const int* seg,
+                            float* x_out, float* theta_out, int* ind_out, int* seg_out, float* x_fin, int* ind_fin,
+                            int* fin_len, int* stop_layer, int64_t* prune0, int64_t* prune1, int* status, int* ws,
+                            const float* conf_thr, float depth_conf, float width_thr, int do_stop, int do_prune,
+                            int layer, int finish, int B, int M, int N, int T, int D, int R, cudaStream_t stream);
 
 /* ---- other assignment heads on the path ----------------------------------------------------------
  * log_double_softmax with a learned bin (gluestick.py:772-783) and log-domain Sinkhorn optimal
