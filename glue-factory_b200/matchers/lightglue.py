@@ -359,11 +359,13 @@ class LightGlue(nn.Module):
         (ops.adaptive_compact, one stop / prune / gather step per layer on the device); the layers run on the same GEMM
         kernels and on the length-aware attention (engine.Ragged), and a stopped pair has no tokens in later layers.  The
         only host read per layer is the kept-token count, which sizes the next layer.  A pair's assignment comes from
-        the head of the layer it stopped at (upstream LightGlue's behaviour; the in-tree reference cannot take that
-        branch: it stacks an empty list after the break, lightglue.py:485-492, 533).  Pairs with the same stop layer and
-        the same point counts (no pruning) run their head as one batch; a pair whose counts no other pair shares runs
-        it alone.  The results are scattered back to the original keypoint indices (lightglue.py:517-526).  See the
-        module docstring for the output shapes at B > 1."""
+        the head of the layer it stopped at (upstream LightGlue's behaviour; the in-tree reference computes it but then
+        fails stacking an empty list after the break, lightglue.py:485-492, 536; the early-stopping fixtures
+        tests/golden/lg_adaptive_*.npz are recorded with a stand-in for that stack by
+        scripts/make_lightglue_adaptive_golden.py).  Pairs with the same stop layer and the same point counts (no
+        pruning) run their head as one batch; a pair whose counts no other pair shares runs it alone.  The results are
+        scattered back to the original keypoint indices (lightglue.py:517-526).  See the module docstring for the output
+        shapes at B > 1."""
         conf = self.conf
         B, M, N = sizes
         dev, D, L = x.device, conf.descriptor_dim, conf.n_layers

@@ -357,8 +357,9 @@ def run_adaptive():
     """Inference-time point pruning (lightglue.py:461-526, 545-558; SURVEY 8f row 4) of the unmodified reference in
     eval mode, fp32 (its pruning branch mixes default-dtype buffers with the model dtype, so fp64 fails).  The seed is
     chosen so that every pruning decision clears its threshold by a margin (checked below), i.e. the fixture does not
-    hinge on fp32 rounding.  Early stopping is not recorded: the reference cannot take that branch without crashing
-    (`torch.stack` of the empty `all_desc0` list after the `break`, lightglue.py:485-492, 533)."""
+    hinge on fp32 rounding.  Early stopping is not recorded here: after the `break` the reference fails at
+    `torch.stack` of the empty `all_desc0` list (lightglue.py:485-492, 536).  scripts/make_lightglue_adaptive_golden.py
+    records it (tests/golden/lg_adaptive_*.npz) with a stand-in for `torch.stack` during the forward call."""
     from gluefactory.models import get_model
 
     conf = dict(synthetic.DEFAULT_CONF, n_layers=5, width_confidence=0.6, depth_confidence=-1, filter_threshold=0.0)

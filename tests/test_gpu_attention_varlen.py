@@ -145,3 +145,68 @@ def test_varlen_equals_uniform_kernel_bitwise(B, Nq, Nk, dtype, hd, H):
                                        torch.full((2 * B,), Nq, **i32), ko, torch.full((2 * B,), Nk, **i32), Nq, scale)
         assert torch.equal(out.view_as(ref), ref)
         assert torch.equal(lse.view(H, 2 * B, Nq).permute(1, 0, 2), ref_lse)
+
+
+def _adaptive_layout(seed):
+    """32 pairs packed back to back, pair-major, without guard rows, as LightGlue's adaptive forward packs them after
+    a stop / prune step: lengths in [1, 2048] (tile edges among them), three stopped pairs of length 0, and the last
+    segment ending at T."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    lens = torch.randint(1, 2049, (64,), generator=g).tolist()
+    lens[:12] = [1, 2, 63, 64, 65, 127, 129, 2047, 2048, 1000, 31, 33]
+    for b in (5, 17, 26):  # stopped pairs
+        lens[2 * b] = lens[2 * b + 1] = 0
+    lens[-2:] = [777, 1531]
+    offs = [0]
+    for n in lens[:-1]:
+        offs.append(offs[-1] + n)
+    return offs, lens, offs[-1] + lens[-1]
+
+
+@pytest.mark.parametrize("cross", [False, True], ids=["self", "cross"])
+@pytest.mark.parametrize("hd,H", [(64, 4), (32, 4), (32, 8)])
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32], ids=["bf16", "fp32"])
+def test_varlen_adaptive_layout_against_fp64(dtype, hd, H, cross):
+    """Segments of unequal lengths back to back: a partial key tile of one sequence reads the first tokens of the next.
+    Those tokens' keys and values are scaled up (keys x 8, values x 64), so a leak would dominate the softmax; each
+    sequence must still equal fp64 attention over its own keys (cross: its partner's, s ^ 1)."""
+    offs, lens, T = _adaptive_layout(seed=hd + H)
+    g = torch.Generator(device="cpu").manual_seed(7 * hd + H + int(cross))
+    q, k, v = (torch.randn(T, H, hd, generator=g) for _ in range(3))
+    for o, n in zip(offs, lens):  # the first tokens of every segment: the keys just past the previous one's end
+        k[o:o + min(n, 16)] *= 8.0
+        v[o:o + min(n, 16)] *= 64.0
+    q, k, v = (t.to(DEV, dtype) for t in (q, k, v))
+    partner = [s ^ 1 for s in range(64)] if cross else list(range(64))
+    i32 = dict(device=DEV, dtype=torch.int32)
+    q_off, q_len = torch.tensor(offs, **i32), torch.tensor(lens, **i32)
+    k_off, k_len = q_off[partner].contiguous(), q_len[partner].contiguous()
+    scale = hd ** -0.5
+    out, lse = ops.attn_fwd_varlen(q, k, v, q_off, q_len, k_off, k_len, max(lens), scale)
+    torch.cuda.synchronize()
+    worst = 0.0
+    for s, (o, n) in enumerate(zip(offs, lens)):
+        ko, kn = offs[partner[s]], lens[partner[s]]
+        if n == 0 or kn == 0:
+            continue
+        got, gl = out[o:o + n], lse[:, o:o + n]
+        if dtype == torch.bfloat16:
+            r = attn_ref(q[o:o + n], k[ko:ko + kn], v[ko:ko + kn], scale)
+            worst = max(worst, _within((got.double() - r["O"]).abs(), r["bO"], f"adaptive layout out s{s}", log=False),
+                        _within((gl.double() - r["lse"]).abs(), r["blse"], f"adaptive layout lse s{s}", log=False))
+        else:
+            Q, K, V = (t.double().permute(1, 0, 2) for t in (q[o:o + n], k[ko:ko + kn], v[ko:ko + kn]))
+            S = scale * Q @ K.transpose(1, 2)
+            P = torch.softmax(S, -1)
+            O = (P @ V).permute(1, 0, 2)
+            L = torch.logsumexp(S, -1)
+            # 2e-5 relative to the magnitudes summed, plus the fp32 rounding of the scores (32 u |q| . |k| each),
+            # which the scaled keys make large: it moves each p by p dS, so O by sum_j p_j dS_j (|v_j| + |O|)
+            dS = 32 * 2.0 ** -24 * scale * (Q.abs() @ K.abs().transpose(1, 2))
+            PdS = P * dS
+            bO = (2e-5 * (1 + P @ V.abs()) + PdS @ V.abs() + PdS.sum(-1, keepdim=True) * (P @ V).abs()).permute(1, 0, 2)
+            bL = 2e-5 * (1 + L.abs()) + PdS.sum(-1)
+            worst = max(worst, _within((got.double() - O).abs(), bO, f"adaptive layout out s{s}", log=False),
+                        _within((gl.double() - L).abs(), bL, f"adaptive layout lse s{s}", log=False))
+    report(f"varlen adaptive layout {dtype} hd{hd} H{H} {'cross' if cross else 'self'}", T=T,
+           max_err_over_bound=worst)
