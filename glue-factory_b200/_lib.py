@@ -35,6 +35,7 @@ SIGNATURES = {
     "lgb200_attn_fwd_varlen": (_i, [_vp] * 9 + [_i, _i, _i, _i, _i, _f, _i, _i, _vp]),
     "lgb200_adaptive_compact_ws_ints": (_i64, [_i, _i]),
     "lgb200_adaptive_compact": (_i, [_vp] * 18 + [_f, _f] + [_i] * 10 + [_vp]),
+    "lgb200_adaptive_compact_varlen": (_i, [_vp] * 19 + [_f, _f] + [_i] * 10 + [_vp]),
     "lgb200_ln_gelu_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _f, _i, _vp]),
     "lgb200_ln_gelu_bwd_parts": (_i, [_i64]),
     "lgb200_ln_gelu_bwd": (_i, [_vp] * 10 + [_i64, _i, _i, _vp]),
@@ -50,6 +51,9 @@ SIGNATURES = {
     "lgb200_assign_fused_stats": (_i, [_vp, _vp, _f] + [_vp] * 10 + [_i, _i, _i, _i, _vp]),
     "lgb200_assign_fused_bwd": (_i, [_vp, _vp, _f] + [_vp] * 9 + [_i, _i, _i, _i, _vp]),
     "lgb200_filter_matches": (_i, [_vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "lgb200_assign_lse_varlen": (_i, [_vp] * 5 + [_i, _i, _i, _vp]),
+    "lgb200_assign_scores_varlen": (_i, [_vp] * 17 + [_i] * 5 + [_vp]),
+    "lgb200_filter_matches_varlen": (_i, [_vp, _vp, _vp, _f] + [_vp] * 7 + [_i] * 5 + [_vp]),
     "lgb200_head_logsig": (_i, [_vp, _vp, _vp, _i64, _vp]),
     "lgb200_head_token_bwd_ws_floats": (_i, [_i]),
     "lgb200_head_token_fwd": (_i, [_vp] * 9 + [_i64, _i, _i, _vp]),
@@ -143,7 +147,8 @@ KERNELS_PER_CALL = {
     "lgb200_attn_fwd_hd": 1, "lgb200_attn_bwd_hd": 3,  # prep + dQ + dKV (fp32: delta + dQ + dKV)
     "lgb200_rope_split_fwd_hd": 1, "lgb200_rope_split_bwd_hd": 1,
     "lgb200_adamw_flat": 1, "lgb200_sgd_flat": 1, "lgb200_rmsprop_flat": 1,
-    "lgb200_attn_fwd_varlen": 1, "lgb200_adaptive_compact": 2,  # decide + gather
+    "lgb200_attn_fwd_varlen": 1, "lgb200_adaptive_compact": 2, "lgb200_adaptive_compact_varlen": 2,  # decide + gather
+    "lgb200_assign_lse_varlen": 2, "lgb200_assign_scores_varlen": 2, "lgb200_filter_matches_varlen": 1,
 }
 launch_count = 0          # running total of kernels launched through `call`
 timed_entry = None        # entry-point name or a set of names: every call of them is bracketed by CUDA events

@@ -37,18 +37,39 @@ __device__ __forceinline__ float4 ld4(const float* p, bool vec, int valid) {
   return r;
 }
 
+// Varlen batches (the packed evaluation head of LightGlue's adaptive / ragged inference): the kernels below are
+// instantiated a second time with kVarlen = true.  Pair g < G then has its own extents m = pairs[g] <= M and
+// n = pairs[G + g] <= N inside the padded [G, M, N] operands (M and N become strides; rows / columns past a pair's
+// extents are never read), and its scores, matches and scores of matches go to batch row pairs[2G + g] of the outputs
+// at the original keypoint indices ind0[g * M + i] / ind1[g * N + j].  Per pair, every value is computed by the same
+// instructions in the same order as a uniform call on [1, m, n].
+struct VarlenPairs {
+  const int* pairs;  // [3, G]: m, n, output batch row
+  const int* ind0;   // [G, M]
+  const int* ind1;   // [G, N]
+  int G, Mo, No;     // outputs: scores [*, Mo + 1, No + 1], m0 / ms0 [*, Mo], m1 / ms1 [*, No]
+};
+
 // ---------------------------------------------------------------------------------------------
 // pass 1: row LSE (final) and per-strip column (max, sumexp) partials
 // ---------------------------------------------------------------------------------------------
+template <bool kVarlen>
 __global__ void __launch_bounds__(256) assign_lse_kernel(const float* __restrict__ sim, float* __restrict__ lse_row,
                                                         float* __restrict__ colpart_m,
-                                                        float* __restrict__ colpart_s, int M, int N, int nstrips) {
+                                                        float* __restrict__ colpart_s, int M, int N, int nstrips,
+                                                        VarlenPairs vp) {
   __shared__ float s_cmax[2][kWarps][kChunk];
   __shared__ float s_csum[2][kWarps][kChunk];
   const int b = blockIdx.y, strip = blockIdx.x;
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const bool vec = (N & 3) == 0;
   const float* base = sim + (int64_t)b * M * N;
+  int Mb = M, Nb = N;  // this pair's extents; M, N are the strides
+  if constexpr (kVarlen) {
+    Mb = min(vp.pairs[b], M);
+    Nb = min(vp.pairs[vp.G + b], N);
+    if (strip * kStripRows >= Mb) return;
+  }
 
   float rm[kRowsPerWarp], rs[kRowsPerWarp];
   int rows[kRowsPerWarp];
@@ -60,20 +81,20 @@ __global__ void __launch_bounds__(256) assign_lse_kernel(const float* __restrict
   }
   auto load_chunk = [&](int c0, float4* dst) {
     const int col = c0 + lane * 4;
-    const int valid = min(4, N - col);  // may be <= 0
+    const int valid = min(4, Nb - col);  // may be <= 0
 #pragma unroll
     for (int t = 0; t < kRowsPerWarp; ++t)
-      dst[t] = (rows[t] < M && valid > 0) ? ld4(base + (int64_t)rows[t] * N + col, vec, valid)
+      dst[t] = (rows[t] < Mb && valid > 0) ? ld4(base + (int64_t)rows[t] * N + col, vec, valid)
                                            : make_float4(kNegInf, kNegInf, kNegInf, kNegInf);
   };
   int buf = 0;
   float4 xn[kRowsPerWarp];
   load_chunk(0, xn);
-  for (int c0 = 0; c0 < N; c0 += kChunk, buf ^= 1) {
+  for (int c0 = 0; c0 < Nb; c0 += kChunk, buf ^= 1) {
     float4 x[kRowsPerWarp];
 #pragma unroll
     for (int t = 0; t < kRowsPerWarp; ++t) x[t] = xn[t];
-    if (c0 + kChunk < N) load_chunk(c0 + kChunk, xn);  // next chunk in flight while this one is reduced
+    if (c0 + kChunk < Nb) load_chunk(c0 + kChunk, xn);  // next chunk in flight while this one is reduced
     // ---- row statistics (online, rescale only when the running max moves)
 #pragma unroll
     for (int t = 0; t < kRowsPerWarp; ++t) {
@@ -110,7 +131,7 @@ __global__ void __launch_bounds__(256) assign_lse_kernel(const float* __restrict
     }
     *reinterpret_cast<float4*>(&s_csum[buf][w][lane * 4]) = cs;
     __syncthreads();
-    if (threadIdx.x < kChunk && c0 + threadIdx.x < N) {
+    if (threadIdx.x < kChunk && c0 + threadIdx.x < Nb) {
       float m = s_cmax[buf][0][threadIdx.x], s = s_csum[buf][0][threadIdx.x];
 #pragma unroll
       for (int ww = 1; ww < kWarps; ++ww) {
@@ -130,22 +151,30 @@ __global__ void __launch_bounds__(256) assign_lse_kernel(const float* __restrict
       float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
       lse_merge(m, s, m2, s2);
     }
-    if (lane == 0 && rows[t] < M) lse_row[(int64_t)b * M + rows[t]] = m + logf(s);
+    if (lane == 0 && rows[t] < Mb) lse_row[(int64_t)b * M + rows[t]] = m + logf(s);
   }
 }
 
 // 32 columns x 8 strip-groups per CTA: max pass (no exp), then one exp per partial; groups merged through smem
+template <bool kVarlen>
 __global__ void __launch_bounds__(256) assign_col_lse_merge_kernel(const float* __restrict__ colpart_m,
                                                                   const float* __restrict__ colpart_s,
-                                                                  float* __restrict__ lse_col, int N, int nstrips) {
+                                                                  float* __restrict__ lse_col, int N, int nstrips,
+                                                                  VarlenPairs vp) {
   __shared__ float s_a[8][33];
   const int b = blockIdx.y, tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int j = blockIdx.x * 32 + tx;
-  const bool ok = j < N;
+  int Nb = N, ns = nstrips;  // this pair's columns and strips; N, nstrips are the strides
+  if constexpr (kVarlen) {
+    Nb = min(vp.pairs[vp.G + b], N);
+    ns = (min(vp.pairs[b], nstrips * kStripRows) + kStripRows - 1) / kStripRows;
+    if (blockIdx.x * 32 >= Nb) return;
+  }
+  const bool ok = j < Nb;
   const float* pm = colpart_m + (int64_t)b * nstrips * N + (ok ? j : 0);
   const float* ps = colpart_s + (int64_t)b * nstrips * N + (ok ? j : 0);
   float m = kNegInf;
-  for (int st = ty; st < nstrips; st += 8) m = fmaxf(m, pm[(int64_t)st * N]);
+  for (int st = ty; st < ns; st += 8) m = fmaxf(m, pm[(int64_t)st * N]);
   s_a[ty][tx] = m;
   __syncthreads();
   float gm = s_a[0][tx];
@@ -153,7 +182,7 @@ __global__ void __launch_bounds__(256) assign_col_lse_merge_kernel(const float* 
   for (int g = 1; g < 8; ++g) gm = fmaxf(gm, s_a[g][tx]);
   const float ref = (gm == kNegInf) ? 0.f : gm;
   float sum = 0.f;
-  for (int st = ty; st < nstrips; st += 8) sum += ps[(int64_t)st * N] * __expf(pm[(int64_t)st * N] - ref);
+  for (int st = ty; st < ns; st += 8) sum += ps[(int64_t)st * N] * __expf(pm[(int64_t)st * N] - ref);
   __syncthreads();
   s_a[ty][tx] = sum;
   __syncthreads();
@@ -187,7 +216,8 @@ struct ScoreArgs {
 
 __device__ __forceinline__ bool better(float v, int i, float bv, int bi) { return v > bv || (v == bv && i < bi); }
 
-__global__ void __launch_bounds__(256) assign_scores_kernel(ScoreArgs a) {
+template <bool kVarlen>
+__global__ void __launch_bounds__(256) assign_scores_kernel(ScoreArgs a, VarlenPairs vp) {
   __shared__ float s_v[2][kWarps][kChunk];
   __shared__ int s_i[2][kWarps][kChunk];
   const int b = blockIdx.y, strip = blockIdx.x;
@@ -196,29 +226,39 @@ __global__ void __launch_bounds__(256) assign_scores_kernel(ScoreArgs a) {
   const bool vec = (N & 3) == 0;
   const float* base = a.sim + (int64_t)b * M * N;
   const uint8_t* gbase = a.gt ? a.gt + (int64_t)b * M * N : nullptr;
+  int Mb = M, Nb = N;  // this pair's extents; M, N are the strides
+  float* sbase = nullptr;  // varlen: row 0 of this pair's scores in the output batch
+  if constexpr (kVarlen) {
+    Mb = min(vp.pairs[b], M);
+    Nb = min(vp.pairs[vp.G + b], N);
+    if (strip * kStripRows >= Mb) return;
+    if (a.scores) sbase = a.scores + (int64_t)vp.pairs[2 * vp.G + b] * (vp.Mo + 1) * (vp.No + 1);
+  }
 
   int rows[kRowsPerWarp];
   float lr[kRowsPerWarp], l0[kRowsPerWarp], bestv[kRowsPerWarp], psum[kRowsPerWarp], esum[kRowsPerWarp];
   int besti[kRowsPerWarp];
+  int64_t orow[kRowsPerWarp];  // varlen: offset of the row's original index in the output scores
 #pragma unroll
   for (int t = 0; t < kRowsPerWarp; ++t) {
     rows[t] = strip * kStripRows + w + kWarps * t;
-    const bool ok = rows[t] < M;
+    const bool ok = rows[t] < Mb;
     lr[t] = ok ? a.lse_row[(int64_t)b * M + rows[t]] : 0.f;
     l0[t] = ok ? a.ls0[(int64_t)b * M + rows[t]] : 0.f;
     bestv[t] = kNegInf;
     besti[t] = 0x7fffffff;
     psum[t] = 0.f;
     esum[t] = 0.f;
+    if constexpr (kVarlen) orow[t] = ok ? (int64_t)vp.ind0[(int64_t)b * M + rows[t]] * (vp.No + 1) : 0;
   }
   auto load_chunk = [&](int c0, float4* dx, uint32_t* dg) {
     const int col = c0 + lane * 4;
-    const int valid = min(4, N - col);
+    const int valid = min(4, Nb - col);
 #pragma unroll
     for (int t = 0; t < kRowsPerWarp; ++t) {
       dx[t] = make_float4(kNegInf, kNegInf, kNegInf, kNegInf);
       dg[t] = 0;
-      if (rows[t] >= M || valid <= 0) continue;
+      if (rows[t] >= Mb || valid <= 0) continue;
       const int64_t roff = (int64_t)rows[t] * N + col;
       dx[t] = ld4(base + roff, vec, valid);
       if (gbase) {
@@ -232,19 +272,21 @@ __global__ void __launch_bounds__(256) assign_scores_kernel(ScoreArgs a) {
   float4 xn[kRowsPerWarp];
   uint32_t gn[kRowsPerWarp];
   load_chunk(0, xn, gn);
-  for (int c0 = 0; c0 < N; c0 += kChunk, buf ^= 1) {
+  for (int c0 = 0; c0 < Nb; c0 += kChunk, buf ^= 1) {
     const int col = c0 + lane * 4;
-    const int valid = min(4, N - col);
+    const int valid = min(4, Nb - col);
     float4 xc[kRowsPerWarp];
     uint32_t gc[kRowsPerWarp];
 #pragma unroll
     for (int t = 0; t < kRowsPerWarp; ++t) { xc[t] = xn[t]; gc[t] = gn[t]; }
-    if (c0 + kChunk < N) load_chunk(c0 + kChunk, xn, gn);  // next chunk in flight while this one is processed
+    if (c0 + kChunk < Nb) load_chunk(c0 + kChunk, xn, gn);  // next chunk in flight while this one is processed
     float lc[4], l1[4];
+    int ocol[4];  // varlen: the columns' original indices
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       lc[e] = e < valid ? a.lse_col[(int64_t)b * N + col + e] : 0.f;
       l1[e] = e < valid ? a.ls1[(int64_t)b * N + col + e] : 0.f;
+      if constexpr (kVarlen) ocol[e] = e < valid ? vp.ind1[(int64_t)b * N + col + e] : 0;
     }
     float cbv[4];
     int cbi[4];
@@ -252,7 +294,7 @@ __global__ void __launch_bounds__(256) assign_scores_kernel(ScoreArgs a) {
     for (int e = 0; e < 4; ++e) { cbv[e] = kNegInf; cbi[e] = 0x7fffffff; }
 #pragma unroll
     for (int t = 0; t < kRowsPerWarp; ++t) {
-      if (rows[t] >= M || valid <= 0) continue;
+      if (rows[t] >= Mb || valid <= 0) continue;
       const float x[4] = {xc[t].x, xc[t].y, xc[t].z, xc[t].w};
       const uint32_t g = gc[t];
       float sc[4];
@@ -267,7 +309,13 @@ __global__ void __launch_bounds__(256) assign_scores_kernel(ScoreArgs a) {
           if (a.row_expsum) esum[t] += __expf(sc[e]);
         }
       }
-      if (a.scores) {
+      if constexpr (kVarlen) {
+        if (sbase) {
+#pragma unroll
+          for (int e = 0; e < 4; ++e)
+            if (e < valid) sbase[orow[t] + ocol[e]] = sc[e];
+        }
+      } else if (a.scores) {
         float* o = a.scores + ((int64_t)b * (M + 1) + rows[t]) * (N + 1) + col;
 #pragma unroll
         for (int e = 0; e < 4; ++e)
@@ -277,7 +325,7 @@ __global__ void __launch_bounds__(256) assign_scores_kernel(ScoreArgs a) {
 #pragma unroll
     for (int e = 0; e < 4; ++e) { s_v[buf][w][lane * 4 + e] = cbv[e]; s_i[buf][w][lane * 4 + e] = cbi[e]; }
     __syncthreads();
-    if (threadIdx.x < kChunk && c0 + threadIdx.x < N) {
+    if (threadIdx.x < kChunk && c0 + threadIdx.x < Nb) {
       float v = s_v[buf][0][threadIdx.x];
       int i = s_i[buf][0][threadIdx.x];
 #pragma unroll
@@ -304,32 +352,43 @@ __global__ void __launch_bounds__(256) assign_scores_kernel(ScoreArgs a) {
     }
     float ps = warp_sum(psum[t]);
     float es = a.row_expsum ? warp_sum(esum[t]) : 0.f;
-    if (lane == 0 && rows[t] < M) {
+    if (lane == 0 && rows[t] < Mb) {
       const int64_t r = (int64_t)b * M + rows[t];
       a.rowmax[r] = v;
       a.rowarg[r] = i;
       if (a.pos_row_sum) a.pos_row_sum[r] = ps;
       const float d0 = a.dust0[r];
       if (a.row_expsum) a.row_expsum[r] = es + __expf(d0);
-      if (a.scores) a.scores[((int64_t)b * (M + 1) + rows[t]) * (N + 1) + N] = d0;
+      if constexpr (kVarlen) {
+        if (sbase) sbase[orow[t] + vp.No] = d0;
+      } else if (a.scores) {
+        a.scores[((int64_t)b * (M + 1) + rows[t]) * (N + 1) + N] = d0;
+      }
     }
   }
 }
 
+template <bool kVarlen>
 __global__ void __launch_bounds__(256) assign_col_arg_merge_kernel(const float* __restrict__ colpart_v,
                                                                   const int* __restrict__ colpart_i,
                                                                   const float* __restrict__ dust1,
                                                                   float* __restrict__ colmax, int* __restrict__ colarg,
                                                                   float* __restrict__ scores, int M, int N,
-                                                                  int nstrips) {
+                                                                  int nstrips, VarlenPairs vp) {
   __shared__ float s_v[8][33];
   __shared__ int s_i[8][33];
   const int b = blockIdx.y, tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int j = blockIdx.x * 32 + tx;
+  int Nb = N, ns = nstrips;  // this pair's columns and strips; N, nstrips are the strides
+  if constexpr (kVarlen) {
+    Nb = min(vp.pairs[vp.G + b], N);
+    ns = (min(vp.pairs[b], M) + kStripRows - 1) / kStripRows;
+    if (blockIdx.x * 32 > Nb) return;
+  }
   float v = kNegInf;
   int i = 0x7fffffff;
-  if (j < N) {
-    for (int st = ty; st < nstrips; st += 8) {
+  if (j < Nb) {
+    for (int st = ty; st < ns; st += 8) {
       const int64_t o = ((int64_t)b * nstrips + st) * N + j;
       const float v2 = colpart_v[o];
       const int i2 = colpart_i[o];
@@ -339,9 +398,17 @@ __global__ void __launch_bounds__(256) assign_col_arg_merge_kernel(const float* 
   s_v[ty][tx] = v;
   s_i[ty][tx] = i;
   __syncthreads();
-  if (ty != 0 || j > N) return;
-  if (j == N) {
-    if (scores) scores[((int64_t)b * (M + 1) + M) * (N + 1) + N] = 0.f;
+  if (ty != 0 || j > Nb) return;
+  float* srow = scores;  // varlen: the dustbin row of this pair in the output batch
+  if constexpr (kVarlen) {
+    if (scores) srow = scores + ((int64_t)vp.pairs[2 * vp.G + b] * (vp.Mo + 1) + vp.Mo) * (vp.No + 1);
+  }
+  if (j == Nb) {
+    if constexpr (kVarlen) {
+      if (scores) srow[vp.No] = 0.f;
+    } else if (scores) {
+      scores[((int64_t)b * (M + 1) + M) * (N + 1) + N] = 0.f;
+    }
     return;
   }
 #pragma unroll
@@ -349,7 +416,11 @@ __global__ void __launch_bounds__(256) assign_col_arg_merge_kernel(const float* 
     if (better(s_v[g][tx], s_i[g][tx], v, i)) { v = s_v[g][tx]; i = s_i[g][tx]; }
   colmax[(int64_t)b * N + j] = v;
   colarg[(int64_t)b * N + j] = i;
-  if (scores) scores[((int64_t)b * (M + 1) + M) * (N + 1) + j] = dust1[(int64_t)b * N + j];
+  if constexpr (kVarlen) {
+    if (scores) srow[vp.ind1[(int64_t)b * N + j]] = dust1[(int64_t)b * N + j];
+  } else if (scores) {
+    scores[((int64_t)b * (M + 1) + M) * (N + 1) + j] = dust1[(int64_t)b * N + j];
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -417,26 +488,38 @@ __global__ void __launch_bounds__(256) assign_bwd_kernel(const float* __restrict
 // ---------------------------------------------------------------------------------------------
 // filter_matches (lightglue.py:293-309) from the row/col argmax of pass 2
 // ---------------------------------------------------------------------------------------------
+template <bool kVarlen>
 __global__ void filter_matches_kernel(const float* __restrict__ rowmax, const int* __restrict__ rowarg,
                                       const int* __restrict__ colarg, float th, int64_t* __restrict__ m0,
                                       int64_t* __restrict__ m1, float* __restrict__ ms0, float* __restrict__ ms1,
-                                      int M, int N) {
+                                      int M, int N, VarlenPairs vp) {
   const int b = blockIdx.y;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   const int* ra = rowarg + (int64_t)b * M;
   const int* ca = colarg + (int64_t)b * N;
   const float* rm = rowmax + (int64_t)b * M;
-  if (t < M) {
+  int Mb = M, Nb = N;  // this pair's extents; M, N are the strides
+  if constexpr (kVarlen) {
+    Mb = min(vp.pairs[b], M);
+    Nb = min(vp.pairs[vp.G + b], N);
+  }
+  if (t < Mb) {
     const int j = ra[t];
-    const bool mutual = (j >= 0 && j < N) && ca[j] == t;
+    const bool mutual = (j >= 0 && j < Nb) && ca[j] == t;
     const float s = mutual ? expf(rm[t]) : 0.f;
     const bool valid = mutual && s > th;
-    m0[(int64_t)b * M + t] = valid ? j : -1;
-    ms0[(int64_t)b * M + t] = s;
+    if constexpr (kVarlen) {  // original indices of both points
+      const int64_t o = (int64_t)vp.pairs[2 * vp.G + b] * vp.Mo + vp.ind0[(int64_t)b * M + t];
+      m0[o] = valid ? vp.ind1[(int64_t)b * N + j] : -1;
+      ms0[o] = s;
+    } else {
+      m0[(int64_t)b * M + t] = valid ? j : -1;
+      ms0[(int64_t)b * M + t] = s;
+    }
   }
-  if (t < N) {
+  if (t < Nb) {
     const int i = ca[t];
-    const bool mutual1 = (i >= 0 && i < M) && ra[i] == t;
+    const bool mutual1 = (i >= 0 && i < Mb) && ra[i] == t;
     float s = 0.f;
     bool valid = false;
     if (mutual1) {
@@ -444,8 +527,14 @@ __global__ void filter_matches_kernel(const float* __restrict__ rowmax, const in
       s = expf(rm[i]);
       valid = s > th;
     }
-    m1[(int64_t)b * N + t] = valid ? i : -1;
-    ms1[(int64_t)b * N + t] = s;
+    if constexpr (kVarlen) {
+      const int64_t o = (int64_t)vp.pairs[2 * vp.G + b] * vp.No + vp.ind1[(int64_t)b * N + t];
+      m1[o] = valid ? vp.ind0[(int64_t)b * M + i] : -1;
+      ms1[o] = s;
+    } else {
+      m1[(int64_t)b * N + t] = valid ? i : -1;
+      ms1[(int64_t)b * N + t] = s;
+    }
   }
 }
 
@@ -656,8 +745,9 @@ int lgb200_assign_lse(const float* sim, float* lse_row, float* lse_col, void* ws
   const int nstrips = (M + kStripRows - 1) / kStripRows;
   float* pm = static_cast<float*>(ws);
   float* ps = pm + (size_t)B * nstrips * N;
-  assign_lse_kernel<<<dim3(nstrips, B), 256, 0, stream>>>(sim, lse_row, pm, ps, M, N, nstrips);
-  assign_col_lse_merge_kernel<<<dim3((N + 31) / 32, B), 256, 0, stream>>>(pm, ps, lse_col, N, nstrips);
+  assign_lse_kernel<false><<<dim3(nstrips, B), 256, 0, stream>>>(sim, lse_row, pm, ps, M, N, nstrips, VarlenPairs{});
+  assign_col_lse_merge_kernel<false><<<dim3((N + 31) / 32, B), 256, 0, stream>>>(pm, ps, lse_col, N, nstrips,
+                                                                                 VarlenPairs{});
   return check_launch("assign_lse");
 }
 
@@ -676,9 +766,9 @@ int lgb200_assign_scores(const float* sim, const float* lse_row, const float* ls
   a.colpart_v = static_cast<float*>(ws);
   a.colpart_i = reinterpret_cast<int*>(a.colpart_v + (size_t)B * nstrips * N);
   a.pos_row_sum = pos_row_sum; a.row_expsum = row_expsum; a.M = M; a.N = N; a.nstrips = nstrips;
-  assign_scores_kernel<<<dim3(nstrips, B), 256, 0, stream>>>(a);
-  assign_col_arg_merge_kernel<<<dim3((N + 1 + 31) / 32, B), 256, 0, stream>>>(a.colpart_v, a.colpart_i, dust1, colmax,
-                                                                              colarg, scores, M, N, nstrips);
+  assign_scores_kernel<false><<<dim3(nstrips, B), 256, 0, stream>>>(a, VarlenPairs{});
+  assign_col_arg_merge_kernel<false><<<dim3((N + 1 + 31) / 32, B), 256, 0, stream>>>(
+      a.colpart_v, a.colpart_i, dust1, colmax, colarg, scores, M, N, nstrips, VarlenPairs{});
   return check_launch("assign_scores");
 }
 
@@ -705,9 +795,70 @@ int lgb200_filter_matches(const float* rowmax, const int* rowarg, const int* col
   LGB_REQUIRE(rowmax && rowarg && colarg && m0 && m1 && ms0 && ms1, kErrInvalid, "filter_matches: null pointer");
   LGB_REQUIRE(B > 0 && M > 0 && N > 0, kErrInvalid, "filter_matches: empty input");
   const int L = M > N ? M : N;
-  filter_matches_kernel<<<dim3((L + 255) / 256, B), 256, 0, stream>>>(rowmax, rowarg, colarg, th, m0, m1, ms0, ms1, M,
-                                                                      N);
+  filter_matches_kernel<false><<<dim3((L + 255) / 256, B), 256, 0, stream>>>(rowmax, rowarg, colarg, th, m0, m1, ms0,
+                                                                             ms1, M, N, VarlenPairs{});
   return check_launch("filter_matches");
+}
+
+static int varlen_pairs(VarlenPairs& vp, const int* pairs, const int* ind0, const int* ind1, int G, int M, int N, int Mo,
+                        int No, const char* what) {
+  LGB_REQUIRE(pairs, kErrInvalid, "%s: null pairs", what);
+  LGB_REQUIRE(G > 0 && G <= 65535 && M > 0 && N > 0 && Mo > 0 && No > 0, kErrInvalid,
+              "%s: bad extents G=%d M=%d N=%d Mo=%d No=%d", what, G, M, N, Mo, No);
+  vp.pairs = pairs; vp.ind0 = ind0; vp.ind1 = ind1; vp.G = G; vp.Mo = Mo; vp.No = No;
+  return 0;
+}
+
+int lgb200_assign_lse_varlen(const float* sim, float* lse_row, float* lse_col, void* ws, const int* pairs, int G, int M,
+                             int N, cudaStream_t stream) {
+  LGB_REQUIRE(sim && lse_row && lse_col && ws, kErrInvalid, "assign_lse_varlen: null pointer");
+  VarlenPairs vp;
+  int rc = varlen_pairs(vp, pairs, nullptr, nullptr, G, M, N, 1, 1, "assign_lse_varlen");
+  if (rc) return rc;
+  const int nstrips = (M + kStripRows - 1) / kStripRows;
+  float* pm = static_cast<float*>(ws);
+  float* ps = pm + (size_t)G * nstrips * N;
+  assign_lse_kernel<true><<<dim3(nstrips, G), 256, 0, stream>>>(sim, lse_row, pm, ps, M, N, nstrips, vp);
+  assign_col_lse_merge_kernel<true><<<dim3((N + 31) / 32, G), 256, 0, stream>>>(pm, ps, lse_col, N, nstrips, vp);
+  return check_launch("assign_lse_varlen");
+}
+
+int lgb200_assign_scores_varlen(const float* sim, const float* lse_row, const float* lse_col, const float* ls0,
+                                const float* ls1, const float* dust0, const float* dust1, float* scores, float* rowmax,
+                                int* rowarg, float* colmax, int* colarg, float* row_expsum, void* ws, const int* pairs,
+                                const int* ind0, const int* ind1, int G, int M, int N, int Mo, int No,
+                                cudaStream_t stream) {
+  LGB_REQUIRE(sim && lse_row && lse_col && ls0 && ls1 && dust0 && dust1 && rowmax && rowarg && colmax && colarg && ws,
+              kErrInvalid, "assign_scores_varlen: null pointer");
+  LGB_REQUIRE(!scores || (ind0 && ind1), kErrInvalid, "assign_scores_varlen: scores need the index maps");
+  VarlenPairs vp;
+  int rc = varlen_pairs(vp, pairs, ind0, ind1, G, M, N, Mo, No, "assign_scores_varlen");
+  if (rc) return rc;
+  const int nstrips = (M + kStripRows - 1) / kStripRows;
+  ScoreArgs a;
+  a.sim = sim; a.lse_row = lse_row; a.lse_col = lse_col; a.ls0 = ls0; a.ls1 = ls1; a.dust0 = dust0; a.dust1 = dust1;
+  a.gt = nullptr; a.scores = scores; a.rowmax = rowmax; a.rowarg = rowarg;
+  a.colpart_v = static_cast<float*>(ws);
+  a.colpart_i = reinterpret_cast<int*>(a.colpart_v + (size_t)G * nstrips * N);
+  a.pos_row_sum = nullptr; a.row_expsum = row_expsum; a.M = M; a.N = N; a.nstrips = nstrips;
+  assign_scores_kernel<true><<<dim3(nstrips, G), 256, 0, stream>>>(a, vp);
+  assign_col_arg_merge_kernel<true><<<dim3((N + 1 + 31) / 32, G), 256, 0, stream>>>(
+      a.colpart_v, a.colpart_i, dust1, colmax, colarg, scores, M, N, nstrips, vp);
+  return check_launch("assign_scores_varlen");
+}
+
+int lgb200_filter_matches_varlen(const float* rowmax, const int* rowarg, const int* colarg, float th, int64_t* m0,
+                                 int64_t* m1, float* ms0, float* ms1, const int* pairs, const int* ind0,
+                                 const int* ind1, int G, int M, int N, int Mo, int No, cudaStream_t stream) {
+  LGB_REQUIRE(rowmax && rowarg && colarg && m0 && m1 && ms0 && ms1 && ind0 && ind1, kErrInvalid,
+              "filter_matches_varlen: null pointer");
+  VarlenPairs vp;
+  int rc = varlen_pairs(vp, pairs, ind0, ind1, G, M, N, Mo, No, "filter_matches_varlen");
+  if (rc) return rc;
+  const int L = M > N ? M : N;
+  filter_matches_kernel<true><<<dim3((L + 255) / 256, G), 256, 0, stream>>>(rowmax, rowarg, colarg, th, m0, m1, ms0,
+                                                                            ms1, M, N, vp);
+  return check_launch("filter_matches_varlen");
 }
 
 }  // extern "C"

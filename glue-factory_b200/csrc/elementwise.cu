@@ -1688,7 +1688,7 @@ __global__ void __launch_bounds__(kAcThreads)
                            int64_t* __restrict__ prune1, int* __restrict__ dst_seg, int* __restrict__ dst_pos,
                            int* __restrict__ cnt, int* __restrict__ state, const float* __restrict__ conf_thr,
                            float depth_conf, float width_thr, int do_stop, int do_prune, int layer, int finish, int B,
-                           int M, int N) {
+                           int M, int N, const int* __restrict__ pair_pts) {
   __shared__ int sh[32];
   __shared__ int s_low;
   const int b = blockIdx.x, S = 2 * B;
@@ -1716,7 +1716,7 @@ __global__ void __launch_bounds__(kAcThreads)
     if ((threadIdx.x & 31) == 0) atomicAdd(&s_low, c);
     __syncthreads();
     // relative to the pair's ORIGINAL point count (lightglue.py:489), in fp32 as the one-pair loop computes it
-    stop = 1.f - (float)s_low / (float)(M + N) > depth_conf;
+    stop = 1.f - (float)s_low / (float)(pair_pts ? pair_pts[b] : M + N) > depth_conf;
   }
   if (stop) {
     for (int i = threadIdx.x; i < n0 + n1; i += blockDim.x) {
@@ -1818,11 +1818,12 @@ extern "C" {
 
 int64_t lgb200_adaptive_compact_ws_ints(int T, int B) { return 2 * (int64_t)T + 3 * (int64_t)B; }
 
-int lgb200_adaptive_compact(const float* x, const float* theta, const int* ind, const float* zt, const int* seg,
-                            float* x_out, float* theta_out, int* ind_out, int* seg_out, float* x_fin, int* ind_fin,
-                            int* fin_len, int* stop_layer, int64_t* prune0, int64_t* prune1, int* status, int* ws,
-                            const float* conf_thr, float depth_conf, float width_thr, int do_stop, int do_prune,
-                            int layer, int finish, int B, int M, int N, int T, int D, int R, cudaStream_t stream) {
+int lgb200_adaptive_compact_varlen(const float* x, const float* theta, const int* ind, const float* zt, const int* seg,
+                                   float* x_out, float* theta_out, int* ind_out, int* seg_out, float* x_fin,
+                                   int* ind_fin, int* fin_len, int* stop_layer, int64_t* prune0, int64_t* prune1,
+                                   int* status, int* ws, const float* conf_thr, const int* pair_pts, float depth_conf,
+                                   float width_thr, int do_stop, int do_prune, int layer, int finish, int B, int M,
+                                   int N, int T, int D, int R, cudaStream_t stream) {
   LGB_REQUIRE(x && theta && ind && seg && x_out && theta_out && ind_out && seg_out && x_fin && ind_fin && fin_len &&
                   stop_layer && prune0 && prune1 && status && ws,
               kErrInvalid, "adaptive_compact: null pointer");
@@ -1838,7 +1839,7 @@ int lgb200_adaptive_compact(const float* x, const float* theta, const int* ind, 
   int* state = cnt + 2 * B;
   adaptive_decide_kernel<<<B, kAcThreads, 0, stream>>>(ind, zt, seg, fin_len, stop_layer, prune0, prune1, dst_seg,
                                                        dst_pos, cnt, state, conf_thr, depth_conf, width_thr, do_stop,
-                                                       do_prune, layer, finish, B, M, N);
+                                                       do_prune, layer, finish, B, M, N, pair_pts);
   int rc = check_launch("adaptive_decide");
   if (rc) return rc;
   const int64_t rows = ((int64_t)T + 7) / 8, cap = 4 * (int64_t)device_sm_count();
@@ -1846,6 +1847,16 @@ int lgb200_adaptive_compact(const float* x, const float* theta, const int* ind, 
       x, theta, ind, dst_seg, dst_pos, cnt, state, x_out, theta_out, ind_out, x_fin, ind_fin, seg_out, status, B, T, D,
       R);
   return check_launch("adaptive_gather");
+}
+
+int lgb200_adaptive_compact(const float* x, const float* theta, const int* ind, const float* zt, const int* seg,
+                            float* x_out, float* theta_out, int* ind_out, int* seg_out, float* x_fin, int* ind_fin,
+                            int* fin_len, int* stop_layer, int64_t* prune0, int64_t* prune1, int* status, int* ws,
+                            const float* conf_thr, float depth_conf, float width_thr, int do_stop, int do_prune,
+                            int layer, int finish, int B, int M, int N, int T, int D, int R, cudaStream_t stream) {
+  return lgb200_adaptive_compact_varlen(x, theta, ind, zt, seg, x_out, theta_out, ind_out, seg_out, x_fin, ind_fin,
+                                        fin_len, stop_layer, prune0, prune1, status, ws, conf_thr, nullptr, depth_conf,
+                                        width_thr, do_stop, do_prune, layer, finish, B, M, N, T, D, R, stream);
 }
 
 }  // extern "C"

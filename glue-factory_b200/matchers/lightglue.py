@@ -27,13 +27,26 @@ looks, DATA_PATH then torch-hub's cache, and never downloaded
 
 Adaptive depth / width (`depth_confidence` / `width_confidence` > 0, eval mode) takes any batch size; every pair
 stops and is pruned on its own, with the result it would have alone.  For one pair the outputs keep the reference's
-shapes: `log_assignment` [1, m+1, n+1] over the m / n points left at the end, `stop_layer` an int.  For B > 1 pairs:
-    log_assignment        [B, M+1, N+1] in the original keypoint indexing; the rows / columns of pruned points are
-                          -inf, the dustbin row and column are kept
-    stop_layer            [B] int64 tensor, the layer whose assignment head each pair used
-    ref_descriptors{0,1}  [B, 1, M|N, D], each pair's final state in the original indexing, zero at pruned points
-    matches*, matching_scores*, prune*: the shapes of the plain forward and the dtypes of the one-pair call (prune*
-                          int64 layer counts with width_confidence, else fp32 n_layers as in the plain forward)
+shapes: `log_assignment` [1, m+1, n+1] over the m / n points left at the end, `stop_layer` an int.
+
+Pairs with their own keypoint counts (eval mode, with or without adaptive depth / width): `data["num_keypoints0"]` /
+`data["num_keypoints1"]`, integer tensors of shape [B] on any device (either or both; a missing one means every row).
+Pair b then uses the first n0_b / n1_b rows of the padded keypoints*, descriptors* and scales* / oris*; the padding is
+never read (NaN or Inf there change nothing), and without a view's image_size its keypoints are normalised by the
+bounding box of its valid points.  Pair b's result equals a one-pair call on its truncated inputs.  The counts are read
+on the host once per call; without depth_confidence and width_confidence there is no host read per layer.  Refused
+with ValueError: counts below 1 or above the padded length, of a shape other than [B] or of a non-integer dtype, and
+counts in training mode (the reference trains on padded views whose padding keypoints take part in matching).
+
+For B > 1 pairs, and for any B with counts, the outputs keep the padded, original keypoint indexing:
+    log_assignment        [B, M+1, N+1], the dustbin row / column at M / N; the rows / columns of pruned and padded
+                          points are -inf
+    stop_layer            [B] int64 tensor, the layer whose assignment head each pair used (n_layers - 1 without
+                          adaptive depth)
+    ref_descriptors{0,1}  [B, 1, M|N, D], each pair's final state, zero at pruned and padded points
+    matches*              [B, M|N] int64, -1 at padding;  matching_scores* fp32, 0 at padding
+    prune*                int64 layer counts with width_confidence, else fp32 n_layers as in the plain forward; 0 at
+                          padding
 `loss` refuses such a pred (ValueError).
 
 conf additions over the reference's default_conf:
@@ -42,6 +55,7 @@ conf additions over the reference's default_conf:
 """
 import copy
 import math
+from typing import NamedTuple
 
 import torch
 import torch.nn.functional as F
@@ -83,6 +97,83 @@ def _merge(base, new):
         else:
             out[k] = copy.deepcopy(v)
     return out
+
+
+def keypoint_counts(data, B, M, N):
+    """data["num_keypoints0/1"] (optional, either or both): pair b uses the first n0_b / n1_b rows of the padded
+    keypoints / descriptors / scales / oris of each view.  Returns None without them, else (n0, n1) int64 CPU tensors
+    of shape [B] (a missing key: every row of that view); the counts' one host read.  Refuses counts of a non-integer
+    dtype, of a shape other than [B], or outside 1 .. the padded length (ValueError)."""
+    if "num_keypoints0" not in data and "num_keypoints1" not in data:
+        return None
+    out = []
+    for key, n in (("num_keypoints0", M), ("num_keypoints1", N)):
+        c = data.get(key)
+        if c is None:
+            out.append(torch.full((B,), n, dtype=torch.int64))
+            continue
+        if not isinstance(c, torch.Tensor) or c.dtype not in (torch.int8, torch.int16, torch.int32, torch.int64,
+                                                                torch.uint8):
+            raise ValueError(f"LightGlue: {key} must be an integer tensor, got "
+                             f"{c.dtype if isinstance(c, torch.Tensor) else type(c).__name__}")
+        if tuple(c.shape) != (B,):
+            raise ValueError(f"LightGlue: {key} must have shape [B] = [{B}], got {list(c.shape)}")
+        out.append(c.detach().to("cpu", torch.int64))
+    for key, c, n in (("num_keypoints0", out[0], M), ("num_keypoints1", out[1], N)):
+        if bool((c < 1).any()) or bool((c > n).any()):
+            raise ValueError(f"LightGlue: {key} must lie in 1 .. {n} (the padded length), got {c.tolist()}")
+    return out[0], out[1]
+
+
+def segment_rows(starts, lens):
+    """For segments k of lens[k] rows starting at starts[k] (int64 tensors): every row starts[k] + i, i < lens[k], in
+    segment order, with its segment k and its index i -- three int64 tensors on the inputs' device."""
+    k = torch.repeat_interleave(torch.arange(lens.numel(), device=lens.device), lens)
+    first = torch.cumsum(lens, 0) - lens
+    i = torch.arange(k.numel(), device=lens.device) - first[k]
+    return starts[k] + i, k, i
+
+
+class RaggedLayout(NamedTuple):
+    """Packed token layout of B pairs with n0[b] / n1[b] points (CPU tensors): tokens [image 0 of every pair; image 1
+    of every pair], segment 2b / 2b + 1 = image 0 / 1 of pair b.  seg [4, 2B] int32 = (offset, length, partner's
+    offset, partner's length); ind [T] int32 = each token's keypoint index; src0 / src1 (int64): the rows of the
+    [B * M] / [B * N] flattened padded views the tokens come from; pid0 / pid1: their pair."""
+    seg: torch.Tensor
+    ind: torch.Tensor
+    src0: torch.Tensor
+    src1: torch.Tensor
+    pid0: torch.Tensor
+    pid1: torch.Tensor
+    n0: torch.Tensor
+    n1: torch.Tensor
+
+
+def ragged_layout(n0, n1, M, N):
+    B = n0.numel()
+    src0, pid0, i0 = segment_rows(torch.arange(B) * M, n0)
+    src1, pid1, i1 = segment_rows(torch.arange(B) * N, n1)
+    off0 = torch.cumsum(n0, 0) - n0
+    off1 = src0.numel() + torch.cumsum(n1, 0) - n1
+    off, ln = torch.stack([off0, off1], 1).reshape(-1), torch.stack([n0, n1], 1).reshape(-1)
+    seg = torch.stack([off, ln, off.view(B, 2).flip(1).reshape(-1), ln.view(B, 2).flip(1).reshape(-1)]).int()
+    return RaggedLayout(seg, torch.cat([i0, i1]).int(), src0, src1, pid0, pid1, n0, n1)
+
+
+def _normalize_packed(kpts, size, pid, B):
+    """normalize_keypoints of packed keypoints kpts [T, 2] of B pairs (pid: each row's pair), per pair: the same
+    arithmetic, with the bounding box of each pair's own rows when there is no image size."""
+    kpts = kpts.float()
+    if size is None:
+        idx = pid[:, None].expand(-1, kpts.shape[1])
+        hi = kpts.new_full((B, kpts.shape[1]), -math.inf).scatter_reduce(0, idx, kpts, "amax")
+        lo = kpts.new_full((B, kpts.shape[1]), math.inf).scatter_reduce(0, idx, kpts, "amin")
+        size = 1 + hi - lo
+    else:
+        size = torch.as_tensor(size, device=kpts.device).to(kpts).reshape(-1, 2).expand(B, 2)
+    shift = size / 2
+    scale = size.max(-1).values / 2
+    return (kpts - shift[pid]) / scale[pid, None]
 
 
 def normalize_keypoints(kpts, size):
@@ -273,36 +364,55 @@ class LightGlue(nn.Module):
     def _forward(self, data):
         for key in self.required_data_keys:
             assert key in data, f"Missing key {key} in data"
-        _lib.load()  # raises unless the CUDA library is built and the device is an H100 (no CPU fallback)
         conf = self.conf
-        adaptive = not self.training and (conf.depth_confidence > 0 or conf.width_confidence > 0)
         kpts0, kpts1 = data["keypoints0"], data["keypoints1"]
         B, M, _ = kpts0.shape
         N = kpts1.shape[1]
         assert M > 0 and N > 0, "empty keypoint sets are not supported"
+        counts = keypoint_counts(data, B, M, N)
+        if counts is not None and self.training:
+            raise ValueError("LightGlue: num_keypoints0/1 are taken in eval mode only (the reference trains on padded "
+                             "views whose padding keypoints take part in matching)")
+        _lib.load()  # raises unless the CUDA library is built and the device is an H100 (no CPU fallback)
+        adaptive = not self.training and (conf.depth_confidence > 0 or conf.width_confidence > 0)
         size0 = data["view0"].get("image_size") if "view0" in data else None
         size1 = data["view1"].get("image_size") if "view1" in data else None
-        kpts0, kpts1 = normalize_keypoints(kpts0, size0), normalize_keypoints(kpts1, size1)
         desc0, desc1 = data["descriptors0"].contiguous(), data["descriptors1"].contiguous()
         assert desc0.shape[-1] == conf.input_dim and desc1.shape[-1] == conf.input_dim
         D = conf.descriptor_dim
-        x = torch.cat([desc0.reshape(B * M, -1), desc1.reshape(B * N, -1)], 0).float()
+        layout = None
+        if counts is None:
+            kpts0, kpts1 = normalize_keypoints(kpts0, size0), normalize_keypoints(kpts1, size1)
+            x = torch.cat([desc0.reshape(B * M, -1), desc1.reshape(B * N, -1)], 0).float()
+        else:
+            # pack the valid rows of every view first: nothing below reads the padding
+            layout = ragged_layout(*counts, M, N)
+            src0, src1, pid0, pid1 = (t.to(kpts0.device) for t in (layout.src0, layout.src1, layout.pid0, layout.pid1))
+            pick = lambda t, n, src: t.reshape(B * n, *t.shape[2:]).index_select(0, src)  # noqa: E731
+            kpts0 = _normalize_packed(pick(kpts0, M, src0), size0, pid0, B)
+            kpts1 = _normalize_packed(pick(kpts1, N, src1), size1, pid1, B)
+            x = torch.cat([pick(desc0, M, src0), pick(desc1, N, src1)], 0).float()
         if not isinstance(self.input_proj, nn.Identity):
             x = self._lin(x, self.input_proj).float()
         # rotary angles, cached for all layers (lightglue.py:456-458); cos/sin are taken in-kernel
         if conf.add_scale_ori:
-            ext = lambda k, sc, o: torch.cat([k, (sc if sc.dim() == 3 else sc[..., None]).float(),  # noqa: E731
-                                              (o if o.dim() == 3 else o[..., None]).float()], -1)
-            kpts0, kpts1 = ext(kpts0, data["scales0"], data["oris0"]), ext(kpts1, data["scales1"], data["oris1"])
+            ext = lambda k, sc, o: torch.cat([k, (sc if sc.dim() == k.dim() else sc[..., None]).float(),  # noqa: E731
+                                              (o if o.dim() == k.dim() else o[..., None]).float()], -1)
+            sc0, o0, sc1, o1 = data["scales0"], data["oris0"], data["scales1"], data["oris1"]
+            if counts is not None:
+                sc0, o0, sc1, o1 = pick(sc0, M, src0), pick(o0, M, src0), pick(sc1, N, src1), pick(o1, N, src1)
+            kpts0, kpts1 = ext(kpts0, sc0, o0), ext(kpts1, sc1, o1)
         kd = kpts0.shape[-1]
-        kp = torch.cat([kpts0.reshape(B * M, kd), kpts1.reshape(B * N, kd)], 0)
+        kp = torch.cat([kpts0.reshape(-1, kd), kpts1.reshape(-1, kd)], 0)
         theta = ops.PosencTheta.apply(kp.float().contiguous(), self.posenc.Wr.weight.float()).contiguous()
         sizes = (B, M, N)
         all0, all1, layers_x = [], [], []
         L = conf.n_layers
         self._refresh_shadow()
-        if adaptive:
-            return self._forward_adaptive(x, theta, sizes)
+        if adaptive or counts is not None:
+            if layout is None:
+                layout = ragged_layout(torch.full((B,), M), torch.full((B,), N), M, N)
+            return self._forward_adaptive(x, theta, sizes, layout, ragged=counts is not None)
         # head -> layer gradient hand-over of the training step (engine.LayerFn / HeadFn docstrings)
         stash = {} if (self.training and torch.is_grad_enabled()) else None
         for i in range(L):
@@ -351,113 +461,133 @@ class LightGlue(nn.Module):
 
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
-    def _forward_adaptive(self, x, theta, sizes):
-        """Inference-time adaptive depth / width (lightglue.py:461-526, 545-576; eval only), every pair on its own: after
-        every layer but the last, (a) a pair stops when the fraction of its confident points exceeds depth_confidence,
-        (b) a pair that goes on drops the points predicted unmatchable (matchability <= 1 - width_confidence) unless their
+    def _forward_adaptive(self, x, theta, sizes, layout, ragged=False):
+        """Inference on packed pairs: adaptive depth / width (lightglue.py:461-526, 545-576; eval only) and batches of
+        pairs with their own keypoint counts (`num_keypoints0/1`, ragged=True), every pair on its own.  After every layer
+        but the last, (a) a pair stops when the fraction of its confident points exceeds depth_confidence, (b) a pair
+        that goes on drops the points predicted unmatchable (matchability <= 1 - width_confidence) unless their
         confidence is still low.  The pairs' tokens stay packed in one [T, D] state whose segments shrink layer by layer
         (ops.adaptive_compact, one stop / prune / gather step per layer on the device); the layers run on the same GEMM
         kernels and on the length-aware attention (engine.Ragged), and a stopped pair has no tokens in later layers.  The
-        only host read per layer is the kept-token count, which sizes the next layer.  A pair's assignment comes from
-        the head of the layer it stopped at (upstream LightGlue's behaviour; the in-tree reference computes it but then
-        fails stacking an empty list after the break, lightglue.py:485-492, 536; the early-stopping fixtures
-        tests/golden/lg_adaptive_*.npz are recorded with a stand-in for that stack by
-        scripts/make_lightglue_adaptive_golden.py).  Pairs with the same stop layer and the same point counts (no
-        pruning) run their head as one batch; a pair whose counts no other pair shares runs it alone.  The results are
-        scattered back to the original keypoint indices (lightglue.py:517-526).  See the module docstring for the output
-        shapes at B > 1."""
+        only host read per layer is the kept-token count, which sizes the next layer; without depth_confidence and
+        width_confidence there is none.  A pair's assignment comes from the head of the layer it stopped at (upstream
+        LightGlue's behaviour; the in-tree reference computes it but then fails stacking an empty list after the break,
+        lightglue.py:485-492, 536; the early-stopping fixtures tests/golden/lg_adaptive_*.npz are recorded with a
+        stand-in for that stack by scripts/make_lightglue_adaptive_golden.py).  The pairs that stopped at the same layer
+        run that layer's head together, on the packed varlen head (ops.assign_varlen), which writes the scores and
+        matches at the original keypoint indices (lightglue.py:517-526).  See the module docstring for the outputs.
+        layout: ragged_layout(n0, n1, M, N) of the packed tokens."""
         conf = self.conf
         B, M, N = sizes
         dev, D, L = x.device, conf.descriptor_dim, conf.n_layers
         do_stop, do_prune = conf.depth_confidence > 0, conf.width_confidence > 0
         i32 = dict(device=dev, dtype=torch.int32)
-        # tokens [image 0 of every pair; image 1 of every pair] as _forward packed them; segment 2b / 2b + 1 = pair b
-        off = torch.stack([torch.arange(B) * M, B * M + torch.arange(B) * N], 1).reshape(-1)
-        ln = torch.tensor([M, N]).repeat(B)
-        seg = torch.stack([off, ln, off.view(B, 2).flip(1).reshape(-1), ln.view(B, 2).flip(1).reshape(-1)]).to(**i32)
-        ind = torch.cat([torch.arange(M, **i32).repeat(B), torch.arange(N, **i32).repeat(B)])
+        n0, n1 = layout.n0, layout.n1
+        seg, ind = layout.seg.to(dev), layout.ind.to(dev)
+        pair_pts = (n0 + n1).to(**i32) if ragged else None
         fin = {"x": torch.empty(B * (M + N), D, device=dev), "ind": torch.empty(B * (M + N), **i32),
                "len": torch.zeros(2 * B, **i32), "stop": torch.full((B,), L - 1, **i32),
-               "prune0": torch.ones(B, M, device=dev, dtype=torch.int64),
-               "prune1": torch.ones(B, N, device=dev, dtype=torch.int64)}
-        ragged = engine.Ragged(seg, max(M, N))
+               "prune0": (torch.arange(M) < n0[:, None]).long().to(dev),
+               "prune1": (torch.arange(N) < n1[:, None]).long().to(dev)}
+        max_len = int(max(n0.max(), n1.max()))
+        ragged_sizes = engine.Ragged(seg, max_len)
         for i in range(L):
             w, params = self._layer_weights(i)
-            x = engine.LayerFn.apply(x, theta, ragged, conf.num_heads, self._cdt, self.transformers[i].self_attn.ffn[1].eps,
-                                     w, None, *params)
+            x = engine.LayerFn.apply(x, theta, ragged_sizes, conf.num_heads, self._cdt,
+                                     self.transformers[i].self_attn.ffn[1].eps, w, None, *params)
+            last = i == L - 1
+            if not (last or do_stop or do_prune):
+                continue  # every pair runs every layer: nothing to decide
             zt = None
-            if i < L - 1:
+            if not last:
                 la, tk = self.log_assignment[i], self.token_confidence[i].token[0]
                 _, zt, _, _ = ops.head_token_fwd(x, la.matchability.weight.view(-1), la.matchability.bias,
                                                  tk.weight.view(-1), tk.bias, self._cdt)
             x, theta, ind, seg, status = ops.adaptive_compact(
-                x, theta, ind, zt, ragged.seg, fin, i, sizes, conf_thr=self.confidence_thresholds[i:i + 1].float(),
-                depth_conf=conf.depth_confidence, width_conf=conf.width_confidence, finish=i == L - 1)
+                x, theta, ind, zt, ragged_sizes.seg, fin, i, sizes, conf_thr=self.confidence_thresholds[i:i + 1].float(),
+                depth_conf=conf.depth_confidence, width_conf=conf.width_confidence, finish=last, pair_pts=pair_pts)
+            if last:
+                break
             kept, emptied = status.tolist()  # the layer loop's one host read: it sizes the next layer
             assert not emptied, "point pruning removed every keypoint of a view"
             if kept == 0:
                 break
             x, theta, ind = x[:kept], theta[:kept], ind[:kept]
-            ragged = engine.Ragged(seg, max(M, N))
-        lens_stop = torch.cat([fin["len"], fin["stop"]]).tolist()
-        lens, stops = lens_stop[:2 * B], lens_stop[2 * B:]
-        xf, indf = fin["x"], fin["ind"].long()
-        m0 = torch.full((B, M), -1, device=dev, dtype=torch.int64)
-        m1 = torch.full((B, N), -1, device=dev, dtype=torch.int64)
-        ms0, ms1 = torch.zeros(B, M, device=dev), torch.zeros(B, N, device=dev)
-        # pairs with the same stop layer and the same point counts share one batched head; after pruning the counts
-        # differ from pair to pair, and such pairs run their head alone
-        groups = {}
-        for b in range(B):
-            groups.setdefault((stops[b], lens[2 * b], lens[2 * b + 1]), []).append(b)
-        heads = []
-        for (layer, m, n), bs in sorted(groups.items()):
-            if len(bs) == 1:
-                base = bs[0] * (M + N)
-                r0, r1 = slice(base, base + m), slice(base + M, base + M + n)
-                d0, d1 = xf[r0].view(1, m, D), xf[r1].view(1, n, D)
-                i0, i1 = indf[r0].view(1, m), indf[r1].view(1, n)
-            else:
-                base = torch.tensor(bs, device=dev)[:, None] * (M + N)
-                r0 = (base + torch.arange(m, device=dev)).view(-1)
-                r1 = (base + M + torch.arange(n, device=dev)).view(-1)
-                d0, d1 = xf.index_select(0, r0).view(-1, m, D), xf.index_select(0, r1).view(-1, n, D)
-                i0, i1 = indf.index_select(0, r0).view(-1, m), indf.index_select(0, r1).view(-1, n)
-            md0, md1, z0, z1 = self._head_inputs(d0, d1, layer)
+            ragged_sizes = engine.Ragged(seg, max_len)
+        lens_stop = torch.cat([fin["len"], fin["stop"]]).cpu()  # sizes the head's padded operands
+        lens, stops = lens_stop[:2 * B].view(B, 2).long(), lens_stop[2 * B:].long()
+        xf, indf = fin["x"], fin["ind"]
+        out = {"scores": torch.full((B, M + 1, N + 1), -math.inf, device=dev),
+               "m0": torch.full((B, M), -1, device=dev, dtype=torch.int64),
+               "m1": torch.full((B, N), -1, device=dev, dtype=torch.int64),
+               "ms0": torch.zeros(B, M, device=dev), "ms1": torch.zeros(B, N, device=dev)}
+        # the final tokens of pair b are rows b (M + N) + i (image 0) and b (M + N) + M + j (image 1) of fin
+        for layer in stops.unique().tolist():  # at most n_layers groups: the pairs that stopped at this layer
+            bs = (stops == layer).nonzero()[:, 0]
+            m, n = lens[bs, 0], lens[bs, 1]
+            rows0, k0, i0 = segment_rows(bs * (M + N), m)
+            rows1, k1, i1 = segment_rows(bs * (M + N) + M, n)
+            lone = torch.cat([(m == 1)[k0], (n == 1)[k1]]).nonzero()[:, 0].tolist()
+            k0, i0, k1, i1 = (t.to(dev) for t in (k0, i0, k1, i1))
+            rows = torch.cat([rows0, rows1]).to(dev)
+            d = xf.index_select(0, rows)
+            md, z = self._head_inputs_packed(d, layer)
+            # cuBLAS takes another summation order for a lone row than for the rows of a longer matrix: the logit of a
+            # view with one point is its own product, as in a one-pair call
+            mw = self.log_assignment[layer].matchability
+            for r in lone:
+                z[r] = F.linear(d[r:r + 1], mw.weight, mw.bias)[0, 0]
+            T0 = rows0.numel()
+            g, Mg, Ng = bs.numel(), int(m.max()), int(n.max())
+
+            def pad(t, k, i, n_, **kw):
+                o = torch.zeros(g, n_, *t.shape[1:], device=dev, **kw)
+                o[k, i] = t
+                return o
+
+            md0, md1 = pad(md[:T0], k0, i0, Mg), pad(md[T0:], k1, i1, Ng)
+            ls, du = F.logsigmoid(z), F.logsigmoid(-z)
+            ls0, du0, ls1, du1 = pad(ls[:T0], k0, i0, Mg), pad(du[:T0], k0, i0, Mg), pad(ls[T0:], k1, i1, Ng), \
+                pad(du[T0:], k1, i1, Ng)
+            ind0 = pad(indf.index_select(0, rows[:T0]), k0, i0, Mg, dtype=torch.int32)
+            ind1 = pad(indf.index_select(0, rows[T0:]), k1, i1, Ng, dtype=torch.int32)
             sim = engine.similarity(md0, md1, self._cdt)
-            st = ops.assign_stats(sim, F.logsigmoid(z0), F.logsigmoid(z1), F.logsigmoid(-z0), F.logsigmoid(-z1),
-                                  dense=True)
-            a0, a1, s0, s1 = ops.filter_matches(st["rowmax"], st["rowarg"], st["colarg"], conf.filter_threshold)
-            pb = torch.tensor(bs, device=dev)[:, None]
-            m0[pb, i0] = torch.where(a0 == -1, -1, i1.gather(1, a0.clamp(min=0)))
-            m1[pb, i1] = torch.where(a1 == -1, -1, i0.gather(1, a1.clamp(min=0)))
-            ms0[pb, i0], ms1[pb, i1] = s0, s1
-            heads.append((pb, d0, d1, i0, i1, st))
+            pairs = torch.stack([m, n, bs]).to(**i32)
+            st = ops.assign_varlen(sim, ls0, ls1, du0, du1, pairs, ind0, ind1, conf.filter_threshold, out)
         if do_prune:
             prune0, prune1 = fin["prune0"], fin["prune1"]
         else:  # without pruning every point sees every layer: fp32 like the plain forward's (lightglue.py:528-529)
-            prune0, prune1 = torch.ones_like(ms0) * L, torch.ones_like(ms1) * L
-        pred = {"matches0": m0, "matches1": m1, "matching_scores0": ms0, "matching_scores1": ms1,
-                "prune0": prune0, "prune1": prune1}
-        if B == 1:  # one pair: the pruned shapes of the reference's one-pair loop
-            _, d0, d1, _, _, st = heads[0]
+            prune0, prune1 = fin["prune0"].float() * L, fin["prune1"].float() * L
+        pred = {"matches0": out["m0"], "matches1": out["m1"], "matching_scores0": out["ms0"],
+                "matching_scores1": out["ms1"], "prune0": prune0, "prune1": prune1}
+        if B == 1 and not ragged:  # one pair: the pruned shapes of the reference's one-pair loop
+            a0, a1 = ind0[0].long(), ind1[0].long()
+            r = torch.cat([a0, a0.new_full((1,), M)])
+            c = torch.cat([a1, a1.new_full((1,), N)])
+            d0, d1 = xf.index_select(0, rows[:T0])[None], xf.index_select(0, rows[T0:])[None]
             # for loss(): one state, which gets head n_layers - 1 as in eval mode; a pruned pred is rejected there
             pred.update({"ref_descriptors0": d0[:, None], "ref_descriptors1": d1[:, None],
-                         "log_assignment": st["scores"], "stop_layer": stops[0],
+                         "log_assignment": out["scores"][0, r[:, None], c[None, :]][None], "stop_layer": int(stops[0]),
                          "_b200_layers": [torch.cat([d0[0], d1[0]])], "_b200_sizes": (1, d0.shape[1], d1.shape[1]),
                          "_b200_row_expsum": st["row_expsum"]})
             return pred
-        # B > 1: the original indexing, -inf / zero at pruned points (see the module docstring)
-        la = torch.full((B, M + 1, N + 1), -math.inf, device=dev)
+        # the original indexing, -inf / zero at pruned and padded points (see the module docstring)
+        rows0, k0, _ = segment_rows(torch.arange(B) * (M + N), lens[:, 0])
+        rows1, k1, _ = segment_rows(torch.arange(B) * (M + N) + M, lens[:, 1])
+        rows0, k0, rows1, k1 = (t.to(dev) for t in (rows0, k0, rows1, k1))
         ref0, ref1 = torch.zeros(B, 1, M, D, device=dev), torch.zeros(B, 1, N, D, device=dev)
-        for pb, d0, d1, i0, i1, st in heads:
-            rows = torch.cat([i0, i0.new_full((i0.shape[0], 1), M)], 1)
-            cols = torch.cat([i1, i1.new_full((i1.shape[0], 1), N)], 1)
-            la[pb[:, :, None], rows[:, :, None], cols[:, None, :]] = st["scores"]
-            ref0[pb, 0, i0], ref1[pb, 0, i1] = d0, d1
-        pred.update({"log_assignment": la, "ref_descriptors0": ref0, "ref_descriptors1": ref1,
-                     "stop_layer": torch.tensor(stops, device=dev, dtype=torch.int64), "_b200_ragged": True})
+        ref0.view(B * M, D)[k0 * M + indf.index_select(0, rows0).long()] = xf.index_select(0, rows0)
+        ref1.view(B * N, D)[k1 * N + indf.index_select(0, rows1).long()] = xf.index_select(0, rows1)
+        pred.update({"log_assignment": out["scores"], "ref_descriptors0": ref0, "ref_descriptors1": ref1,
+                     "stop_layer": fin["stop"].long(), "_b200_ragged": True})
         return pred
+
+    def _head_inputs_packed(self, d, i):
+        """final_proj / matchability of layer i over packed tokens d [T, D] (lightglue.py:280-285)."""
+        la = self.log_assignment[i]
+        md = self._lin(d, la.final_proj).float() / d.shape[-1]**0.25
+        z = F.linear(d, la.matchability.weight, la.matchability.bias).squeeze(-1)
+        return md, z
 
     # ------------------------------------------------------------------------------------------
     def _loss(self, pred, data):
@@ -465,8 +595,9 @@ class LightGlue(nn.Module):
         yields the NLL and the token-confidence BCE; the O(M+N) terms are two small fused kernels."""
         conf = self.conf
         if pred.get("_b200_ragged"):
-            raise ValueError("LightGlue.loss cannot be taken on the pred of an adaptive forward over several pairs: each "
-                             "pair stopped and was pruned on its own (depth_confidence / width_confidence)")
+            raise ValueError("LightGlue.loss cannot be taken on the pred of an adaptive forward over several pairs or "
+                             "of a forward with num_keypoints0/1: each pair stopped, was pruned or was truncated on its "
+                             "own")
         layers_x = pred.get("_b200_layers")
         if layers_x is None:
             raise ValueError("LightGlue.loss needs the pred of this module's own forward: pred['_b200_layers'] is missing")

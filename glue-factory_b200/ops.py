@@ -752,12 +752,14 @@ def head_token_fwd(x, wm, bm, wt, bt, cdt):
 
 
 def adaptive_compact(x, theta, ind, zt, seg, fin, layer, sizes, conf_thr=None, depth_conf=-1.0, width_conf=-1.0,
-                     finish=False):
+                     finish=False, pair_pts=None):
     """One layer's stop / prune step of adaptive depth / width on a batch of pairs (lgb200_adaptive_compact,
     include/lgb200.h).  x [T, D], theta [T, R] fp32, ind [T] int32, zt [T, 2] (None when finish), seg [4, 2B] int32.
     fin: dict of the per-batch outputs updated in place -- x [B (M + N), D], ind [B (M + N)], len [2B], stop [B]
-    (int32) and prune0 [B, M] / prune1 [B, N] (int64).  Returns (x, theta, ind, seg, status): the packed state of the
-    next layer with T rows of capacity, and status [2] int32 = (kept tokens, emptied-view flag), still on the device."""
+    (int32) and prune0 [B, M] / prune1 [B, N] (int64).  pair_pts: None, or [B] int32 = each pair's original point count
+    when the pairs have different sizes (M, N are then the padded sizes; lgb200_adaptive_compact_varlen).  Returns
+    (x, theta, ind, seg, status): the packed state of the next layer with T rows of capacity, and status [2] int32 =
+    (kept tokens, emptied-view flag), still on the device."""
     B, M, N = sizes
     T, D = x.shape
     R = theta.shape[1]
@@ -773,10 +775,17 @@ def adaptive_compact(x, theta, ind, zt, seg, fin, layer, sizes, conf_thr=None, d
     status = torch.empty(2, device=dev, dtype=torch.int32)
     ws = torch.empty(_lib.load().lgb200_adaptive_compact_ws_ints(T, B), device=dev, dtype=torch.int32)
     do_stop, do_prune = depth_conf > 0, width_conf > 0
-    call("lgb200_adaptive_compact", ptr(x), ptr(theta), ptr(ind), ptr(zt), ptr(seg), ptr(x_out), ptr(theta_out),
-         ptr(ind_out), ptr(seg_out), ptr(fin["x"]), ptr(fin["ind"]), ptr(fin["len"]), ptr(fin["stop"]),
-         ptr(fin["prune0"]), ptr(fin["prune1"]), ptr(status), ptr(ws), ptr(conf_thr), float(depth_conf),
-         float(1 - width_conf), int(do_stop), int(do_prune), int(layer), int(finish), B, M, N, T, D, R, stream_ptr())
+    args = (ptr(x), ptr(theta), ptr(ind), ptr(zt), ptr(seg), ptr(x_out), ptr(theta_out), ptr(ind_out), ptr(seg_out),
+            ptr(fin["x"]), ptr(fin["ind"]), ptr(fin["len"]), ptr(fin["stop"]), ptr(fin["prune0"]), ptr(fin["prune1"]),
+            ptr(status), ptr(ws), ptr(conf_thr))
+    rest = (float(depth_conf), float(1 - width_conf), int(do_stop), int(do_prune), int(layer), int(finish), B, M, N, T,
+            D, R, stream_ptr())
+    if pair_pts is None:
+        call("lgb200_adaptive_compact", *args, *rest)
+    else:
+        _chk(pair_pts, torch.int32)
+        assert pair_pts.shape == (B,) and pair_pts.device == x.device
+        call("lgb200_adaptive_compact_varlen", *args, ptr(pair_pts), *rest)
     return x_out, theta_out, ind_out, seg_out, status
 
 
@@ -812,6 +821,41 @@ def filter_matches(rowmax, rowarg, colarg, th):
     call("lgb200_filter_matches", ptr(rowmax), ptr(rowarg), ptr(colarg), float(th), ptr(m0), ptr(m1), ptr(ms0),
          ptr(ms1), B, M, N, stream_ptr())
     return m0, m1, ms0, ms1
+
+
+def assign_varlen(sim, ls0, ls1, dust0, dust1, pairs, ind0, ind1, th, out):
+    """The evaluation head (assign_stats(dense=True) + filter_matches) over G pairs of different sizes in one pass each
+    (lgb200_assign_{lse,scores}_varlen + lgb200_filter_matches_varlen, include/lgb200.h).  sim [G, M, N] fp32 padded;
+    ls0 / dust0 [G, M], ls1 / dust1 [G, N]; pairs [3, G] int32 = (m, n, output batch row); ind0 [G, M] / ind1 [G, N]
+    int32 original keypoint indices; nothing past a pair's (m, n) is read.  `out` holds the batch outputs, written in
+    place at the original indices: scores [Bo, Mo + 1, No + 1], m0 / ms0 [Bo, Mo] (int64 / fp32), m1 / ms1 [Bo, No].
+    Returns the padded per-row statistics (rowmax, rowarg, row_expsum [G, M]; colmax, colarg [G, N])."""
+    _chk(sim, torch.float32)
+    for t in (pairs, ind0, ind1):
+        _chk(t, torch.int32)
+    G, M, N = sim.shape
+    assert pairs.shape == (3, G) and ind0.shape == (G, M) and ind1.shape == (G, N), (pairs.shape, ind0.shape, ind1.shape)
+    scores, m0, m1, ms0, ms1 = (out[k] for k in ("scores", "m0", "m1", "ms0", "ms1"))
+    _chk(scores, torch.float32), _chk(m0, torch.int64), _chk(m1, torch.int64), _chk(ms0, torch.float32)
+    _chk(ms1, torch.float32)
+    Mo, No = m0.shape[1], m1.shape[1]
+    assert scores.shape[1:] == (Mo + 1, No + 1) and ms0.shape == m0.shape and ms1.shape == m1.shape
+    dev = sim.device
+    f = lambda *s: torch.empty(*s, device=dev, dtype=torch.float32)  # noqa: E731
+    st = {"lse_row": f(G, M), "lse_col": f(G, N), "rowmax": f(G, M), "colmax": f(G, N), "row_expsum": f(G, M),
+          "rowarg": torch.empty(G, M, device=dev, dtype=torch.int32),
+          "colarg": torch.empty(G, N, device=dev, dtype=torch.int32)}
+    ws = torch.empty(_lib.load().lgb200_assign_ws_bytes(G, M, N), device=dev, dtype=torch.uint8)
+    call("lgb200_assign_lse_varlen", ptr(sim), ptr(st["lse_row"]), ptr(st["lse_col"]), ptr(ws), ptr(pairs), G, M, N,
+         stream_ptr())
+    ls0, ls1, dust0, dust1 = (t.detach().float().contiguous() for t in (ls0, ls1, dust0, dust1))
+    assert ls0.shape == dust0.shape == (G, M) and ls1.shape == dust1.shape == (G, N)
+    call("lgb200_assign_scores_varlen", ptr(sim), ptr(st["lse_row"]), ptr(st["lse_col"]), ptr(ls0), ptr(ls1), ptr(dust0),
+         ptr(dust1), ptr(scores), ptr(st["rowmax"]), ptr(st["rowarg"]), ptr(st["colmax"]), ptr(st["colarg"]),
+         ptr(st["row_expsum"]), ptr(ws), ptr(pairs), ptr(ind0), ptr(ind1), G, M, N, Mo, No, stream_ptr())
+    call("lgb200_filter_matches_varlen", ptr(st["rowmax"]), ptr(st["rowarg"]), ptr(st["colarg"]), float(th), ptr(m0),
+         ptr(m1), ptr(ms0), ptr(ms1), ptr(pairs), ptr(ind0), ptr(ind1), G, M, N, Mo, No, stream_ptr())
+    return st
 
 
 def _log_double_softmax_fwd(sim, bin_score):

@@ -197,6 +197,27 @@ int lgb200_assign_fused_bwd(const void* md0, const void* md1, float alpha, const
                             cudaStream_t stream);
 int lgb200_filter_matches(const float* rowmax, const int* rowarg, const int* colarg, float th, int64_t* m0,
                           int64_t* m1, float* ms0, float* ms1, int B, int M, int N, cudaStream_t stream);
+/* Varlen forms of lgb200_assign_lse / lgb200_assign_scores (evaluation: no gt, no pos_row_sum) / lgb200_filter_matches:
+ * one launch each over G pairs of different sizes (the packed evaluation head of LightGlue's adaptive / ragged
+ * inference).  pairs [3, G] int32 (device) = (m, n, output batch row) of each pair, 1 <= m <= M, 1 <= n <= N; the
+ * operands are padded: sim [G, M, N], ls0 / dust0 [G, M], ls1 / dust1 [G, N], and so are the intermediates lse_row /
+ * rowmax / rowarg / row_expsum [G, M] and lse_col / colmax / colarg [G, N]; entries past a pair's extents are never read
+ * (they may hold NaN) and, in the intermediates, never written.  ws: lgb200_assign_ws_bytes(G, M, N).  ind0 [G, M] /
+ * ind1 [G, N] int32 (device): each row's / column's original keypoint index (< Mo / < No, distinct within a pair).
+ * Pair g's scores go to scores [*, Mo + 1, No + 1] at row pairs[2G + g]: (ind0 i, ind1 j) for i < m, j < n, the
+ * dustbin column No, the dustbin row Mo and the corner; every other entry keeps its contents.  filter_matches_varlen
+ * writes m0 / ms0 [*, Mo] at ind0 and m1 / ms1 [*, No] at ind1 of that row, the matches themselves as original
+ * indices.  Per pair the values are bit-identical to a uniform call on [1, m, n] (same kernels, same order).      */
+int lgb200_assign_lse_varlen(const float* sim, float* lse_row, float* lse_col, void* ws, const int* pairs, int G, int M,
+                             int N, cudaStream_t stream);
+int lgb200_assign_scores_varlen(const float* sim, const float* lse_row, const float* lse_col, const float* ls0,
+                                const float* ls1, const float* dust0, const float* dust1, float* scores, float* rowmax,
+                                int* rowarg, float* colmax, int* colarg, float* row_expsum, void* ws, const int* pairs,
+                                const int* ind0, const int* ind1, int G, int M, int N, int Mo, int No,
+                                cudaStream_t stream);
+int lgb200_filter_matches_varlen(const float* rowmax, const int* rowarg, const int* colarg, float th, int64_t* m0,
+                                 int64_t* m1, float* ms0, float* ms1, const int* pairs, const int* ind0,
+                                 const int* ind1, int G, int M, int N, int Mo, int No, cudaStream_t stream);
 
 /* O(M+N) terms of one supervised layer (replaces the logsigmoid / weighted-sum / clamp / BCE tensor ops of
  * lightglue.py:264-267, losses.py:13-25, lightglue.py:81-94).  zt [T,2] = per token (matchability logit,
@@ -254,6 +275,15 @@ int lgb200_adaptive_compact(const float* x, const float* theta, const int* ind, 
                             int* fin_len, int* stop_layer, int64_t* prune0, int64_t* prune1, int* status, int* ws,
                             const float* conf_thr, float depth_conf, float width_thr, int do_stop, int do_prune,
                             int layer, int finish, int B, int M, int N, int T, int D, int R, cudaStream_t stream);
+/* The same step for pairs of different original sizes (LightGlue's ragged batches): pair_pts [B] int32 (device) =
+ * each pair's original point count m_b + n_b, which replaces M + N in the stop test; M / N are the padded sizes that
+ * lay out x_fin and prune0 / prune1.  pair_pts NULL is lgb200_adaptive_compact.                                    */
+int lgb200_adaptive_compact_varlen(const float* x, const float* theta, const int* ind, const float* zt, const int* seg,
+                                   float* x_out, float* theta_out, int* ind_out, int* seg_out, float* x_fin,
+                                   int* ind_fin, int* fin_len, int* stop_layer, int64_t* prune0, int64_t* prune1,
+                                   int* status, int* ws, const float* conf_thr, const int* pair_pts, float depth_conf,
+                                   float width_thr, int do_stop, int do_prune, int layer, int finish, int B, int M,
+                                   int N, int T, int D, int R, cudaStream_t stream);
 
 /* ---- other assignment heads on the path ----------------------------------------------------------
  * log_double_softmax with a learned bin (gluestick.py:772-783) and log-domain Sinkhorn optimal
