@@ -20,30 +20,139 @@ __device__ __forceinline__ float logaddexp_f(float a, float b) {
   return m + log1pf(expf(-fabsf(a - b)));
 }
 
+// Varlen batches (GlueStick's packed evaluation heads): pair g < G of the padded [G, M, N] sim has its own extents
+// m = pairs[g] <= M, n = pairs[G + g] <= N (M and N become strides; nothing past a pair's extents is read).  Its scores
+// go to batch row pairs[2G + g] of the output [*, Mo + 1, No + 1] at the same row / column indices, with its dustbin
+// row and column at Mo / No; every other entry keeps its contents.  The row max / argmax of the inner block (first
+// index on ties) go to rowmax / rowarg [G, M], for lgb200_filter_matches_varlen.
+struct LdsVarlen {
+  const int* pairs;  // [3, G]: m, n, output batch row
+  float* rowmax;     // [G, M]
+  int* rowarg;       // [G, M]
+  int G, Mo, No;
+};
+
 // scores from precomputed lse_row / lse_col of the UNBORDERED sim
+template <bool kVarlen>
 __global__ void __launch_bounds__(256) lds_scores_kernel(const float* __restrict__ sim, const float* __restrict__ lse_row,
                                                         const float* __restrict__ lse_col, float beta,
                                                         const float* __restrict__ beta_dev,
-                                                        float* __restrict__ scores, int M, int N) {
+                                                        float* __restrict__ scores, int M, int N, LdsVarlen vp) {
   if (beta_dev) beta = __ldg(beta_dev);  // the learnt bin score read from device memory (no host read-back)
   const int b = blockIdx.y;
   const int i = blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
-  if (i > M) return;
-  float* orow = scores + ((int64_t)b * (M + 1) + i) * (N + 1);
-  if (i == M) {
-    for (int j = lane; j <= N; j += 32)
-      orow[j] = j < N ? beta - logaddexp_f(lse_col[(int64_t)b * N + j], beta) : 0.f;
+  int Mb = M, Nb = N, Mp = M, Np = N;  // this pair's extents (M, N are the strides) and the output's
+  int64_t ob = b;                      // output batch row
+  if constexpr (kVarlen) {
+    Mb = min(vp.pairs[b], M);
+    Nb = min(vp.pairs[vp.G + b], N);
+    Mp = vp.Mo;
+    Np = vp.No;
+    ob = vp.pairs[2 * vp.G + b];
+  }
+  if (i > Mb) return;
+  float* orow = scores + (ob * (Mp + 1) + ((kVarlen && i == Mb) ? Mp : i)) * (Np + 1);
+  if (i == Mb) {
+    for (int j = lane; j <= Nb; j += 32)
+      orow[(kVarlen && j == Nb) ? Np : j] = j < Nb ? beta - logaddexp_f(lse_col[(int64_t)b * N + j], beta) : 0.f;
     return;
   }
   const float lr = logaddexp_f(lse_row[(int64_t)b * M + i], beta);
   const float* srow = sim + ((int64_t)b * M + i) * N;
-  for (int j = lane; j < N; j += 32) {
+  float best = kNInf;
+  int arg = 0x7fffffff;
+  for (int j = lane; j < Nb; j += 32) {
     const float x = srow[j];
     const float lc = logaddexp_f(lse_col[(int64_t)b * N + j], beta);
-    orow[j] = ((x - lr) + (x - lc)) * 0.5f;
+    const float s = ((x - lr) + (x - lc)) * 0.5f;
+    orow[j] = s;
+    if constexpr (kVarlen) {
+      if (s > best || arg == 0x7fffffff) best = s, arg = j;
+    }
   }
-  if (lane == 0) orow[N] = beta - lr;
+  if (lane == 0) orow[Np] = beta - lr;
+  if constexpr (kVarlen) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float v2 = __shfl_xor_sync(0xffffffffu, best, o);
+      const int a2 = __shfl_xor_sync(0xffffffffu, arg, o);
+      if (a2 != 0x7fffffff && (arg == 0x7fffffff || v2 > best || (v2 == best && a2 < arg))) best = v2, arg = a2;
+    }
+    if (lane == 0) {
+      vp.rowmax[(int64_t)b * M + i] = best;
+      vp.rowarg[(int64_t)b * M + i] = arg;
+    }
+  }
+}
+
+// column argmax of a varlen pair's inner scores as written by lds_scores_kernel<true> (first row on ties; thread per
+// column, rows in order)
+__global__ void __launch_bounds__(256) lds_colarg_varlen_kernel(const float* __restrict__ scores, int* __restrict__ colarg,
+                                                               int N, LdsVarlen vp) {
+  const int b = blockIdx.y, j = blockIdx.x * 256 + threadIdx.x;
+  const int Mb = vp.pairs[b], Nb = min(vp.pairs[vp.G + b], N);
+  if (j >= Nb) return;
+  const int64_t pitch = vp.No + 1;
+  const float* col = scores + (int64_t)vp.pairs[2 * vp.G + b] * (vp.Mo + 1) * pitch + j;
+  float best = col[0];
+  int arg = 0;
+  for (int i = 1; i < Mb; ++i) {
+    const float x = col[(int64_t)i * pitch];
+    if (x > best) best = x, arg = i;
+  }
+  colarg[(int64_t)b * N + j] = arg;
+}
+
+// raw line scores (gluestick.py:348-361) of a varlen pair straight from its endpoint similarity block:
+//   raw[g, i, j] = 0.5 * max(s[a0, c0] + s[a1, c1], s[a0, c1] + s[a1, c0]),
+// a0 / a1 = junc0[g, 2i], [2i + 1], c0 / c1 = junc1[g, 2j], [2j + 1], s = sim[g] ([P0, P1] pitch).  Same operations
+// in the same order as the torch formula (two gathers, two adds, maximum, scale).  Thread per (i, j), j fastest.
+__global__ void __launch_bounds__(256) line_scores_varlen_kernel(const float* __restrict__ sim,
+                                                                const int* __restrict__ junc0,
+                                                                const int* __restrict__ junc1, float* __restrict__ raw,
+                                                                const int* __restrict__ pairs, int G, int P0, int P1,
+                                                                int L0, int L1) {
+  const int g = blockIdx.z, i = blockIdx.y;
+  const int j = blockIdx.x * 256 + threadIdx.x;
+  const int Lb0 = min(pairs[g], L0), Lb1 = min(pairs[G + g], L1);
+  if (i >= Lb0 || j >= Lb1) return;
+  const float* s = sim + (int64_t)g * P0 * P1;
+  const int a0 = __ldg(junc0 + (int64_t)g * 2 * L0 + 2 * i), a1 = __ldg(junc0 + (int64_t)g * 2 * L0 + 2 * i + 1);
+  const int c0 = __ldg(junc1 + (int64_t)g * 2 * L1 + 2 * j), c1 = __ldg(junc1 + (int64_t)g * 2 * L1 + 2 * j + 1);
+  const float* r0 = s + (int64_t)a0 * P1;
+  const float* r1 = s + (int64_t)a1 * P1;
+  const float straight = __fadd_rn(__ldg(r0 + c0), __ldg(r1 + c1));
+  const float swapped = __fadd_rn(__ldg(r0 + c1), __ldg(r1 + c0));
+  raw[((int64_t)g * L0 + i) * L1 + j] = 0.5f * fmaxf(straight, swapped);
+}
+
+// x[row] += mean of the endpoint updates upd[e] whose target row is `row` (the LineLayer's scatter-mean over
+// junctions, gluestick.py:682-690).  order [E]: the endpoints sorted stably by target row, tgt_sorted [E] their rows;
+// each run of equal rows is summed in that order (a fixed order: no atomics, and a pair's sums do not depend on the
+// other pairs, whose rows differ).  Warp per sorted position; the warp at the start of a run owns the run.
+__global__ void __launch_bounds__(256) junction_mean_kernel(float* __restrict__ x, const float* __restrict__ upd,
+                                                           const int* __restrict__ order,
+                                                           const int* __restrict__ tgt_sorted, int E, int D) {
+  const int k = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (k >= E) return;
+  const int row = __ldg(tgt_sorted + k);
+  if (k > 0 && __ldg(tgt_sorted + k - 1) == row) return;
+  int end = k + 1;
+  while (end < E && __ldg(tgt_sorted + end) == row) ++end;
+  const float cnt = (float)(end - k);
+  for (int c = lane * 4; c < D; c += 128) {
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int e = k; e < end; ++e) {
+      const float4 u = __ldg(reinterpret_cast<const float4*>(upd + (int64_t)__ldg(order + e) * D + c));
+      s.x = __fadd_rn(s.x, u.x); s.y = __fadd_rn(s.y, u.y); s.z = __fadd_rn(s.z, u.z); s.w = __fadd_rn(s.w, u.w);
+    }
+    float4* xr = reinterpret_cast<float4*>(x + (int64_t)row * D + c);
+    float4 v = *xr;
+    v.x = __fadd_rn(v.x, __fdiv_rn(s.x, cnt)); v.y = __fadd_rn(v.y, __fdiv_rn(s.y, cnt));
+    v.z = __fadd_rn(v.z, __fdiv_rn(s.z, cnt)); v.w = __fadd_rn(v.w, __fdiv_rn(s.w, cnt));
+    *xr = v;
+  }
 }
 
 // ---- Sinkhorn -------------------------------------------------------------------------------------
@@ -576,8 +685,49 @@ static int log_double_softmax_impl(const float* sim, float bin_score, const floa
   void* sub = lse_col + (size_t)B * N;
   int rc = lgb200_assign_lse(sim, lse_row, lse_col, sub, B, M, N, stream);
   if (rc) return rc;
-  lds_scores_kernel<<<dim3((M + 1 + 7) / 8, B), 256, 0, stream>>>(sim, lse_row, lse_col, bin_score, bin_dev, scores, M, N);
+  lds_scores_kernel<false><<<dim3((M + 1 + 7) / 8, B), 256, 0, stream>>>(sim, lse_row, lse_col, bin_score, bin_dev,
+                                                                          scores, M, N, LdsVarlen{});
   return check_launch("log_double_softmax");
+}
+
+int lgb200_log_double_softmax_varlen(const float* sim, const float* bin_score_dev, float* scores, float* rowmax,
+                                     int* rowarg, int* colarg, void* ws, const int* pairs, int G, int M, int N, int Mo,
+                                     int No, cudaStream_t stream) {
+  LGB_REQUIRE(sim && bin_score_dev && scores && rowmax && rowarg && colarg && ws && pairs, kErrInvalid,
+              "log_double_softmax_varlen: null pointer");
+  LGB_REQUIRE(G > 0 && G <= 65535 && M > 0 && N > 0 && Mo > 0 && No > 0, kErrInvalid,
+              "log_double_softmax_varlen: bad extents G=%d M=%d N=%d Mo=%d No=%d", G, M, N, Mo, No);
+  // ws layout as lgb200_log_double_softmax's: [lse_row G*M][lse_col G*N][assign_lse scratch]
+  float* lse_row = static_cast<float*>(ws);
+  float* lse_col = lse_row + (size_t)G * M;
+  void* sub = lse_col + (size_t)G * N;
+  int rc = lgb200_assign_lse_varlen(sim, lse_row, lse_col, sub, pairs, G, M, N, stream);
+  if (rc) return rc;
+  const LdsVarlen vp{pairs, rowmax, rowarg, G, Mo, No};
+  lds_scores_kernel<true><<<dim3((M + 1 + 7) / 8, G), 256, 0, stream>>>(sim, lse_row, lse_col, 0.f, bin_score_dev,
+                                                                        scores, M, N, vp);
+  if ((rc = check_launch("log_double_softmax_varlen"))) return rc;
+  lds_colarg_varlen_kernel<<<dim3((N + 255) / 256, G), 256, 0, stream>>>(scores, colarg, N, vp);
+  return check_launch("log_double_softmax_varlen");
+}
+
+int lgb200_line_scores_varlen(const float* sim, const int* junc0, const int* junc1, float* raw, const int* pairs, int G,
+                              int P0, int P1, int L0, int L1, cudaStream_t stream) {
+  LGB_REQUIRE(sim && junc0 && junc1 && raw && pairs, kErrInvalid, "line_scores_varlen: null pointer");
+  LGB_REQUIRE(G > 0 && G <= 65535 && P0 > 0 && P1 > 0 && L0 > 0 && L0 <= 65535 && L1 > 0, kErrInvalid,
+              "line_scores_varlen: bad extents G=%d P0=%d P1=%d L0=%d L1=%d", G, P0, P1, L0, L1);
+  line_scores_varlen_kernel<<<dim3((L1 + 255) / 256, L0, G), 256, 0, stream>>>(sim, junc0, junc1, raw, pairs, G, P0, P1,
+                                                                                L0, L1);
+  return check_launch("line_scores_varlen");
+}
+
+int lgb200_junction_mean_varlen(float* x, const float* upd, const int* order, const int* tgt_sorted, int E, int D,
+                                cudaStream_t stream) {
+  LGB_REQUIRE(x && upd && order && tgt_sorted, kErrInvalid, "junction_mean_varlen: null pointer");
+  LGB_REQUIRE(E > 0 && D > 0 && D % 4 == 0, kErrInvalid, "junction_mean_varlen: bad extents E=%d D=%d", E, D);
+  LGB_REQUIRE(((uintptr_t)x | (uintptr_t)upd) % 16 == 0, kErrInvalid, "junction_mean_varlen: x / upd not 16-byte aligned");
+  junction_mean_kernel<<<(E + 7) / 8, 256, 0, stream>>>(x, upd, order, tgt_sorted, E, D);
+  return check_launch("junction_mean_varlen");
 }
 
 static int sk_launch(const void* fn, const SkPlan& p, size_t smem, void** args, cudaStream_t stream, const char* what) {

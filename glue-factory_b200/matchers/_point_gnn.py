@@ -46,25 +46,35 @@ class PointGNN(nn.Module):
     def _bf16(self):
         return self.conf.precision == "bf16"
 
-    def _conv(self, x, conv, w=None, b=None, keep_bf16=False):
+    def _conv(self, x, conv, w=None, b=None, keep_bf16=False, rowwise=False):
         """Conv1d(kernel 1) on token-major x [T, C_in]; w / b override the module's parameters (permuted views).
         bf16 mode: x may already be bf16 (no second cast), and keep_bf16 leaves the GEMM's bf16 output as it is for a
-        consumer that rounds to bf16 anyway (the next GEMM, BatchNorm + ReLU in front of one, the attention kernels)."""
+        consumer that rounds to bf16 anyway (the next GEMM, BatchNorm + ReLU in front of one, the attention kernels).
+        rowwise (bf16 mode, packed batches): a layer too narrow for the wgmma GEMM sums its inputs in index order
+        elementwise instead of on cuBLAS, which picks its kernel and summation order by the row count: a row's result
+        then does not depend on the other pairs of the batch."""
         w = conv.weight[:, :, 0] if w is None else w
         b = conv.bias if b is None else b
         if self._bf16 and w.shape[1] % 64 == 0 and w.shape[0] % 8 == 0:
             y = ops.LinearFn.apply(x.to(torch.bfloat16).contiguous(), w, b)
             return y if keep_bf16 else y.float()
+        if rowwise and self._bf16:
+            x, w = x.float(), w.float()
+            y = x[:, :1] * w[:, 0]
+            for k in range(1, w.shape[1]):
+                y = torch.addcmul(y, x[:, k:k + 1], w[:, k])
+            return y + b
         return F.linear(x.float(), w, b)
 
-    def _mlp(self, x, seq, stats=None):
-        """`stats`: None or a list that receives (BatchNorm module, batch statistics) of every training-mode BatchNorm."""
+    def _mlp(self, x, seq, stats=None, rowwise=False):
+        """`stats`: None or a list that receives (BatchNorm module, batch statistics) of every training-mode BatchNorm.
+        `rowwise`: as in _conv."""
         mods = list(seq)
         for i, m in enumerate(mods):
             if isinstance(m, nn.Conv1d):
                 # an inner layer's output only feeds BatchNorm / ReLU and the next GEMM, which rounds it to bf16 at the
                 # same point either way: keep it bf16 (BatchNorm still accumulates its statistics in fp64)
-                x = self._conv(x, m, keep_bf16=self._bf16 and i < len(mods) - 1)
+                x = self._conv(x, m, keep_bf16=self._bf16 and i < len(mods) - 1, rowwise=rowwise)
             elif isinstance(m, _BatchNorm):
                 # BatchNorm1d, or SyncBatchNorm after convert_sync_batchnorm (statistics summed over its process
                 # group), fused with the ReLU that MLP() puts behind it; [T, C]: statistics over all tokens of this call
@@ -95,6 +105,28 @@ class PointGNN(nn.Module):
         shp = lambda t: t.to(cdt).view(B, -1, 4, D // 4)  # noqa: E731  head-major thanks to the permuted rows
         o = ops.Attention.apply(shp(q), shp(k), shp(v), 0, (D // 4) ** -0.5)
         return self._conv(o.reshape(-1, D), attn.merge, merge_w, attn.merge.bias)
+
+    def _attention_packed(self, x, attn, seg, max_len, cross, wts):
+        """MultiHeadedAttention over packed pairs (eval): x [T, D] holds every view's tokens, seg [4, S] int32 on the
+        device = (offset, length, partner's offset, partner's length) per view (lightglue.RaggedLayout.seg).  Each view
+        attends to its own tokens (self) or to its partner's (cross) on ops.attn_fwd_varlen; max_len bounds every
+        length."""
+        T, D = x.shape
+        proj_w, merge_w = wts
+        if self._bf16:
+            x = x.to(torch.bfloat16)
+        q, k, v = (self._conv(x, p, w, b, keep_bf16=True) for p, (w, b) in zip(attn.proj, proj_w))
+        cdt = torch.bfloat16 if self._bf16 else torch.float32
+        shp = lambda t: t.to(cdt).contiguous().view(T, 4, D // 4)  # noqa: E731  head-major thanks to the permuted rows
+        off, ln, poff, pln = seg
+        o, _ = ops.attn_fwd_varlen(shp(q), shp(k), shp(v), off, ln, poff if cross else off, pln if cross else ln,
+                                   max_len, (D // 4) ** -0.5)
+        return self._conv(o.reshape(T, D), attn.merge, merge_w, attn.merge.bias)
+
+    def _gnn_layer_packed(self, x, prop, cross, seg, max_len):
+        """_gnn_layer over packed pairs (see _attention_packed): x + MLP([x ; MHA(x, src)]) for every token at once."""
+        msg = self._attention_packed(x, prop.attn, seg, max_len, cross, self._attn_weights(prop.attn))
+        return x + self._mlp(torch.cat([x, msg], 1), prop.mlp)
 
     def _gnn_layer(self, d0, d1, prop, cross, B, stats=None):
         """One AttentionalPropagation `prop` applied to both images: x + MLP([x ; MHA(x, src)]), src the other image's

@@ -23,6 +23,9 @@ node features are token-major [B*N, D] like in the LightGlue plugin, so
     before the DDP wrap): their statistics and backward sums are then all-reduced over the module's process group
     between the two passes, so every rank normalises with the global batch's statistics like the reference;
   * the LineLayer's gather / scatter-mean over junctions and the O(lines^2) line-score gathers are torch ops.
+Batches of pairs of different sizes (eval, `num_keypoints0/1`, `num_lines0/1`) run `_forward_packed`: packed tokens,
+length-aware attention, a fixed-order junction mean and the varlen heads (`ops.log_double_softmax_varlen`,
+`ops.line_scores_varlen`, `ops.junction_mean_`); see INTEGRATION.md for its outputs and refusals.
 `precision: "bf16"` (default) rounds GEMM / attention operands to bf16 (the reference forces its attention to fp32,
 gluestick.py:17-22; the fp32 mode reproduces that); `precision: "fp32"` is the parity path (fp32 cuBLAS linears,
 CUDA-core attention).  No CPU fallback.
@@ -46,7 +49,7 @@ from torch import nn
 from .. import _lib, ops
 from . import _weights
 from ._point_gnn import PointGNN
-from .lightglue import _Conf, _merge, _to_plain, matcher_metrics
+from .lightglue import _Conf, _merge, _to_plain, keypoint_counts, matcher_metrics, ragged_layout, segment_rows
 
 
 def MLP(channels, do_bn=True):
@@ -229,6 +232,9 @@ class GlueStick(PointGNN):
         B, n0 = kp0.shape[:2]
         n1 = kp1.shape[1]
         L0, L1 = data["lines0"].shape[1], data["lines1"].shape[1]
+        counts = self._counts(data, B, n0, n1, L0, L1)
+        if counts is not None:
+            return self._forward_packed(data, *counts)
         if n0 == 0 or n1 == 0:  # nothing to match: no computation
             return _empty_pred(B, n0, n1, L0, L1, kp0.device)
         _lib.load()  # raises unless the CUDA library is built and the device is an H100 (no CPU fallback)
@@ -302,6 +308,139 @@ class GlueStick(PointGNN):
         lscores = ops.log_double_softmax(raw.contiguous(), self.line_bin_score)
         return (lscores, *self._matches(lscores.detach()), raw)
 
+    # ------------------------------------------------------------------------------------------ packed batches
+    def _counts(self, data, B, M, N, L0, L1):
+        """The optional per-pair counts num_keypoints0/1 (1 .. padded length) and num_lines0/1 (0 .. padded length) as
+        int64 CPU tensors (n0, n1, l0, l1), a missing key meaning every row of that view; None without any of them."""
+        kc = keypoint_counts(data, B, M, N, owner="GlueStick")
+        lc = keypoint_counts(data, B, L0, L1, keys=("num_lines0", "num_lines1"), low=0, owner="GlueStick")
+        if kc is None and lc is None:
+            return None
+        if self.training:
+            raise ValueError("GlueStick: num_keypoints0/1 and num_lines0/1 are taken in eval mode only (BatchNorm "
+                             "normalises training batches with their own statistics, padding included)")
+        full = lambda n: torch.full((B,), n, dtype=torch.int64)  # noqa: E731
+        kc = kc if kc is not None else (full(M), full(N))
+        lc = lc if lc is not None else (full(L0), full(L1))
+        return (*kc, *lc)
+
+    @torch.no_grad()
+    def _forward_packed(self, data, n0, n1, l0, l1):
+        """Eval forward over B pairs with their own counts: pair b uses the first n0_b / n1_b keypoints and l0_b / l1_b
+        lines of the padded views, and gets what a one-pair call on those truncated inputs returns, in the padded
+        original indexing (see README, "Batches of pairs of different sizes").  The valid rows are gathered once into
+        the packed token layout [view 0 of every pair; view 1 of every pair] (lightglue.ragged_layout); the encoders,
+        GEMMs and BatchNorms run token-wise over it, attention is length-aware (_attention_packed), the LineLayer
+        averages endpoints into junctions in a fixed order (ops.junction_mean_), and the heads run once over per-pair
+        zero-padded operands on the varlen kernels.  The padding is never read."""
+        _lib.load()  # raises unless the CUDA library is built and the device is an H100 (no CPU fallback)
+        kp0, kp1 = data["keypoints0"], data["keypoints1"]
+        (B, M), N = kp0.shape[:2], kp1.shape[1]
+        Lp0, Lp1 = data["lines0"].shape[1], data["lines1"].shape[1]
+        dev, D = kp0.device, self.conf.descriptor_dim
+        layout = ragged_layout(n0, n1, M, N)
+        src0, src1, pid0, pid1 = (t.to(dev) for t in (layout.src0, layout.src1, layout.pid0, layout.pid1))
+        pick = lambda t, n, src: t.reshape(B * n, *t.shape[2:]).index_select(0, src)  # noqa: E731
+        size0 = _image_size(data["view0"], kp0).to(dev).expand(B, 2)
+        size1 = _image_size(data["view1"], kp1).to(dev).expand(B, 2)
+        x = torch.cat([pick(data["descriptors0"], M, src0), pick(data["descriptors1"], N, src1)], 0).float()
+        if self.conf.input_dim != D:
+            x = self._conv(x, self.input_proj)
+        k = torch.cat([_norm_kpts_packed(pick(kp0.float(), M, src0), size0, pid0),
+                       _norm_kpts_packed(pick(kp1.float(), N, src1), size1, pid1)], 0)
+        s = torch.cat([pick(data["keypoint_scores0"], M, src0), pick(data["keypoint_scores1"], N, src1)], 0).float()
+        x = x + self._mlp(torch.cat([k, s[:, None]], -1), self.kenc.encoder, rowwise=True)
+
+        # a pair with no lines in either view runs no LineLayer and no line head (gluestick.py:213-240, 257-317)
+        lined = (l0 > 0) & (l1 > 0)
+        tok_off = layout.seg[0].long().view(B, 2)
+        views = [endpoint_layout(l, n, Lp, lined) for l, n, Lp in ((l0, n0, Lp0), (l1, n1, Lp1))]
+        lines = bool(lined.any())
+        if lines:
+            enc, tgt, bad = [], [], []
+            for v, (lay, size) in enumerate(zip(views, (size0, size1))):
+                lsrc, lpid, esrc, epid, ssrc, bound = (t.to(dev) for t in lay)
+                enc.append(_endpoint_inputs(data[f"lines{v}"], data[f"line_scores{v}"], size, lsrc, lpid, ssrc))
+                junc = data[f"lines_junc_idx{v}"].reshape(-1).index_select(0, esrc).long()
+                bad.append(((junc < 0) | (junc >= bound)).any())
+                tgt.append(tok_off[:, v].to(dev)[epid] + junc)
+            if bool(torch.stack(bad).any()):  # the junction check's one host read
+                raise ValueError("GlueStick: lines_junc_idx0/1 of pair b's first num_lines lines must lie in "
+                                 "0 .. min(num_keypoints, 2 * num_lines) - 1")
+            enc = self._mlp(torch.cat(enc, 0), self.lenc.encoder, rowwise=True)
+            tgt = torch.cat(tgt).int()
+            order, tgt_sorted = junction_order(tgt)
+            jl = (tgt, order, tgt_sorted, enc)
+        seg, max_len = layout.seg.to(dev), int(max(n0.max(), n1.max()))
+        inter = {}
+        for i, layer in enumerate(self.gnn.layers):
+            x = self._gnn_layer_packed(x, layer.update, layer.type == "cross", seg, max_len)
+            if layer.type == "self" and lines:
+                for _ in range(self.conf.num_line_iterations):
+                    x = self._line_layer_packed(x, jl, self.gnn.line_layers[i // 2])
+            if (lines and self.conf.inter_supervision and layer.type == "cross"
+                    and i // 2 in self.conf.inter_supervision):
+                inter[i // 2] = x
+        # points (keypoints and line junctions together)
+        out = _padded_outputs(B, M, N, dev)
+        md = self._conv(x, self.final_proj)
+        T0 = src0.numel()
+        sim = self._padded_similarity(md[:T0], md[T0:], pid0, layout.src0 % M, pid1, layout.src1 % N, B,
+                                      int(n0.max()), int(n1.max()))
+        pairs = torch.stack([n0, n1, torch.arange(B)]).to(dev, torch.int32)
+        ops.log_double_softmax_varlen(sim, self.bin_score, pairs, self.conf.filter_threshold, out)
+        pred = {"log_assignment": out["scores"], "matches0": out["m0"], "matches1": out["m1"],
+                "matching_scores0": out["ms0"], "matching_scores1": out["ms1"], "_b200_packed": True}
+        lh = _line_head_layout(data, lined, n0, n1, l0, l1, layout, dev) if lines else None
+        heads = [("line_", self.final_line_proj, x)]
+        heads += [(f"line_{blk}_", self.inter_line_proj[self.layer2idx[blk]], inter.get(blk))
+                  for blk in self.conf.inter_supervision or []]
+        for prefix, proj, xf in heads:
+            lo = _padded_outputs(B, Lp0, Lp1, dev)
+            raw = kp0.new_zeros(B, Lp0, Lp1, dtype=torch.float32)
+            if lines:
+                raw_g = self._line_head_packed(xf, proj, lh, lo)
+                raw[lh["bs"], :raw_g.shape[1], :raw_g.shape[2]] = raw_g
+            pred.update({prefix + "log_assignment": lo["scores"], prefix + "matches0": lo["m0"],
+                         prefix + "matches1": lo["m1"], prefix + "matching_scores0": lo["ms0"],
+                         prefix + "matching_scores1": lo["ms1"]})
+            if prefix == "line_":
+                pred["raw_line_scores"] = raw
+        return pred
+
+    def _line_layer_packed(self, x, jl, layer):
+        """LineLayer (gluestick.py:589-691) over the endpoints of every lined pair and both views at once: each
+        endpoint's update from [its junction ; the other end's junction ; its encoding], then every junction's token
+        gets the mean of its endpoints' updates, added in place in a fixed order (ops.junction_mean_)."""
+        tgt, order, tgt_sorted, enc = jl
+        D = x.shape[1]
+        ld = x.index_select(0, tgt)
+        other = ld.view(-1, 2, D).flip(1).reshape(-1, D)
+        upd = self._mlp(torch.cat([ld, other, enc], 1), layer.mlp)
+        return ops.junction_mean_(x, upd.float().contiguous(), order, tgt_sorted)
+
+    def _padded_similarity(self, a, b, k0, i0, k1, i1, G, Mg, Ng):
+        """The similarity of G pairs whose rows a [T0, D] / b [T1, D] are packed (row r: pair k[r], index i[r]), on
+        per-pair zero-padded [G, Mg, Ng] operands; the padded sizes are rounded up to 8 so that bf16 always runs the
+        batched wgmma GEMM, whose entries do not depend on the padding."""
+        Mg, Ng, D = -(-Mg // 8) * 8, -(-Ng // 8) * 8, a.shape[1]
+        pa, pb = a.new_zeros(G, Mg, D), b.new_zeros(G, Ng, D)
+        pa[k0, i0.to(a.device)] = a
+        pb[k1, i1.to(b.device)] = b
+        return self._similarity(pa.view(-1, D), pb.view(-1, D), G)
+
+    def _line_head_packed(self, x, proj, lh, out):
+        """_line_head of every lined pair at once: projection of each pair's first min(n, 2 L) tokens, one padded
+        similarity, the raw line scores straight from it (ops.line_scores_varlen) and the varlen log_double_softmax +
+        match filter into `out`.  Returns the raw scores [G, Lg0, Lg1] of the lined pairs."""
+        md = self._conv(x.index_select(0, lh["rows"]), proj)
+        T0 = lh["k0"].numel()
+        s = self._padded_similarity(md[:T0], md[T0:], lh["k0"], lh["i0"], lh["k1"], lh["i1"], lh["G"], lh["P0"],
+                                    lh["P1"])
+        raw = ops.line_scores_varlen(s, lh["junc0"], lh["junc1"], lh["pairs"], lh["Lg0"], lh["Lg1"])
+        ops.log_double_softmax_varlen(raw, self.line_bin_score, lh["pairs"], self.conf.filter_threshold, out)
+        return raw
+
     def _sub_loss(self, pred, data, losses, bin_score, prefix, block=None):
         """gluestick.py:379-415; `block`: an intermediate line head (pred keys line_{block}_*, ground truth gt_line_*),
         weighted by its loss.inter_supervision entry and without the statistics entries."""
@@ -331,6 +470,9 @@ class GlueStick(PointGNN):
 
     def loss(self, pred, data):
         """gluestick.py:417-462."""
+        if pred.get("_b200_packed"):
+            raise ValueError("GlueStick.loss cannot be taken on the pred of a forward with num_keypoints0/1 or "
+                             "num_lines0/1: each pair was truncated on its own")
         if data["lines0"].shape[1] == 0 or data["lines1"].shape[1] == 0:
             raise ValueError("gluefactory_b200 gluestick: the line loss needs lines in both views (lines0 has "
                              f"{data['lines0'].shape[1]}, lines1 {data['lines1'].shape[1]})")
@@ -355,6 +497,79 @@ def _image_size(view, kpts):
         return view["image_size"]
     h, w = view["image"].shape[-2:]
     return kpts.new_tensor([[w, h]])
+
+
+def _norm_kpts_packed(kpts, size, pid):
+    """PointGNN._norm_kpts of packed points kpts [T, 2] (pid: each row's pair; size [B, 2]): the same arithmetic."""
+    size = size.to(kpts)
+    return (kpts - (size / 2)[pid]) / (size.max(1, keepdim=True).values * 0.7)[pid]
+
+
+def endpoint_layout(nl, nk, Lp, lined):
+    """The line endpoints of one view over B pairs (CPU int64 tensors; nl / nk: each pair's line / keypoint counts, Lp
+    the padded line count, lined: the pairs whose line layers run).  Lines of lined pairs in pair order, endpoints
+    2 l, 2 l + 1 of line l in line order.  Returns
+      lsrc, lpid: each line's row of the flattened [B * Lp] lines and its pair;
+      esrc, epid: each endpoint's entry of the flattened [B * 2 Lp] junction indices and its pair;
+      ssrc: the row of the flattened [B * Lp] line scores each endpoint takes: line e % nl of its pair for endpoint e,
+            as the reference tiles the scores over the interleaved endpoints (`scores.repeat(1, 2)`, gluestick.py:520);
+      bound: each endpoint's junction-index bound min(nk, 2 nl) (the rows the line head's gathers see)."""
+    B = nl.numel()
+    n = torch.where(lined, nl, torch.zeros_like(nl))
+    lsrc, lpid, li = segment_rows(torch.arange(B) * Lp, n)
+    e = (2 * li[:, None] + torch.arange(2)).reshape(-1)
+    epid = lpid.repeat_interleave(2)
+    esrc = epid * 2 * Lp + e
+    ssrc = epid * Lp + e % n[epid].clamp(min=1)
+    bound = torch.minimum(nk, 2 * nl)[epid]
+    return lsrc, lpid, esrc, epid, ssrc, bound
+
+
+def junction_order(tgt):
+    """The endpoints sorted stably by their target token rows tgt [E] int32: (order, tgt_sorted), both int32.  Built once
+    per forward; every LineLayer sums each junction's endpoints in this order."""
+    tgt_sorted, order = torch.sort(tgt, stable=True)
+    return order.int(), tgt_sorted.int()
+
+
+def _endpoint_inputs(lines, scores, size, lsrc, lpid, ssrc):
+    """The endpoint encoder's input [2 nl, 5] of the packed lines (gluestick.py:512-521, as GlueStick._forward's
+    line_enc): normalised endpoint, offset to the other end (negated for the second), tiled line score."""
+    ln = lines.float().reshape(-1, 2, 2).index_select(0, lsrc)
+    ln = _norm_kpts_packed(ln.reshape(-1, 2), size, lpid.repeat_interleave(2)).reshape(-1, 2, 2)
+    off = ln[:, 1] - ln[:, 0]
+    off = torch.stack([off, -off], 1).reshape(-1, 2)
+    sc = scores.reshape(-1).index_select(0, ssrc).float()
+    return torch.cat([ln.reshape(-1, 2), off, sc[:, None]], -1)
+
+
+def _line_head_layout(data, lined, n0, n1, l0, l1, layout, dev):
+    """The packed line heads' operands, shared by the final and the intermediate heads: the lined pairs bs, the token
+    rows of each one's first min(n, 2 L) tokens per view (with their pair k and index i in the group), the junction
+    indices [G, 2 Lg] and pairs [3, G] = (l0, l1, batch row)."""
+    bs = lined.nonzero()[:, 0]
+    tok_off = layout.seg[0].long().view(-1, 2)[bs]
+    lh = {"bs": bs.to(dev), "G": bs.numel()}
+    rows = []
+    for v, (nk, nl) in enumerate(((n0, l0), (n1, l1))):
+        p = torch.minimum(nk, 2 * nl)[bs]
+        r, k, i = segment_rows(tok_off[:, v], p)
+        rows.append(r)
+        Lg = int(nl[bs].max())
+        lh.update({f"k{v}": k.to(dev), f"i{v}": i.to(dev), f"P{v}": int(p.max()), f"Lg{v}": Lg,
+                   f"junc{v}": data[f"lines_junc_idx{v}"].reshape(len(nk), -1)[bs.to(dev), :2 * Lg].int().contiguous()})
+    lh["rows"] = torch.cat(rows).to(dev)
+    lh["pairs"] = torch.stack([l0[bs], l1[bs], bs]).to(dev, torch.int32)
+    return lh
+
+
+def _padded_outputs(B, M, N, dev):
+    """A head's outputs in the padded original indexing: -inf log-assignment, -1 matches and 0 scores wherever a pair's
+    own head writes nothing."""
+    return {"scores": torch.full((B, M + 1, N + 1), float("-inf"), device=dev),
+            "m0": torch.full((B, M), -1, device=dev, dtype=torch.int64),
+            "m1": torch.full((B, N), -1, device=dev, dtype=torch.int64),
+            "ms0": torch.zeros(B, M, device=dev), "ms1": torch.zeros(B, N, device=dev)}
 
 
 def _no_line_outputs(B, L0, L1, device):

@@ -99,29 +99,30 @@ def _merge(base, new):
     return out
 
 
-def keypoint_counts(data, B, M, N):
+def keypoint_counts(data, B, M, N, keys=("num_keypoints0", "num_keypoints1"), low=1, owner="LightGlue"):
     """data["num_keypoints0/1"] (optional, either or both): pair b uses the first n0_b / n1_b rows of the padded
     keypoints / descriptors / scales / oris of each view.  Returns None without them, else (n0, n1) int64 CPU tensors
     of shape [B] (a missing key: every row of that view); the counts' one host read.  Refuses counts of a non-integer
-    dtype, of a shape other than [B], or outside 1 .. the padded length (ValueError)."""
-    if "num_keypoints0" not in data and "num_keypoints1" not in data:
+    dtype, of a shape other than [B], or outside `low` .. the padded length (ValueError).  `keys` / `owner`: the same
+    for other per-view counts (GlueStick's num_lines0/1, low 0) and the name in the messages."""
+    if keys[0] not in data and keys[1] not in data:
         return None
     out = []
-    for key, n in (("num_keypoints0", M), ("num_keypoints1", N)):
+    for key, n in ((keys[0], M), (keys[1], N)):
         c = data.get(key)
         if c is None:
             out.append(torch.full((B,), n, dtype=torch.int64))
             continue
         if not isinstance(c, torch.Tensor) or c.dtype not in (torch.int8, torch.int16, torch.int32, torch.int64,
                                                                 torch.uint8):
-            raise ValueError(f"LightGlue: {key} must be an integer tensor, got "
+            raise ValueError(f"{owner}: {key} must be an integer tensor, got "
                              f"{c.dtype if isinstance(c, torch.Tensor) else type(c).__name__}")
         if tuple(c.shape) != (B,):
-            raise ValueError(f"LightGlue: {key} must have shape [B] = [{B}], got {list(c.shape)}")
+            raise ValueError(f"{owner}: {key} must have shape [B] = [{B}], got {list(c.shape)}")
         out.append(c.detach().to("cpu", torch.int64))
-    for key, c, n in (("num_keypoints0", out[0], M), ("num_keypoints1", out[1], N)):
-        if bool((c < 1).any()) or bool((c > n).any()):
-            raise ValueError(f"LightGlue: {key} must lie in 1 .. {n} (the padded length), got {c.tolist()}")
+    for key, c, n in ((keys[0], out[0], M), (keys[1], out[1], N)):
+        if bool((c < low).any()) or bool((c > n).any()):
+            raise ValueError(f"{owner}: {key} must lie in {low} .. {n} (the padded length), got {c.tolist()}")
     return out[0], out[1]
 
 

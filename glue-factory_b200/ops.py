@@ -880,6 +880,59 @@ def log_double_softmax(sim, bin_score):
     return _log_double_softmax_fwd(sim, bin_score)
 
 
+def log_double_softmax_varlen(sim, bin_score, pairs, th, out):
+    """GlueStick's evaluation head (log_double_softmax + _get_matches, gluestick.py:318-331, 772-783) over G pairs of
+    different sizes (lgb200_log_double_softmax_varlen + lgb200_filter_matches_varlen, include/lgb200.h).  sim [G, M, N]
+    fp32 padded; bin_score a CUDA tensor (read on the device); pairs [3, G] int32 = (m, n, output batch row); nothing
+    past a pair's (m, n) is read.  `out` holds the batch outputs, written in place: scores [Bo, Mo + 1, No + 1] (pair
+    block top-left, dustbins at Mo / No), m0 / ms0 [Bo, Mo] (int64 / fp32), m1 / ms1 [Bo, No]; other entries are kept."""
+    _chk(sim, torch.float32), _chk(pairs, torch.int32)
+    G, M, N = sim.shape
+    assert pairs.shape == (3, G), pairs.shape
+    scores, m0, m1, ms0, ms1 = (out[k] for k in ("scores", "m0", "m1", "ms0", "ms1"))
+    _chk(scores, torch.float32), _chk(m0, torch.int64), _chk(m1, torch.int64), _chk(ms0, torch.float32)
+    _chk(ms1, torch.float32)
+    Mo, No = m0.shape[1], m1.shape[1]
+    assert scores.shape[1:] == (Mo + 1, No + 1) and ms0.shape == m0.shape and ms1.shape == m1.shape
+    bs = _bin_dev(bin_score)
+    assert bs is not None, "log_double_softmax_varlen: the bin score must be a CUDA tensor"
+    dev = sim.device
+    rowmax = torch.empty(G, M, device=dev, dtype=torch.float32)
+    rowarg = torch.empty(G, M, device=dev, dtype=torch.int32)
+    colarg = torch.empty(G, N, device=dev, dtype=torch.int32)
+    ws = torch.empty(_lib.load().lgb200_heads_ws_bytes(G, M, N), device=dev, dtype=torch.uint8)
+    call("lgb200_log_double_softmax_varlen", ptr(sim), ptr(bs), ptr(scores), ptr(rowmax), ptr(rowarg), ptr(colarg),
+         ptr(ws), ptr(pairs), G, M, N, Mo, No, stream_ptr())
+    ind0 = torch.arange(M, device=dev, dtype=torch.int32).expand(G, M).contiguous()
+    ind1 = torch.arange(N, device=dev, dtype=torch.int32).expand(G, N).contiguous()
+    call("lgb200_filter_matches_varlen", ptr(rowmax), ptr(rowarg), ptr(colarg), float(th), ptr(m0), ptr(m1), ptr(ms0),
+         ptr(ms1), ptr(pairs), ptr(ind0), ptr(ind1), G, M, N, Mo, No, stream_ptr())
+
+
+def line_scores_varlen(sim, junc0, junc1, pairs, L0, L1):
+    """raw line scores [G, L0, L1] fp32 (gluestick.py:348-361) of G pairs from their endpoint similarity blocks sim
+    [G, P0, P1] fp32 and junction indices junc0 [G, 2 L0] / junc1 [G, 2 L1] int32; pairs [2+, G] int32 = each pair's
+    line counts (m, n).  Entries past (m, n) are zero."""
+    _chk(sim, torch.float32), _chk(junc0, torch.int32), _chk(junc1, torch.int32), _chk(pairs, torch.int32)
+    G, P0, P1 = sim.shape
+    assert junc0.shape == (G, 2 * L0) and junc1.shape == (G, 2 * L1) and pairs.shape[1] == G
+    raw = torch.zeros(G, L0, L1, device=sim.device, dtype=torch.float32)
+    call("lgb200_line_scores_varlen", ptr(sim), ptr(junc0), ptr(junc1), ptr(raw), ptr(pairs), G, P0, P1, L0, L1,
+         stream_ptr())
+    return raw
+
+
+def junction_mean_(x, upd, order, tgt_sorted):
+    """x [T, D] fp32 += (in place) the mean of the endpoint updates upd [E, D] fp32 per target row, summed in the order
+    `order` [E] int32 (the endpoints sorted stably by target row; tgt_sorted [E] int32 their rows).  Returns x."""
+    _chk(x, torch.float32), _chk(upd, torch.float32), _chk(order, torch.int32), _chk(tgt_sorted, torch.int32)
+    E, D = upd.shape
+    assert x.shape[1] == D and order.shape == tgt_sorted.shape == (E,)
+    if E:
+        call("lgb200_junction_mean_varlen", ptr(x), ptr(upd), ptr(order), ptr(tgt_sorted), E, D, stream_ptr())
+    return x
+
+
 def _bin_dev(alpha):
     """A CUDA tensor bin score as a 1-element fp32 device vector (read by the kernels: no host read-back), else None."""
     if torch.is_tensor(alpha) and alpha.is_cuda:

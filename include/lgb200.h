@@ -295,6 +295,27 @@ int lgb200_log_double_softmax(const float* sim, float bin_score, float* scores, 
 /* the same with the (learnt) bin score read from device memory: no host read-back, capturable into a CUDA graph */
 int lgb200_log_double_softmax_dev(const float* sim, const float* bin_score_dev, float* scores, void* ws, int B, int M,
                                   int N, cudaStream_t stream);
+/* GlueStick's packed evaluation heads over G pairs of different sizes (eval only, no backward).
+ * log_double_softmax_varlen: sim [G, M, N] fp32 padded; pairs [3, G] int32 (device) = (m <= M, n <= N, output batch
+ * row) per pair; nothing past a pair's (m, n) is read.  Pair g's scores go to scores [*, Mo + 1, No + 1] at row
+ * pairs[2G + g]: (i, j) for i < m, j < n, its dustbin column at No, its dustbin row at Mo and the corner (Mo, No); every
+ * other entry keeps its contents.  rowmax / rowarg [G, M] and colarg [G, N] receive the max / argmax of each row and
+ * the argmax of each column of the inner block (first index on ties), the input of lgb200_filter_matches_varlen with
+ * identity index maps.  ws: lgb200_heads_ws_bytes(G, M, N).  Per pair, the scores are bit-identical to
+ * lgb200_log_double_softmax on [1, m, n].
+ * line_scores_varlen: raw [G, L0, L1] (i < m, j < n of pairs [2, G]; other entries untouched) from the endpoint
+ * similarity sim [G, P0, P1] and the junction indices junc0 [G, 2 L0] / junc1 [G, 2 L1] (< P0 / P1 for the pair's
+ * first 2m / 2n entries, not checked here): 0.5 max(s[a0,c0] + s[a1,c1], s[a0,c1] + s[a1,c0]) (gluestick.py:348-361).
+ * junction_mean_varlen: x [*, D] fp32 += per target row, the mean of the endpoint updates upd [E, D] fp32 aimed at it;
+ * order [E] int32 = the endpoints sorted stably by target row, tgt_sorted [E] = their rows in that order.  Each mean is
+ * summed in that order (deterministic).  D % 4 == 0, x and upd 16-byte aligned.                                     */
+int lgb200_log_double_softmax_varlen(const float* sim, const float* bin_score_dev, float* scores, float* rowmax,
+                                     int* rowarg, int* colarg, void* ws, const int* pairs, int G, int M, int N, int Mo,
+                                     int No, cudaStream_t stream);
+int lgb200_line_scores_varlen(const float* sim, const int* junc0, const int* junc1, float* raw, const int* pairs, int G,
+                              int P0, int P1, int L0, int L1, cudaStream_t stream);
+int lgb200_junction_mean_varlen(float* x, const float* upd, const int* order, const int* tgt_sorted, int E, int D,
+                                cudaStream_t stream);
 int lgb200_sinkhorn(const float* sim, float alpha, int iters, float* out, void* ws, int B, int M, int N,
                     cudaStream_t stream);
 /* The same iterations with their potentials kept (uh [iters,B,M+1], vh [iters,B,N+1], both or neither; out may be
