@@ -71,6 +71,8 @@ SIGNATURES = {
     "lgb200_sinkhorn_bwd": (_i, [_vp, _f, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "lgb200_sinkhorn_fwd_dev": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "lgb200_sinkhorn_bwd_dev": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "lgb200_sinkhorn_varlen_ws_bytes": (_sz, [_i, _i, _i]),
+    "lgb200_sinkhorn_varlen": (_i, [_vp, _vp, _i, _vp, _vp, _vp] + [_i] * 5 + [_vp]),
     "lgb200_ot_nll_fwd": (_i, [_vp] * 7 + [_i, _i, _i, _vp]),
     "lgb200_ot_nll_bwd": (_i, [_vp] * 8 + [_i, _i, _i, _vp]),
     "lgb200_ot_filter_stats": (_i, [_vp] * 4 + [_i, _i, _i, _vp]),
@@ -153,6 +155,7 @@ KERNELS_PER_CALL = {
     "lgb200_attn_fwd_varlen": 1, "lgb200_adaptive_compact": 2, "lgb200_adaptive_compact_varlen": 2,  # decide + gather
     "lgb200_assign_lse_varlen": 2, "lgb200_assign_scores_varlen": 2, "lgb200_filter_matches_varlen": 1,
     "lgb200_log_double_softmax_varlen": 4, "lgb200_line_scores_varlen": 1, "lgb200_junction_mean_varlen": 1,
+    "lgb200_sinkhorn_varlen": 2,  # item table + persistent iterations
 }
 launch_count = 0          # running total of kernels launched through `call`
 timed_entry = None        # entry-point name or a set of names: every call of them is bracketed by CUDA events

@@ -528,6 +528,201 @@ static size_t sk_ws_floats(int B, int M, int N) {
   return (size_t)B * (M + N + 2) + 2 * parts * (N + 1) + 64;
 }
 
+// ---- packed Sinkhorn (SuperGlue's packed evaluation head): G pairs of their own sizes in one persistent launch ----
+// Pair g < G of the padded sim [G, M, N] has m = pairs[g] <= M rows and n = pairs[G + g] <= N columns (M and N are
+// strides: nothing past (m, n) is read).  Its strips are kSkvRows rows each, S = ceil(m / kSkvRows) of them, the last
+// one owning the dustbin row; in the merge phase strip s of the pair owns the columns [s C, (s + 1) C) of its n + 1,
+// C = ceil((n + 1) / S).  So a pair's strip geometry and every summation order are functions of (m, n) alone, never
+// of G, the other pairs or the grid: a pair's result is bit-identical in any batch.  Work item = (pair, strip), items
+// of a pair consecutive; the item table is built on the device (sk_varlen_items_kernel), so no host read sizes the
+// launch.  Iterations as sk_fwd_persistent_kernel (two grid barriers each); no strip cache (a 32-row strip of a wide
+// pair does not fit in shared memory, and a CTA may own several items).  Output: pair g's block goes to row
+// pairs[2G + g] of out [*, Mo + 1, No + 1], its dustbin column at No, its dustbin row at Mo; other entries are kept.
+constexpr int kSkvRows = 32;  // one row per warp of the 1024-thread CTA in the row phase
+
+struct SkvGeom {
+  const int* pairs;  // [3, G]: m, n, output batch row
+  const int2* tab;   // [items]: (pair, strip)
+  const int* start;  // [G + 1]: each pair's first item; start[G] = item count
+  int G, M, N, Mo, No;
+};
+
+__device__ __forceinline__ int skv_strips(int m) { return m > 0 ? (m + kSkvRows - 1) / kSkvRows : 0; }
+
+// one CTA: the pairs' first items (serial prefix over G, thread 0), then the table (warp per pair); resets the barrier
+__global__ void __launch_bounds__(1024) sk_varlen_items_kernel(const int* __restrict__ pairs, int G, int M, int N,
+                                                              int2* __restrict__ tab, int* __restrict__ start,
+                                                              unsigned* __restrict__ bar) {
+  if (threadIdx.x == 0) {
+    int acc = 0;
+    for (int g = 0; g < G; ++g) {
+      start[g] = acc;
+      acc += min(pairs[G + g], N) > 0 ? skv_strips(min(pairs[g], M)) : 0;
+    }
+    start[G] = acc;
+    *bar = 0u;
+  }
+  __syncthreads();
+  for (int g = threadIdx.x >> 5; g < G; g += 32) {
+    const int s0 = start[g], S = start[g + 1] - s0;
+    for (int s = threadIdx.x & 31; s < S; s += 32) tab[s0 + s] = make_int2(g, s);
+  }
+}
+
+__global__ void __launch_bounds__(kSkThreads, 1)
+sk_fwd_varlen_kernel(const float* __restrict__ sim, const float* __restrict__ alpha_dev, int iters,
+                     float* __restrict__ out, float* __restrict__ u, float* __restrict__ v, float* __restrict__ pm,
+                     float* __restrict__ ps, unsigned* __restrict__ bar, SkvGeom q) {
+  extern __shared__ float sk_smem[];
+  const int M = q.M, N = q.N, G = q.G;
+  float* vsm = sk_smem;                  // n + 1
+  float* usm = vsm + sk_pad(N + 1);      // kSkvRows + 1
+  const float alpha = __ldg(alpha_dev);  // the learnt bin score read from device memory (no host read-back)
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int items = __ldcg(q.start + G);
+  unsigned target = 0;
+  for (int it = 0; it < iters; ++it) {
+    // ---- row phase
+    for (int w = blockIdx.x; w < items; w += gridDim.x) {
+      const int2 e = __ldg(q.tab + w);
+      const int b = e.x, s = e.y;
+      const int m = min(q.pairs[b], M), n = min(q.pairs[G + b], N), S = skv_strips(m);
+      const int i0 = s * kSkvRows, i1 = min(m, i0 + kSkvRows);
+      const int nrows = i1 - i0 + (s == S - 1 ? 1 : 0);
+      const float norm = -logf((float)(m + n));
+      for (int j = tid; j <= n; j += kSkThreads) vsm[j] = it ? __ldcg(v + (int64_t)b * (N + 1) + j) : 0.f;
+      __syncthreads();
+      for (int r = warp; r < nrows; r += 32) {
+        const int i = i0 + r;
+        float mx = kNInf, sm = 0.f;
+        if (i < m) {
+          const float* row = sim + ((int64_t)b * M + i) * N;
+          int j = lane;
+          for (; j + 224 < n; j += 256) {  // eight loads in flight per lane
+            float x[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) x[k] = row[j + 32 * k];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) x[k] += vsm[j + 32 * k];
+            lse4(mx, sm, x[0], x[1], x[2], x[3]);
+            lse4(mx, sm, x[4], x[5], x[6], x[7]);
+          }
+          for (; j + 96 < n; j += 128)
+            lse4(mx, sm, row[j] + vsm[j], row[j + 32] + vsm[j + 32], row[j + 64] + vsm[j + 64], row[j + 96] + vsm[j + 96]);
+          for (; j < n; j += 32) lse1(mx, sm, row[j] + vsm[j]);
+        } else {
+          for (int j = lane; j < n; j += 32) lse1(mx, sm, alpha + vsm[j]);
+        }
+        lse_warp(mx, sm);
+        if (lane == 0) {
+          lse1(mx, sm, alpha + vsm[n]);
+          const float ui = (i < m ? norm : logf((float)n) + norm) - (mx + logf(sm));
+          usm[r] = ui;
+          u[(int64_t)b * (M + 1) + i] = ui;
+        }
+      }
+      __syncthreads();
+      // column partials over the strip's dense rows (the dustbin row is added in the merge)
+      for (int j = tid; j <= n; j += kSkThreads) {
+        float mx = kNInf, sm = 0.f;
+        if (j < n) {
+          const float* col = sim + ((int64_t)b * M + i0) * N + j;
+          int r = 0;
+          for (; r + 7 < i1 - i0; r += 8) {
+            float x[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) x[k] = col[(int64_t)(r + k) * N];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) x[k] += usm[r + k];
+            lse4(mx, sm, x[0], x[1], x[2], x[3]);
+            lse4(mx, sm, x[4], x[5], x[6], x[7]);
+          }
+          for (; r + 3 < i1 - i0; r += 4)
+            lse4(mx, sm, col[(int64_t)r * N] + usm[r], col[(int64_t)(r + 1) * N] + usm[r + 1],
+                 col[(int64_t)(r + 2) * N] + usm[r + 2], col[(int64_t)(r + 3) * N] + usm[r + 3]);
+          for (; r < i1 - i0; ++r) lse1(mx, sm, col[(int64_t)r * N] + usm[r]);
+        } else {
+          for (int r = 0; r < i1 - i0; ++r) lse1(mx, sm, alpha + usm[r]);
+        }
+        pm[(int64_t)w * (N + 1) + j] = mx;
+        ps[(int64_t)w * (N + 1) + j] = sm;
+      }
+      __syncthreads();
+    }
+    sk_grid_barrier(bar, target);
+    // ---- merge phase: warp per column of the item's slice, the pair's S partials in strip order
+    for (int w = blockIdx.x; w < items; w += gridDim.x) {
+      const int2 e = __ldg(q.tab + w);
+      const int b = e.x, s = e.y;
+      const int m = min(q.pairs[b], M), n = min(q.pairs[G + b], N), S = skv_strips(m);
+      const int C = (n + S) / S, j0 = s * C, j1 = min(n + 1, j0 + C);
+      const int64_t p_first = w - s;  // item of the pair's strip 0
+      const float norm = -logf((float)(m + n));
+      const float ubin = alpha + __ldcg(u + (int64_t)b * (M + 1) + m);
+      for (int j = j0 + warp; j < j1; j += 32) {
+        float mx = kNInf, sm = 0.f;
+        for (int p0 = 0; p0 < S; p0 += 128) {  // four partial pairs in flight per lane
+          float m2[4], s2[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int p = p0 + k * 32 + lane;
+            const int64_t o = (p_first + (p < S ? p : 0)) * (N + 1) + j;
+            m2[k] = p < S ? __ldcg(pm + o) : kNInf;
+            s2[k] = p < S ? __ldcg(ps + o) : 0.f;
+          }
+          const float mn = fmaxf(fmaxf(fmaxf(m2[0], m2[1]), fmaxf(m2[2], m2[3])), mx);
+          if (mn != kNInf) {
+            sm = sm * __expf(mx - mn);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) sm += s2[k] * __expf(m2[k] - mn);
+            mx = mn;
+          }
+        }
+        lse_warp(mx, sm);
+        if (lane == 0) {
+          lse1(mx, sm, ubin);
+          v[(int64_t)b * (N + 1) + j] = (j < n ? norm : logf((float)m) + norm) - (mx + logf(sm));
+        }
+      }
+    }
+    sk_grid_barrier(bar, target);
+  }
+  // ---- output: out = Z + u + v - norm, at the pair's output row with the dustbins at (Mo, No)
+  for (int w = blockIdx.x; w < items; w += gridDim.x) {
+    const int2 e = __ldg(q.tab + w);
+    const int b = e.x, s = e.y;
+    const int m = min(q.pairs[b], M), n = min(q.pairs[G + b], N), S = skv_strips(m);
+    const int i0 = s * kSkvRows, i1 = min(m, i0 + kSkvRows);
+    const int nrows = i1 - i0 + (s == S - 1 ? 1 : 0);
+    const float norm = -logf((float)(m + n));
+    const int64_t pitch = q.No + 1;
+    float* ob = out + (int64_t)q.pairs[2 * G + b] * (q.Mo + 1) * pitch;
+    for (int j = tid; j <= n; j += kSkThreads) vsm[j] = iters ? __ldcg(v + (int64_t)b * (N + 1) + j) : 0.f;
+    __syncthreads();
+    for (int r = warp; r < nrows; r += 32) {
+      const int i = i0 + r;
+      const float ui = (iters ? __ldcg(u + (int64_t)b * (M + 1) + i) : 0.f) - norm;
+      if (i < m) {
+        const float* row = sim + ((int64_t)b * M + i) * N;
+        float* orow = ob + (int64_t)i * pitch;
+        for (int j = lane; j < n; j += 32) orow[j] = row[j] + ui + vsm[j];
+        if (lane == 0) orow[q.No] = alpha + ui + vsm[n];
+      } else {
+        float* orow = ob + (int64_t)q.Mo * pitch;
+        for (int j = lane; j <= n; j += 32) orow[j < n ? j : q.No] = alpha + ui + vsm[j];
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// the item table (two ints per item, at most G * ceil(M / kSkvRows) items), the pairs' first items (G + 1), the
+// barrier word, u [G, M + 1], v [G, N + 1] and two partial planes of items x (N + 1), in 4-byte words
+static size_t skv_ws_floats(int G, int M, int N) {
+  const size_t items = (size_t)G * ((M + kSkvRows - 1) / kSkvRows);
+  return 2 * items + G + 2 + (size_t)G * (M + N + 2) + 2 * items * (N + 1);
+}
+
 // ---- dense Sinkhorn output Z [B,M+1,N+1] (row pitch N+1): NLL head and match-filter statistics -----------------------
 // SuperGlue's loss (superglue.py:322-352) and match filter (:301-311) read only the inner block and the two dustbins of
 // Z: the reference builds dense fp32 copies of the mask and of mask * Z for it.  Here one pass reads the byte mask and
@@ -808,6 +1003,33 @@ int lgb200_sinkhorn_bwd_dev(const float* sim, const float* alpha_dev, int iters,
                             cudaStream_t stream) {
   LGB_REQUIRE(alpha_dev, kErrInvalid, "sinkhorn_bwd: null bin score pointer");
   return sinkhorn_bwd_impl(sim, 0.f, alpha_dev, iters, grad, uh, vh, dsim, dzr, dzc, ws, B, M, N, stream);
+}
+
+size_t lgb200_sinkhorn_varlen_ws_bytes(int G, int M, int N) { return 4 * skv_ws_floats(G, M, N); }
+
+int lgb200_sinkhorn_varlen(const float* sim, const float* alpha_dev, int iters, float* out, void* ws, const int* pairs,
+                           int G, int M, int N, int Mo, int No, cudaStream_t stream) {
+  LGB_REQUIRE(sim && alpha_dev && out && ws && pairs, kErrInvalid, "sinkhorn_varlen: null pointer");
+  LGB_REQUIRE(G > 0 && M > 0 && N > 0 && Mo > 0 && No > 0 && iters >= 0, kErrInvalid,
+              "sinkhorn_varlen: bad arguments G=%d M=%d N=%d Mo=%d No=%d iters=%d", G, M, N, Mo, No, iters);
+  const size_t items = (size_t)G * ((M + kSkvRows - 1) / kSkvRows);
+  // ws layout: [item table][first items G + 1][barrier][u][v][pm][ps]; the int2 table first keeps it aligned
+  int2* tab = static_cast<int2*>(ws);
+  int* start = reinterpret_cast<int*>(tab + items);
+  unsigned* bar = reinterpret_cast<unsigned*>(start + G + 1);
+  float* u = reinterpret_cast<float*>(bar + 1);
+  float* v = u + (size_t)G * (M + 1);
+  float* pm = v + (size_t)G * (N + 1);
+  float* ps = pm + items * (N + 1);
+  sk_varlen_items_kernel<<<1, 1024, 0, stream>>>(pairs, G, M, N, tab, start, bar);
+  if (int rc = check_launch("sinkhorn_varlen")) return rc;
+  SkPlan p{};
+  const int nsm = device_sm_count();
+  p.grid = items < (size_t)nsm ? (int)items : nsm;
+  const size_t smem = ((size_t)sk_pad(N + 1) + sk_pad(kSkvRows + 1)) * 4;
+  SkvGeom q{pairs, tab, start, G, M, N, Mo, No};
+  void* args[] = {&sim, &alpha_dev, &iters, &out, &u, &v, &pm, &ps, &bar, &q};
+  return sk_launch((const void*)sk_fwd_varlen_kernel, p, smem, args, stream, "sinkhorn_varlen");
 }
 
 int lgb200_ot_nll_fwd(const float* Z, const uint8_t* mask, const float* neg0, const float* neg1, float* pos, float* neg,

@@ -152,3 +152,28 @@ class PointGNN(nn.Module):
         if self._bf16 and a.shape[1] % 8 == 0 and b.shape[1] % 8 == 0:
             return _BmmNT.apply(a.to(torch.bfloat16).contiguous(), b.to(torch.bfloat16).contiguous(), D ** -0.5)
         return torch.bmm(a, b.transpose(1, 2)) / D ** 0.5
+
+    def _padded_similarity(self, a, b, k0, i0, k1, i1, G, Mg, Ng):
+        """The similarity of G pairs whose rows a [T0, D] / b [T1, D] are packed (row r: pair k[r], index i[r]), on
+        per-pair zero-padded [G, Mg, Ng] operands; the padded sizes are rounded up to 8 so that bf16 always runs the
+        batched wgmma GEMM, whose entries do not depend on the padding."""
+        Mg, Ng, D = -(-Mg // 8) * 8, -(-Ng // 8) * 8, a.shape[1]
+        pa, pb = a.new_zeros(G, Mg, D), b.new_zeros(G, Ng, D)
+        pa[k0, i0.to(a.device)] = a
+        pb[k1, i1.to(b.device)] = b
+        return self._similarity(pa.view(-1, D), pb.view(-1, D), G)
+
+
+def _norm_kpts_packed(kpts, size, pid):
+    """PointGNN._norm_kpts of packed points kpts [T, 2] (pid: each row's pair; size [B, 2]): the same arithmetic."""
+    size = size.to(kpts)
+    return (kpts - (size / 2)[pid]) / (size.max(1, keepdim=True).values * 0.7)[pid]
+
+
+def _padded_outputs(B, M, N, dev):
+    """A head's outputs in the padded original indexing: -inf log-assignment, -1 matches and 0 scores wherever a pair's
+    own head writes nothing."""
+    return {"scores": torch.full((B, M + 1, N + 1), float("-inf"), device=dev),
+            "m0": torch.full((B, M), -1, device=dev, dtype=torch.int64),
+            "m1": torch.full((B, N), -1, device=dev, dtype=torch.int64),
+            "ms0": torch.zeros(B, M, device=dev), "ms1": torch.zeros(B, N, device=dev)}

@@ -48,7 +48,7 @@ from torch import nn
 
 from .. import _lib, ops
 from . import _weights
-from ._point_gnn import PointGNN
+from ._point_gnn import PointGNN, _norm_kpts_packed, _padded_outputs
 from .lightglue import _Conf, _merge, _to_plain, keypoint_counts, matcher_metrics, ragged_layout, segment_rows
 
 
@@ -419,16 +419,6 @@ class GlueStick(PointGNN):
         upd = self._mlp(torch.cat([ld, other, enc], 1), layer.mlp)
         return ops.junction_mean_(x, upd.float().contiguous(), order, tgt_sorted)
 
-    def _padded_similarity(self, a, b, k0, i0, k1, i1, G, Mg, Ng):
-        """The similarity of G pairs whose rows a [T0, D] / b [T1, D] are packed (row r: pair k[r], index i[r]), on
-        per-pair zero-padded [G, Mg, Ng] operands; the padded sizes are rounded up to 8 so that bf16 always runs the
-        batched wgmma GEMM, whose entries do not depend on the padding."""
-        Mg, Ng, D = -(-Mg // 8) * 8, -(-Ng // 8) * 8, a.shape[1]
-        pa, pb = a.new_zeros(G, Mg, D), b.new_zeros(G, Ng, D)
-        pa[k0, i0.to(a.device)] = a
-        pb[k1, i1.to(b.device)] = b
-        return self._similarity(pa.view(-1, D), pb.view(-1, D), G)
-
     def _line_head_packed(self, x, proj, lh, out):
         """_line_head of every lined pair at once: projection of each pair's first min(n, 2 L) tokens, one padded
         similarity, the raw line scores straight from it (ops.line_scores_varlen) and the varlen log_double_softmax +
@@ -499,12 +489,6 @@ def _image_size(view, kpts):
     return kpts.new_tensor([[w, h]])
 
 
-def _norm_kpts_packed(kpts, size, pid):
-    """PointGNN._norm_kpts of packed points kpts [T, 2] (pid: each row's pair; size [B, 2]): the same arithmetic."""
-    size = size.to(kpts)
-    return (kpts - (size / 2)[pid]) / (size.max(1, keepdim=True).values * 0.7)[pid]
-
-
 def endpoint_layout(nl, nk, Lp, lined):
     """The line endpoints of one view over B pairs (CPU int64 tensors; nl / nk: each pair's line / keypoint counts, Lp
     the padded line count, lined: the pairs whose line layers run).  Lines of lined pairs in pair order, endpoints
@@ -561,15 +545,6 @@ def _line_head_layout(data, lined, n0, n1, l0, l1, layout, dev):
     lh["rows"] = torch.cat(rows).to(dev)
     lh["pairs"] = torch.stack([l0[bs], l1[bs], bs]).to(dev, torch.int32)
     return lh
-
-
-def _padded_outputs(B, M, N, dev):
-    """A head's outputs in the padded original indexing: -inf log-assignment, -1 matches and 0 scores wherever a pair's
-    own head writes nothing."""
-    return {"scores": torch.full((B, M + 1, N + 1), float("-inf"), device=dev),
-            "m0": torch.full((B, M), -1, device=dev, dtype=torch.int64),
-            "m1": torch.full((B, N), -1, device=dev, dtype=torch.int64),
-            "ms0": torch.zeros(B, M, device=dev), "ms1": torch.zeros(B, N, device=dev)}
 
 
 def _no_line_outputs(B, L0, L1, device):

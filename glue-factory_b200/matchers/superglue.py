@@ -11,6 +11,9 @@ kernels that read the bin score on the device (`ops.log_optimal_transport`); the
 pass over the byte ground-truth mask (`ops.ot_nll`), and the match filter (superglue.py:301-311) runs on the row /
 column argmax of that output (`ops.ot_filter_stats` + `ops.filter_matches`).  The Sinkhorn head is fp32 in both
 precisions; in bf16 mode its cost comes from the fp32-output wgmma GEMM.  No CPU fallback.
+Batches of pairs of different sizes (eval, `num_keypoints0/1`) run `_forward_packed`: packed tokens, length-aware
+attention and one packed Sinkhorn launch for every pair (`ops.log_optimal_transport_varlen`); see INTEGRATION.md for
+its outputs and refusals.
 
 Deliberate differences from the reference:
   * `loss` returns `(losses, metrics)` like every other matcher (TwoViewPipeline.loss unpacks two values,
@@ -32,9 +35,9 @@ import torch
 from torch import nn
 
 from .. import _lib, ops
-from ._point_gnn import PointGNN
+from ._point_gnn import PointGNN, _norm_kpts_packed, _padded_outputs
 from .gluestick import MLP
-from .lightglue import _Conf, _merge, _to_plain, matcher_metrics
+from .lightglue import _Conf, _merge, _to_plain, keypoint_counts, matcher_metrics, ragged_layout
 
 
 class KeypointEncoder(nn.Module):
@@ -132,6 +135,12 @@ class SuperGlue(PointGNN):
         for key in self.required_data_keys:
             assert key in data, f"Missing key {key} in data"
         kp0, kp1 = data["keypoints0"], data["keypoints1"]
+        counts = keypoint_counts(data, kp0.shape[0], kp0.shape[1], kp1.shape[1], owner="SuperGlue")
+        if counts is not None:
+            if self.training:
+                raise ValueError("SuperGlue: num_keypoints0/1 are taken in eval mode only (BatchNorm normalises "
+                                 "training batches with their own statistics, padding included)")
+            return self._forward_packed(data, *counts)
         if kp0.shape[1] == 0 or kp1.shape[1] == 0:  # no keypoints (superglue.py:270-277)
             shape0, shape1 = kp0.shape[:-1], kp1.shape[:-1]
             return {"matches0": kp0.new_full(shape0, -1, dtype=torch.int),
@@ -167,6 +176,52 @@ class SuperGlue(PointGNN):
         return {"sinkhorn_cost": cost, "log_assignment": scores, "matches0": m0, "matches1": m1,
                 "matching_scores0": ms0, "matching_scores1": ms1}
 
+    @torch.no_grad()
+    def _forward_packed(self, data, n0, n1):
+        """Eval forward over B pairs with their own keypoint counts: pair b uses the first n0_b / n1_b rows of the
+        padded views and gets what a one-pair call on those truncated inputs returns, in the padded original indexing
+        (see INTEGRATION.md).  The valid rows are gathered once into the packed token layout (lightglue.ragged_layout);
+        the keypoint encoder, the GNN layers (length-aware attention) and final_proj run token-wise over it, the
+        similarity is one batched GEMM over per-pair zero-padded operands, and the Sinkhorn iterations of every pair
+        run in one launch (ops.log_optimal_transport_varlen).  The padding is never read."""
+        _lib.load()  # raises unless the CUDA library is built and the device is an H100 (no CPU fallback)
+        kp0, kp1 = data["keypoints0"], data["keypoints1"]
+        (B, M), N = kp0.shape[:2], kp1.shape[1]
+        dev, D = kp0.device, self.conf.descriptor_dim
+        layout = ragged_layout(n0, n1, M, N)
+        src0, src1, pid0, pid1 = (t.to(dev) for t in (layout.src0, layout.src1, layout.pid0, layout.pid1))
+        pick = lambda t, n, src: t.reshape(B * n, *t.shape[2:]).index_select(0, src)  # noqa: E731
+        size0 = self._image_size(data["view0"], kp0).to(dev).expand(B, 2)
+        size1 = self._image_size(data["view1"], kp1).to(dev).expand(B, 2)
+        k = torch.cat([_norm_kpts_packed(pick(kp0.float(), M, src0), size0, pid0),
+                       _norm_kpts_packed(pick(kp1.float(), N, src1), size1, pid1)], 0)
+        if not torch.cuda.is_current_stream_capturing():  # a host read-back: eager mode only; valid rows only
+            assert torch.all(k >= -1) and torch.all(k <= 1)
+        if self.conf.use_scores:
+            s = torch.cat([pick(data["keypoint_scores0"], M, src0), pick(data["keypoint_scores1"], N, src1)], 0)
+            k = torch.cat([k, s.float()[:, None]], -1)
+        x = torch.cat([pick(data["descriptors0"], M, src0), pick(data["descriptors1"], N, src1)], 0).float()
+        x = x + self._mlp(k, self.kenc.encoder, rowwise=True)
+        seg, max_len = layout.seg.to(dev), int(max(n0.max(), n1.max()))
+        for layer, name in zip(self.gnn.layers, self.gnn.names):
+            x = self._gnn_layer_packed(x, layer, name == "cross", seg, max_len)
+        md = self._conv(x, self.final_proj)
+        T0 = src0.numel()
+        Mg, Ng = int(n0.max()), int(n1.max())
+        sim = self._padded_similarity(md[:T0], md[T0:], pid0, layout.src0 % M, pid1, layout.src1 % N, B, Mg, Ng)
+        pairs = torch.stack([n0, n1, torch.arange(B)]).to(dev, torch.int32)
+        scores = ops.log_optimal_transport_varlen(sim, self.bin_score, self.conf.num_sinkhorn_iterations, pairs,
+                                                  _padded_outputs(B, M, N, dev)["scores"])
+        # a padding row or column of `scores` is all -inf: its argmax is never mutual, and a valid row's max and
+        # argmax only see its own pair's block
+        m0, m1, ms0, ms1 = ops.filter_matches(*ops.ot_filter_stats(scores), self.conf.filter_threshold)
+        inside = ((torch.arange(Mg, device=dev) < n0.to(dev)[:, None])[:, :, None]
+                  & (torch.arange(Ng, device=dev) < n1.to(dev)[:, None])[:, None, :])
+        cost = sim.new_zeros(B, M, N)
+        cost[:, :Mg, :Ng] = torch.where(inside, sim[:, :Mg, :Ng], 0.0)
+        return {"sinkhorn_cost": cost, "log_assignment": scores, "matches0": m0, "matches1": m1,
+                "matching_scores0": ms0, "matching_scores1": ms1, "_b200_packed": True}
+
     @staticmethod
     def _bn_update_on_backward(d0, d1, stats):
         """The reference's checkpointed layer is recomputed in training mode when the backward first reaches it; that
@@ -182,6 +237,9 @@ class SuperGlue(PointGNN):
 
     def loss(self, pred, data):
         """superglue.py:322-352, returned as (losses, metrics) like the other matchers."""
+        if pred.get("_b200_packed"):
+            raise ValueError("SuperGlue.loss cannot be taken on the pred of a forward with num_keypoints0/1: each pair "
+                             "was truncated on its own")
         with torch.autocast(device_type="cuda", enabled=False):
             nll_pos, nll_neg, num_pos, num_neg = ops.ot_nll(pred["log_assignment"], data["gt_assignment"],
                                                             data["gt_matches0"], data["gt_matches1"])

@@ -995,6 +995,24 @@ def log_optimal_transport(sim, alpha, iters):
     return _log_optimal_transport_fwd(sim, alpha if _bin_dev(alpha) is not None else float(alpha), iters)
 
 
+def log_optimal_transport_varlen(sim, alpha, iters, pairs, out):
+    """SuperGlue's evaluation head (superglue.py:186-214) over G pairs of different sizes in one persistent launch
+    (lgb200_sinkhorn_varlen, include/lgb200.h).  sim [G, M, N] fp32 padded; alpha a CUDA tensor (read on the device);
+    pairs [3, G] int32 = (m, n, output batch row); nothing past a pair's (m, n) is read.  Pair g's result is written in
+    place into out [Bo, Mo + 1, No + 1] fp32: its block top-left of row pairs[2, g], its dustbins at Mo / No; every other
+    entry is kept.  Forward only."""
+    _chk(sim, torch.float32), _chk(pairs, torch.int32), _chk(out, torch.float32)
+    G, M, N = sim.shape
+    assert pairs.shape == (3, G) and out.dim() == 3, (pairs.shape, out.shape)
+    a_dev = _bin_dev(alpha)
+    assert a_dev is not None, "log_optimal_transport_varlen: the bin score must be a CUDA tensor"
+    Mo, No = out.shape[1] - 1, out.shape[2] - 1
+    ws = torch.empty(_lib.load().lgb200_sinkhorn_varlen_ws_bytes(G, M, N), device=sim.device, dtype=torch.uint8)
+    call("lgb200_sinkhorn_varlen", ptr(sim), ptr(a_dev), int(iters), ptr(out), ptr(ws), ptr(pairs), G, M, N, Mo, No,
+         stream_ptr())
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # SuperGlue's NLL head and match filter on the dense Sinkhorn output (superglue.py:301-311, 322-352)
 # ------------------------------------------------------------------------------------------------

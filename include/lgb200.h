@@ -333,6 +333,17 @@ int lgb200_sinkhorn_fwd_dev(const float* sim, const float* alpha_dev, int iters,
 int lgb200_sinkhorn_bwd_dev(const float* sim, const float* alpha_dev, int iters, const float* grad, const float* uh,
                             const float* vh, float* dsim, float* dzr, float* dzc, void* ws, int B, int M, int N,
                             cudaStream_t stream);
+/* SuperGlue's packed evaluation head: the Sinkhorn iterations over G pairs of different sizes in one persistent
+ * cooperative launch (eval only, no potentials, no backward).  sim [G, M, N] fp32 padded; pairs [3, G] int32 (device)
+ * = (m <= M, n <= N, output batch row) per pair; nothing past a pair's (m, n) is read; alpha_dev the bin score on the
+ * device; iters >= 0.  Per pair, superglue.py:186-214 with norm = -log(m + n): out = Z + u + v - norm, pair g's block
+ * at row pairs[2G + g] of out [*, Mo + 1, No + 1]: (i, j) for i < m, j < n, its dustbin column at No, its dustbin row
+ * at Mo and the corner (Mo, No); every other entry keeps its contents.  A pair's strip geometry and summation orders
+ * depend on its (m, n) only, so its result is bit-identical whatever the other pairs of the call; it equals
+ * lgb200_sinkhorn_fwd_dev on [1, m, n] up to the order of the column merges.  ws: lgb200_sinkhorn_varlen_ws_bytes. */
+size_t lgb200_sinkhorn_varlen_ws_bytes(int G, int M, int N);
+int lgb200_sinkhorn_varlen(const float* sim, const float* alpha_dev, int iters, float* out, void* ws, const int* pairs,
+                           int G, int M, int N, int Mo, int No, cudaStream_t stream);
 /* NLL head on the dense Sinkhorn output Z [B,M+1,N+1] (row pitch N+1; superglue.py:322-352), gt mask u8 [B,M,N],
  * neg0 [B,M] / neg1 [B,N] the 0/1 unmatched indicators (fp32).  Forward, per pair: pos = sum mask * Z[:M,:N],
  * neg = sum neg0 * Z[:M,N] + sum neg1 * Z[M,:N], in a fixed order (two calls are bit-identical); ws: at least
