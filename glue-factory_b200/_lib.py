@@ -66,6 +66,9 @@ SIGNATURES = {
     "lgb200_log_double_softmax_varlen": (_i, [_vp] * 8 + [_i] * 5 + [_vp]),
     "lgb200_line_scores_varlen": (_i, [_vp] * 5 + [_i] * 5 + [_vp]),
     "lgb200_junction_mean_varlen": (_i, [_vp] * 4 + [_i, _i, _vp]),
+    "lgb200_line_scores_train": (_i, [_vp] * 5 + [_i] * 5 + [_vp]),
+    "lgb200_line_scores_bwd": (_i, [_vp] * 10 + [_i] * 5 + [_vp]),
+    "lgb200_junction_sum": (_i, [_vp] * 4 + [_i, _i, _i, _vp]),
     "lgb200_sinkhorn": (_i, [_vp, _f, _i, _vp, _vp, _i, _i, _i, _vp]),
     "lgb200_sinkhorn_fwd": (_i, [_vp, _f, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "lgb200_sinkhorn_bwd": (_i, [_vp, _f, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
@@ -155,6 +158,7 @@ KERNELS_PER_CALL = {
     "lgb200_attn_fwd_varlen": 1, "lgb200_adaptive_compact": 2, "lgb200_adaptive_compact_varlen": 2,  # decide + gather
     "lgb200_assign_lse_varlen": 2, "lgb200_assign_scores_varlen": 2, "lgb200_filter_matches_varlen": 1,
     "lgb200_log_double_softmax_varlen": 4, "lgb200_line_scores_varlen": 1, "lgb200_junction_mean_varlen": 1,
+    "lgb200_line_scores_train": 1, "lgb200_line_scores_bwd": 1, "lgb200_junction_sum": 1,
     "lgb200_sinkhorn_varlen": 2,  # item table + persistent iterations
 }
 launch_count = 0          # running total of kernels launched through `call`

@@ -108,6 +108,9 @@ __global__ void __launch_bounds__(256) lds_colarg_varlen_kernel(const float* __r
 //   raw[g, i, j] = 0.5 * max(s[a0, c0] + s[a1, c1], s[a0, c1] + s[a1, c0]),
 // a0 / a1 = junc0[g, 2i], [2i + 1], c0 / c1 = junc1[g, 2j], [2j + 1], s = sim[g] ([P0, P1] pitch).  Same operations
 // in the same order as the torch formula (two gathers, two adds, maximum, scale).  Thread per (i, j), j fastest.
+// kTrain (the training path): the maximum propagates a NaN like torch.maximum (fmaxf drops a one-sided one), and a
+// junction index outside [0, P0) / [0, P1) gives NaN instead of a read outside the pair's block.
+template <bool kTrain>
 __global__ void __launch_bounds__(256) line_scores_varlen_kernel(const float* __restrict__ sim,
                                                                 const int* __restrict__ junc0,
                                                                 const int* __restrict__ junc1, float* __restrict__ raw,
@@ -120,20 +123,84 @@ __global__ void __launch_bounds__(256) line_scores_varlen_kernel(const float* __
   const float* s = sim + (int64_t)g * P0 * P1;
   const int a0 = __ldg(junc0 + (int64_t)g * 2 * L0 + 2 * i), a1 = __ldg(junc0 + (int64_t)g * 2 * L0 + 2 * i + 1);
   const int c0 = __ldg(junc1 + (int64_t)g * 2 * L1 + 2 * j), c1 = __ldg(junc1 + (int64_t)g * 2 * L1 + 2 * j + 1);
+  if constexpr (kTrain) {
+    if ((unsigned)a0 >= (unsigned)P0 || (unsigned)a1 >= (unsigned)P0 || (unsigned)c0 >= (unsigned)P1 ||
+        (unsigned)c1 >= (unsigned)P1) {
+      raw[((int64_t)g * L0 + i) * L1 + j] = __int_as_float(0x7fffffff);
+      return;
+    }
+  }
   const float* r0 = s + (int64_t)a0 * P1;
   const float* r1 = s + (int64_t)a1 * P1;
   const float straight = __fadd_rn(__ldg(r0 + c0), __ldg(r1 + c1));
   const float swapped = __fadd_rn(__ldg(r0 + c1), __ldg(r1 + c0));
-  raw[((int64_t)g * L0 + i) * L1 + j] = 0.5f * fmaxf(straight, swapped);
+  float m = fmaxf(straight, swapped);
+  if constexpr (kTrain) m = isnan(straight) ? straight : isnan(swapped) ? swapped : m;
+  raw[((int64_t)g * L0 + i) * L1 + j] = 0.5f * m;
+}
+
+// d sim of line_scores_varlen_kernel<true> (the autograd of the torch formula, summed in a fixed order): for each
+// (r, c) of pair g, every endpoint k0 of view 0 at junction r (CSR: order0[ptr0[g, r] .. ptr0[g, r + 1]), indices into
+// junc0's flat [G, 2 L0], sorted) meets every endpoint k1 of view 1 at junction c.  Their lines i = k0 / 2, j = k1 / 2
+// take s[r, c] in the straight branch when k0 and k1 are the same end (k0 % 2 == k1 % 2), else in the swapped one, and
+// the branch passes on 0.5 * graw[g, i, j] times torch.maximum's weight: 1 to the larger branch, 0 to the smaller
+// (skipped, so a non-finite graw there does not leak), 1/2 to each on an exact tie, 1 to both when either is NaN.
+// Lines past a pair's (m, n), lines with a junction index outside the block and entries of another pair are skipped.  Thread per (r, c),
+// c fastest: the view-0 list is the same for the whole CTA.  Entries no line touches get 0.
+__global__ void __launch_bounds__(256) line_scores_bwd_kernel(const float* __restrict__ graw,
+                                                             const float* __restrict__ sim,
+                                                             const int* __restrict__ junc0,
+                                                             const int* __restrict__ junc1,
+                                                             const int* __restrict__ order0,
+                                                             const int* __restrict__ ptr0,
+                                                             const int* __restrict__ order1,
+                                                             const int* __restrict__ ptr1, const int* __restrict__ pairs,
+                                                             float* __restrict__ dsim, int G, int P0, int P1, int L0,
+                                                             int L1) {
+  const int g = blockIdx.z, r = blockIdx.y;
+  const int c = blockIdx.x * 256 + threadIdx.x;
+  if (c >= P1) return;
+  const int Lb0 = min(pairs[g], L0), Lb1 = min(pairs[G + g], L1);
+  const float* s = sim + (int64_t)g * P0 * P1;
+  const int64_t e0 = (int64_t)g * 2 * L0, e1 = (int64_t)g * 2 * L1;  // pair g's first entries of junc0 / junc1
+  const int b0 = __ldg(ptr0 + (int64_t)g * (P0 + 1) + r), n0 = __ldg(ptr0 + (int64_t)g * (P0 + 1) + r + 1);
+  const int b1 = __ldg(ptr1 + (int64_t)g * (P1 + 1) + c), n1 = __ldg(ptr1 + (int64_t)g * (P1 + 1) + c + 1);
+  float acc = 0.f;
+  for (int p = b0; p < n0; ++p) {
+    const int k0 = __ldg(order0 + p) - (int)e0, i = k0 >> 1;
+    if ((unsigned)i >= (unsigned)Lb0) continue;  // also an endpoint of another pair (a junction index >= n)
+    const int a0 = __ldg(junc0 + e0 + 2 * i), a1 = __ldg(junc0 + e0 + 2 * i + 1);
+    if ((unsigned)a0 >= (unsigned)P0 || (unsigned)a1 >= (unsigned)P0) continue;
+    const float* r0 = s + (int64_t)a0 * P1;
+    const float* r1 = s + (int64_t)a1 * P1;
+    for (int q = b1; q < n1; ++q) {
+      const int k1 = __ldg(order1 + q) - (int)e1, j = k1 >> 1;
+      if ((unsigned)j >= (unsigned)Lb1) continue;
+      const int c0 = __ldg(junc1 + e1 + 2 * j), c1 = __ldg(junc1 + e1 + 2 * j + 1);
+      if ((unsigned)c0 >= (unsigned)P1 || (unsigned)c1 >= (unsigned)P1) continue;
+      const float straight = __fadd_rn(__ldg(r0 + c0), __ldg(r1 + c1));
+      const float swapped = __fadd_rn(__ldg(r0 + c1), __ldg(r1 + c0));
+      const bool mine_straight = (k0 & 1) == (k1 & 1);
+      const float mine = mine_straight ? straight : swapped, other = mine_straight ? swapped : straight;
+      if (mine < other) continue;  // false with a NaN on either side: both branches get the gradient
+      const float d = __fmul_rn(__ldg(graw + ((int64_t)g * L0 + i) * L1 + j), 0.5f);
+      acc = __fadd_rn(acc, mine == other ? __fmul_rn(d, 0.5f) : d);
+    }
+  }
+  dsim[((int64_t)g * P0 + r) * P1 + c] = acc;
 }
 
 // x[row] += mean of the endpoint updates upd[e] whose target row is `row` (the LineLayer's scatter-mean over
 // junctions, gluestick.py:682-690).  order [E]: the endpoints sorted stably by target row, tgt_sorted [E] their rows;
 // each run of equal rows is summed in that order (a fixed order: no atomics, and a pair's sums do not depend on the
 // other pairs, whose rows differ).  Warp per sorted position; the warp at the start of a run owns the run.
+// kPartnerSum: the backward of the LineLayer's endpoint gather instead, x[row] += the sum over the run of
+// upd[e, :D] + upd[e ^ 1, D:2D] (endpoint e read its own junction into columns 0..D-1 and its line's other end e ^ 1
+// read it into columns D..2D-1); upd has row pitch ld.
+template <bool kPartnerSum>
 __global__ void __launch_bounds__(256) junction_mean_kernel(float* __restrict__ x, const float* __restrict__ upd,
                                                            const int* __restrict__ order,
-                                                           const int* __restrict__ tgt_sorted, int E, int D) {
+                                                           const int* __restrict__ tgt_sorted, int E, int D, int ld) {
   const int k = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (k >= E) return;
   const int row = __ldg(tgt_sorted + k);
@@ -144,13 +211,25 @@ __global__ void __launch_bounds__(256) junction_mean_kernel(float* __restrict__ 
   for (int c = lane * 4; c < D; c += 128) {
     float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int e = k; e < end; ++e) {
-      const float4 u = __ldg(reinterpret_cast<const float4*>(upd + (int64_t)__ldg(order + e) * D + c));
-      s.x = __fadd_rn(s.x, u.x); s.y = __fadd_rn(s.y, u.y); s.z = __fadd_rn(s.z, u.z); s.w = __fadd_rn(s.w, u.w);
+      if constexpr (kPartnerSum) {
+        const int o = __ldg(order + e);
+        const float4 u = __ldg(reinterpret_cast<const float4*>(upd + (int64_t)o * ld + c));
+        const float4 w = __ldg(reinterpret_cast<const float4*>(upd + (int64_t)(o ^ 1) * ld + D + c));
+        s.x = __fadd_rn(s.x, u.x); s.y = __fadd_rn(s.y, u.y); s.z = __fadd_rn(s.z, u.z); s.w = __fadd_rn(s.w, u.w);
+        s.x = __fadd_rn(s.x, w.x); s.y = __fadd_rn(s.y, w.y); s.z = __fadd_rn(s.z, w.z); s.w = __fadd_rn(s.w, w.w);
+      } else {
+        const float4 u = __ldg(reinterpret_cast<const float4*>(upd + (int64_t)__ldg(order + e) * D + c));
+        s.x = __fadd_rn(s.x, u.x); s.y = __fadd_rn(s.y, u.y); s.z = __fadd_rn(s.z, u.z); s.w = __fadd_rn(s.w, u.w);
+      }
     }
     float4* xr = reinterpret_cast<float4*>(x + (int64_t)row * D + c);
     float4 v = *xr;
-    v.x = __fadd_rn(v.x, __fdiv_rn(s.x, cnt)); v.y = __fadd_rn(v.y, __fdiv_rn(s.y, cnt));
-    v.z = __fadd_rn(v.z, __fdiv_rn(s.z, cnt)); v.w = __fadd_rn(v.w, __fdiv_rn(s.w, cnt));
+    if constexpr (kPartnerSum) {
+      v.x = __fadd_rn(v.x, s.x); v.y = __fadd_rn(v.y, s.y); v.z = __fadd_rn(v.z, s.z); v.w = __fadd_rn(v.w, s.w);
+    } else {
+      v.x = __fadd_rn(v.x, __fdiv_rn(s.x, cnt)); v.y = __fadd_rn(v.y, __fdiv_rn(s.y, cnt));
+      v.z = __fadd_rn(v.z, __fdiv_rn(s.z, cnt)); v.w = __fadd_rn(v.w, __fdiv_rn(s.w, cnt));
+    }
     *xr = v;
   }
 }
@@ -906,14 +985,41 @@ int lgb200_log_double_softmax_varlen(const float* sim, const float* bin_score_de
   return check_launch("log_double_softmax_varlen");
 }
 
+static int line_scores_launch(bool train, const float* sim, const int* junc0, const int* junc1, float* raw,
+                              const int* pairs, int G, int P0, int P1, int L0, int L1, cudaStream_t stream,
+                              const char* what) {
+  LGB_REQUIRE(sim && junc0 && junc1 && raw && pairs, kErrInvalid, "%s: null pointer", what);
+  LGB_REQUIRE(G > 0 && G <= 65535 && P0 > 0 && P1 > 0 && L0 > 0 && L0 <= 65535 && L1 > 0, kErrInvalid,
+              "%s: bad extents G=%d P0=%d P1=%d L0=%d L1=%d", what, G, P0, P1, L0, L1);
+  const dim3 grid((L1 + 255) / 256, L0, G);
+  if (train)
+    line_scores_varlen_kernel<true><<<grid, 256, 0, stream>>>(sim, junc0, junc1, raw, pairs, G, P0, P1, L0, L1);
+  else
+    line_scores_varlen_kernel<false><<<grid, 256, 0, stream>>>(sim, junc0, junc1, raw, pairs, G, P0, P1, L0, L1);
+  return check_launch(what);
+}
+
 int lgb200_line_scores_varlen(const float* sim, const int* junc0, const int* junc1, float* raw, const int* pairs, int G,
                               int P0, int P1, int L0, int L1, cudaStream_t stream) {
-  LGB_REQUIRE(sim && junc0 && junc1 && raw && pairs, kErrInvalid, "line_scores_varlen: null pointer");
-  LGB_REQUIRE(G > 0 && G <= 65535 && P0 > 0 && P1 > 0 && L0 > 0 && L0 <= 65535 && L1 > 0, kErrInvalid,
-              "line_scores_varlen: bad extents G=%d P0=%d P1=%d L0=%d L1=%d", G, P0, P1, L0, L1);
-  line_scores_varlen_kernel<<<dim3((L1 + 255) / 256, L0, G), 256, 0, stream>>>(sim, junc0, junc1, raw, pairs, G, P0, P1,
-                                                                                L0, L1);
-  return check_launch("line_scores_varlen");
+  return line_scores_launch(false, sim, junc0, junc1, raw, pairs, G, P0, P1, L0, L1, stream, "line_scores_varlen");
+}
+
+int lgb200_line_scores_train(const float* sim, const int* junc0, const int* junc1, float* raw, const int* pairs, int G,
+                             int P0, int P1, int L0, int L1, cudaStream_t stream) {
+  return line_scores_launch(true, sim, junc0, junc1, raw, pairs, G, P0, P1, L0, L1, stream, "line_scores_train");
+}
+
+int lgb200_line_scores_bwd(const float* graw, const float* sim, const int* junc0, const int* junc1, const int* order0,
+                           const int* ptr0, const int* order1, const int* ptr1, const int* pairs, float* dsim, int G,
+                           int P0, int P1, int L0, int L1, cudaStream_t stream) {
+  LGB_REQUIRE(graw && sim && junc0 && junc1 && order0 && ptr0 && order1 && ptr1 && pairs && dsim, kErrInvalid,
+              "line_scores_bwd: null pointer");
+  LGB_REQUIRE(G > 0 && G <= 65535 && P0 > 0 && P0 <= 65535 && P1 > 0 && L0 > 0 && L1 > 0, kErrInvalid,
+              "line_scores_bwd: bad extents G=%d P0=%d P1=%d L0=%d L1=%d", G, P0, P1, L0, L1);
+  line_scores_bwd_kernel<<<dim3((P1 + 255) / 256, P0, G), 256, 0, stream>>>(graw, sim, junc0, junc1, order0, ptr0,
+                                                                             order1, ptr1, pairs, dsim, G, P0, P1, L0,
+                                                                             L1);
+  return check_launch("line_scores_bwd");
 }
 
 int lgb200_junction_mean_varlen(float* x, const float* upd, const int* order, const int* tgt_sorted, int E, int D,
@@ -921,8 +1027,18 @@ int lgb200_junction_mean_varlen(float* x, const float* upd, const int* order, co
   LGB_REQUIRE(x && upd && order && tgt_sorted, kErrInvalid, "junction_mean_varlen: null pointer");
   LGB_REQUIRE(E > 0 && D > 0 && D % 4 == 0, kErrInvalid, "junction_mean_varlen: bad extents E=%d D=%d", E, D);
   LGB_REQUIRE(((uintptr_t)x | (uintptr_t)upd) % 16 == 0, kErrInvalid, "junction_mean_varlen: x / upd not 16-byte aligned");
-  junction_mean_kernel<<<(E + 7) / 8, 256, 0, stream>>>(x, upd, order, tgt_sorted, E, D);
+  junction_mean_kernel<false><<<(E + 7) / 8, 256, 0, stream>>>(x, upd, order, tgt_sorted, E, D, D);
   return check_launch("junction_mean_varlen");
+}
+
+int lgb200_junction_sum(float* x, const float* src, const int* order, const int* tgt_sorted, int E, int D, int ld,
+                        cudaStream_t stream) {
+  LGB_REQUIRE(x && src && order && tgt_sorted, kErrInvalid, "junction_sum: null pointer");
+  LGB_REQUIRE(E > 0 && E % 2 == 0 && D > 0 && D % 4 == 0 && ld >= 2 * D && ld % 4 == 0, kErrInvalid,
+              "junction_sum: bad extents E=%d D=%d ld=%d", E, D, ld);
+  LGB_REQUIRE(((uintptr_t)x | (uintptr_t)src) % 16 == 0, kErrInvalid, "junction_sum: x / src not 16-byte aligned");
+  junction_mean_kernel<true><<<(E + 7) / 8, 256, 0, stream>>>(x, src, order, tgt_sorted, E, D, ld);
+  return check_launch("junction_sum");
 }
 
 static int sk_launch(const void* fn, const SkPlan& p, size_t smem, void** args, cudaStream_t stream, const char* what) {

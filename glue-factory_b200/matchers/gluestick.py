@@ -22,10 +22,13 @@ node features are token-major [B*N, D] like in the LightGlue plugin, so
     glue-factory's distributed trainer the BatchNorms are `nn.SyncBatchNorm` (train.py:337-339, convert_sync_batchnorm
     before the DDP wrap): their statistics and backward sums are then all-reduced over the module's process group
     between the two passes, so every rank normalises with the global batch's statistics like the reference;
-  * the LineLayer's gather / scatter-mean over junctions and the O(lines^2) line-score gathers are torch ops.
+  * the LineLayer's gather and mean over junctions, and the line scores from the junction similarity, are kernels that
+    sum in a fixed order in both directions (`ops.JunctionGather`, `ops.JunctionMean`, `ops.LineScores`): the endpoints
+    are sorted stably by junction once per forward (`junction_layout`), so a wireframe with shared junctions trains to
+    the same bits on every run.
 Batches of pairs of different sizes (eval, `num_keypoints0/1`, `num_lines0/1`) run `_forward_packed`: packed tokens,
-length-aware attention, a fixed-order junction mean and the varlen heads (`ops.log_double_softmax_varlen`,
-`ops.line_scores_varlen`, `ops.junction_mean_`); see INTEGRATION.md for its outputs and refusals.
+length-aware attention, the same LineLayer on a packed JunctionLayout and the varlen heads
+(`ops.log_double_softmax_varlen`, `ops.line_scores_varlen`); see INTEGRATION.md for its outputs and refusals.
 `precision: "bf16"` (default) rounds GEMM / attention operands to bf16 (the reference forces its attention to fp32,
 gluestick.py:17-22; the fp32 mode reproduces that); `precision: "fp32"` is the parity path (fp32 cuBLAS linears,
 CUDA-core attention).  No CPU fallback.
@@ -43,6 +46,8 @@ the local disk only (matchers/_weights.py).
 
 Not built (raise NotImplementedError): `line_attention`, `skip_init`.
 """
+from typing import NamedTuple, Optional
+
 import torch
 from torch import nn
 
@@ -197,21 +202,12 @@ class GlueStick(PointGNN):
             raise ValueError(f"gluefactory_b200 gluestick: loss.inter_supervision {list(weights)} has fewer weights than "
                              f"inter_supervision {list(conf.inter_supervision)} has entries")
 
-    def _line_layer(self, d0, d1, enc0, enc1, idx0, idx1, layer, B):
-        """LineLayer (gluestick.py:589-691, line_attention = False)."""
-        out = []
-        for d, enc, idx in ((d0, enc0, idx0), (d1, enc1, idx1)):
-            D = d.shape[1]
-            n = d.shape[0] // B
-            n2 = idx.shape[1]
-            flat = (idx + torch.arange(B, device=idx.device)[:, None] * n).reshape(-1)  # rows of the [B*n, D] matrix
-            ld = d.index_select(0, flat)
-            other = ld.view(B, n2 // 2, 2, D).flip(2).reshape(B * n2, D)
-            upd = self._mlp(torch.cat([ld, other, enc], 1), layer.mlp)
-            acc = torch.zeros_like(d).scatter_reduce(0, flat[:, None].expand(-1, D), upd.to(d.dtype), reduce="mean",
-                                                     include_self=False)
-            out.append(d + acc)
-        return out[0], out[1]
+    def _line_layer(self, x, enc, lay, layer):
+        """LineLayer (gluestick.py:589-691, line_attention = False) over the endpoints of a JunctionLayout `lay` into the
+        token rows x [T, D]: each endpoint's update from [its junction ; the other end's junction ; its encoding enc],
+        then every junction's row gets the mean of its endpoints' updates, summed in the layout's fixed order."""
+        upd = self._mlp(torch.cat([ops.JunctionGather.apply(x, lay.tgt, lay.order, lay.tgt_sorted), enc], 1), layer.mlp)
+        return ops.JunctionMean.apply(x, upd, lay.tgt, lay.order, lay.tgt_sorted)
 
     def _matches(self, scores):
         """_get_matches (gluestick.py:318-331) on the filter kernel."""
@@ -265,12 +261,15 @@ class GlueStick(PointGNN):
             enc0 = line_enc(data["lines0"], data["line_scores0"], size0)
             enc1 = line_enc(data["lines1"], data["line_scores1"], size1)
             idx0, idx1 = data["lines_junc_idx0"].reshape(B, -1), data["lines_junc_idx1"].reshape(B, -1)
+            lay0 = junction_layout(idx0, n0, min(n0, 2 * L0))
+            lay1 = junction_layout(idx1, n1, min(n1, 2 * L1))
         inter = {}  # block -> both images' features after its cross layer (gluestick.py:762-768)
         for i, layer in enumerate(self.gnn.layers):
             d0, d1 = self._gnn_layer(d0, d1, layer.update, layer.type == "cross", B)
             if layer.type == "self" and lines:
                 for _ in range(self.conf.num_line_iterations):
-                    d0, d1 = self._line_layer(d0, d1, enc0, enc1, idx0, idx1, self.gnn.line_layers[i // 2], B)
+                    line_layer = self.gnn.line_layers[i // 2]
+                    d0, d1 = self._line_layer(d0, enc0, lay0, line_layer), self._line_layer(d1, enc1, lay1, line_layer)
             if (lines and self.conf.inter_supervision and layer.type == "cross"
                     and i // 2 in self.conf.inter_supervision):
                 inter[i // 2] = (d0, d1)
@@ -282,30 +281,30 @@ class GlueStick(PointGNN):
         if not lines:
             pred.update(_no_line_outputs(B, L0, L1, kp0.device), raw_line_scores=kp0.new_zeros(B, L0, L1))
             return pred
-        lscores, lm0, lm1, lms0, lms1, raw = self._line_head(d0, d1, idx0, idx1, L0, L1, self.final_line_proj, B)
+        lscores, lm0, lm1, lms0, lms1, raw = self._line_head(d0, d1, lay0, lay1, L0, L1, self.final_line_proj, B)
         pred.update({"line_log_assignment": lscores, "line_matches0": lm0, "line_matches1": lm1,
                      "line_matching_scores0": lms0, "line_matching_scores1": lms1, "raw_line_scores": raw})
         for block in self.conf.inter_supervision or []:
             proj = self.inter_line_proj[self.layer2idx[block]]
-            la, lm0, lm1, lms0, lms1, _ = self._line_head(*inter[block], idx0, idx1, L0, L1, proj, B)
+            la, lm0, lm1, lms0, lms1, _ = self._line_head(*inter[block], lay0, lay1, L0, L1, proj, B)
             pred.update({f"line_{block}_log_assignment": la, f"line_{block}_matches0": lm0,
                          f"line_{block}_matches1": lm1, f"line_{block}_matching_scores0": lms0,
                          f"line_{block}_matching_scores1": lms1})
         return pred
 
-    def _line_head(self, d0, d1, idx0, idx1, L0, L1, proj, B):
-        """_get_line_matches (gluestick.py:336-376) with the projection `proj`: junction similarity gathered per endpoint
-        pair, best of the two endpoint orderings, log_double_softmax with the line bin score, match filtering.
+    def _line_head(self, d0, d1, lay0, lay1, L0, L1, proj, B):
+        """_get_line_matches (gluestick.py:336-376) with the projection `proj`: junction similarity, best of the two
+        endpoint orderings per line pair (ops.LineScores, from the JunctionLayouts lay0 / lay1), log_double_softmax with
+        the line bin score, match filtering.
         Returns (log-assignment, matches0, matches1, matching_scores0, matching_scores1, raw line scores)."""
         D = d0.shape[1]
         ld0 = d0.view(B, -1, D)[:, :2 * L0].reshape(-1, D)
         ld1 = d1.view(B, -1, D)[:, :2 * L1].reshape(-1, D)
         s = self._similarity(self._conv(ld0, proj), self._conv(ld1, proj), B)
-        n20, n21 = idx0.shape[1], idx1.shape[1]
-        s = torch.gather(s, 2, idx1[:, None, :].expand(B, s.shape[1], n21))
-        s = torch.gather(s, 1, idx0[:, :, None].expand(B, n20, n21)).reshape(B, n20 // 2, 2, n21 // 2, 2)
-        raw = 0.5 * torch.maximum(s[:, :, 0, :, 0] + s[:, :, 1, :, 1], s[:, :, 0, :, 1] + s[:, :, 1, :, 0])
-        lscores = ops.log_double_softmax(raw.contiguous(), self.line_bin_score)
+        full = lambda n: torch.full((B,), n, dtype=torch.int32, device=s.device)  # noqa: E731
+        raw = ops.LineScores.apply(s.contiguous(), lay0.junc, lay1.junc, torch.stack([full(L0), full(L1)]), lay0.order,
+                                   lay0.ptr, lay1.order, lay1.ptr)
+        lscores = ops.log_double_softmax(raw, self.line_bin_score)
         return (lscores, *self._matches(lscores.detach()), raw)
 
     # ------------------------------------------------------------------------------------------ packed batches
@@ -330,9 +329,9 @@ class GlueStick(PointGNN):
         lines of the padded views, and gets what a one-pair call on those truncated inputs returns, in the padded
         original indexing (see README, "Batches of pairs of different sizes").  The valid rows are gathered once into
         the packed token layout [view 0 of every pair; view 1 of every pair] (lightglue.ragged_layout); the encoders,
-        GEMMs and BatchNorms run token-wise over it, attention is length-aware (_attention_packed), the LineLayer
-        averages endpoints into junctions in a fixed order (ops.junction_mean_), and the heads run once over per-pair
-        zero-padded operands on the varlen kernels.  The padding is never read."""
+        GEMMs and BatchNorms run token-wise over it, attention is length-aware (_attention_packed), the LineLayer runs
+        once over the endpoints of every lined pair and both views (eval-mode BatchNorm), and the heads run once over
+        per-pair zero-padded operands on the varlen kernels.  The padding is never read."""
         _lib.load()  # raises unless the CUDA library is built and the device is an H100 (no CPU fallback)
         kp0, kp1 = data["keypoints0"], data["keypoints1"]
         (B, M), N = kp0.shape[:2], kp1.shape[1]
@@ -369,15 +368,14 @@ class GlueStick(PointGNN):
                                  "0 .. min(num_keypoints, 2 * num_lines) - 1")
             enc = self._mlp(torch.cat(enc, 0), self.lenc.encoder, rowwise=True)
             tgt = torch.cat(tgt).int()
-            order, tgt_sorted = junction_order(tgt)
-            jl = (tgt, order, tgt_sorted, enc)
+            lay = JunctionLayout(tgt, *junction_order(tgt), None, None)
         seg, max_len = layout.seg.to(dev), int(max(n0.max(), n1.max()))
         inter = {}
         for i, layer in enumerate(self.gnn.layers):
             x = self._gnn_layer_packed(x, layer.update, layer.type == "cross", seg, max_len)
             if layer.type == "self" and lines:
                 for _ in range(self.conf.num_line_iterations):
-                    x = self._line_layer_packed(x, jl, self.gnn.line_layers[i // 2])
+                    x = self._line_layer(x, enc, lay, self.gnn.line_layers[i // 2])
             if (lines and self.conf.inter_supervision and layer.type == "cross"
                     and i // 2 in self.conf.inter_supervision):
                 inter[i // 2] = x
@@ -407,17 +405,6 @@ class GlueStick(PointGNN):
             if prefix == "line_":
                 pred["raw_line_scores"] = raw
         return pred
-
-    def _line_layer_packed(self, x, jl, layer):
-        """LineLayer (gluestick.py:589-691) over the endpoints of every lined pair and both views at once: each
-        endpoint's update from [its junction ; the other end's junction ; its encoding], then every junction's token
-        gets the mean of its endpoints' updates, added in place in a fixed order (ops.junction_mean_)."""
-        tgt, order, tgt_sorted, enc = jl
-        D = x.shape[1]
-        ld = x.index_select(0, tgt)
-        other = ld.view(-1, 2, D).flip(1).reshape(-1, D)
-        upd = self._mlp(torch.cat([ld, other, enc], 1), layer.mlp)
-        return ops.junction_mean_(x, upd.float().contiguous(), order, tgt_sorted)
 
     def _line_head_packed(self, x, proj, lh, out):
         """_line_head of every lined pair at once: projection of each pair's first min(n, 2 L) tokens, one padded
@@ -514,6 +501,32 @@ def junction_order(tgt):
     per forward; every LineLayer sums each junction's endpoints in this order."""
     tgt_sorted, order = torch.sort(tgt, stable=True)
     return order.int(), tgt_sorted.int()
+
+
+class JunctionLayout(NamedTuple):
+    """The line endpoints of one forward and the junction rows they read and update, built once per forward.
+    tgt [E] int32: each endpoint's token row (endpoints 2 l, 2 l + 1 of line l); order / tgt_sorted: junction_order(tgt).
+    Uniform batches (junction_layout) also carry the line heads' operands: junc [B, 2 L] int32 the junction indices,
+    ptr [B, P + 1] int32 the endpoints at junction r < P of pair b, order[ptr[b, r] .. ptr[b, r + 1])."""
+    tgt: torch.Tensor
+    order: torch.Tensor
+    tgt_sorted: torch.Tensor
+    junc: Optional[torch.Tensor]
+    ptr: Optional[torch.Tensor]
+
+
+def junction_layout(idx, n, P):
+    """JunctionLayout of one view of a uniform batch: idx [B, 2 L] the junction indices (lines_junc_idx), n the nodes
+    per pair (token row of pair b's junction j: b * n + j), P the rows of the line heads' similarity (min(n, 2 L)).
+    No host read: it is built inside a captured training step."""
+    B = idx.shape[0]
+    junc = idx.int().contiguous()
+    base = torch.arange(B, device=idx.device, dtype=torch.int32)[:, None] * n
+    tgt = (junc + base).reshape(-1)
+    order, tgt_sorted = junction_order(tgt)
+    rows = (base + torch.arange(P + 1, device=idx.device, dtype=torch.int32)).reshape(-1)
+    ptr = torch.searchsorted(tgt_sorted, rows, out_int32=True).view(B, P + 1)
+    return JunctionLayout(tgt, order, tgt_sorted, junc, ptr)
 
 
 def _endpoint_inputs(lines, scores, size, lsrc, lpid, ssrc):

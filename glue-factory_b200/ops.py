@@ -933,6 +933,104 @@ def junction_mean_(x, upd, order, tgt_sorted):
     return x
 
 
+def _junction_sum_(x, src, order, tgt_sorted):
+    """x [T, D] fp32 += (in place) per target row, the sum over the endpoints e aimed at it of src[e, :D] +
+    src[e ^ 1, D:2D] (src [E, >= 2D] fp32 with unit inner stride), in the order `order` (lgb200_junction_sum)."""
+    _chk(x, torch.float32), _chk(order, torch.int32), _chk(tgt_sorted, torch.int32)
+    E, D = src.shape[0], x.shape[1]
+    if src.dtype != torch.float32 or src.stride(1) != 1 or src.stride(0) % 4 or src.data_ptr() % 16:
+        src = src.float().contiguous()
+    _chk(src, strided_rows=True)
+    assert src.shape[1] >= 2 * D and order.shape == tgt_sorted.shape == (E,)
+    if E:
+        call("lgb200_junction_sum", ptr(x), ptr(src), ptr(order), ptr(tgt_sorted), E, D, src.stride(0), stream_ptr())
+    return x
+
+
+class JunctionGather(torch.autograd.Function):
+    """The LineLayer's endpoint gather (gluestick.py:664-675): x [T, D] fp32 -> [E, 2D] = [x[tgt[e]] ; x[tgt[e ^ 1]]]
+    (endpoint e's junction, then its line's other end's).  tgt [E] int32; order / tgt_sorted [E] int32: the endpoints
+    sorted stably by tgt (gluestick.junction_order).  Backward: per junction row, the sum of its endpoints' two column
+    blocks in that order (lgb200_junction_sum), so it has no atomics and gives the same bits on every run."""
+
+    @staticmethod
+    def forward(ctx, x, tgt, order, tgt_sorted):
+        E, D = tgt.numel(), x.shape[1]
+        both = torch.stack([tgt, tgt.view(-1, 2).flip(1).reshape(-1)], 1).reshape(-1)
+        ctx.save_for_backward(order, tgt_sorted)
+        ctx.T = x.shape[0]
+        return x.index_select(0, both).view(E, 2 * D)
+
+    @staticmethod
+    def backward(ctx, g):
+        order, tgt_sorted = ctx.saved_tensors
+        dx = torch.zeros(ctx.T, g.shape[1] // 2, device=g.device, dtype=torch.float32)
+        return _junction_sum_(dx, g, order, tgt_sorted), None, None, None
+
+
+class JunctionMean(torch.autograd.Function):
+    """x [T, D] fp32 + per target row, the mean of the endpoint updates upd [E, D] aimed at it (the LineLayer's
+    scatter-mean, gluestick.py:682-690), summed in the order `order` (lgb200_junction_mean_varlen on a copy of x).
+    tgt [E] int32 each endpoint's row; order / tgt_sorted as for JunctionGather.  Backward: dx = g, d upd[e] =
+    g[tgt[e]] / (number of endpoints at tgt[e]), the same division as the forward's."""
+
+    @staticmethod
+    def forward(ctx, x, upd, tgt, order, tgt_sorted):
+        out = junction_mean_(x.float().clone(), upd.float().contiguous(), order, tgt_sorted)
+        ctx.save_for_backward(tgt, tgt_sorted)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        tgt, tgt_sorted = ctx.saved_tensors
+        cnt = torch.searchsorted(tgt_sorted, tgt, right=True) - torch.searchsorted(tgt_sorted, tgt)
+        return g, g.index_select(0, tgt) / cnt[:, None].float(), None, None, None
+
+
+def _line_scores_train(sim, junc0, junc1, pairs):
+    _chk(sim, torch.float32), _chk(junc0, torch.int32), _chk(junc1, torch.int32), _chk(pairs, torch.int32)
+    G, P0, P1 = sim.shape
+    L0, L1 = junc0.shape[1] // 2, junc1.shape[1] // 2
+    assert junc0.shape == (G, 2 * L0) and junc1.shape == (G, 2 * L1) and pairs.shape[1] == G
+    raw = torch.zeros(G, L0, L1, device=sim.device, dtype=torch.float32)
+    call("lgb200_line_scores_train", ptr(sim), ptr(junc0), ptr(junc1), ptr(raw), ptr(pairs), G, P0, P1, L0, L1,
+         stream_ptr())
+    return raw
+
+
+def line_scores_bwd(graw, sim, junc0, junc1, order0, ptr0, order1, ptr1, pairs):
+    """d sim [G, P0, P1] of LineScores (lgb200_line_scores_bwd): every entry written, 0 where no line reads it."""
+    graw = graw.float().contiguous()
+    for t in (order0, ptr0, order1, ptr1):
+        _chk(t, torch.int32)
+    G, P0, P1 = sim.shape
+    L0, L1 = junc0.shape[1] // 2, junc1.shape[1] // 2
+    assert graw.shape == (G, L0, L1) and ptr0.shape == (G, P0 + 1) and ptr1.shape == (G, P1 + 1)
+    assert order0.shape == (G * 2 * L0,) and order1.shape == (G * 2 * L1,)
+    dsim = torch.empty_like(sim)
+    call("lgb200_line_scores_bwd", ptr(graw), ptr(sim), ptr(junc0), ptr(junc1), ptr(order0), ptr(ptr0), ptr(order1),
+         ptr(ptr1), ptr(pairs), ptr(dsim), G, P0, P1, L0, L1, stream_ptr())
+    return dsim
+
+
+class LineScores(torch.autograd.Function):
+    """raw line scores [G, L0, L1] = 0.5 * maximum(s[a0,c0] + s[a1,c1], s[a0,c1] + s[a1,c0]) (gluestick.py:348-361) from
+    sim [G, P0, P1] fp32 and the junction indices junc0 [G, 2 L0] / junc1 [G, 2 L1] int32; pairs [2+, G] int32: each
+    pair's line counts (m, n), raw is 0 past them.  Forward: lgb200_line_scores_train, bit-identical to the torch formula
+    (NaN included).  order0 / ptr0, order1 / ptr1: each view's endpoints per junction (gluestick.junction_layout), for the
+    backward, lgb200_line_scores_bwd: torch's gradient summed in a fixed order."""
+
+    @staticmethod
+    def forward(ctx, sim, junc0, junc1, pairs, order0, ptr0, order1, ptr1):
+        ctx.save_for_backward(sim, junc0, junc1, pairs, order0, ptr0, order1, ptr1)
+        return _line_scores_train(sim, junc0, junc1, pairs)
+
+    @staticmethod
+    def backward(ctx, graw):
+        sim, junc0, junc1, pairs, *csr = ctx.saved_tensors
+        return (line_scores_bwd(graw, sim, junc0, junc1, *csr, pairs), *([None] * 7))
+
+
 def _bin_dev(alpha):
     """A CUDA tensor bin score as a 1-element fp32 device vector (read by the kernels: no host read-back), else None."""
     if torch.is_tensor(alpha) and alpha.is_cuda:

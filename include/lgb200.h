@@ -316,6 +316,26 @@ int lgb200_line_scores_varlen(const float* sim, const int* junc0, const int* jun
                               int P0, int P1, int L0, int L1, cudaStream_t stream);
 int lgb200_junction_mean_varlen(float* x, const float* upd, const int* order, const int* tgt_sorted, int E, int D,
                                 cudaStream_t stream);
+/* GlueStick's LineLayer and line heads in training, summed in a fixed order (no atomics: the same bits on every run).
+ * line_scores_train: lgb200_line_scores_varlen with torch.maximum's NaN rule (a NaN in either branch gives NaN), and
+ * NaN for a line with a junction index outside [0, P0) / [0, P1) (nothing outside the pair's block is read).
+ * line_scores_bwd: dsim [G, P0, P1] (every entry written, 0 where no line reads it) from graw = dL/draw [G, L0, L1],
+ * the autograd of the torch formula: torch.maximum's backward (the larger branch takes the gradient, each takes half on
+ * an exact tie, both take it when either is NaN), the gathers' backward summed per (r, c) over the endpoints at
+ * junctions r and c in CSR order.  order0 [G * 2 L0] int32: entries of junc0's flat [G, 2 L0], each pair's endpoints
+ * sorted stably by junction index; ptr0 [G, P0 + 1] int32: junction r of pair g has order0[ptr0[g, r] ..
+ * ptr0[g, r + 1]); likewise order1 / ptr1.  Lines past a pair's (m, n) of pairs [2+, G] are skipped.
+ * junction_sum: x [*, D] fp32 += per target row, the sum over the endpoints e aimed at it (order / tgt_sorted as for
+ * junction_mean_varlen) of src[e, 0 .. D-1] + src[e ^ 1, D .. 2D-1], src [E, ld] fp32 with row pitch ld >= 2D: the
+ * backward of the LineLayer's gather of [x[tgt[e]] ; x[tgt[e ^ 1]]].  E even, D % 4 == 0, ld % 4 == 0, x and src 16-byte
+ * aligned.                                                                                                          */
+int lgb200_line_scores_train(const float* sim, const int* junc0, const int* junc1, float* raw, const int* pairs, int G,
+                             int P0, int P1, int L0, int L1, cudaStream_t stream);
+int lgb200_line_scores_bwd(const float* graw, const float* sim, const int* junc0, const int* junc1, const int* order0,
+                           const int* ptr0, const int* order1, const int* ptr1, const int* pairs, float* dsim, int G,
+                           int P0, int P1, int L0, int L1, cudaStream_t stream);
+int lgb200_junction_sum(float* x, const float* src, const int* order, const int* tgt_sorted, int E, int D, int ld,
+                        cudaStream_t stream);
 int lgb200_sinkhorn(const float* sim, float alpha, int iters, float* out, void* ws, int B, int M, int N,
                     cudaStream_t stream);
 /* The same iterations with their potentials kept (uh [iters,B,M+1], vh [iters,B,N+1], both or neither; out may be
