@@ -50,6 +50,9 @@ SIGNATURES = {
     "lgb200_assign_fused_lse": (_i, [_vp, _vp, _f, _vp, _vp, _i, _i, _i, _i, _vp]),
     "lgb200_assign_fused_stats": (_i, [_vp, _vp, _f] + [_vp] * 10 + [_i, _i, _i, _i, _vp]),
     "lgb200_assign_fused_bwd": (_i, [_vp, _vp, _f] + [_vp] * 9 + [_i, _i, _i, _i, _vp]),
+    "lgb200_assign_pos_fwd": (_i, [_vp, _vp, _vp, _f] + [_vp] * 5 + [_i] * 4 + [_vp]),
+    "lgb200_assign_pos_bwd": (_i, [_vp] * 7 + [_i] * 4 + [_vp]),
+    "lgb200_assign_bwd_sparse": (_i, [_vp] * 8 + [_i, _i, _i, _i, _vp]),
     "lgb200_filter_matches": (_i, [_vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "lgb200_assign_lse_varlen": (_i, [_vp] * 5 + [_i, _i, _i, _vp]),
     "lgb200_assign_scores_varlen": (_i, [_vp] * 17 + [_i] * 5 + [_vp]),
@@ -78,6 +81,8 @@ SIGNATURES = {
     "lgb200_sinkhorn_varlen": (_i, [_vp, _vp, _i, _vp, _vp, _vp] + [_i] * 5 + [_vp]),
     "lgb200_ot_nll_fwd": (_i, [_vp] * 7 + [_i, _i, _i, _vp]),
     "lgb200_ot_nll_bwd": (_i, [_vp] * 8 + [_i, _i, _i, _vp]),
+    "lgb200_ot_nll_fwd_sparse": (_i, [_vp] * 8 + [_i, _i, _i, _vp]),
+    "lgb200_ot_nll_bwd_sparse": (_i, [_vp] * 8 + [_i, _i, _i, _vp]),
     "lgb200_ot_filter_stats": (_i, [_vp] * 4 + [_i, _i, _i, _vp]),
     "lgb200_gt_homography_ws_bytes": (_sz, [_i, _i, _i]),
     "lgb200_gt_from_homography": (_i, [_vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
@@ -160,6 +165,8 @@ KERNELS_PER_CALL = {
     "lgb200_log_double_softmax_varlen": 4, "lgb200_line_scores_varlen": 1, "lgb200_junction_mean_varlen": 1,
     "lgb200_line_scores_train": 1, "lgb200_line_scores_bwd": 1, "lgb200_junction_sum": 1,
     "lgb200_sinkhorn_varlen": 2,  # item table + persistent iterations
+    "lgb200_ot_nll_fwd_sparse": 2, "lgb200_assign_pos_fwd": 1, "lgb200_assign_pos_bwd": 1,
+    "lgb200_assign_bwd_sparse": 1, "lgb200_ot_nll_bwd_sparse": 1,
 }
 launch_count = 0          # running total of kernels launched through `call`
 timed_entry = None        # entry-point name or a set of names: every call of them is bracketed by CUDA events

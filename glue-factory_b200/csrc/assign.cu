@@ -428,12 +428,14 @@ __global__ void __launch_bounds__(256) assign_col_arg_merge_kernel(const float* 
 //   dsim_ij = 2 c_b gt_ij - exp(sim_ij - lse_row_i) a_row_i - exp(sim_ij - lse_col_j) a_col_j
 // (SURVEY.md Appendix A.4; here a_row_i = c_b * rowcount_i(gt), a_col_j = c_b * colcount_j(gt): the
 //  kernel takes the counts and applies c_b itself)
+// GtT = uint8_t: gt is the [B,M,N] byte mask.  GtT = int64_t: gt is the match list gt_matches0 [B,M] (one-to-one
+// labels), and gt_ij = (gt[i] == j); every other instruction is the same, so dsim is bit-identical to the mask's.
 // ---------------------------------------------------------------------------------------------
-template <typename OutT>
+template <typename OutT, typename GtT>
 __global__ void __launch_bounds__(256) assign_bwd_kernel(const float* __restrict__ sim,
                                                         const float* __restrict__ lse_row,
                                                         const float* __restrict__ lse_col,
-                                                        const uint8_t* __restrict__ gt, const float* __restrict__ gcoef,
+                                                        const GtT* __restrict__ gt, const float* __restrict__ gcoef,
                                                         const float* __restrict__ a_row,
                                                         const float* __restrict__ a_col, OutT* __restrict__ dsim, int M,
                                                         int N) {
@@ -447,14 +449,20 @@ __global__ void __launch_bounds__(256) assign_bwd_kernel(const float* __restrict
   const float lr = lse_row[(int64_t)b * M + row];
   const float ar = gc * a_row[(int64_t)b * M + row];
   const int64_t roff = ((int64_t)b * M + row) * N;
+  int64_t jpos = -1;
+  if constexpr (sizeof(GtT) == 8) jpos = gt[(int64_t)b * M + row];
   for (int col = lane * 4; col < N; col += 128) {
     const int valid = min(4, N - col);
     float4 x4 = ld4(sim + roff + col, vec, valid);
     float x[4] = {x4.x, x4.y, x4.z, x4.w};
     uint32_t g = 0;
-    if (vec && valid >= 4) g = *reinterpret_cast<const uint32_t*>(gt + roff + col);
-    else
-      for (int e = 0; e < valid; ++e) g |= (uint32_t)gt[roff + col + e] << (8 * e);
+    if constexpr (sizeof(GtT) == 8) {
+      if (jpos >= col && jpos < col + valid) g = 0xffu << (8 * (int)(jpos - col));
+    } else {
+      if (vec && valid >= 4) g = *reinterpret_cast<const uint32_t*>(gt + roff + col);
+      else
+        for (int e = 0; e < valid; ++e) g |= (uint32_t)gt[roff + col + e] << (8 * e);
+    }
     float d[4];
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
@@ -483,6 +491,95 @@ __global__ void __launch_bounds__(256) assign_bwd_kernel(const float* __restrict
       }
     }
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Positive term from match lists: with one-to-one labels row i has its only positive at j = gt0[i] >= 0, so the
+// positive part of the NLL is one entry per row and its gradient one rank-1 update per row and per column
+// (no [B,M,N] mask is read).  One warp per row; every sum runs in a fixed order.
+// ---------------------------------------------------------------------------------------------
+// pos_row_sum_i = 2 alpha md0_i . md1_j - lse_row_i - lse_col_j   (kSim = false: bf16 operands, fp32 accumulate)
+//              = (sim_ij - lse_row_i) + (sim_ij - lse_col_j)     (kSim = true: assign_scores' arithmetic, so the result
+//                                                                 is bit-identical to the mask's on consistent lists)
+// 0 when the row has no positive, NaN when j >= N or gt1[j] != i (the two lists disagree).
+template <bool kSim>
+__global__ void __launch_bounds__(256) assign_pos_fwd_kernel(const __nv_bfloat16* __restrict__ md0,
+                                                            const __nv_bfloat16* __restrict__ md1,
+                                                            const float* __restrict__ sim, float alpha,
+                                                            const float* __restrict__ lse_row,
+                                                            const float* __restrict__ lse_col,
+                                                            const int64_t* __restrict__ gt0,
+                                                            const int64_t* __restrict__ gt1,
+                                                            float* __restrict__ pos_row_sum, int M, int N, int D) {
+  const int b = blockIdx.y, i = blockIdx.x * kWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (i >= M) return;
+  const int64_t r = (int64_t)b * M + i;
+  const int64_t j = gt0[r];  // warp-uniform: every branch below is taken by the whole warp
+  float v = 0.f;
+  if (j >= 0) {
+    if (j >= N || gt1[(int64_t)b * N + j] != i) {
+      v = NAN;
+    } else {
+      const float lr = lse_row[r], lc = lse_col[(int64_t)b * N + j];
+      if constexpr (kSim) {
+        const float x = sim[r * N + j];
+        v = (x - lr) + (x - lc);
+      } else {
+        const __nv_bfloat162* a = reinterpret_cast<const __nv_bfloat162*>(md0 + r * D);
+        const __nv_bfloat162* c = reinterpret_cast<const __nv_bfloat162*>(md1 + ((int64_t)b * N + j) * D);
+        float s = 0.f;
+        for (int k = lane; k < D / 2; k += 32) {
+          const float2 x = __bfloat1622float2(a[k]), y = __bfloat1622float2(c[k]);
+          s = fmaf(x.x, y.x, s);
+          s = fmaf(x.y, y.y, s);
+        }
+        v = fmaf(warp_sum(s), 2.f * alpha, -lr) - lc;
+      }
+    }
+  }
+  if (lane == 0) pos_row_sum[r] = v;
+}
+
+// dmd0_i += 2 gcoef_b md1_{gt0[i]} and dmd1_j += 2 gcoef_b md0_{gt1[j]} (bf16 in place, fp32 arithmetic): the dsim =
+// 2 gcoef entries at the positives, which the mask-free fused backward leaves out.  Warps [0, M) of a pair take the
+// rows of image 0, warps [M, M + N) the columns of image 1; an index outside the other image adds nothing.
+__global__ void __launch_bounds__(256) assign_pos_bwd_kernel(const __nv_bfloat16* __restrict__ md0,
+                                                            const __nv_bfloat16* __restrict__ md1,
+                                                            const float* __restrict__ gcoef,
+                                                            const int64_t* __restrict__ gt0,
+                                                            const int64_t* __restrict__ gt1,
+                                                            __nv_bfloat16* __restrict__ dmd0,
+                                                            __nv_bfloat16* __restrict__ dmd1, int M, int N, int D) {
+  const int b = blockIdx.y, w = blockIdx.x * kWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (w >= M + N) return;
+  const bool side1 = w >= M;
+  const int64_t r = side1 ? (int64_t)b * N + (w - M) : (int64_t)b * M + w;
+  const int64_t k = side1 ? gt1[r] : gt0[r];
+  if (k < 0 || k >= (side1 ? M : N)) return;
+  const __nv_bfloat162* src =
+      reinterpret_cast<const __nv_bfloat162*>(side1 ? md0 + ((int64_t)b * M + k) * D : md1 + ((int64_t)b * N + k) * D);
+  __nv_bfloat162* dst = reinterpret_cast<__nv_bfloat162*>((side1 ? dmd1 : dmd0) + r * D);
+  const float c = 2.f * gcoef[b];
+  for (int e = lane; e < D / 2; e += 32) {
+    const float2 s = __bfloat1622float2(src[e]), d = __bfloat1622float2(dst[e]);
+    dst[e] = __floats2bfloat162_rn(fmaf(c, s.x, d.x), fmaf(c, s.y, d.y));
+  }
+}
+
+template <typename GtT>
+static int launch_assign_bwd(const float* sim, const float* lse_row, const float* lse_col, const GtT* gt,
+                             const float* gcoef, const float* a_row, const float* a_col, void* dsim, int out_dtype,
+                             int B, int M, int N, cudaStream_t stream, const char* what) {
+  dim3 grid((M + kWarps - 1) / kWarps, B);
+  if (out_dtype == LGB200_F32)
+    assign_bwd_kernel<float, GtT><<<grid, 256, 0, stream>>>(sim, lse_row, lse_col, gt, gcoef, a_row, a_col,
+                                                            static_cast<float*>(dsim), M, N);
+  else if (out_dtype == LGB200_BF16)
+    assign_bwd_kernel<__nv_bfloat16, GtT><<<grid, 256, 0, stream>>>(sim, lse_row, lse_col, gt, gcoef, a_row, a_col,
+                                                                    static_cast<__nv_bfloat16*>(dsim), M, N);
+  else
+    LGB_REQUIRE(false, kErrInvalid, "%s: bad out_dtype %d", what, out_dtype);
+  return check_launch(what);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -778,16 +875,53 @@ int lgb200_assign_bwd(const float* sim, const float* lse_row, const float* lse_c
   LGB_REQUIRE(sim && lse_row && lse_col && gt && gcoef && a_row && a_col && dsim, kErrInvalid,
               "assign_bwd: null pointer");
   LGB_REQUIRE(B > 0 && M > 0 && N > 0, kErrInvalid, "assign_bwd: empty input");
+  return launch_assign_bwd(sim, lse_row, lse_col, gt, gcoef, a_row, a_col, dsim, out_dtype, B, M, N, stream,
+                           "assign_bwd");
+}
+
+int lgb200_assign_bwd_sparse(const float* sim, const float* lse_row, const float* lse_col, const int64_t* gt0,
+                             const float* gcoef, const float* a_row, const float* a_col, void* dsim, int out_dtype,
+                             int B, int M, int N, cudaStream_t stream) {
+  LGB_REQUIRE(sim && lse_row && lse_col && gt0 && gcoef && a_row && a_col && dsim, kErrInvalid,
+              "assign_bwd_sparse: null pointer");
+  LGB_REQUIRE(B > 0 && M > 0 && N > 0, kErrInvalid, "assign_bwd_sparse: empty input");
+  return launch_assign_bwd(sim, lse_row, lse_col, gt0, gcoef, a_row, a_col, dsim, out_dtype, B, M, N, stream,
+                           "assign_bwd_sparse");
+}
+
+int lgb200_assign_pos_fwd(const void* md0, const void* md1, const float* sim, float alpha, const float* lse_row,
+                          const float* lse_col, const int64_t* gt0, const int64_t* gt1, float* pos_row_sum, int B,
+                          int M, int N, int D, cudaStream_t stream) {
+  LGB_REQUIRE(lse_row && lse_col && gt0 && gt1 && pos_row_sum, kErrInvalid, "assign_pos_fwd: null pointer");
+  LGB_REQUIRE((sim != nullptr) != (md0 != nullptr && md1 != nullptr) && (md0 == nullptr) == (md1 == nullptr),
+              kErrInvalid, "assign_pos_fwd: pass either sim or both descriptor matrices");
+  LGB_REQUIRE(B > 0 && M > 0 && N > 0, kErrInvalid, "assign_pos_fwd: empty input B=%d M=%d N=%d", B, M, N);
   dim3 grid((M + kWarps - 1) / kWarps, B);
-  if (out_dtype == LGB200_F32)
-    assign_bwd_kernel<float><<<grid, 256, 0, stream>>>(sim, lse_row, lse_col, gt, gcoef, a_row, a_col,
-                                                       static_cast<float*>(dsim), M, N);
-  else if (out_dtype == LGB200_BF16)
-    assign_bwd_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(sim, lse_row, lse_col, gt, gcoef, a_row, a_col,
-                                                               static_cast<__nv_bfloat16*>(dsim), M, N);
-  else
-    LGB_REQUIRE(false, kErrInvalid, "assign_bwd: bad out_dtype %d", out_dtype);
-  return check_launch("assign_bwd");
+  if (sim) {
+    assign_pos_fwd_kernel<true><<<grid, 256, 0, stream>>>(nullptr, nullptr, sim, alpha, lse_row, lse_col, gt0, gt1,
+                                                          pos_row_sum, M, N, 0);
+  } else {
+    LGB_REQUIRE(D > 0 && D % 2 == 0 && ((reinterpret_cast<uintptr_t>(md0) | reinterpret_cast<uintptr_t>(md1)) & 3) == 0,
+                kErrInvalid, "assign_pos_fwd: descriptor width %d must be even, rows 4-byte aligned", D);
+    assign_pos_fwd_kernel<false><<<grid, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(md0),
+                                                           static_cast<const __nv_bfloat16*>(md1), nullptr, alpha,
+                                                           lse_row, lse_col, gt0, gt1, pos_row_sum, M, N, D);
+  }
+  return check_launch("assign_pos_fwd");
+}
+
+int lgb200_assign_pos_bwd(const void* md0, const void* md1, const float* gcoef, const int64_t* gt0, const int64_t* gt1,
+                          void* dmd0, void* dmd1, int B, int M, int N, int D, cudaStream_t stream) {
+  LGB_REQUIRE(md0 && md1 && gcoef && gt0 && gt1 && dmd0 && dmd1, kErrInvalid, "assign_pos_bwd: null pointer");
+  LGB_REQUIRE(B > 0 && M > 0 && N > 0, kErrInvalid, "assign_pos_bwd: empty input B=%d M=%d N=%d", B, M, N);
+  LGB_REQUIRE(D > 0 && D % 2 == 0 &&
+                  ((reinterpret_cast<uintptr_t>(md0) | reinterpret_cast<uintptr_t>(md1) |
+                    reinterpret_cast<uintptr_t>(dmd0) | reinterpret_cast<uintptr_t>(dmd1)) & 3) == 0,
+              kErrInvalid, "assign_pos_bwd: descriptor width %d must be even, rows 4-byte aligned", D);
+  assign_pos_bwd_kernel<<<dim3((M + N + kWarps - 1) / kWarps, B), 256, 0, stream>>>(
+      static_cast<const __nv_bfloat16*>(md0), static_cast<const __nv_bfloat16*>(md1), gcoef, gt0, gt1,
+      static_cast<__nv_bfloat16*>(dmd0), static_cast<__nv_bfloat16*>(dmd1), M, N, D);
+  return check_launch("assign_pos_bwd");
 }
 
 int lgb200_filter_matches(const float* rowmax, const int* rowarg, const int* colarg, float th, int64_t* m0,

@@ -12,7 +12,9 @@
 //   quad (16 of the tile's columns each), whose running values are merged at the end of the item.
 //   A producer warpgroup fills each stage: the B tile by TMA and, for STATS / BWD, the tile's side data next to it --
 //   the 128 x 64 mask tile (gt for direction 0, gt_t for direction 1) and the two per-column fp32 vectors the
-//   elementwise work reads -- so the consumers' inner loop makes no global loads.
+//   elementwise work reads -- so the consumers' inner loop makes no global loads.  Without a mask (labels given as
+//   match lists) no mask tile is staged and STATS / BWD have no positive term: lgb200_assign_pos_fwd / _bwd
+//   (assign.cu) supply it, one entry per row.
 //
 //   LSE  : running (max, sum exp2) per row -> lse_row [B,M] (dir 0), lse_col [B,N] (dir 1).
 //   STATS: scores in the reference's association order ((s - lse_r) + (s - lse_c)) + (lsig0 + lsig1); running
@@ -480,8 +482,11 @@ int lgb200_assign_fused_bwd(const void* md0, const void* md1, float alpha, const
                             const uint8_t* gt, const uint8_t* gt_t, const float* gcoef, const float* rowcnt,
                             const float* colcnt, void* dmd0, void* dmd1, int B, int M, int N, int D,
                             cudaStream_t stream) {
-  LGB_REQUIRE(lse_row && lse_col && gt && gt_t && gcoef && rowcnt && colcnt && dmd0 && dmd1, kErrInvalid,
+  LGB_REQUIRE(lse_row && lse_col && gcoef && rowcnt && colcnt && dmd0 && dmd1, kErrInvalid,
               "assign_fused_bwd: null pointer");
+  // both masks NULL: no mask tile is staged and dsim has no positive term (lgb200_assign_pos_bwd adds it)
+  LGB_REQUIRE((gt == nullptr) == (gt_t == nullptr), kErrInvalid,
+              "assign_fused_bwd: gt and gt_t must both be set or both be null");
   AssignTcArgs a = {};
   a.alpha = alpha; a.B = B; a.M = M; a.N = N; a.D = D;
   a.lse_row = const_cast<float*>(lse_row); a.lse_col = const_cast<float*>(lse_col);

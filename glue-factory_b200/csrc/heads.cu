@@ -878,6 +878,50 @@ __global__ void __launch_bounds__(256) ot_nll_bwd_kernel(const uint8_t* __restri
   }
 }
 
+// The same two kernels with the positives given as match lists gt0 [B,M] / gt1 [B,N] (int64, one-to-one): row i's
+// positive is Z[i, gt0[i]].  Thread t adds it when gt0[i] % 256 == t, so every thread sees the same entries in the same
+// order as in ot_nll_part_kernel and the partials, the sums and dZ are bit-identical to the mask's.  A row whose
+// partner disagrees (gt0[i] >= N, or gt1[gt0[i]] != i) adds NaN to its strip.
+__global__ void __launch_bounds__(256) ot_nll_part_sparse_kernel(const float* __restrict__ Z,
+                                                                const int64_t* __restrict__ gt0,
+                                                                const int64_t* __restrict__ gt1,
+                                                                float* __restrict__ part, int M, int N) {
+  __shared__ double red[8];
+  const int b = blockIdx.y, r0 = blockIdx.x * kOtRows, r1 = min(M, r0 + kOtRows);
+  float acc = 0.f;
+  for (int i = r0; i < r1; ++i) {
+    const int64_t j = __ldg(gt0 + (int64_t)b * M + i);
+    if (j < 0 || j % 256 != threadIdx.x) continue;
+    if (j >= N || __ldg(gt1 + (int64_t)b * N + j) != i) acc += NAN;
+    else acc += __ldg(Z + ((int64_t)b * (M + 1) + i) * (N + 1) + j);
+  }
+  const double t = ot_block_sum((double)acc, red);
+  if (threadIdx.x == 0) part[(int64_t)b * gridDim.x + blockIdx.x] = (float)t;
+}
+
+__global__ void __launch_bounds__(256) ot_nll_bwd_sparse_kernel(const int64_t* __restrict__ gt0,
+                                                               const float* __restrict__ neg0,
+                                                               const float* __restrict__ neg1,
+                                                               const float* __restrict__ num_pos,
+                                                               const float* __restrict__ num_neg,
+                                                               const float* __restrict__ gpos,
+                                                               const float* __restrict__ gneg, float* __restrict__ dZ,
+                                                               int M, int N) {
+  const int b = blockIdx.y, r0 = blockIdx.x * kOtRows, r1 = min(M + 1, r0 + kOtRows);
+  const float cp = -(__ldg(gpos + b) / __ldg(num_pos + b)), cn = -(__ldg(gneg + b) / __ldg(num_neg + b));
+  for (int i = r0; i < r1; ++i) {
+    float* drow = dZ + ((int64_t)b * (M + 1) + i) * (N + 1);
+    if (i < M) {
+      const int64_t jp = __ldg(gt0 + (int64_t)b * M + i);
+      for (int j = threadIdx.x; j < N; j += 256) drow[j] = j == jp ? cp : 0.f;
+      if (threadIdx.x == 0) drow[N] = __ldg(neg0 + (int64_t)b * M + i) * cn;
+    } else {
+      for (int j = threadIdx.x; j < N; j += 256) drow[j] = __ldg(neg1 + (int64_t)b * N + j) * cn;
+      if (threadIdx.x == 0) drow[N] = 0.f;
+    }
+  }
+}
+
 // row max / argmax of Z's inner block, first index on ties (warp per row)
 __global__ void __launch_bounds__(256) ot_rowmax_kernel(const float* __restrict__ Z, float* __restrict__ rowmax,
                                                        int* __restrict__ rowarg, int M, int N) {
@@ -1168,6 +1212,30 @@ int lgb200_ot_nll_bwd(const uint8_t* mask, const float* neg0, const float* neg1,
   ot_nll_bwd_kernel<<<dim3((M + 1 + kOtRows - 1) / kOtRows, B), 256, 0, stream>>>(mask, neg0, neg1, num_pos, num_neg,
                                                                                  gpos, gneg, dZ, M, N);
   return check_launch("ot_nll_bwd");
+}
+
+int lgb200_ot_nll_fwd_sparse(const float* Z, const int64_t* gt0, const int64_t* gt1, const float* neg0,
+                             const float* neg1, float* pos, float* neg, void* ws, int B, int M, int N,
+                             cudaStream_t stream) {
+  LGB_REQUIRE(Z && gt0 && gt1 && neg0 && neg1 && pos && neg && ws, kErrInvalid, "ot_nll_fwd_sparse: null pointer");
+  LGB_REQUIRE(B > 0 && M > 0 && N > 0, kErrInvalid, "ot_nll_fwd_sparse: empty input");
+  const int nparts = (M + kOtRows - 1) / kOtRows;
+  float* part = static_cast<float*>(ws);
+  ot_nll_part_sparse_kernel<<<dim3(nparts, B), 256, 0, stream>>>(Z, gt0, gt1, part, M, N);
+  if (int rc = check_launch("ot_nll_fwd_sparse")) return rc;
+  ot_nll_final_kernel<<<B, 256, 0, stream>>>(Z, neg0, neg1, part, nparts, pos, neg, M, N);
+  return check_launch("ot_nll_fwd_sparse");
+}
+
+int lgb200_ot_nll_bwd_sparse(const int64_t* gt0, const float* neg0, const float* neg1, const float* num_pos,
+                             const float* num_neg, const float* gpos, const float* gneg, float* dZ, int B, int M, int N,
+                             cudaStream_t stream) {
+  LGB_REQUIRE(gt0 && neg0 && neg1 && num_pos && num_neg && gpos && gneg && dZ, kErrInvalid,
+              "ot_nll_bwd_sparse: null pointer");
+  LGB_REQUIRE(B > 0 && M > 0 && N > 0, kErrInvalid, "ot_nll_bwd_sparse: empty input");
+  ot_nll_bwd_sparse_kernel<<<dim3((M + 1 + kOtRows - 1) / kOtRows, B), 256, 0, stream>>>(gt0, neg0, neg1, num_pos,
+                                                                                        num_neg, gpos, gneg, dZ, M, N);
+  return check_launch("ot_nll_bwd_sparse");
 }
 
 int lgb200_ot_filter_stats(const float* Z, float* rowmax, int* rowarg, int* colarg, int B, int M, int N,

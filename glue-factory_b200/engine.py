@@ -62,16 +62,18 @@ def similarity(md0, md1, cdt, alpha=1.0):
     return sim.mul_(alpha) if alpha != 1 else sim
 
 
-def assign_unfused_bwd(md0, md1, sim, lse_row, lse_col, gt_u8, gcoef, rowcnt, colcnt):
+def assign_unfused_bwd(md0, md1, sim, lse_row, lse_col, gt_u8, gcoef, rowcnt, colcnt, gt0=None):
     """d(mdesc0) [B, M, D], d(mdesc1) [B, N, D] (md0's dtype) of the NLL through a stored sim: dsim = gcoef (2 gt -
     softmax_row rowcnt - softmax_col colcnt) from lgb200_assign_bwd, then dsim md1 and dsim^T md0.  The unfused
-    counterpart of ops.assign_fused_bwd, for fp32 and for operands assign_fused_ok rejects."""
+    counterpart of ops.assign_fused_bwd, for fp32 and for operands assign_fused_ok rejects.  gt_u8 None: gt is the
+    match list gt0 [B, M] int64 (lgb200_assign_bwd_sparse, the same dsim)."""
     B, M, N = sim.shape
     cdt = md0.dtype
     tc = cdt == torch.bfloat16 and N % 8 == 0 and M % 8 == 0
     dsim = torch.empty(B, M, N, device=sim.device, dtype=torch.bfloat16 if tc else torch.float32)
-    ops.call("lgb200_assign_bwd", ops.ptr(sim), ops.ptr(lse_row), ops.ptr(lse_col), ops.ptr(gt_u8), ops.ptr(gcoef),
-             ops.ptr(rowcnt), ops.ptr(colcnt), ops.ptr(dsim), ops._code(dsim.dtype), B, M, N, ops.stream_ptr())
+    ops.call("lgb200_assign_bwd" if gt_u8 is not None else "lgb200_assign_bwd_sparse", ops.ptr(sim), ops.ptr(lse_row),
+             ops.ptr(lse_col), ops.ptr(gt_u8 if gt_u8 is not None else gt0), ops.ptr(gcoef), ops.ptr(rowcnt),
+             ops.ptr(colcnt), ops.ptr(dsim), ops._code(dsim.dtype), B, M, N, ops.stream_ptr())
     if tc:
         dmd0 = ops.gemm_bf16(dsim, md1, a_mn_major=False, b_mn_major=True, out_dtype=cdt)  # dsim   md1
         dmd1 = ops.gemm_bf16(dsim, md0, a_mn_major=True, b_mn_major=True, out_dtype=cdt)   # dsim^T md0
@@ -312,7 +314,9 @@ class HeadFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, sizes, cdt, gt, bal, fin, stash, wfp, bfp, Wfp_p, bfp_p, wm, bm, wt, bt):
         """stash: None, or (dict, key): the backward then leaves the gradient w.r.t. x in dict[key] for the LayerFn that
-        produced x (which merges it with the next layer's gradient in one fused pass) instead of returning it."""
+        produced x (which merges it with the next layer's gradient in one fused pass) instead of returning it.
+        gt["u8"] None: the labels are the match lists gt["m0"] / gt["m1"] (int64), and the positive term is one entry per
+        row (ops.assign_pos_fwd / assign_pos_bwd, lgb200_assign_bwd_sparse) instead of a pass over the mask."""
         B, M, N = sizes
         D = x.shape[1]
         t0 = B * M
@@ -326,7 +330,8 @@ class HeadFn(torch.autograd.Function):
         md0, md1 = md[:t0].view(B, M, D), md[t0:].view(B, N, D)
         alpha = float(D) ** -0.5
         ls0, ls1, du0, du1 = ls[:t0].view(B, M), ls[t0:].view(B, N), du[:t0].view(B, M), du[t0:].view(B, N)
-        fused = ops.assign_fused_ok(md, D) and gt.get("u8_t") is not None
+        sparse = gt["u8"] is None
+        fused = ops.assign_fused_ok(md, D) and (sparse or gt.get("u8_t") is not None)
         if fused:
             # GEMM + LSE, then GEMM + scores / argmax / positives: the similarity matrix stays in tensor memory
             sim = None
@@ -334,6 +339,10 @@ class HeadFn(torch.autograd.Function):
         else:
             sim = similarity(md0, md1, cdt, alpha)
             st = ops.assign_stats(sim, ls0, ls1, du0, du1, gt_u8=gt["u8"], dense=False)
+        if sparse:
+            st["pos_row_sum"] = (ops.assign_pos_fwd(gt["m0"], gt["m1"], st["lse_row"], st["lse_col"], alpha, md0, md1)
+                                 if fused else
+                                 ops.assign_pos_fwd(gt["m0"], gt["m1"], st["lse_row"], st["lse_col"], alpha, sim=sim))
         out = torch.empty(4, B, device=dev, dtype=torch.float32)
         f0, f1 = (fin if (fin is not None and has_tok) else (None, None))
         hws = torch.empty(4 * B * ((M + N + 255) // 256), device=dev, dtype=torch.float32)
@@ -347,9 +356,9 @@ class HeadFn(torch.autograd.Function):
                  ops.ptr(gt["num_pos"]), ops.ptr(gt["num_neg"]), float(bal), ops.ptr(out[0]), ops.ptr(out[1]),
                  ops.ptr(out[2]), ops.ptr(out[3]), ops.ptr(hws), ops.ptr(cnt), B, M, N, ops.stream_ptr())
         nll, nll_pos, nll_neg, conf = out[0], out[1], out[2], out[3]
-        saved = [x, x16, md, sim if sim is not None else gt["u8_t"], st["lse_row"], st["lse_col"], zt, st["rowmax"],
+        saved = [x, x16, md, sim if sim is not None else gt.get("u8_t"), st["lse_row"], st["lse_col"], zt, st["rowmax"],
                  st["rowarg"], st["colmax"], st["colarg"], wfp, wm, gt["u8"], gt["rowcnt"], gt["colcnt"], gt["neg0"],
-                 gt["neg1"], gt["num_pos"], gt["num_neg"]]
+                 gt["neg1"], gt["num_pos"], gt["num_neg"], gt.get("m0"), gt.get("m1")]
         if f0 is not None:
             saved += [f0, f1]
         ctx.save_for_backward(*saved)
@@ -362,9 +371,9 @@ class HeadFn(torch.autograd.Function):
     def backward(ctx, g_nll, g_conf, *_):
         sv = ctx.saved_tensors
         (x, x16, md, sim, lse_row, lse_col, zt, rowmax, rowarg, colmax, colarg, wfp, wm, gt_u8, rowcnt, colcnt, neg0,
-         neg1, num_pos, num_neg) = sv[:20]
+         neg1, num_pos, num_neg, gt0, gt1) = sv[:22]
         (B, M, N), cdt, bal, alpha, has_tok, has_fin, fused = ctx.meta
-        f0, f1 = (sv[20], sv[21]) if has_fin else (None, None)
+        f0, f1 = (sv[22], sv[23]) if has_fin else (None, None)
         D = x.shape[1]
         t0 = B * M
         g_nll = g_nll.float().contiguous()
@@ -387,8 +396,10 @@ class HeadFn(torch.autograd.Function):
                 dmd = torch.empty(t0 + B * N, D, device=x.device, dtype=cdt)
                 ops.assign_fused_bwd(md0, md1, alpha, lse_row, lse_col, gt_u8, sim, gc, rowcnt, colcnt, dmd[:t0],
                                      dmd[t0:])
+                if gt_u8 is None:
+                    ops.assign_pos_bwd(md0, md1, gc, gt0, gt1, dmd[:t0], dmd[t0:])
             else:
-                dmd0, dmd1 = assign_unfused_bwd(md0, md1, sim, lse_row, lse_col, gt_u8, gc, rowcnt, colcnt)
+                dmd0, dmd1 = assign_unfused_bwd(md0, md1, sim, lse_row, lse_col, gt_u8, gc, rowcnt, colcnt, gt0)
                 dmd = torch.cat([dmd0.reshape(t0, D), dmd1.reshape(B * N, D)], 0)
         dWfp = _wgrad(dmd, x16) if need_wfp else None
         dbfp = _bgrad(dmd) if need_bfp else None

@@ -422,13 +422,19 @@ class GlueStick(PointGNN):
         """gluestick.py:379-415; `block`: an intermediate line head (pred keys line_{block}_*, ground truth gt_line_*),
         weighted by its loss.inter_supervision entry and without the statistics entries."""
         suffix = "" if block is None else f"{block}_"
-        positive = data["gt_" + prefix + "assignment"].float()
-        num_pos = positive.sum((1, 2)).clamp(min=1.0)
+        la = pred[prefix + suffix + "log_assignment"]
+        positive = data.get("gt_" + prefix + "assignment")
+        if positive is None:  # labels as one-to-one match lists: one gathered entry per row
+            pos_sum, num_pos = _list_positive_sum(la, data["gt_" + prefix + "matches0"],
+                                                  data["gt_" + prefix + "matches1"])
+        else:
+            positive = positive.float()
+            num_pos = positive.sum((1, 2)).clamp(min=1.0)
+            pos_sum = (la[:, :-1, :-1] * positive).sum((1, 2))
         neg0 = (data["gt_" + prefix + "matches0"] == -1).float()
         neg1 = (data["gt_" + prefix + "matches1"] == -1).float()
         num_neg = (neg0.sum(1) + neg1.sum(1)).clamp(min=1.0)
-        la = pred[prefix + suffix + "log_assignment"]
-        nll_pos = -(la[:, :-1, :-1] * positive).sum((1, 2)) / num_pos
+        nll_pos = -pos_sum / num_pos
         nll_neg = (-(la[:, :-1, -1] * neg0).sum(1) - (la[:, -1, :-1] * neg1).sum(1)) / num_neg
         bal = self.conf.loss.nll_balancing
         nll = bal * nll_pos + (1 - bal) * nll_neg
@@ -465,6 +471,21 @@ class GlueStick(PointGNN):
                 for block in self.conf.inter_supervision or []:
                     metrics.update(_line_metrics(pred, data, f"line_{block}_"))
             return losses, metrics
+
+
+def _list_positive_sum(la, gt0, gt1):
+    """(sum_i la[b, i, gt0[b, i]] over the rows with gt0 >= 0, num_pos) for one-to-one match lists gt0 [B, M] /
+    gt1 [B, N]: the positive part of gluestick.py:389-393 without the [B, M, N] mask, by torch gathers (the gather's
+    backward writes one entry per row: no index repeats).  NaN for a pair whose lists disagree."""
+    gt0, gt1 = gt0.long(), gt1.long()
+    M, N = gt0.shape[1], gt1.shape[1]
+    _, _, num_pos = ops.match_list_counts(gt0, gt1)
+    pos = gt0 >= 0
+    j = gt0.clamp(0, N - 1)
+    bad = pos & ((gt0 >= N) | (gt1.gather(1, j) != torch.arange(M, device=gt0.device)))
+    v = la[:, :-1, :-1].gather(2, j[..., None])[..., 0]
+    s = torch.where(pos, v, torch.zeros_like(v)).sum(1)
+    return torch.where(bad.any(1), torch.full_like(s, float("nan")), s), num_pos
 
 
 def _image_size(view, kpts):

@@ -603,21 +603,34 @@ class LightGlue(nn.Module):
         if layers_x is None:
             raise ValueError("LightGlue.loss needs the pred of this module's own forward: pred['_b200_layers'] is missing")
         (B, M, N), L = pred["_b200_sizes"], len(layers_x)
-        gt = data["gt_assignment"]
-        if tuple(gt.shape) != (B, M, N):
-            raise ValueError(f"gt_assignment has shape {tuple(gt.shape)} but the forward ran on (B, M, N) = {(B, M, N)}; "
-                             "the loss cannot be taken after point pruning (width_confidence)")
-        gt_u8 = gt.contiguous().view(torch.uint8) if gt.dtype == torch.bool else gt.to(torch.uint8).contiguous()
-        # both counts in one pass over the 4.2 MB/pair mask (`gt.sum(2)` / `gt.sum(1)` each widen it first: int64 by
-        # default, fp32 with dtype=)
-        rowcnt, colcnt = ops.mask_counts(gt_u8)
+        gt = data.get("gt_assignment")
+        m0 = m1 = None
+        if gt is None:
+            # labels as match lists (a ground-truth component with dense_assignment: False): one-to-one positives,
+            # (i, j) <=> gt_matches0[i] = j >= 0; a pair whose two lists disagree gets a NaN loss (ops.match_list_counts)
+            m0, m1 = (data[k].long().contiguous() for k in ("gt_matches0", "gt_matches1"))
+            if tuple(m0.shape) != (B, M) or tuple(m1.shape) != (B, N):
+                raise ValueError(f"gt_matches0/1 have shapes {tuple(m0.shape)} / {tuple(m1.shape)} but the forward ran "
+                                 f"on (B, M, N) = {(B, M, N)}; the loss cannot be taken after point pruning "
+                                 "(width_confidence)")
+            gt_u8 = None
+            rowcnt, colcnt, num_pos = ops.match_list_counts(m0, m1)
+        else:
+            if tuple(gt.shape) != (B, M, N):
+                raise ValueError(f"gt_assignment has shape {tuple(gt.shape)} but the forward ran on (B, M, N) = "
+                                 f"{(B, M, N)}; the loss cannot be taken after point pruning (width_confidence)")
+            gt_u8 = gt.contiguous().view(torch.uint8) if gt.dtype == torch.bool else gt.to(torch.uint8).contiguous()
+            # both counts in one pass over the 4.2 MB/pair mask (`gt.sum(2)` / `gt.sum(1)` each widen it first: int64 by
+            # default, fp32 with dtype=)
+            rowcnt, colcnt = ops.mask_counts(gt_u8)
+            num_pos = rowcnt.sum(1).clamp(min=1.0)
         neg0 = (data["gt_matches0"] == -1).float()
         neg1 = (data["gt_matches1"] == -1).float()
-        num_pos = rowcnt.sum(1).clamp(min=1.0)
         num_neg0, num_neg1 = neg0.sum(1).clamp(min=1.0), neg1.sum(1).clamp(min=1.0)
         gtd = {"u8": gt_u8, "rowcnt": rowcnt.contiguous(), "colcnt": colcnt.contiguous(), "neg0": neg0.contiguous(),
-               "neg1": neg1.contiguous(), "num_pos": num_pos.contiguous(), "num_neg": (num_neg0 + num_neg1).contiguous()}
-        if self._bf16 and torch.is_grad_enabled():
+               "neg1": neg1.contiguous(), "num_pos": num_pos.contiguous(), "num_neg": (num_neg0 + num_neg1).contiguous(),
+               "m0": m0, "m1": m1}
+        if self._bf16 and torch.is_grad_enabled() and gt_u8 is not None:
             # the fused backward walks the mask by columns as well: one transposed copy per step, shared by all layers
             gt_t = data.get("gt_assignment_t")  # written by the plugin's ground-truth components when asked to
             gtd["u8_t"] = (gt_t.contiguous().view(torch.uint8) if gt_t is not None and gt_t.dtype == torch.bool

@@ -241,7 +241,7 @@ class SuperGlue(PointGNN):
             raise ValueError("SuperGlue.loss cannot be taken on the pred of a forward with num_keypoints0/1: each pair "
                              "was truncated on its own")
         with torch.autocast(device_type="cuda", enabled=False):
-            nll_pos, nll_neg, num_pos, num_neg = ops.ot_nll(pred["log_assignment"], data["gt_assignment"],
+            nll_pos, nll_neg, num_pos, num_neg = ops.ot_nll(pred["log_assignment"], data.get("gt_assignment"),
                                                             data["gt_matches0"], data["gt_matches1"])
             bal = self.conf.loss.nll_balancing
             nll = bal * nll_pos + (1 - bal) * nll_neg

@@ -554,14 +554,62 @@ def assign_fused_stats(md0, md1, alpha, ls0, ls1, gt_u8=None):
 
 def assign_fused_bwd(md0, md1, alpha, lse_row, lse_col, gt_u8, gt_t_u8, gcoef, rowcnt, colcnt, dmd0, dmd1):
     """d(mdesc0), d(mdesc1) (bf16, written into dmd0 [B*M, D] / dmd1 [B*N, D]) of the NLL through sim: dsim is
-    recomputed per tile from the two LSE vectors and contracted with the other image's descriptors in the same kernel."""
+    recomputed per tile from the two LSE vectors and contracted with the other image's descriptors in the same kernel.
+    gt_u8 = gt_t_u8 = None (labels as match lists): without the positive term, which assign_pos_bwd then adds."""
     B, M, D = md0.shape
     N = md1.shape[1]
     for t in (lse_row, lse_col, gcoef, rowcnt, colcnt):
         _chk(t, torch.float32)
-    _chk(gt_u8), _chk(gt_t_u8), _chk(dmd0, torch.bfloat16), _chk(dmd1, torch.bfloat16)
+    if gt_u8 is not None or gt_t_u8 is not None:
+        _chk(gt_u8), _chk(gt_t_u8)
+    _chk(dmd0, torch.bfloat16), _chk(dmd1, torch.bfloat16)
     call("lgb200_assign_fused_bwd", ptr(md0), ptr(md1), float(alpha), ptr(lse_row), ptr(lse_col), ptr(gt_u8), ptr(gt_t_u8),
          ptr(gcoef), ptr(rowcnt), ptr(colcnt), ptr(dmd0), ptr(dmd1), B, M, N, D, stream_ptr())
+
+
+def match_list_counts(gt0, gt1):
+    """Labels as match lists gt0 [B,M] / gt1 [B,N] (one-to-one; -1 unmatched, -2 ignored) -> (rowcnt [B,M] = (gt0 >= 0),
+    colcnt [B,N] = (gt1 >= 0) as fp32, num_pos [B] = the positives clamped at 1).  num_pos is NaN for a pair whose two
+    lists hold different numbers of positives; with the per-row check gt1[gt0[i]] == i that the loss kernels make, equal
+    counts mean the lists agree (gt1[j] = i <=> gt0[i] = j).  Device ops only: no host read."""
+    rowcnt, colcnt = (gt0 >= 0).float(), (gt1 >= 0).float()
+    n0, n1 = rowcnt.sum(1), colcnt.sum(1)
+    num_pos = torch.where(n0 == n1, n0, torch.full_like(n0, float("nan"))).clamp(min=1.0)
+    return rowcnt.contiguous(), colcnt.contiguous(), num_pos.contiguous()
+
+
+def assign_pos_fwd(gt0, gt1, lse_row, lse_col, alpha, md0=None, md1=None, sim=None):
+    """pos_row_sum [B,M] of match-list labels (lgb200_assign_pos_fwd): the positive entry of row i, j = gt0[i],
+    from sim [B,M,N] fp32 ((sim - lse_row) + (sim - lse_col), as assign_stats computes it from the mask) or from the
+    bf16 descriptors md0 [B,M,D] / md1 [B,N,D] (2 alpha md0_i . md1_j - lse_row_i - lse_col_j); 0 without a positive,
+    NaN where the lists disagree."""
+    _chk(gt0, torch.int64), _chk(gt1, torch.int64), _chk(lse_row, torch.float32), _chk(lse_col, torch.float32)
+    B, M = gt0.shape
+    N = gt1.shape[1]
+    D = 0
+    if sim is not None:
+        _chk(sim, torch.float32)
+        assert sim.shape == (B, M, N)
+    else:
+        _chk(md0, torch.bfloat16), _chk(md1, torch.bfloat16)
+        D = md0.shape[2]
+        assert md0.shape == (B, M, D) and md1.shape == (B, N, D)
+    out = torch.empty(B, M, device=gt0.device, dtype=torch.float32)
+    call("lgb200_assign_pos_fwd", ptr(md0), ptr(md1), ptr(sim), float(alpha), ptr(lse_row), ptr(lse_col), ptr(gt0),
+         ptr(gt1), ptr(out), B, M, N, D, stream_ptr())
+    return out
+
+
+def assign_pos_bwd(md0, md1, gcoef, gt0, gt1, dmd0, dmd1):
+    """dmd0 [B*M, D] += 2 gcoef_b md1[gt0[i]], dmd1 [B*N, D] += 2 gcoef_b md0[gt1[j]] in place (bf16;
+    lgb200_assign_pos_bwd): the positive term that assign_fused_bwd leaves out without masks."""
+    _chk(md0, torch.bfloat16), _chk(md1, torch.bfloat16), _chk(gcoef, torch.float32)
+    _chk(gt0, torch.int64), _chk(gt1, torch.int64), _chk(dmd0, torch.bfloat16), _chk(dmd1, torch.bfloat16)
+    B, M, D = md0.shape
+    N = md1.shape[1]
+    assert gt0.shape == (B, M) and gt1.shape == (B, N) and dmd0.numel() == B * M * D and dmd1.numel() == B * N * D
+    call("lgb200_assign_pos_bwd", ptr(md0), ptr(md1), ptr(gcoef), ptr(gt0), ptr(gt1), ptr(dmd0), ptr(dmd1), B, M, N, D,
+         stream_ptr())
 
 
 def head_logsig(zt):
@@ -1114,28 +1162,47 @@ def log_optimal_transport_varlen(sim, alpha, iters, pairs, out):
 # ------------------------------------------------------------------------------------------------
 # SuperGlue's NLL head and match filter on the dense Sinkhorn output (superglue.py:301-311, 322-352)
 # ------------------------------------------------------------------------------------------------
-def ot_nll_sums(Z, mask_u8, neg0, neg1):
+def ot_nll_sums(Z, mask_u8, neg0, neg1, gt0=None, gt1=None):
     """Z [B,M+1,N+1] fp32, mask u8 [B,M,N], neg0 [B,M] / neg1 [B,N] fp32 0/1 -> (pos, neg) [B]:
-    pos = sum mask * Z[:, :M, :N], neg = sum neg0 * Z[:, :M, N] + sum neg1 * Z[:, M, :N] (lgb200_ot_nll_fwd)."""
-    _chk(Z, torch.float32), _chk(mask_u8, torch.uint8), _chk(neg0, torch.float32), _chk(neg1, torch.float32)
+    pos = sum mask * Z[:, :M, :N], neg = sum neg0 * Z[:, :M, N] + sum neg1 * Z[:, M, :N] (lgb200_ot_nll_fwd).
+    mask_u8 None: the positives are the match lists gt0 [B,M] / gt1 [B,N] int64 (lgb200_ot_nll_fwd_sparse, the same
+    bits; NaN pos for a pair whose lists disagree)."""
+    _chk(Z, torch.float32), _chk(neg0, torch.float32), _chk(neg1, torch.float32)
     B, M1, N1 = Z.shape
     M, N = M1 - 1, N1 - 1
-    assert mask_u8.shape == (B, M, N) and neg0.shape == (B, M) and neg1.shape == (B, N)
+    assert neg0.shape == (B, M) and neg1.shape == (B, N)
     pos = torch.empty(B, device=Z.device, dtype=torch.float32)
     neg = torch.empty_like(pos)
     ws = torch.empty(_lib.load().lgb200_heads_ws_bytes(B, M, N), device=Z.device, dtype=torch.uint8)
+    if mask_u8 is None:
+        _chk(gt0, torch.int64), _chk(gt1, torch.int64)
+        assert gt0.shape == (B, M) and gt1.shape == (B, N)
+        call("lgb200_ot_nll_fwd_sparse", ptr(Z), ptr(gt0), ptr(gt1), ptr(neg0), ptr(neg1), ptr(pos), ptr(neg), ptr(ws),
+             B, M, N, stream_ptr())
+        return pos, neg
+    _chk(mask_u8, torch.uint8)
+    assert mask_u8.shape == (B, M, N)
     call("lgb200_ot_nll_fwd", ptr(Z), ptr(mask_u8), ptr(neg0), ptr(neg1), ptr(pos), ptr(neg), ptr(ws), B, M, N,
          stream_ptr())
     return pos, neg
 
 
-def ot_nll_bwd(mask_u8, neg0, neg1, num_pos, num_neg, gpos, gneg):
+def ot_nll_bwd(mask_u8, neg0, neg1, num_pos, num_neg, gpos, gneg, gt0=None):
     """dZ [B,M+1,N+1] of nll_pos = -pos / num_pos and nll_neg = -neg / num_neg for incoming gradients gpos, gneg [B]
-    (lgb200_ot_nll_bwd: everything read on the device, linear in the incoming gradients)."""
-    B, M, N = mask_u8.shape
+    (lgb200_ot_nll_bwd: everything read on the device, linear in the incoming gradients).  mask_u8 None: the positives
+    are the match list gt0 [B,M] int64 (lgb200_ot_nll_bwd_sparse, the same bits)."""
+    B, M = neg0.shape
+    N = neg1.shape[1]
     for t in (neg0, neg1, num_pos, num_neg, gpos, gneg):
         _chk(t, torch.float32)
-    dZ = torch.empty(B, M + 1, N + 1, device=mask_u8.device, dtype=torch.float32)
+    dZ = torch.empty(B, M + 1, N + 1, device=neg0.device, dtype=torch.float32)
+    if mask_u8 is None:
+        _chk(gt0, torch.int64)
+        assert gt0.shape == (B, M)
+        call("lgb200_ot_nll_bwd_sparse", ptr(gt0), ptr(neg0), ptr(neg1), ptr(num_pos), ptr(num_neg), ptr(gpos),
+             ptr(gneg), ptr(dZ), B, M, N, stream_ptr())
+        return dZ
+    assert mask_u8.shape == (B, M, N)
     call("lgb200_ot_nll_bwd", ptr(mask_u8), ptr(neg0), ptr(neg1), ptr(num_pos), ptr(num_neg), ptr(gpos), ptr(gneg),
          ptr(dZ), B, M, N, stream_ptr())
     return dZ
@@ -1143,31 +1210,39 @@ def ot_nll_bwd(mask_u8, neg0, neg1, num_pos, num_neg, gpos, gneg):
 
 class OtNllFn(torch.autograd.Function):
     """(nll_pos, nll_neg) [B] of superglue.py:325-336 from the dense log assignment Z, differentiable w.r.t. Z; the
-    reference's dense fp32 copies of the mask and of mask * Z are never formed."""
+    reference's dense fp32 copies of the mask and of mask * Z are never formed.  mask_u8 None: the positives are the
+    match lists gt0 / gt1."""
 
     @staticmethod
-    def forward(ctx, Z, mask_u8, neg0, neg1, num_pos, num_neg):
-        pos, neg = ot_nll_sums(Z, mask_u8, neg0, neg1)
-        ctx.save_for_backward(mask_u8, neg0, neg1, num_pos, num_neg)
+    def forward(ctx, Z, mask_u8, neg0, neg1, num_pos, num_neg, gt0=None, gt1=None):
+        pos, neg = ot_nll_sums(Z, mask_u8, neg0, neg1, gt0, gt1)
+        ctx.save_for_backward(mask_u8, neg0, neg1, num_pos, num_neg, gt0)
         return -pos / num_pos, -neg / num_neg
 
     @staticmethod
     def backward(ctx, gpos, gneg):
-        mask_u8, neg0, neg1, num_pos, num_neg = ctx.saved_tensors
+        mask_u8, neg0, neg1, num_pos, num_neg, gt0 = ctx.saved_tensors
         z = torch.zeros_like(num_pos)
         gpos = z if gpos is None else gpos.float().contiguous()
         gneg = z if gneg is None else gneg.float().contiguous()
-        return ot_nll_bwd(mask_u8, neg0, neg1, num_pos, num_neg, gpos, gneg), None, None, None, None, None
+        return ot_nll_bwd(mask_u8, neg0, neg1, num_pos, num_neg, gpos, gneg, gt0), None, None, None, None, None, None, None
 
 
 def ot_nll(Z, gt_assignment, gt_matches0, gt_matches1):
-    """superglue.py:325-336 -> (nll_pos, nll_neg, num_pos, num_neg) [B]; counts from lgb200_mask_counts."""
-    mask = gt_assignment.to(torch.uint8).contiguous()
+    """superglue.py:325-336 -> (nll_pos, nll_neg, num_pos, num_neg) [B]; counts from lgb200_mask_counts.
+    gt_assignment None: the positives come from the one-to-one match lists gt_matches0/1 (match_list_counts); the
+    losses and dZ are then bit-identical to the mask's, and NaN for a pair whose lists disagree."""
     neg0 = (gt_matches0 == -1).float().contiguous()
     neg1 = (gt_matches1 == -1).float().contiguous()
+    num_neg = (neg0.sum(1) + neg1.sum(1)).clamp(min=1.0)
+    if gt_assignment is None:
+        gt0, gt1 = gt_matches0.long().contiguous(), gt_matches1.long().contiguous()
+        _, _, num_pos = match_list_counts(gt0, gt1)
+        nll_pos, nll_neg = OtNllFn.apply(Z.contiguous(), None, neg0, neg1, num_pos, num_neg, gt0, gt1)
+        return nll_pos, nll_neg, num_pos, num_neg
+    mask = gt_assignment.to(torch.uint8).contiguous()
     rowcnt, _ = mask_counts(mask)
     num_pos = rowcnt.sum(1).clamp(min=1.0)
-    num_neg = (neg0.sum(1) + neg1.sum(1)).clamp(min=1.0)
     nll_pos, nll_neg = OtNllFn.apply(Z.contiguous(), mask, neg0, neg1, num_pos, num_neg)
     return nll_pos, nll_neg, num_pos, num_neg
 

@@ -190,11 +190,30 @@ int lgb200_assign_fused_stats(const void* md0, const void* md1, float alpha, con
                               float* colmax, int* colarg, float* pos_row_sum, int B, int M, int N, int D,
                               cudaStream_t stream);
 /* dmd0 [B*M, D], dmd1 [B*N, D] bf16 = dsim . md1, dsim^T . md0 with
- * dsim = gcoef[b] (2 gt - softmax_row rowcnt - softmax_col colcnt); gt_t = the [B,N,M] transpose of gt. */
+ * dsim = gcoef[b] (2 gt - softmax_row rowcnt - softmax_col colcnt); gt_t = the [B,N,M] transpose of gt.  gt and gt_t
+ * both NULL: dsim without the 2 gt term (labels given as match lists; lgb200_assign_pos_bwd adds it). */
 int lgb200_assign_fused_bwd(const void* md0, const void* md1, float alpha, const float* lse_row, const float* lse_col,
                             const uint8_t* gt, const uint8_t* gt_t, const float* gcoef, const float* rowcnt,
                             const float* colcnt, void* dmd0, void* dmd1, int B, int M, int N, int D,
                             cudaStream_t stream);
+/* ---- positive term from match lists (one-to-one labels; replaces the mask reads of losses.py:6-25 as used by
+ * lightglue.py:578-627).  gt0 [B,M], gt1 [B,N] int64 (gt_matches0/1): row i's only positive is j = gt0[i] >= 0, and the
+ * lists must agree, gt1[j] = i <=> gt0[i] = j.  rowcnt = (gt0 >= 0), colcnt = (gt1 >= 0) as floats.
+ * pos_fwd: pos_row_sum [B,M] = the dense pos_row_sum of lgb200_assign_scores / _fused_stats: from sim (fp32 [B,M,N],
+ * bit-identical to the mask's) or from md0 [B,M,D] / md1 [B,N,D] bf16 (2 alpha md0_i . md1_j - lse_row_i - lse_col_j,
+ * fp32 accumulate); exactly one of sim and (md0, md1) is set.  0 without a positive; NaN where gt0[i] >= N or
+ * gt1[gt0[i]] != i, so an inconsistent pair's loss is NaN.
+ * pos_bwd: dmd0_i += 2 gcoef_b md1_{gt0[i]}, dmd1_j += 2 gcoef_b md0_{gt1[j]} in place (bf16), after
+ * lgb200_assign_fused_bwd without masks.
+ * bwd_sparse: lgb200_assign_bwd with gt_ij = (gt0[i] == j); bit-identical to it on consistent lists. */
+int lgb200_assign_pos_fwd(const void* md0, const void* md1, const float* sim, float alpha, const float* lse_row,
+                          const float* lse_col, const int64_t* gt0, const int64_t* gt1, float* pos_row_sum, int B,
+                          int M, int N, int D, cudaStream_t stream);
+int lgb200_assign_pos_bwd(const void* md0, const void* md1, const float* gcoef, const int64_t* gt0, const int64_t* gt1,
+                          void* dmd0, void* dmd1, int B, int M, int N, int D, cudaStream_t stream);
+int lgb200_assign_bwd_sparse(const float* sim, const float* lse_row, const float* lse_col, const int64_t* gt0,
+                             const float* gcoef, const float* rowcnt, const float* colcnt, void* dsim, int out_dtype,
+                             int B, int M, int N, cudaStream_t stream);
 int lgb200_filter_matches(const float* rowmax, const int* rowarg, const int* colarg, float th, int64_t* m0,
                           int64_t* m1, float* ms0, float* ms1, int B, int M, int N, cudaStream_t stream);
 /* Varlen forms of lgb200_assign_lse / lgb200_assign_scores (evaluation: no gt, no pos_row_sum) / lgb200_filter_matches:
@@ -375,6 +394,15 @@ int lgb200_ot_nll_fwd(const float* Z, const uint8_t* mask, const float* neg0, co
 int lgb200_ot_nll_bwd(const uint8_t* mask, const float* neg0, const float* neg1, const float* num_pos,
                       const float* num_neg, const float* gpos, const float* gneg, float* dZ, int B, int M, int N,
                       cudaStream_t stream);
+/* The same with the positives given as match lists (replaces the mask of superglue.py:325-336): gt0 [B,M], gt1 [B,N]
+ * int64, one-to-one, positive (i, j) <=> gt0[i] = j >= 0.  pos, neg and dZ are bit-identical to lgb200_ot_nll_fwd /
+ * _bwd on the equivalent mask; a row with gt0[i] >= N or gt1[gt0[i]] != i makes its pair's pos NaN. */
+int lgb200_ot_nll_fwd_sparse(const float* Z, const int64_t* gt0, const int64_t* gt1, const float* neg0,
+                             const float* neg1, float* pos, float* neg, void* ws, int B, int M, int N,
+                             cudaStream_t stream);
+int lgb200_ot_nll_bwd_sparse(const int64_t* gt0, const float* neg0, const float* neg1, const float* num_pos,
+                             const float* num_neg, const float* gpos, const float* gneg, float* dZ, int B, int M, int N,
+                             cudaStream_t stream);
 /* Row max / argmax and column argmax of the inner block Z[:, :M, :N] (row pitch N+1), first index on ties like
  * torch's CPU max: the inputs of lgb200_filter_matches for SuperGlue's filter (superglue.py:301-311).             */
 int lgb200_ot_filter_stats(const float* Z, float* rowmax, int* rowarg, int* colarg, int B, int M, int N,
