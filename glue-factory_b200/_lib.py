@@ -114,6 +114,12 @@ SIGNATURES = {
     "lgb200_residual_add_cast": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _vp]),
     "lgb200_add_f32_cast": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _vp]),
     "lgb200_residual_add_cast_pitched": (_i, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i, _vp]),
+    "lgb200_sp_conv1a": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "lgb200_sp_conv": (_i, [_vp, _i, _vp, _vp, _vp] + [_i] * 7 + [_vp]),
+    "lgb200_sp_nms": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "lgb200_sp_count": (_i, [_vp, _f, _vp, _i, _i, _i, _vp]),
+    "lgb200_sp_select": (_i, [_vp, _f, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "lgb200_sp_sample": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
 }
 
 

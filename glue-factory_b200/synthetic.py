@@ -421,3 +421,35 @@ def line_gt_scene(kind, B, L0, L1, seed, W=640, H=480):
     res.update(extra)
     res["image_size"] = (H, W)
     return res
+
+
+def make_superpoint_weights(state_dict_like, seed=0, dtype=torch.float32):
+    """Deterministic SuperPoint weights (names / shapes from `state_dict_like`): He-uniform conv weights
+    U(-sqrt(6 / fan_in), ..), so activations keep their scale through the ReLU stack, biases U(-0.05, 0.05), and
+    convPb's weights 4x larger, so the 65-way softmax gives peaked score maps with keypoints above the threshold."""
+    rs = np.random.RandomState(seed)
+    out = {}
+    for k, v in state_dict_like.items():
+        shp = tuple(v.shape)
+        if k.endswith("weight"):
+            bound = math.sqrt(6.0 / (shp[1] * shp[2] * shp[3])) * (4.0 if k.startswith("convPb") else 1.0)
+        else:
+            bound = 0.05
+        out[k] = torch.from_numpy(rs.uniform(-bound, bound, size=shp)).to(dtype)
+    return out
+
+
+def make_superpoint_images(B, C, H, W, seed=0):
+    """[B, C, H, W] float32 images in [0, 1]: a few Gaussian blobs and edges over low-amplitude noise."""
+    rs = np.random.RandomState(seed)
+    yy, xx = np.mgrid[0:H, 0:W].astype(np.float64)
+    out = np.empty((B, C, H, W), np.float32)
+    for b in range(B):
+        for c in range(C):
+            img = 0.1 * rs.standard_normal((H, W))
+            for _ in range(12):
+                cy, cx, s, a = rs.uniform(0, H), rs.uniform(0, W), rs.uniform(1.5, 6.0), rs.uniform(-1, 1)
+                img += a * np.exp(-((yy - cy) ** 2 + (xx - cx) ** 2) / (2 * s * s))
+            img += 0.5 * (xx > rs.uniform(0, W)) * (yy > rs.uniform(0, H))
+            out[b, c] = (img - img.min()) / (img.max() - img.min())
+    return torch.from_numpy(out)

@@ -577,6 +577,47 @@ int lgb200_gt_line_matches(const float* lines0, const float* lines1, const float
                            double min_visibility_th, int64_t* matches0, int64_t* matches1, uint8_t* assignment,
                            void* ws, int B, int L0, int L1, cudaStream_t stream);
 
+/* ---- SuperPoint keypoint extraction, inference only (gluefactory_nonfree/superpoint.py, SuperPoint._forward) ------
+ * Activations are NHWC bf16, dense descriptors NHWC fp32, score maps [B, H, W] fp32.
+ * lgb200_sp_conv1a: image [B, C, H, W] fp32 (C = 3: gray = (r .299 + g .587) + b .114), weight [64, 9] / bias [64]
+ *   fp32 -> ReLU(conv3x3) as NHWC bf16 [B, H, W, 64] (16-byte aligned).
+ * lgb200_sp_conv: implicit-GEMM conv on wgmma.  x [B, H, W, ldx] bf16 (Cin channels used, Cin % 64 == 0),
+ *   weight [Npad, ksize * ksize * Cin] bf16 (K ordered (tap, channel)), bias [Npad] fp32, with Npad a multiple of the
+ *   tile width (64 for Cout 64, else 128; 256 for the normalising epilogue); the padding rows are zero.
+ *   epilogue LGB200_SP_RELU:    out [B, H, W, Cout] bf16 = ReLU(conv + bias)
+ *            LGB200_SP_POOL:    out [B, H/2, W/2, Cout] bf16 = maxpool2x2(ReLU(conv + bias)), floor sizes
+ *            LGB200_SP_SOFTMAX: Cout 65; out [B, 8H, 8W] fp32 = softmax over the 65 channels, channel c < 64 of pixel
+ *                               (y, x) at (8y + c/8, 8x + c%8)
+ *            LGB200_SP_L2N:     Cout 256; out [B, H, W, 256] fp32 = (conv + bias) / max(||conv + bias||, 1e-12)
+ * lgb200_sp_nms: simple_nms(scores, radius) (radius <= 9), then -1 on the remove_borders frame: rows < rb, cols < rb,
+ *   and rows >= int(h) - rb, cols >= int(w) - rb with (w, h) = image_size[b] ([B, 2] fp32, or NULL for H, W), each
+ *   start resolved like a Python slice start.
+ * lgb200_sp_count: counts[b] = number of pixels of nms[b] above threshold.
+ * lgb200_sp_select: per image, the candidates above threshold: all of them in row-major order when k <= 0 or there
+ *   are at most k, else the k largest in descending score order, exact ties to the lower row-major index (k <=
+ *   LGB200_SP_MAX_K).  keypoints [B, cap, 2] (x, y), scores [B, cap]; counts[b] (may be NULL) = slots filled.  Slots
+ *   past that are padding with score 0: coordinate i = lo_i + uniform[b, j, i] (hi_i - lo_i), [lo_i, hi_i] the range of
+ *   the kept keypoints' coordinate i, or [0, *pad_hi] when none is kept; zeros when uniform is NULL.  No host read.
+ * lgb200_sp_sample: desc [B, h, w, C] fp32 (C 128 or 256), keypoints [B, K, 2] in score-map pixels -> out [B, K, C] =
+ *   L2-normalised bilinear grid_sample (zeros padding) of desc at the keypoints, with legacy != 0 the reference's
+ *   sample_descriptors (align_corners=True), else sample_descriptors_fix_sampling.                                 */
+#define LGB200_SP_RELU 0
+#define LGB200_SP_POOL 1
+#define LGB200_SP_SOFTMAX 2
+#define LGB200_SP_L2N 3
+#define LGB200_SP_MAX_K 16384
+int lgb200_sp_conv1a(const float* image, int C, const float* weight, const float* bias, void* out, int B, int H,
+                     int W, cudaStream_t stream);
+int lgb200_sp_conv(const void* x, int ldx, const void* weight, const float* bias, void* out, int B, int H, int W,
+                   int Cin, int Cout, int ksize, int epilogue, cudaStream_t stream);
+int lgb200_sp_nms(const float* scores, const float* image_size, float* out, int B, int H, int W, int radius,
+                  int remove_borders, cudaStream_t stream);
+int lgb200_sp_count(const float* nms, float threshold, int* counts, int B, int H, int W, cudaStream_t stream);
+int lgb200_sp_select(const float* nms, float threshold, int k, int cap, const float* uniform, const float* pad_hi,
+                     float* keypoints, float* scores, int* counts, int B, int H, int W, cudaStream_t stream);
+int lgb200_sp_sample(const float* desc, const float* keypoints, float* out, int B, int K, int h, int w, int C,
+                     int legacy, cudaStream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
