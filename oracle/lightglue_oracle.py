@@ -220,8 +220,8 @@ def filter_matches(scores, th):
     inner = scores[:, :-1, :-1]
     max0, max1 = inner.max(2), inner.max(1)
     m0, m1 = max0.indices, max1.indices
-    i0 = torch.arange(m0.shape[1])[None]
-    i1 = torch.arange(m1.shape[1])[None]
+    i0 = torch.arange(m0.shape[1], device=m0.device)[None]
+    i1 = torch.arange(m1.shape[1], device=m1.device)[None]
     mutual0 = i0 == m1.gather(1, m0)
     mutual1 = i1 == m0.gather(1, m1)
     ms0 = torch.where(mutual0, max0.values.exp(), max0.values.new_zeros(()))
@@ -234,12 +234,14 @@ def filter_matches(scores, th):
 # ----------------------------------------------------------------------------
 # forward
 # ----------------------------------------------------------------------------
-def lightglue_forward(w, data, conf, rnd=_id):
+def lightglue_forward(w, data, conf, rnd=_id, layer=None):
     """lightglue.py:412-543, training-mode path (no early stop / pruning).
 
     conf: dict with n_layers, num_heads, filter_threshold.
+    layer: stands in for transformer_layer (same signature), e.g. the same layer under activation checkpointing.
     Returns the reference's pred dict.
     """
+    layer = transformer_layer if layer is None else layer
     L, H = conf["n_layers"], conf["num_heads"]
     k0 = normalize_keypoints(data["keypoints0"], data["view0"]["image_size"])
     k1 = normalize_keypoints(data["keypoints1"], data["view1"]["image_size"])
@@ -252,7 +254,7 @@ def lightglue_forward(w, data, conf, rnd=_id):
     th0, th1 = posenc_angles(w, k0), posenc_angles(w, k1)
     all0, all1 = [], []
     for i in range(L):
-        d0, d1 = transformer_layer(d0, d1, th0, th1, w, i, H, rnd)
+        d0, d1 = layer(d0, d1, th0, th1, w, i, H, rnd)
         all0.append(d0)
         all1.append(d1)
     scores, _ = match_assignment(d0, d1, w, L - 1, rnd)

@@ -278,15 +278,18 @@ def check_matches(tag, pred, rp, th, thr):
     return s0, s1
 
 
-def check_lg(tag, conf, pred, losses, grads, ref, precision, kind, training=True):
+def check_lg(tag, conf, pred, losses, grads, ref, precision, kind, training=True, bars=None):
     """One run against one reference: kind 'fp64' or 'mirror'.  ref = (pred, losses, grads, heads) of the fp64 oracle;
-    for 'mirror' the mirror's (pred, losses, grads) with the fp64 heads for the scales and margins."""
+    for 'mirror' the mirror's (pred, losses, grads) with the fp64 heads for the scales and margins.
+    bars: {"tol", "gtol", "thr"} in place of this file's bars (derived for at most 3 layers), for deeper models."""
     rp, rl, rg, heads = ref
     B = pred["log_assignment"].shape[0]
     L = len(heads)
     tol = TOL32 if precision == "fp32" else (TOLM if kind == "mirror" else TOLB)
     gtol = GRAD_TOL["fp32" if precision == "fp32" else kind if kind == "mirror" else "bf16"]
     thr = MARGIN[precision]
+    if bars is not None:
+        tol, gtol, thr = bars["tol"], bars["gtol"], bars["thr"]
     if kind == "fp64":
         check_matches(tag, pred, rp, conf.get("filter_threshold", 0.0), thr)
     th = conf.get("filter_threshold", 0.0)
@@ -318,10 +321,16 @@ def check_lg(tag, conf, pred, losses, grads, ref, precision, kind, training=True
     if training and kind == "fp64":
         check_final_targets(tag, pred, heads, thr)
     if grads is not None:
-        G = max(v.double().norm().item() for v in rg.values())
-        for k, g in grads.items():
-            r = rg[k].double()
-            _ratio(f"grad {precision} {kind}:{tag}:{k}", (g - r).norm().item(), gtol * max(r.norm().item(), GRAD_FLOOR * G))
+        check_grads(tag, grads, rg, gtol, precision, kind)
+
+
+def check_grads(tag, grads, rg, gtol, precision, kind):
+    """Every parameter's gradient as its own tensor: ||g - ref|| <= gtol max(||ref||, GRAD_FLOOR G)."""
+    G = max(v.double().norm().item() for v in rg.values())
+    for k, g in grads.items():
+        r = rg[k].double()
+        _ratio(f"grad {precision} {kind}:{tag}:{k}", (g.double() - r).norm().item(),
+               gtol * max(r.norm().item(), GRAD_FLOOR * G))
 
 
 def conf_term_bound(heads, b, tol, thr):

@@ -51,6 +51,14 @@ Fused assignment head (assign_fused_stats / assign_fused_bwd), per pair, s = alp
                + (N/4 + 4) U32 sum_j gt |2 s - lse_row - lse_col|
   dmd0      (2 UBF |dsim| + 2 ddsim + N UACC |dsim|) |md1| + UBF |dmd0|, ddsim = gc (Pr rowcnt eps_r' + Pc colcnt eps_c'),
             eps' = es + b(lse) + EX2 + 4 U32 (|s| + |lse|): dsim is rounded to bf16 before its product; dmd1 likewise.
+  labels as match lists (gt = gt_t = NULL): STATS reads no mask for its LSE / max / argmax outputs, which must equal the
+            mask mode's bit for bit.  assign_pos_fwd from the descriptors is held to the bound of
+            tests/test_gpu_sparse_labels.py, (2 D + 8) U32 (2 alpha |md0_i| . |md1_j| + |lse_row_i| + |lse_col_j|) at
+            the kernel's own LSEs.  The fused backward then rounds X = dsim' md1 to bf16, dsim' = dsim without its
+            2 gc entries at the positives, and assign_pos_bwd adds 2 gc md1[gt0[i]] to that bf16 value in one fp32 fma
+            and rounds again: dmd0 is within b1 = (2 UBF |dsim'| + 2 ddsim + N UACC |dsim'|) |md1| + UBF |X| (the
+            mask mode's bound for the partial product) plus (UBF + U32) (|dmd0| + b1) for the second rounding of a
+            value already off by b1; dmd1 likewise.
 
 Every check takes a NaN as a failure (unwritten outputs show as NaN) and records its largest err / bound through
 tests.util.report.  Attention outputs, lse, dq / dk / dv and d(mdesc) land in buffers with NaN-pattern guard rows on
@@ -222,8 +230,9 @@ def _lse_with_bound(s, es, dim):
     return lse, b, P
 
 
-def assign_ref(md0, md1, alpha, ls0, ls1, gt, gc):
-    """fp64 assignment head of one pair: md0 [M,D], md1 [N,D] bf16, ls0 [M], ls1 [N], gt [M,N] bool, gc scalar."""
+def assign_ref(md0, md1, alpha, ls0, ls1, gt, gc, lists=False):
+    """fp64 assignment head of one pair: md0 [M,D], md1 [N,D] bf16, ls0 [M], ls1 [N], gt [M,N] bool, gc scalar.
+    lists: the d(mdesc) bounds of the mask-free backward followed by assign_pos_bwd (module docstring)."""
     A, Bm = md0.double(), md1.double()
     D = A.shape[1]
     s = alpha * (A @ Bm.t())
@@ -248,8 +257,15 @@ def assign_ref(md0, md1, alpha, ls0, ls1, gt, gc):
     M, N = s.shape
     r["dmd0"] = dsim @ Bm
     r["dmd1"] = dsim.t() @ A
-    r["b_dmd0"] = ((2 * UBF + N * UACC) * dsim.abs() + 2 * ddsim) @ Bm.abs() + UBF * r["dmd0"].abs()
-    r["b_dmd1"] = ((2 * UBF + M * UACC) * dsim.abs() + 2 * ddsim).t() @ A.abs() + UBF * r["dmd1"].abs()
+    if not lists:
+        r["b_dmd0"] = ((2 * UBF + N * UACC) * dsim.abs() + 2 * ddsim) @ Bm.abs() + UBF * r["dmd0"].abs()
+        r["b_dmd1"] = ((2 * UBF + M * UACC) * dsim.abs() + 2 * ddsim).t() @ A.abs() + UBF * r["dmd1"].abs()
+        return r
+    part = dsim - 2 * gc * g  # what the fused kernel contracts without masks
+    b1 = ((2 * UBF + N * UACC) * part.abs() + 2 * ddsim) @ Bm.abs() + UBF * (part @ Bm).abs()
+    r["b_dmd0"] = b1 + (UBF + U32) * (r["dmd0"].abs() + b1)
+    b1 = ((2 * UBF + M * UACC) * part.abs() + 2 * ddsim).t() @ A.abs() + UBF * (part.t() @ A).abs()
+    r["b_dmd1"] = b1 + (UBF + U32) * (r["dmd1"].abs() + b1)
     return r
 
 
@@ -667,30 +683,74 @@ def _assign_inputs(B, M, N, D, seed):
     return md0, md1, D ** -0.5, ls0, ls1, gt, gc
 
 
+def _assign_lists(B, M, N, seed):
+    """One-to-one match lists gt0 [B,M] / gt1 [B,N] with -1 and -2 labels: pair 0 without positives, every other pair
+    with min(M, N) // 3 positives at random rows and columns; a tenth of the unmatched points ignored."""
+    g = torch.Generator().manual_seed(seed)
+    m0 = torch.full((B, M), -1, dtype=torch.long)
+    m1 = torch.full((B, N), -1, dtype=torch.long)
+    K = max(1, min(M, N) // 3)
+    for b in range(1, B):
+        i, j = torch.randperm(M, generator=g)[:K], torch.randperm(N, generator=g)[:K]
+        m0[b, i], m1[b, j] = j, i
+    m0[(torch.rand(B, M, generator=g) < 0.1) & (m0 < 0)] = -2
+    m1[(torch.rand(B, N, generator=g) < 0.1) & (m1 < 0)] = -2
+    return m0.to(DEV), m1.to(DEV)
+
+
 ASSIGN_SHAPES = [(32, 2048, 2048, 256), (32, 2048, 2048, 128), (4, 384, 320, 64), (4, 300, 257, 128), (4, 191, 321, 192), (4, 1000, 777, 256)]
 
 
+# every shape with the mask (ids as before the lists mode existed) and with match lists ("-lists")
+ASSIGN_CASES = [pytest.param(*s, labels, id="-".join(map(str, s)) + ("" if labels == "mask" else "-lists"))
+                for labels in ("mask", "lists") for s in ASSIGN_SHAPES]
+
+
 @GPU
-@pytest.mark.parametrize("B,M,N,D", ASSIGN_SHAPES)
-def test_assign_fused_against_fp64(B, M, N, D):
+@pytest.mark.parametrize("B,M,N,D,labels", ASSIGN_CASES)
+def test_assign_fused_against_fp64(B, M, N, D, labels):
     md0, md1, alpha, ls0, ls1, gt, gc = _assign_inputs(B, M, N, D, seed=B + M + N + D)
+    if labels == "lists":  # the same labels as a mask, for the mask mode's outputs and the reference
+        m0, m1 = _assign_lists(B, M, N, seed=B * M + N + D)
+        gt = torch.zeros(B, M, N, device=DEV, dtype=torch.bool).scatter_(2, m0.clamp(min=0)[..., None],
+                                                                       (m0 >= 0)[..., None])
     gt_u8 = gt.view(torch.uint8)
     f = ops.assign_fused_stats(md0, md1, alpha, ls0, ls1, gt_u8=gt_u8)
     rowcnt, colcnt = gt_u8.sum(2, dtype=torch.float32), gt_u8.sum(1, dtype=torch.float32)
     g0 = _guarded((B * M, D), torch.bfloat16, 2 * D)
     g1 = _guarded((B * N, D), torch.bfloat16, 2 * D)
-    gt_t = gt_u8.transpose(1, 2).contiguous()
-    ops.assign_fused_bwd(md0, md1, alpha, f["lse_row"], f["lse_col"], gt_u8, gt_t, gc, rowcnt, colcnt, g0[1], g1[1])
+    if labels == "mask":
+        gt_t = gt_u8.transpose(1, 2).contiguous()
+        ops.assign_fused_bwd(md0, md1, alpha, f["lse_row"], f["lse_col"], gt_u8, gt_t, gc, rowcnt, colcnt, g0[1], g1[1])
+    else:
+        fl = ops.assign_fused_stats(md0, md1, alpha, ls0, ls1, gt_u8=None)
+        assert fl["pos_row_sum"] is None
+        for k in ("lse_row", "lse_col", "rowmax", "rowarg", "colmax", "colarg"):
+            assert torch.equal(fl[k], f[k]), k  # STATS reads no mask for these
+        rowcnt, colcnt, _ = ops.match_list_counts(m0, m1)
+        pos = ops.assign_pos_fwd(m0, m1, fl["lse_row"], fl["lse_col"], alpha, md0, md1)
+        a, c = md0.double(), md1.double()
+        j = m0.clamp(min=0)
+        cj = c.gather(1, j[..., None].expand(-1, -1, D))
+        lcj = fl["lse_col"].double().gather(1, j)
+        lr = fl["lse_row"].double()
+        want = torch.where(m0 >= 0, 2 * alpha * (a * cj).sum(-1) - lr - lcj, torch.zeros_like(lr))
+        bound = torch.where(m0 >= 0, (2 * D + 8) * U32 * (2 * alpha * (a.abs() * cj.abs()).sum(-1) + lr.abs() + lcj.abs()),
+                            torch.zeros_like(lr))
+        _within((pos.double() - want).abs(), bound, f"assign lists B={B} M={M} N={N} D={D} pos_fwd")
+        del a, c, cj, fl
+        ops.assign_fused_bwd(md0, md1, alpha, f["lse_row"], f["lse_col"], None, None, gc, rowcnt, colcnt, g0[1], g1[1])
+        ops.assign_pos_bwd(md0, md1, gc, m0, m1, g0[1], g1[1])
     dmd0, dmd1 = g0[1].view(B, M, D), g1[1].view(B, N, D)
     if B == 32:  # the benchmark's launch: a second call is bit-identical
         f2 = ops.assign_fused_stats(md0, md1, alpha, ls0, ls1, gt_u8=gt_u8)
         assert all(torch.equal(f[k], f2[k]) for k in ("lse_row", "lse_col", "rowmax", "rowarg", "colmax", "colarg",
                                                       "pos_row_sum"))
         del f2
-    tag = f"assign B={B} M={M} N={N} D={D}"
+    tag = f"assign {labels} B={B} M={M} N={N} D={D}"
     w = _Worst(tag)
     for b in range(B):
-        r = assign_ref(md0[b], md1[b], alpha, ls0[b], ls1[b], gt[b], gc[b].item())
+        r = assign_ref(md0[b], md1[b], alpha, ls0[b], ls1[b], gt[b], gc[b].item(), lists=labels == "lists")
         for k in ("lse_row", "lse_col", "rowmax", "colmax"):
             w(k, (f[k][b].double() - r[k]).abs(), r["b_" + k])
         w("pos_row_sum", (f["pos_row_sum"][b].double() - r["pos_row_sum"]).abs(), r["b_pos"])
@@ -698,7 +758,7 @@ def test_assign_fused_against_fp64(B, M, N, D):
         check_argmax(f["colarg"][b], r["sc"], r["b_colmax"], 0, f"{tag} b={b} colarg")
         w("dmd0", (dmd0[b].double() - r["dmd0"]).abs(), r["b_dmd0"])
         w("dmd1", (dmd1[b].double() - r["dmd1"]).abs(), r["b_dmd1"])
-        if b % 4 == 1:  # no positives: nothing to differentiate
+        if (b == 0) if labels == "lists" else (b % 4 == 1):  # no positives: nothing to differentiate
             assert not dmd0[b].any() and not dmd1[b].any() and not f["pos_row_sum"][b].any()
         del r
     w.report()
