@@ -120,6 +120,9 @@ SIGNATURES = {
     "lgb200_sp_count": (_i, [_vp, _f, _vp, _i, _i, _i, _vp]),
     "lgb200_sp_select": (_i, [_vp, _f, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "lgb200_sp_sample": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "lgb200_spo_conv1a": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "lgb200_spo_conv": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp] + [_i] * 7 + [_vp]),
+    "lgb200_spo_bn_apply": (_i, [_vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _i, _i, _vp]),
 }
 
 

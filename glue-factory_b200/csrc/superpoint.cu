@@ -15,6 +15,12 @@
 //              padding for force_num_keypoints.
 //  sp_sample   bilinear grid_sample of the dense descriptors (legacy align_corners=True, or the fixed variant),
 //              L2-normalised, one warp per keypoint, written as [B, K, C].
+//
+// SuperPoint-open (gluefactory/models/extractors/superpoint_open.py) puts a BatchNorm after every conv.  With running
+// statistics (eval mode) its affine y = scale x + shift is folded into the conv epilogues above (AFF): after the ReLU
+// and before the pool in the encoder, before the softmax / L2 normalisation in the heads.  With batch statistics
+// (training mode) the convs write the pre-BatchNorm activations (ReLU, or RAW fp32 for the heads), lgb200_bn_stats
+// sums them, and spo_bn_apply normalises: plain, + 2x2 max-pool, + softmax / depth-to-space, + L2 normalisation.
 #include <algorithm>
 
 #include "common.cuh"
@@ -38,12 +44,22 @@ __device__ __forceinline__ void sp_cp_wait() {
 // ---------------------------------------------------------------------------------------------
 // one thread per (pixel, 8 output channels); gray = (r * .299 + g * .587) + b * .114 rounded per op like torch's
 // (image * scale).sum(1)
+// AFF: ReLU then the per-channel affine scale * x + shift (an eval-mode BatchNorm)
+template <bool AFF>
 __global__ void __launch_bounds__(256) sp_conv1a_kernel(const float* __restrict__ img, int C,
                                                         const float* __restrict__ w, const float* __restrict__ bias,
-                                                        __nv_bfloat16* __restrict__ out, int B, int H, int W) {
+                                                        __nv_bfloat16* __restrict__ out, int B, int H, int W,
+                                                        const float* __restrict__ scale,
+                                                        const float* __restrict__ shift) {
   __shared__ float sw[64 * 9], sb[64];
+  __shared__ float ss[AFF ? 64 : 1], sh[AFF ? 64 : 1];
   for (int i = threadIdx.x; i < 64 * 9; i += blockDim.x) sw[i] = w[i];
   for (int i = threadIdx.x; i < 64; i += blockDim.x) sb[i] = bias[i];
+  if constexpr (AFF)
+    for (int i = threadIdx.x; i < 64; i += blockDim.x) {
+      ss[i] = scale[i];
+      sh[i] = shift[i];
+    }
   __syncthreads();
   const int64_t n = (int64_t)B * H * W * 8;
   const int64_t HW = (int64_t)H * W;
@@ -80,6 +96,7 @@ __global__ void __launch_bounds__(256) sp_conv1a_kernel(const float* __restrict_
 #pragma unroll
         for (int k = 0; k < 9; ++k) a = fmaf(sw[c * 9 + k], v[k], a);
         r[h] = fmaxf(a, 0.f);
+        if constexpr (AFF) r[h] = fmaf(r[h], ss[c], sh[c]);
       }
       packed[c2] = pack_bf16(r[0], r[1]);
     }
@@ -93,7 +110,7 @@ __global__ void __launch_bounds__(256) sp_conv1a_kernel(const float* __restrict_
 constexpr int SP_TY = 8, SP_TX = 16, SP_TM = SP_TY * SP_TX;  // output tile: 8 pixel rows x 16 columns
 constexpr int SP_STAGES = 3;
 constexpr int SP_THREADS = 256;
-enum { SP_EP_RELU = 0, SP_EP_POOL = 1, SP_EP_SOFTMAX = 2, SP_EP_L2N = 3 };
+enum { SP_EP_RELU = 0, SP_EP_POOL = 1, SP_EP_SOFTMAX = 2, SP_EP_L2N = 3, SP_EP_RAW = 4 };
 
 template <int BN>
 __host__ __device__ constexpr int sp_stage_bytes() { return (SP_TM + BN) * 128; }
@@ -107,11 +124,13 @@ __host__ __device__ constexpr int sp_smem_bytes() {
 // row r, 16-byte chunk c of a 128-byte-swizzled K-major block
 __device__ __forceinline__ int sw128(int r, int c) { return r * 128 + ((c ^ (r & 7)) << 4); }
 
-template <int BN, int EP>
+// AFF: the staged values (after the ReLU of the encoder epilogues) become scale * v + shift before the epilogue
+// proper.  SP_EP_RAW: conv + bias as fp32 [B, H, W, BN * tiles_n].
+template <int BN, int EP, bool AFF = false>
 __global__ void __launch_bounds__(SP_THREADS)
     sp_conv_kernel(const __nv_bfloat16* __restrict__ x, int ldx, const __nv_bfloat16* __restrict__ w,
                    const float* __restrict__ bias, void* __restrict__ out, int H, int W, int Cin, int Cout, int ks,
-                   int tiles_n) {
+                   int tiles_n, const float* __restrict__ scale, const float* __restrict__ shift) {
   extern __shared__ uint8_t sp_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(sp_raw) + 1023) & ~uintptr_t(1023));
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
@@ -199,6 +218,7 @@ __global__ void __launch_bounds__(SP_THREADS)
             const int col = sub * 128 + 8 * j + 2 * (lane & 3) + c;
             float v = d[sub][4 * j + 2 * i + c] + bias[n0 + col];
             if (EP == SP_EP_RELU || EP == SP_EP_POOL) v = fmaxf(v, 0.f);
+            if constexpr (AFF) v = fmaf(v, scale[n0 + col], shift[n0 + col]);
             st[(rbase + 8 * i) * LD + col] = v;
           }
   }
@@ -252,6 +272,16 @@ __global__ void __launch_bounds__(SP_THREADS)
         o[(int64_t)(8 * yy + cy) * (8 * W) + 8 * xx + cx] = expf(st[m * LD + cy * 8 + cx] - mx[m]) / inv[m];
       }
     }
+  } else if constexpr (EP == SP_EP_RAW) {
+    const int ld = BN * tiles_n;
+    float* o = static_cast<float*>(out) + (int64_t)b * H * W * ld;
+    for (int q = tid; q < SP_TM * BN / 4; q += SP_THREADS) {
+      const int m = q / (BN / 4), c = 4 * (q % (BN / 4));
+      const int yy = y0 + (m >> 4), xx = x0 + (m & 15);
+      if (yy < H && xx < W)
+        *reinterpret_cast<float4*>(o + ((int64_t)yy * W + xx) * ld + n0 + c) =
+            make_float4(st[m * LD + c], st[m * LD + c + 1], st[m * LD + c + 2], st[m * LD + c + 3]);
+    }
   } else {
     // L2 normalisation over the BN (= Cout) channels of a pixel: one warp per pixel, fp32 NHWC out
     float* o = static_cast<float*>(out) + (int64_t)b * H * W * Cout;
@@ -267,15 +297,72 @@ __global__ void __launch_bounds__(SP_THREADS)
   }
 }
 
-template <int BN, int EP>
-static int launch_sp_conv(const __nv_bfloat16* x, int ldx, const __nv_bfloat16* w, const float* bias, void* out, int B,
-                          int H, int W, int Cin, int Cout, int ks, int tiles_n, cudaStream_t st) {
-  auto k = sp_conv_kernel<BN, EP>;
+template <int BN, int EP, bool AFF>
+static int launch_sp_conv(const __nv_bfloat16* x, int ldx, const __nv_bfloat16* w, const float* bias,
+                          const float* scale, const float* shift, void* out, int B, int H, int W, int Cin, int Cout,
+                          int ks, int tiles_n, cudaStream_t st) {
+  auto k = sp_conv_kernel<BN, EP, AFF>;
   constexpr int smem = sp_smem_bytes<BN>();
   if (ensure_dyn_smem(reinterpret_cast<const void*>(k), smem)) return kErrCuda;
   dim3 grid((W + SP_TX - 1) / SP_TX, ((H + SP_TY - 1) / SP_TY) * tiles_n, B);
-  k<<<grid, SP_THREADS, smem, st>>>(x, ldx, w, bias, out, H, W, Cin, Cout, ks, tiles_n);
+  k<<<grid, SP_THREADS, smem, st>>>(x, ldx, w, bias, out, H, W, Cin, Cout, ks, tiles_n, scale, shift);
   return check_launch("sp_conv");
+}
+
+// the shape checks and instantiation choice of lgb200_sp_conv (AFF false) and lgb200_spo_conv (AFF true, or RAW)
+template <bool AFF>
+static int sp_conv_dispatch(const void* x, int ldx, const void* weight, const float* bias, const float* scale,
+                            const float* shift, void* out, int B, int H, int W, int Cin, int Cout, int ksize,
+                            int epilogue, cudaStream_t stream) {
+  LGB_REQUIRE(x && weight && bias && out, kErrInvalid, "sp_conv: null pointer");
+  LGB_REQUIRE(!AFF || epilogue == SP_EP_RAW || (scale && shift), kErrInvalid, "sp_conv: null scale / shift");
+  LGB_REQUIRE(B > 0 && H > 0 && W > 0 && B <= 65535, kErrInvalid, "sp_conv: bad extents B=%d H=%d W=%d", B, H, W);
+  LGB_REQUIRE(ksize == 1 || ksize == 3, kErrInvalid, "sp_conv: ksize %d (1 or 3)", ksize);
+  LGB_REQUIRE(Cin % 64 == 0 && Cin > 0 && ldx >= Cin && ldx % 8 == 0, kErrInvalid,
+              "sp_conv: Cin %d must be a multiple of 64 and ldx %d >= Cin a multiple of 8", Cin, ldx);
+  LGB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(weight)) & 15) == 0, kErrInvalid,
+              "sp_conv: x and weight must be 16-byte aligned");
+  const int ty = (H + SP_TY - 1) / SP_TY;
+  auto grid_ok = [&](int tiles_n) { return (int64_t)ty * tiles_n <= 65535; };
+  const __nv_bfloat16 *xb = (const __nv_bfloat16*)x, *wb = (const __nv_bfloat16*)weight;
+  switch (epilogue) {
+    case SP_EP_RELU:
+    case SP_EP_POOL: {
+      LGB_REQUIRE(Cout % 64 == 0, kErrInvalid, "sp_conv: Cout %d must be a multiple of 64", Cout);
+      if (Cout == 64) {
+        LGB_REQUIRE(grid_ok(1), kErrInvalid, "sp_conv: image too tall");
+        return epilogue == SP_EP_RELU
+                   ? launch_sp_conv<64, SP_EP_RELU, AFF>(xb, ldx, wb, bias, scale, shift, out, B, H, W, Cin, Cout,
+                                                         ksize, 1, stream)
+                   : launch_sp_conv<64, SP_EP_POOL, AFF>(xb, ldx, wb, bias, scale, shift, out, B, H, W, Cin, Cout,
+                                                         ksize, 1, stream);
+      }
+      LGB_REQUIRE(Cout % 128 == 0 && grid_ok(Cout / 128), kErrInvalid, "sp_conv: Cout %d (64 or a multiple of 128)",
+                  Cout);
+      return epilogue == SP_EP_RELU
+                 ? launch_sp_conv<128, SP_EP_RELU, AFF>(xb, ldx, wb, bias, scale, shift, out, B, H, W, Cin, Cout,
+                                                        ksize, Cout / 128, stream)
+                 : launch_sp_conv<128, SP_EP_POOL, AFF>(xb, ldx, wb, bias, scale, shift, out, B, H, W, Cin, Cout,
+                                                        ksize, Cout / 128, stream);
+    }
+    case SP_EP_SOFTMAX:
+      LGB_REQUIRE(Cout == 65 && grid_ok(1), kErrInvalid, "sp_conv: the softmax epilogue takes Cout 65 (got %d)", Cout);
+      return launch_sp_conv<128, SP_EP_SOFTMAX, AFF>(xb, ldx, wb, bias, scale, shift, out, B, H, W, Cin, Cout, ksize,
+                                                     1, stream);
+    case SP_EP_L2N:
+      LGB_REQUIRE(Cout == 256 && grid_ok(1), kErrInvalid, "sp_conv: the normalising epilogue takes Cout 256 (got %d)",
+                  Cout);
+      LGB_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, kErrInvalid, "sp_conv: out must be 16-byte aligned");
+      return launch_sp_conv<256, SP_EP_L2N, AFF>(xb, ldx, wb, bias, scale, shift, out, B, H, W, Cin, Cout, ksize, 1,
+                                                 stream);
+    case SP_EP_RAW:
+      LGB_REQUIRE(Cout > 0 && grid_ok((Cout + 127) / 128), kErrInvalid, "sp_conv: raw epilogue, Cout %d", Cout);
+      LGB_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, kErrInvalid, "sp_conv: out must be 16-byte aligned");
+      return launch_sp_conv<128, SP_EP_RAW, false>(xb, ldx, wb, bias, nullptr, nullptr, out, B, H, W, Cin, Cout, ksize,
+                                                   (Cout + 127) / 128, stream);
+    default:
+      LGB_REQUIRE(false, kErrInvalid, "sp_conv: unknown epilogue %d", epilogue);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -637,6 +724,168 @@ __global__ void __launch_bounds__(256) sp_sample_kernel(const float* __restrict_
     *reinterpret_cast<float4*>(o + c) = make_float4(acc[c] * r, acc[c + 1] * r, acc[c + 2] * r, acc[c + 3] * r);
 }
 
+// ---------------------------------------------------------------------------------------------
+// training-mode BatchNorm of SuperPoint-open from batch statistics
+// ---------------------------------------------------------------------------------------------
+// sums = [sum x (C) | sum x^2 (C) | count] in fp64 (lgb200_bn_stats, possibly summed across ranks): mean and biased
+// variance as bn_relu_fwd_kernel forms them, y = (x - mean) rstd gamma + beta.  Every CTA fills its own copy.
+enum { SPO_BN_PLAIN = 0, SPO_BN_POOL = 1, SPO_BN_SOFTMAX = 2, SPO_BN_L2N = 3 };
+constexpr int SPO_BN_MAXC = 512;
+constexpr int SPO_BN_THREADS = 256;
+
+struct SpoBnSmem {
+  float mu[SPO_BN_MAXC], rs[SPO_BN_MAXC], g[SPO_BN_MAXC], b[SPO_BN_MAXC];
+};
+
+__device__ __forceinline__ void spo_bn_setup(SpoBnSmem& sm, const double* __restrict__ sums,
+                                             const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
+                                             int C) {
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const double n = sums[2 * C];
+    const double m = sums[c] / n;
+    const double var = fmax(sums[C + c] / n - m * m, 0.0);
+    sm.mu[c] = (float)m;
+    sm.rs[c] = 1.f / sqrtf((float)var + eps);
+    sm.g[c] = gamma[c];
+    sm.b[c] = beta[c];
+  }
+  __syncthreads();
+}
+
+__device__ __forceinline__ float spo_bn(const SpoBnSmem& sm, int c, float v) {
+  return fmaf((v - sm.mu[c]) * sm.rs[c], sm.g[c], sm.b[c]);
+}
+
+__device__ __forceinline__ void spo_unpack8(const uint4& u, float* v) {
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    v[2 * i] = __uint_as_float(w[i] << 16);
+    v[2 * i + 1] = __uint_as_float(w[i] & 0xFFFF0000u);
+  }
+}
+
+// PLAIN: bf16 [B, H, W, C] -> bf16 [B, H, W, C].  POOL: -> bf16 [B, H/2, W/2, C], the 2x2 max of the normalised
+// values (floor sizes).  One thread per 8 channels of an output pixel, 16-byte loads and stores.
+template <int OP>
+__global__ void __launch_bounds__(SPO_BN_THREADS)
+    spo_bn_nhwc_kernel(const __nv_bfloat16* __restrict__ x, const double* __restrict__ sums,
+                       const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
+                       __nv_bfloat16* __restrict__ out, int B, int H, int W, int C) {
+  __shared__ SpoBnSmem sm;
+  spo_bn_setup(sm, sums, gamma, beta, eps, C);
+  // C / 8 divides the grid stride (C a power of two <= 512), so a thread keeps its 8 channels
+  const int cv = C / 8;
+  const int Ho = OP == SPO_BN_POOL ? H / 2 : H, Wo = OP == SPO_BN_POOL ? W / 2 : W;
+  const int64_t np = (int64_t)B * Ho * Wo;
+  const int start = blockIdx.x * blockDim.x + threadIdx.x, c0 = (start % cv) * 8;
+  const int pstride = gridDim.x * blockDim.x / cv;
+  for (int64_t p = start / cv; p < np; p += pstride) {
+    float r[8];
+    if constexpr (OP == SPO_BN_PLAIN) {
+      float v[8];
+      spo_unpack8(*reinterpret_cast<const uint4*>(x + p * C + c0), v);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) r[e] = spo_bn(sm, c0 + e, v[e]);
+    } else {
+      const int px = (int)(p % Wo), py = (int)((p / Wo) % Ho), b = (int)(p / ((int64_t)Wo * Ho));
+      const __nv_bfloat16* xb = x + (((int64_t)b * H + 2 * py) * W + 2 * px) * C + c0;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) r[e] = -INFINITY;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        float v[8];
+        spo_unpack8(*reinterpret_cast<const uint4*>(xb + ((int64_t)(q >> 1) * W + (q & 1)) * C), v);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) r[e] = fmaxf(r[e], spo_bn(sm, c0 + e, v[e]));
+      }
+    }
+    *reinterpret_cast<uint4*>(out + p * C + c0) =
+        make_uint4(pack_bf16(r[0], r[1]), pack_bf16(r[2], r[3]), pack_bf16(r[4], r[5]), pack_bf16(r[6], r[7]));
+  }
+}
+
+// SOFTMAX: logits fp32 [B, h, w, 128] (channels 65.. ignored) -> normalise the 65 -> softmax -> depth-to-space score
+// map fp32 [B, 8h, 8w].  16 lanes per pixel: lane j holds channels 4j .. 4j + 3 (score row j / 2, columns
+// 4 (j & 1) .. + 3 of the pixel's 8x8 cell) and every lane the dustbin, channel 64.
+__global__ void __launch_bounds__(SPO_BN_THREADS)
+    spo_bn_softmax_kernel(const float* __restrict__ x, const double* __restrict__ sums,
+                          const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
+                          float* __restrict__ out, int B, int h, int w) {
+  __shared__ SpoBnSmem sm;
+  spo_bn_setup(sm, sums, gamma, beta, eps, 65);
+  const int lane = threadIdx.x & 31, j = lane & 15;
+  const unsigned mask = 0xFFFFu << (lane & 16);
+  const int64_t np = (int64_t)B * h * w;
+  for (int64_t p = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 4; p < np;
+       p += ((int64_t)gridDim.x * blockDim.x) >> 4) {
+    const float4 q = *reinterpret_cast<const float4*>(x + p * 128 + 4 * j);
+    float v[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+    for (int t = 0; t < 4; ++t) v[t] = spo_bn(sm, 4 * j + t, v[t]);
+    const float dust = spo_bn(sm, 64, x[p * 128 + 64]);
+    float m = fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3]));
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(mask, m, o));
+    m = fmaxf(m, dust);
+    float e[4], s;
+#pragma unroll
+    for (int t = 0; t < 4; ++t) e[t] = expf(v[t] - m);
+    s = (e[0] + e[1]) + (e[2] + e[3]);
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) s += __shfl_xor_sync(mask, s, o);
+    s += expf(dust - m);
+    const int xx = (int)(p % w), yy = (int)((p / w) % h), b = (int)(p / ((int64_t)w * h));
+    float* o = out + ((int64_t)b * 8 * h + 8 * yy + (j >> 1)) * (8 * (int64_t)w) + 8 * xx + 4 * (j & 1);
+    *reinterpret_cast<float4*>(o) = make_float4(e[0] / s, e[1] / s, e[2] / s, e[3] / s);
+  }
+}
+
+// L2N: fp32 [T, 256] -> normalise -> divide by max(||.||, 1e-12) per pixel, fp32 [T, 256].  One warp per pixel.
+__global__ void __launch_bounds__(SPO_BN_THREADS)
+    spo_bn_l2n_kernel(const float* __restrict__ x, const double* __restrict__ sums, const float* __restrict__ gamma,
+                      const float* __restrict__ beta, float eps, float* __restrict__ out, int64_t T) {
+  __shared__ SpoBnSmem sm;
+  spo_bn_setup(sm, sums, gamma, beta, eps, 256);
+  const int lane = threadIdx.x & 31;
+  for (int64_t p = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; p < T;
+       p += ((int64_t)gridDim.x * blockDim.x) >> 5) {
+    const float* xp = x + p * 256 + 8 * lane;
+    const float4 a = *reinterpret_cast<const float4*>(xp), c = *reinterpret_cast<const float4*>(xp + 4);
+    float v[8] = {a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w};
+    float ss = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      v[e] = spo_bn(sm, 8 * lane + e, v[e]);
+      ss += v[e] * v[e];
+    }
+    ss = warp_sum(ss);
+    const float r = 1.f / fmaxf(sqrtf(ss), 1e-12f);
+    float* op = out + p * 256 + 8 * lane;
+    *reinterpret_cast<float4*>(op) = make_float4(v[0] * r, v[1] * r, v[2] * r, v[3] * r);
+    *reinterpret_cast<float4*>(op + 4) = make_float4(v[4] * r, v[5] * r, v[6] * r, v[7] * r);
+  }
+}
+
+static int sp_conv1a_launch(bool aff, const float* image, int C, const float* weight, const float* bias,
+                            const float* scale, const float* shift, void* out, int B, int H, int W,
+                            cudaStream_t stream) {
+  LGB_REQUIRE(image && weight && bias && out, kErrInvalid, "sp_conv1a: null pointer");
+  LGB_REQUIRE(!aff || (scale && shift), kErrInvalid, "sp_conv1a: null scale / shift");
+  LGB_REQUIRE(C == 1 || C == 3, kErrInvalid, "sp_conv1a: image has %d channels (1 or 3)", C);
+  LGB_REQUIRE(B > 0 && H > 0 && W > 0, kErrInvalid, "sp_conv1a: empty image");
+  LGB_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, kErrInvalid, "sp_conv1a: out must be 16-byte aligned");
+  const int64_t n = (int64_t)B * H * W * 8;
+  const int blocks = (int)std::min<int64_t>((n + 255) / 256, 65535LL * 16);
+  if (aff)
+    sp_conv1a_kernel<true><<<blocks, 256, 0, stream>>>(image, C, weight, bias, static_cast<__nv_bfloat16*>(out), B,
+                                                        H, W, scale, shift);
+  else
+    sp_conv1a_kernel<false><<<blocks, 256, 0, stream>>>(image, C, weight, bias, static_cast<__nv_bfloat16*>(out), B,
+                                                         H, W, nullptr, nullptr);
+  return check_launch("sp_conv1a");
+}
+
 }  // namespace lgb
 
 using namespace lgb;
@@ -645,60 +894,14 @@ extern "C" {
 
 int lgb200_sp_conv1a(const float* image, int C, const float* weight, const float* bias, void* out, int B, int H,
                      int W, cudaStream_t stream) {
-  LGB_REQUIRE(image && weight && bias && out, kErrInvalid, "sp_conv1a: null pointer");
-  LGB_REQUIRE(C == 1 || C == 3, kErrInvalid, "sp_conv1a: image has %d channels (1 or 3)", C);
-  LGB_REQUIRE(B > 0 && H > 0 && W > 0, kErrInvalid, "sp_conv1a: empty image");
-  LGB_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, kErrInvalid, "sp_conv1a: out must be 16-byte aligned");
-  const int64_t n = (int64_t)B * H * W * 8;
-  const int blocks = (int)std::min<int64_t>((n + 255) / 256, 65535LL * 16);
-  sp_conv1a_kernel<<<blocks, 256, 0, stream>>>(image, C, weight, bias, static_cast<__nv_bfloat16*>(out), B, H, W);
-  return check_launch("sp_conv1a");
+  return sp_conv1a_launch(false, image, C, weight, bias, nullptr, nullptr, out, B, H, W, stream);
 }
 
 int lgb200_sp_conv(const void* x, int ldx, const void* weight, const float* bias, void* out, int B, int H, int W,
                    int Cin, int Cout, int ksize, int epilogue, cudaStream_t stream) {
-  LGB_REQUIRE(x && weight && bias && out, kErrInvalid, "sp_conv: null pointer");
-  LGB_REQUIRE(B > 0 && H > 0 && W > 0 && B <= 65535, kErrInvalid, "sp_conv: bad extents B=%d H=%d W=%d", B, H, W);
-  LGB_REQUIRE(ksize == 1 || ksize == 3, kErrInvalid, "sp_conv: ksize %d (1 or 3)", ksize);
-  LGB_REQUIRE(Cin % 64 == 0 && Cin > 0 && ldx >= Cin && ldx % 8 == 0, kErrInvalid,
-              "sp_conv: Cin %d must be a multiple of 64 and ldx %d >= Cin a multiple of 8", Cin, ldx);
-  LGB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(weight)) & 15) == 0, kErrInvalid,
-              "sp_conv: x and weight must be 16-byte aligned");
-  const int ty = (H + SP_TY - 1) / SP_TY;
-  auto grid_ok = [&](int tiles_n) { return (int64_t)ty * tiles_n <= 65535; };
-  switch (epilogue) {
-    case SP_EP_RELU:
-    case SP_EP_POOL: {
-      LGB_REQUIRE(Cout % 64 == 0, kErrInvalid, "sp_conv: Cout %d must be a multiple of 64", Cout);
-      if (Cout == 64) {
-        LGB_REQUIRE(grid_ok(1), kErrInvalid, "sp_conv: image too tall");
-        return epilogue == SP_EP_RELU
-                   ? launch_sp_conv<64, SP_EP_RELU>((const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)weight, bias,
-                                                    out, B, H, W, Cin, Cout, ksize, 1, stream)
-                   : launch_sp_conv<64, SP_EP_POOL>((const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)weight, bias,
-                                                    out, B, H, W, Cin, Cout, ksize, 1, stream);
-      }
-      LGB_REQUIRE(Cout % 128 == 0 && grid_ok(Cout / 128), kErrInvalid, "sp_conv: Cout %d (64 or a multiple of 128)",
-                  Cout);
-      return epilogue == SP_EP_RELU
-                 ? launch_sp_conv<128, SP_EP_RELU>((const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)weight, bias,
-                                                   out, B, H, W, Cin, Cout, ksize, Cout / 128, stream)
-                 : launch_sp_conv<128, SP_EP_POOL>((const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)weight, bias,
-                                                   out, B, H, W, Cin, Cout, ksize, Cout / 128, stream);
-    }
-    case SP_EP_SOFTMAX:
-      LGB_REQUIRE(Cout == 65 && grid_ok(1), kErrInvalid, "sp_conv: the softmax epilogue takes Cout 65 (got %d)", Cout);
-      return launch_sp_conv<128, SP_EP_SOFTMAX>((const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)weight, bias, out,
-                                                B, H, W, Cin, Cout, ksize, 1, stream);
-    case SP_EP_L2N:
-      LGB_REQUIRE(Cout == 256 && grid_ok(1), kErrInvalid, "sp_conv: the normalising epilogue takes Cout 256 (got %d)",
-                  Cout);
-      LGB_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, kErrInvalid, "sp_conv: out must be 16-byte aligned");
-      return launch_sp_conv<256, SP_EP_L2N>((const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)weight, bias, out, B,
-                                            H, W, Cin, Cout, ksize, 1, stream);
-    default:
-      LGB_REQUIRE(false, kErrInvalid, "sp_conv: unknown epilogue %d", epilogue);
-  }
+  LGB_REQUIRE(epilogue != SP_EP_RAW, kErrInvalid, "sp_conv: unknown epilogue %d", epilogue);
+  return sp_conv_dispatch<false>(x, ldx, weight, bias, nullptr, nullptr, out, B, H, W, Cin, Cout, ksize, epilogue,
+                                 stream);
 }
 
 int lgb200_sp_nms(const float* scores, const float* image_size, float* out, int B, int H, int W, int radius,
@@ -754,6 +957,59 @@ int lgb200_sp_sample(const float* desc, const float* keypoints, float* out, int 
   else
     sp_sample_kernel<4><<<blocks, 256, 0, stream>>>(desc, keypoints, out, B, K, h, w, legacy);
   return check_launch("sp_sample");
+}
+
+int lgb200_spo_conv1a(const float* image, int C, const float* weight, const float* bias, const float* scale,
+                      const float* shift, void* out, int B, int H, int W, cudaStream_t stream) {
+  return sp_conv1a_launch(true, image, C, weight, bias, scale, shift, out, B, H, W, stream);
+}
+
+int lgb200_spo_conv(const void* x, int ldx, const void* weight, const float* bias, const float* scale,
+                    const float* shift, void* out, int B, int H, int W, int Cin, int Cout, int ksize, int epilogue,
+                    cudaStream_t stream) {
+  return sp_conv_dispatch<true>(x, ldx, weight, bias, scale, shift, out, B, H, W, Cin, Cout, ksize, epilogue, stream);
+}
+
+int lgb200_spo_bn_apply(const void* x, const double* sums, const float* gamma, const float* beta, float eps,
+                        void* out, int B, int H, int W, int C, int op, cudaStream_t stream) {
+  LGB_REQUIRE(x && sums && gamma && beta && out && x != out, kErrInvalid, "spo_bn_apply: null or aliased pointer");
+  LGB_REQUIRE(B > 0 && H > 0 && W > 0, kErrInvalid, "spo_bn_apply: bad extents B=%d H=%d W=%d", B, H, W);
+  LGB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out)) & 15) == 0, kErrInvalid,
+              "spo_bn_apply: x and out must be 16-byte aligned");
+  const int64_t T = (int64_t)B * H * W;
+  auto grid = [&](int64_t threads) {
+    return (unsigned)std::min<int64_t>((threads + SPO_BN_THREADS - 1) / SPO_BN_THREADS, 8LL * device_sm_count());
+  };
+  switch (op) {
+    case SPO_BN_PLAIN:
+    case SPO_BN_POOL: {
+      LGB_REQUIRE(C >= 8 && C <= SPO_BN_MAXC && (C & (C - 1)) == 0, kErrUnsupported,
+                  "spo_bn_apply: C %d is not a power of two in [8, %d]", C, SPO_BN_MAXC);
+      LGB_REQUIRE(op == SPO_BN_PLAIN || (H >= 2 && W >= 2), kErrInvalid, "spo_bn_apply: %dx%d map too small to pool",
+                  H, W);
+      const int64_t n = op == SPO_BN_PLAIN ? T * (C / 8) : (int64_t)B * (H / 2) * (W / 2) * (C / 8);
+      if (op == SPO_BN_PLAIN)
+        spo_bn_nhwc_kernel<SPO_BN_PLAIN><<<grid(n), SPO_BN_THREADS, 0, stream>>>(
+            (const __nv_bfloat16*)x, sums, gamma, beta, eps, (__nv_bfloat16*)out, B, H, W, C);
+      else
+        spo_bn_nhwc_kernel<SPO_BN_POOL><<<grid(n), SPO_BN_THREADS, 0, stream>>>(
+            (const __nv_bfloat16*)x, sums, gamma, beta, eps, (__nv_bfloat16*)out, B, H, W, C);
+      break;
+    }
+    case SPO_BN_SOFTMAX:
+      LGB_REQUIRE(C == 65, kErrInvalid, "spo_bn_apply: the softmax op takes C 65 (got %d)", C);
+      spo_bn_softmax_kernel<<<grid(T * 16), SPO_BN_THREADS, 0, stream>>>((const float*)x, sums, gamma, beta, eps,
+                                                                        (float*)out, B, H, W);
+      break;
+    case SPO_BN_L2N:
+      LGB_REQUIRE(C == 256, kErrInvalid, "spo_bn_apply: the normalising op takes C 256 (got %d)", C);
+      spo_bn_l2n_kernel<<<grid(T * 32), SPO_BN_THREADS, 0, stream>>>((const float*)x, sums, gamma, beta, eps,
+                                                                    (float*)out, T);
+      break;
+    default:
+      LGB_REQUIRE(false, kErrInvalid, "spo_bn_apply: unknown op %d", op);
+  }
+  return check_launch("spo_bn_apply");
 }
 
 }  // extern "C"

@@ -97,6 +97,32 @@ def select(nms_scores, threshold, k, cap, uniform=None, pad_hi=None):
     return kpts, scores, counts
 
 
+def select_keypoints(s, threshold, max_kps, force, image_size, image_hw):
+    """Keypoints [B, n, 2] (x, y) and scores [B, n] from the NMS'd score map s [B, H, W].  With `force` (max_kps > 0):
+    n = max_kps, padded on the device inside the kept keypoints' range, or (0, min(image_size)) when none is kept
+    (image_size [B, 2] on the device, or None for the image's own (H, W) = image_hw); nothing is read back to the host.
+    Without it: every image's count is read back and must agree, as torch.stack requires."""
+    B = s.shape[0]
+    dev = s.device
+    if force:
+        if max_kps <= 0:
+            raise AssertionError("force_num_keypoints needs max_num_keypoints > 0")
+        uniform = torch.rand(B, max_kps, 2, device=dev)
+        if image_size is not None:
+            pad_hi = image_size.min().reshape(1)
+        else:
+            pad_hi = torch.full((1,), float(min(image_hw)), device=dev)
+        kpts, kscores, _ = select(s, threshold, max_kps, max_kps, uniform, pad_hi)
+    else:
+        counts = count(s, threshold).tolist()
+        kept = [min(c, max_kps) if max_kps > 0 else c for c in counts]
+        if any(c != kept[0] for c in kept):
+            raise RuntimeError(f"stack expects each tensor to be equal size, but got keypoint counts {kept}: pass "
+                               "force_num_keypoints with B > 1")
+        kpts, kscores, _ = select(s, threshold, max_kps, kept[0])
+    return kpts, kscores
+
+
 def sample(desc_nhwc, kpts, legacy):
     """L2-normalised bilinear samples [B, K, C] of desc [B, h, w, C] fp32 at kpts [B, K, 2] (score-map pixels)."""
     B, h, w, C = desc_nhwc.shape
@@ -271,7 +297,6 @@ class SuperPoint(nn.Module):
 
     def _sparse(self, data, image, scores, desc):
         conf = self.conf
-        B = image.shape[0]
         dev = image.device
         image_size = data.get("image_size")
         if image_size is not None:
@@ -280,22 +305,8 @@ class SuperPoint(nn.Module):
         max_kps = conf.max_num_keypoints
         if not self.training and conf.max_num_keypoints_val is not None:
             max_kps = conf.max_num_keypoints_val
-        if conf.force_num_keypoints:
-            if max_kps <= 0:
-                raise AssertionError("force_num_keypoints needs max_num_keypoints > 0")
-            uniform = torch.rand(B, max_kps, 2, device=dev)
-            if image_size is not None:
-                pad_hi = image_size.min().reshape(1)
-            else:
-                pad_hi = torch.full((1,), float(min(image.shape[-2:])), device=dev)
-            kpts, kscores, _ = select(s, conf.detection_threshold, max_kps, max_kps, uniform, pad_hi)
-        else:
-            counts = count(s, conf.detection_threshold).tolist()
-            kept = [min(c, max_kps) if max_kps > 0 else c for c in counts]
-            if any(c != kept[0] for c in kept):
-                raise RuntimeError(f"stack expects each tensor to be equal size, but got keypoint counts {kept}: pass "
-                                   "force_num_keypoints with B > 1")
-            kpts, kscores, _ = select(s, conf.detection_threshold, max_kps, kept[0])
+        kpts, kscores = select_keypoints(s, conf.detection_threshold, max_kps, conf.force_num_keypoints, image_size,
+                                         image.shape[-2:])
         pred = {
             "keypoints": kpts + 0.5,
             "keypoint_scores": kscores,

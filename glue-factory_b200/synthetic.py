@@ -453,3 +453,35 @@ def make_superpoint_images(B, C, H, W, seed=0):
             img += 0.5 * (xx > rs.uniform(0, W)) * (yy > rs.uniform(0, H))
             out[b, c] = (img - img.min()) / (img.max() - img.min())
     return torch.from_numpy(out)
+
+
+def make_superpoint_open_weights(state_dict_like, seed=0, dtype=torch.float32):
+    """Deterministic SuperPoint-open weights (names / shapes from `state_dict_like`).  Convs as
+    make_superpoint_weights (He-uniform, biases U(-0.05, 0.05)), detector.1's weights 4x larger so that keypoints
+    clear the detection threshold.  BatchNorms: gamma of either sign with |gamma| in [0.5, 1.5] (a 2x2 max-pool placed
+    before the affine gives a different map), beta U(-0.1, 0.1), running_mean U(0, 0.5), running_var U(0.5, 2),
+    num_batches_tracked 0."""
+    rs = np.random.RandomState(seed)
+    out = {}
+    for k, v in state_dict_like.items():
+        shp = tuple(v.shape)
+        if k.endswith("num_batches_tracked"):
+            out[k] = torch.zeros((), dtype=torch.long)
+            continue
+        if k.endswith("conv.weight"):
+            bound = math.sqrt(6.0 / (shp[1] * shp[2] * shp[3])) * (4.0 if k.startswith("detector.1") else 1.0)
+            w = rs.uniform(-bound, bound, size=shp)
+        elif k.endswith("conv.bias"):
+            w = rs.uniform(-0.05, 0.05, size=shp)
+        elif k.endswith("bn.weight"):
+            w = rs.uniform(0.5, 1.5, size=shp) * rs.choice([-1.0, 1.0], size=shp)
+        elif k.endswith("bn.bias"):
+            w = rs.uniform(-0.1, 0.1, size=shp)
+        elif k.endswith("running_mean"):
+            w = rs.uniform(0.0, 0.5, size=shp)
+        elif k.endswith("running_var"):
+            w = rs.uniform(0.5, 2.0, size=shp)
+        else:
+            raise KeyError(k)
+        out[k] = torch.from_numpy(w).to(dtype)
+    return out

@@ -618,6 +618,42 @@ int lgb200_sp_select(const float* nms, float threshold, int k, int cap, const fl
 int lgb200_sp_sample(const float* desc, const float* keypoints, float* out, int B, int K, int h, int w, int C,
                      int legacy, cudaStream_t stream);
 
+/* ---- SuperPoint-open, inference only (gluefactory/models/extractors/superpoint_open.py): every conv is a VGGBlock
+ * conv -> ReLU (not after detector.1 / descriptor.1) -> BatchNorm2d, the pools after the BatchNorm (:59-75, :99-115).
+ * Same layouts and kernels as the lgb200_sp_* calls above; the keypoints go through lgb200_sp_nms (image_size NULL:
+ * the fixed border frame of :143-149), lgb200_sp_select and lgb200_sp_sample at kpts + 0.5 (fixed mode: :20-31).
+ * lgb200_spo_conv1a: lgb200_sp_conv1a followed by the eval-mode BatchNorm as a per-channel affine:
+ *   out = ReLU(conv3x3) * scale[c] + shift[c] (backbone.0.0, :101 and :128).
+ * lgb200_spo_conv: lgb200_sp_conv with the eval-mode BatchNorm affine scale / shift [Npad] fp32 (padding zero) in the
+ *   epilogue (:101-115 with running statistics):
+ *   epilogue LGB200_SP_RELU:    ReLU -> affine, bf16
+ *            LGB200_SP_POOL:    ReLU -> affine -> 2x2 max-pool, bf16 (the MaxPool2d after the block, :103)
+ *            LGB200_SP_SOFTMAX: affine -> softmax -> depth-to-space (detector.1 and :134-140)
+ *            LGB200_SP_L2N:     affine -> L2 normalisation (descriptor.1 and :129-131)
+ *            LGB200_SPO_RAW:    conv + bias, no affine (scale / shift unused): out [B, H, W, Npad] fp32 with Npad =
+ *                               Cout rounded up to 128 (the training-mode head logits ahead of their BatchNorm).
+ * lgb200_spo_bn_apply: training-mode BatchNorm2d from batch statistics, sums = [sum x (C) | sum x^2 (C) | count]
+ *   fp64 (lgb200_bn_stats of the pre-BatchNorm activation, possibly summed across ranks); mean and biased variance,
+ *   y = (x - mean) / sqrt(var + eps) * gamma + beta.  x [B, H, W, .] NHWC, out must not alias x.
+ *   op LGB200_SPO_BN_PLAIN:   bf16 C (a power of two in [8, 512]) -> bf16 (:101, :109, :113)
+ *      LGB200_SPO_BN_POOL:    bf16 -> 2x2 floor max-pool -> bf16 [B, H/2, W/2, C] (:101-103)
+ *      LGB200_SPO_BN_SOFTMAX: fp32 [B, H, W, 128] logits, C 65 -> softmax -> depth-to-space fp32 [B, 8H, 8W]
+ *                             (:110 and :134-140)
+ *      LGB200_SPO_BN_L2N:     fp32 C 256 -> L2 normalisation -> fp32 (:114 and :129-131)
+ *   The running statistics are not touched: lgb200_bn_running_update does that step.  No atomics, fixed order.  */
+#define LGB200_SPO_RAW 4
+#define LGB200_SPO_BN_PLAIN 0
+#define LGB200_SPO_BN_POOL 1
+#define LGB200_SPO_BN_SOFTMAX 2
+#define LGB200_SPO_BN_L2N 3
+int lgb200_spo_conv1a(const float* image, int C, const float* weight, const float* bias, const float* scale,
+                      const float* shift, void* out, int B, int H, int W, cudaStream_t stream);
+int lgb200_spo_conv(const void* x, int ldx, const void* weight, const float* bias, const float* scale,
+                    const float* shift, void* out, int B, int H, int W, int Cin, int Cout, int ksize, int epilogue,
+                    cudaStream_t stream);
+int lgb200_spo_bn_apply(const void* x, const double* sums, const float* gamma, const float* beta, float eps,
+                        void* out, int B, int H, int W, int C, int op, cudaStream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
